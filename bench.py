@@ -29,7 +29,7 @@ def _peaks():
   if os.path.exists(path):
     with open(path) as f:
       return float(json.load(f)['hbm_gbs']), 'measured'
-  return 6650.0, 'fallback'
+  return 3350.0, 'H100 SXM data sheet'
 
 
 class ClockSampler(threading.Thread):
@@ -72,8 +72,8 @@ class ClockSampler(threading.Thread):
 
 def usable_cores():
   """Host CPUs this process may actually use: the affinity mask capped by the cgroup CPU
-  quota (cpu.max).  On the GPU boxes 128 logical CPUs are visible but the container's quota
-  is 16; more threads than that only add throttling."""
+  quota (cpu.max).  A container may see many more logical CPUs than its quota lets it use;
+  more threads than the quota only add throttling."""
   try:
     n = len(os.sched_getaffinity(0))
   except AttributeError:
@@ -220,7 +220,7 @@ class Bench(object):
     self.actions = torch.from_numpy(wl.sample_actions(np.random.RandomState(7 + rank), T, E)).to(self.dev)
     self.H, self.W = wl.image_size[1], wl.image_size[0]
     self.frame_bytes = E * self.H * self.W * 3
-    # frame ring larger than L2 (126 MB) so that every step's frame writes reach HBM
+    # frame ring larger than L2 (50 MB on H100) so that every step's frame writes reach HBM
     self.n_ring = max(2, int(np.ceil(160e6 / self.frame_bytes)) + 1)
     self.ring = [self.raster.new_frames() for _ in range(self.n_ring)]
     self.gathered, self.peer, self.inflight, self.n_gslots = None, None, [], 2
@@ -273,18 +273,18 @@ class Bench(object):
       self.wait_for(lambda it: it[2] == dst)   # everyone is done with the step that last used dst
       if self.gather == 'ce':
         # variant: render into this rank's block, then copy-engine pushes to the peers
-        eng.step(self.actions[t % T], raster, peer.own_slab(dst))
+        self.last = eng.step(self.actions[t % T], raster, peer.own_slab(dst))
         self.inflight.append((peer.push(dst), -1, dst))
       else:
         # the per-env records ride along as ONE all-gather behind the kernel (SURVEY 8e); it is also
         # the completion barrier of the frame stores: it cannot finish before every rank's kernel has
-        eng.step_gather(self.actions[t % T], raster, peer.slot(dst))
+        self.last = eng.step_gather(self.actions[t % T], raster, peer.slot(dst))
         self.inflight.append((dist.all_gather_into_tensor(self.out_all[dst], eng.out_bytes, async_op=True),
                               -1, dst))
       return
     self.wait_for(lambda it: it[1] == slot)    # the gather that last read this ring buffer
     fr = self.ring[slot]
-    eng.step(self.actions[t % T], raster, fr)
+    self.last = eng.step(self.actions[t % T], raster, fr)
     if self.world > 1 and gather:
       # the single collective of the path as a separate NCCL all-gather.  It runs on NCCL's
       # stream and overlaps the next step's compute.
@@ -331,18 +331,38 @@ class Bench(object):
       if total >= 1e3 * min_seconds or len(blocks) >= 200:
         return blocks
 
-  def run(self, min_seconds, sampler=None):
-    """Warm-up, the timed blocks, the sharded variant at N > 1 and the render kernel alone."""
+  def outputs(self, max_bytes=64 * 10 ** 6):
+    """What the last step returned to its caller, as float32/float64 host arrays: the per-env
+    reward, step type, success and status, and the frames of a fixed, seeded sample of envs
+    (all of them if they fit) with their env indices, in at most `max_bytes` in all."""
+    last = self.last
+    out = dict(reward=last.reward.cpu().numpy().astype(np.float64),
+               step_type=last.step_type.cpu().numpy().astype(np.float32),
+               success=last.success.cpu().numpy().astype(np.float32),
+               status=last.status.cpu().numpy().astype(np.float32))
+    n_frames = last.frames.shape[0]   # all ranks' envs where the frames are gathered
+    per_env = 4 * self.H * self.W * 3 + 8
+    n = min(n_frames, (max_bytes - sum(a.nbytes for a in out.values())) // per_env)
+    idx = (np.sort(np.random.RandomState(0).choice(n_frames, n, replace=False)) if n < n_frames
+           else np.arange(n_frames))
+    out['frames'] = last.frames[self.torch.from_numpy(idx).to(last.frames.device)].cpu().numpy().astype(np.float32)
+    out['frames_env_index'] = idx.astype(np.float64)
+    return out
+
+  def run(self, min_seconds, sampler=None, keep_outputs=False):
+    """Warm-up, the timed blocks, the sharded variant at N > 1 and the render kernel alone.
+    `keep_outputs`: return the last timed step's outputs (see outputs()) under 'outputs'."""
     torch = self.torch
+    if sampler:   # before the warm-up, so that no idle gap lets the clocks drop before the timed steps
+      sampler.start()
+      time.sleep(0.3)
     for t in range(self.warmup):
       self.one_step(t)
     self.barrier()
-    if sampler:
-      sampler.start()
-      time.sleep(0.3)
     launches0 = self.eng.launch_count()
     blocks = self.timed_blocks(min_seconds, True, self.warmup)
     launches = (self.eng.launch_count() - launches0) // len(blocks)
+    outputs = self.outputs() if keep_outputs else None
     ms = float(np.median(blocks))
     res = dict(value=self.world * self.E * self.steps / (ms * 1e-3), ms_per_step=ms / self.steps,
                launches=int(launches), timed=dict(
@@ -359,7 +379,7 @@ class Bench(object):
       ingest = (self.world - 1) * self.frame_bytes
       res['nvlink'] = dict(ingest_bytes_per_gpu_per_step=int(ingest),
                            achieved_gbs_per_direction_per_gpu=ingest / (ms / self.steps * 1e-3) / 1e9,
-                           nominal_gbs_per_direction=900.0)
+                           nominal_gbs_per_direction=450.0)   # H100 SXM, NVLink 4
     # dominant kernel alone: launches of the render kernel, CUDA events on its stream
     evr0, evr1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     n_r = max(20, min(self.steps, 100))
@@ -372,14 +392,16 @@ class Bench(object):
     evr1.record()
     torch.cuda.synchronize()
     res['render_ms'] = evr0.elapsed_time(evr1) / n_r
+    if outputs is not None:
+      res['outputs'] = outputs
     return res
 
-  def roofline(self, render_ms, traffic=None):
+  def roofline(self, render_ms):
     peak, peak_kind = _peaks()
     alg_bytes = self.wl.algorithmic_bytes() * self.E
     achieved = alg_bytes / (render_ms * 1e-3) / 1e9
     return dict(bound='hbm', achieved=achieved, peak=peak, unit='GB/s', frac=achieved / peak,
-                traffic=traffic, peak_kind=peak_kind, kernel='render_kernel', kernel_ms=render_ms,
+                peak_kind=peak_kind, kernel='render_kernel', kernel_ms=render_ms,
                 algorithmic_bytes_per_launch=alg_bytes)
 
   def e2e(self):
@@ -414,17 +436,6 @@ class Bench(object):
                 d2h_gbs_per_gpu=d2h / (dt / n_e2e) / 1e9,
                 path='swb_step_host: pinned host actions -> H2D -> step+render -> D2H frames, '
                      'reward, step_type, success, status -> stream sync')
-
-
-def _traffic(key):
-  """DRAM bytes per render launch from the committed ncu capture (profiles/traffic.json):
-  a record, not a live measurement -- ncu cannot run inside the timed process."""
-  tpath = os.path.join(ROOT, 'profiles', 'traffic.json')
-  if not os.path.exists(tpath):
-    return None, None
-  with open(tpath) as f:
-    d = json.load(f)
-  return d.get(key), d.get('source')
 
 
 def api_rate(wl, E, local_rank, steps):
@@ -462,7 +473,9 @@ def api_rate(wl, E, local_rank, steps):
 def main():
   ap = argparse.ArgumentParser()
   ap.add_argument('--gpus', type=int, default=1)
-  ap.add_argument('--steps', type=int, default=200)
+  ap.add_argument('--steps', type=int, default=None,
+                  help='timed steps of the headline: one block of exactly this many (default 5000, '
+                       'about 1 s at C2 on an H100; 200 for --impl reference)')
   ap.add_argument('--warmup', type=int, default=20)
   ap.add_argument('--impl', default='b200', choices=['b200', 'reference'])
   ap.add_argument('--workload', default='c2', choices=['c2', 'c3', 'c4', 'c5'])
@@ -471,7 +484,11 @@ def main():
                        '(default: c3,c4,c5 at N=1; c4,c5 at N>1; "none" to skip)')
   ap.add_argument('--envs', type=int, default=0, help='override envs per GPU')
   ap.add_argument('--min-seconds', type=float, default=1.0,
-                  help='the block of --steps timed steps is repeated until this much time is timed')
+                  help='the other configs\' blocks of timed steps are repeated until this much time '
+                       'is timed; the headline times exactly --steps steps and warns if they took '
+                       'less than this')
+  ap.add_argument('--dump-outputs', default=None, metavar='DIR',
+                  help='write what the last timed headline step computed to DIR/<name>.npy')
   ap.add_argument('--gather', default='peer', choices=['peer', 'ce', 'nccl'],
                   help='N>1 frame gather: stores into peer memory from the render kernel, or a '
                        'separate NCCL all-gather')
@@ -481,6 +498,8 @@ def main():
   args = ap.parse_args()
   if args.warmup < 3:
     args.warmup = 3
+  if args.steps is None:
+    args.steps = 200 if args.impl == 'reference' else 5000
   from spriteworld_b200 import workloads
   wl = workloads.WORKLOADS[args.workload]()
   if args.impl == 'reference':
@@ -509,8 +528,18 @@ def main():
 
   sampler = ClockSampler(local_rank) if rank == 0 else None
   b = Bench(wl, args, world, rank, local_rank, args.steps, args.warmup, E=args.envs or None)
-  res = b.run(args.min_seconds, sampler)
+  # one block of exactly --steps timed steps: the same arguments then end in the same state, so
+  # the dumped outputs of two builds can be compared
+  res = b.run(0, sampler, keep_outputs=bool(args.dump_outputs) and rank == 0)
+  if rank == 0 and res['timed']['seconds'] < args.min_seconds:
+    sys.stderr.write('warning: the headline block of %d steps took %.3f s (< --min-seconds %.1f): '
+                     'the number is dominated by clock and scheduler noise; raise --steps\n'
+                     % (args.steps, res['timed']['seconds'], args.min_seconds))
   clocks = sampler.stop() if sampler else None
+  if 'outputs' in res:
+    os.makedirs(args.dump_outputs, exist_ok=True)
+    for name, a in res.pop('outputs').items():
+      np.save(os.path.join(args.dump_outputs, name + '.npy'), a)
   e2e = None if args.no_e2e else b.e2e()
   collective = ('none' if world == 1 else
                 'frames stored into every rank\'s gathered buffer by the render kernel '
@@ -529,10 +558,7 @@ def main():
                       'configs are under "configs", measured in the same run')
   if numa is not None:
     cfg['numa_node'] = numa
-  traffic, traffic_src = _traffic(args.workload)
-  roof = b.roofline(res['render_ms'], traffic)
-  if traffic_src:
-    roof['traffic_source'] = traffic_src
+  roof = b.roofline(res['render_ms'])
   headline_E = b.E
   b.close()
 
@@ -556,10 +582,9 @@ def main():
     w2 = workloads.WORKLOADS[key]()
     b2 = Bench(w2, args, world, rank, local_rank, min(args.steps, 100), 5)
     r2 = b2.run(min(args.min_seconds, 0.5))
-    t2, _ = _traffic(key)
     entry = dict(value=r2['value'], unit=UNIT, ms_per_step=r2['ms_per_step'], n_gpus=world,
                  config=workload_config(w2, b2.E), timed=r2['timed'],
-                 roofline=b2.roofline(r2['render_ms'], t2), gpu_launches=r2['launches'])
+                 roofline=b2.roofline(r2['render_ms']), gpu_launches=r2['launches'])
     for k in ('frames_sharded', 'nvlink'):
       if k in r2:
         entry[k] = r2[k]

@@ -1,2 +1,2 @@
-"""spriteworld_b200: B200-native batched Spriteworld step+render engine."""
+"""spriteworld_b200: H100-native batched Spriteworld step+render engine."""
 __version__ = '0.1.0'

@@ -85,7 +85,7 @@ def load():
   if not os.path.exists(_LIB_PATH):
     raise NativeError(
         'spriteworld_b200: %s is missing. Build it with `python -m spriteworld_b200.build` '
-        '(nvcc, sm_100a). There is no CPU fallback.' % _LIB_PATH)
+        '(nvcc, sm_90a). There is no CPU fallback.' % _LIB_PATH)
   L = ctypes.CDLL(_LIB_PATH)
   vp, ci = ctypes.c_void_p, ctypes.c_int32
   L.swb_last_error.restype = ctypes.c_char_p

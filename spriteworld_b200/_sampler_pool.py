@@ -2,7 +2,8 @@
 
 `init_sprites()` stays on the host (north_star), and in Python: a scene costs about 2-3 us to
 draw and pack with NumPy, GIL-bound, so threads do not scale it.  At C2's reset rate (every env
-every 20 steps) 4096 envs at 20 M env-steps/s want ~1 M scenes/s; a few processes deliver that.
+every 20 steps) the ~18.6 M env-steps/s of C2 on an H100 want ~0.9 M scenes/s, more than one
+core draws.
 Each worker holds the generator, the task filters and the colour map (sent once, cloudpickle:
 generators are closures), receives (n, seed) and writes the packed scene arrays
 (scene.arrays_from_layout: what the in-process path uploads) into its block of POSIX shared
@@ -90,7 +91,7 @@ class SamplerPool(object):
     self._n_slots, self._cap = int(n_slots), int(capacity)
     self.worker_seconds = 0.0   # time the workers spent sampling and packing (summed)
     # The workers run single-threaded NumPy.  Without this every worker starts an OpenBLAS/OpenMP
-    # pool of one thread per visible CPU (64 on the GPU boxes, whose containers may use 16):
+    # pool of one thread per visible CPU, and a container may see many more CPUs than it may use:
     # hundreds of threads spinning at start-up exhaust the container's CPU quota and the cgroup
     # throttles the whole process tree for seconds.
     pinned = ('OMP_NUM_THREADS', 'OPENBLAS_NUM_THREADS', 'MKL_NUM_THREADS', 'NUMEXPR_NUM_THREADS')

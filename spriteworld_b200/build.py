@@ -1,4 +1,4 @@
-"""Builds spriteworld_b200/csrc/libspriteworld_b200.so with nvcc for sm_100a (in-tree), and the
+"""Builds spriteworld_b200/csrc/libspriteworld_b200.so with nvcc for sm_90a (in-tree), and the
 small host-side helper csrc/libswb_host.so (C, gcc: scene packing for the batched environment's
 refill; optional -- without it the NumPy path runs).
 
@@ -16,7 +16,7 @@ HEADERS = ['swb_device.cuh', 'swb_render.cuh', 'swb_step.cuh', 'swb_tables.h',
            os.path.join('..', '..', 'include', 'spriteworld_b200.h')]
 
 NVCC_FLAGS = [
-    '-gencode', 'arch=compute_100a,code=sm_100a', '-O3', '-lineinfo', '-std=c++17',
+    '-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17',
     # parity: the reference's float/double arithmetic is never FMA-contracted
     '-fmad=false',
     '-Xcompiler', '-fPIC', '-shared', '-lcudart',
@@ -31,10 +31,13 @@ def _nvcc():
 
 
 def is_stale():
+  """True if the library is missing or older than its sources or this file (which holds the
+  compiler flags, e.g. the target architecture)."""
   if not os.path.exists(LIB):
     return True
   t = os.path.getmtime(LIB)
-  return any(os.path.getmtime(os.path.join(CSRC, f)) > t for f in SOURCES + HEADERS)
+  inputs = [os.path.join(CSRC, f) for f in SOURCES + HEADERS] + [os.path.abspath(__file__)]
+  return any(os.path.getmtime(f) > t for f in inputs)
 
 
 HOST_LIB = os.path.join(CSRC, 'libswb_host.so')
@@ -45,7 +48,8 @@ HOST_FLAGS = ['-O3', '-ffp-contract=off', '-fPIC', '-shared', '-Wall', '-Wextra'
 
 def build_host(force=False):
   """libswb_host.so (gcc).  Returns its path, or None if there is no C compiler."""
-  if not force and os.path.exists(HOST_LIB) and os.path.getmtime(HOST_LIB) >= os.path.getmtime(HOST_SRC):
+  if not force and os.path.exists(HOST_LIB) and os.path.getmtime(HOST_LIB) >= max(
+      os.path.getmtime(HOST_SRC), os.path.getmtime(os.path.abspath(__file__))):
     return HOST_LIB
   cc = shutil.which('gcc') or shutil.which('cc')
   if not cc:

@@ -176,7 +176,7 @@ int swb_engine_create(const swb_config *cfg, swb_engine **out) {
   eng->device = cfg->device;
   if (cudaDeviceGetAttribute(&eng->n_sms, cudaDevAttrMultiProcessorCount, cfg->device) != cudaSuccess ||
       eng->n_sms < 1)
-    eng->n_sms = 148;
+    eng->n_sms = 132;
   StepCfg &sc = eng->step_cfg;
   memset(&sc, 0, sizeof sc);
   sc.action_kind = cfg->action_kind;

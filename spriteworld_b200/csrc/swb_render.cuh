@@ -224,7 +224,7 @@ __device__ __forceinline__ void mma_u8s8(int (&d)[4], const uint32_t (&a)[4], co
 
 // The kernel's dynamic shared memory, at namespace scope so that its shared-window address
 // can be taken by name (mov.u32 r, symbol: a link-time constant; converting a generic pointer
-// costs five instructions on sm_100 and is rematerialised at every use)
+// costs extra instructions and is rematerialised at every use)
 extern __shared__ __align__(16) unsigned char g_render_smem[];
 __device__ __forceinline__ uint32_t render_smem_base() {
   uint32_t a;

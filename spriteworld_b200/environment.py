@@ -1,4 +1,4 @@
-"""Spriteworld environments on the B200 engine.
+"""Spriteworld environments on the H100 engine.
 
 `Environment` is the drop-in for the reference's `spriteworld/environment.py:27-161`: same
 constructor, `reset()/step()/observation_spec()/action_spec()/state()/success()`, dm_env
@@ -67,7 +67,7 @@ def _require_compilable(task, action_space):
     if missing:
       raise NotImplementedError(
           '%s %r cannot run on the device: it has no %s(). User-defined tasks and action spaces '
-          '(the reference accepts any duck-typed object) are out of scope of the B200 engine; '
+          '(the reference accepts any duck-typed object) are out of scope of the GPU engine; '
           'compose spriteworld_b200.tasks / action_spaces classes instead.'
           % (what, type(obj).__name__, '/'.join(missing)))
 
@@ -290,9 +290,8 @@ class BatchedEnvironment(object):
         RandomState drawn from `rng`, so what a block draws does not depend on timing).
       refill_procs: worker processes that sample and pack the blocks' scenes at the same time
         (_sampler_pool; NumPy sampling is GIL-bound, threads do not scale it).  0 (default): the
-        refill thread samples block after block.  Opt-in: in isolation eight workers deliver
-        2 M scenes/s on the GPU box, but next to a stepping process they were measured running
-        one after the other there (DESIGN.md section 4), slower than the in-process sampler.
+        refill thread samples block after block.  Opt-in: next to a stepping process the
+        workers have been seen running one after the other (DESIGN.md section 4).
     """
     self._task, self._action_space = task, action_space
     self._renderers = renderers

@@ -1,4 +1,4 @@
-"""Generates tests/golden/*.npz by RUNNING THE UNMODIFIED REFERENCE.
+"""Generates tests/golden/*.npz and *.json by RUNNING THE UNMODIFIED REFERENCE.
 
 Run in the build container only (needs /root/reference):
 
@@ -6,9 +6,11 @@ Run in the build container only (needs /root/reference):
 
 The reference is imported through oracle/refshim (alias patches + stand-ins for the
 absent matplotlib/dm_env; SURVEY.md App. E).  Nothing here is used at test time except
-the .npz files it writes; /root/reference does not exist on the GPU box.
+the files it writes; /root/reference does not exist on the GPU box.
 
 Fixtures
+  reference_surface.json  public classes (attributes, constructor parameters) and functions
+                     (parameters) of the reference's modules on and around the path
   render_cases.npz   scenes (sprite factor arrays) + the frames PILRenderer produced
   episodes_<cfg>.npz per-env scene pools, action scripts and the per-step outputs of
                      Environment.step (positions, reward, step_type, success, frames)
@@ -436,7 +438,50 @@ def sampling_cases(seed=5, n_scenes=12):
   print('sampling.npz: %d config/mode pairs' % (len(blob) // 7))
 
 
+SURFACE_MODULES = [
+    'action_spaces', 'constants', 'environment', 'factor_distributions', 'gym_wrapper', 'shapes',
+    'sprite', 'sprite_generators', 'tasks', 'renderers', 'renderers.abstract_renderer',
+    'renderers.color_maps', 'renderers.handcrafted', 'renderers.pil_renderer',
+    'configs.cobra.common']
+
+
+def reference_surface():
+  """reference_surface.json: every public class (its public attributes and constructor
+  parameters), function (its parameters) and other name of the reference's modules on and
+  around the path (demo_ui / run_demo / example_run_loop are out of scope, DESIGN.md section 8)."""
+  import importlib
+  import importlib.util
+  import inspect
+  # the reference's gym_wrapper needs gym; the reference's own tests/ shadows ours on sys.path
+  spec = importlib.util.spec_from_file_location(
+      'swb_reference_suite', os.path.join(ROOT, 'tests', 'test_reference_suite.py'))
+  suite = importlib.util.module_from_spec(spec)
+  spec.loader.exec_module(suite)
+  sys.modules.update({k: v for k, v in suite._third_party_stand_ins().items() if k.startswith('gym')})
+  surface = {}
+  for m in SURFACE_MODULES:
+    ref = importlib.import_module('spriteworld.' + m)
+    names = surface[m] = {}
+    for name, obj in vars(ref).items():
+      if name.startswith('_') or inspect.ismodule(obj) or type(obj).__name__ == '_Feature':
+        continue   # private, submodule, `from __future__ import ...`
+      if getattr(obj, '__module__', ref.__name__) != ref.__name__ and (
+          inspect.isclass(obj) or inspect.isfunction(obj)) and m != 'renderers':
+        continue   # imported helper; `renderers` re-exports its classes on purpose
+      entry = names[name] = {}
+      if inspect.isclass(obj):
+        entry['attrs'] = sorted(a for a in vars(obj) if not a.startswith('_'))
+        if '__init__' in vars(obj):
+          entry['init'] = [p for p in inspect.signature(obj.__init__).parameters if p != 'self']
+      elif inspect.isfunction(obj):
+        entry['params'] = list(inspect.signature(obj).parameters)
+  with open(os.path.join(OUT, 'reference_surface.json'), 'w') as f:
+    json.dump(surface, f, indent=1, sort_keys=True)
+    f.write('\n')
+
+
 def main():
+  reference_surface()
   sampling_cases()
   render_cases()
   run_episodes('goal_finding', bench_like_goal_finding, n_envs=12, n_steps=60, n_slots=5,

@@ -7,7 +7,8 @@ are; the ones that call tasks, action spaces, the PIL renderer or whole environm
 device, so here the engine is replaced by the oracle-backed double (tests/oracle_engine.py):
 what is under test is this package's host layer -- task / action compilation, scene packing,
 the plugin protocol, the config modules -- the device arithmetic has its own parity tests
-(`-m gpu`).  Skipped where /root/reference does not exist (the GPU boxes).
+(`-m gpu`).  The runs of the reference's test files are skipped where the reference is not
+installed (SPRITEWORLD_REFERENCE).
 """
 import importlib
 import importlib.abc
@@ -20,7 +21,7 @@ import pytest
 
 REF_TESTS = os.path.join(os.environ.get('SPRITEWORLD_REFERENCE', '/root/reference'), 'tests')
 
-pytestmark = pytest.mark.skipif(not os.path.isdir(REF_TESTS), reason='reference tests not present')
+needs_reference = pytest.mark.skipif(not os.path.isdir(REF_TESTS), reason='reference tests not present')
 
 
 class _Alias(importlib.abc.MetaPathFinder, importlib.abc.Loader):
@@ -99,6 +100,7 @@ def _run(rel):
   return result.testsRun, problems
 
 
+@needs_reference
 @pytest.mark.parametrize('rel,n_tests', [
     ('factor_distributions_test', 39), ('sprite_generators_test', 7), ('shapes_test', 21),
     ('sprite_test', 16), ('renderers/handcrafted_test', 24)])
@@ -108,6 +110,7 @@ def test_reference_host_tests(reference_alias, rel, n_tests):
   assert ran == n_tests
 
 
+@needs_reference
 @pytest.mark.parametrize('rel,n_tests', [
     ('tasks_test', 85), ('action_spaces_test', 30), ('renderers/pil_renderer_test', 5),
     ('configs/configs_test', 8), ('environment_test', 7), ('gym_wrapper_test', 2)])
@@ -119,53 +122,27 @@ def test_reference_protocol_tests_on_oracle_engine(reference_alias, monkeypatch,
   assert ran == n_tests
 
 
-SURFACE_MODULES = [
-    'action_spaces', 'constants', 'environment', 'factor_distributions', 'gym_wrapper', 'shapes',
-    'sprite', 'sprite_generators', 'tasks', 'renderers', 'renderers.abstract_renderer',
-    'renderers.color_maps', 'renderers.handcrafted', 'renderers.pil_renderer',
-    'configs.cobra.common']
-
-
 def test_public_surface_of_the_reference_is_present():
   """Every public class, function, method and constructor parameter of the reference's modules
-  on and around the path exists under the same name in spriteworld_b200 (demo_ui / run_demo /
-  example_run_loop are out of scope, DESIGN.md section 8)."""
+  on and around the path (as recorded from the reference in tests/golden/reference_surface.json
+  by tests/golden/make_golden.py) exists under the same name in spriteworld_b200."""
   import inspect
-  from oracle.refshim import loader
-  stand_ins = _third_party_stand_ins()
-  sys.modules.update(stand_ins)
-  try:
-    loader.load_reference()
-    missing = []
-    for m in SURFACE_MODULES:
-      ref = importlib.import_module('spriteworld.' + m)
-      ours = importlib.import_module('spriteworld_b200.' + m)
-      for name, obj in vars(ref).items():
-        if name.startswith('_') or inspect.ismodule(obj) or type(obj).__name__ == '_Feature':
-          continue   # private, submodule, `from __future__ import ...`
-        if getattr(obj, '__module__', ref.__name__) != ref.__name__ and (
-            inspect.isclass(obj) or inspect.isfunction(obj)) and m != 'renderers':
-          continue   # imported helper; `renderers` re-exports its classes on purpose
-        if not hasattr(ours, name):
-          missing.append('%s.%s' % (m, name))
-          continue
-        mine = getattr(ours, name)
-        if inspect.isclass(obj):
-          missing += ['%s.%s.%s' % (m, name, a) for a in vars(obj)
-                      if not a.startswith('_') and not hasattr(mine, a)]
-          if '__init__' in vars(obj):
-            want = [p for p in inspect.signature(obj.__init__).parameters if p != 'self']
-            have = [p for p in inspect.signature(mine.__init__).parameters if p != 'self']
-            if want != have[:len(want)]:
-              missing.append('%s.%s(%s)' % (m, name, ', '.join(want)))
-        elif inspect.isfunction(obj):
-          want = list(inspect.signature(obj).parameters)
-          have = list(inspect.signature(mine).parameters)
-          if want != have[:len(want)]:
-            missing.append('%s.%s(%s)' % (m, name, ', '.join(want)))
-    assert not missing, missing
-  finally:
-    for name in stand_ins:
-      sys.modules.pop(name, None)
-    for name in [n for n in sys.modules if n == 'spriteworld' or n.startswith('spriteworld.')]:
-      del sys.modules[name]
+  import json
+  with open(os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden',
+                         'reference_surface.json')) as f:
+    surface = json.load(f)
+  missing = []
+  for m, names in sorted(surface.items()):
+    ours = importlib.import_module('spriteworld_b200.' + m)
+    for name, entry in sorted(names.items()):
+      if not hasattr(ours, name):
+        missing.append('%s.%s' % (m, name))
+        continue
+      mine = getattr(ours, name)
+      missing += ['%s.%s.%s' % (m, name, a) for a in entry.get('attrs', ()) if not hasattr(mine, a)]
+      for key, fn in (('init', lambda: mine.__init__), ('params', lambda: mine)):
+        if key in entry:
+          have = [p for p in inspect.signature(fn()).parameters if p != 'self']
+          if entry[key] != have[:len(entry[key])]:
+            missing.append('%s.%s(%s)' % (m, name, ', '.join(entry[key])))
+  assert not missing, missing

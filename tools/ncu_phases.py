@@ -21,8 +21,9 @@ print('total inst (line-attributed)',tot,'samples',tots)
 for k,a in sorted(agg.items(), key=lambda kv:-kv[1][0])[:top]:
     print('%9d %5.1f%% samp %5.1f%%  %s:%d  %s'%(a[0],100*a[0]/tot,100*a[1]/max(tots,1),k[0],k[1],a[2][:95]))
 print('--- buckets')
+import os
 import re
-SRC='/root/repo/spriteworld_b200/csrc/swb_render.cuh'
+SRC=os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), 'spriteworld_b200', 'csrc', 'swb_render.cuh')
 marks=[('A',r'// ---- phase A'),('B_pre',r'// ---- phase B'),('B1',r'^    // B1$'),('B2',r'^    // B2$'),('bgfill',r'// background fill'),('C_pre',r'// ---- phase C'),('H',r'---- H pass'),('V',r'---- V pass'),('D',r'// ---- phase D')]
 lines=open(SRC).read().split('\n')
 starts=[]
