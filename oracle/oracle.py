@@ -142,10 +142,14 @@ def polygon_fill(canvas, xy, rgb, corner_join=1):
 
 
 def lanczos_resize(img, out_w, out_h, return_hpass=False):
+  """Image.resize(..., LANCZOS).  return_hpass: also the first pass's image when both sizes
+  change: (h, out_w) for the horizontal pass, or (out_h, w) for an image more than 100 times
+  taller than wide, which Pillow shrinks vertically first."""
   img = np.ascontiguousarray(img, dtype=np.uint8)
   h, w = img.shape[:2]
   out = np.empty((out_h, out_w, 3), np.uint8)
-  tmp = np.empty((h, out_w, 3), np.uint8) if return_hpass else None
+  mid = (out_h, w) if h > 100 * w and out_h < h else (h, out_w)
+  tmp = np.empty(mid + (3,), np.uint8) if return_hpass else None
   lib().swo_lanczos_resize(_p(img), w, h, _p(out), out_w, out_h,
                            _p(tmp) if tmp is not None else None)
   return (out, tmp) if return_hpass else out

@@ -253,72 +253,94 @@ static inline uint8_t clip8(int in) {
   return (uint8_t)(v < 0 ? 0 : (v > 255 ? 255 : v));
 }
 
+/* One LANCZOS pass of ImagingResample over an RGB image: horizontal (inW -> outW columns of
+ * H rows) or vertical (inH -> outH rows of W columns), each output clip8'ed to uint8. */
+static void hpass(const uint8_t *in, int inW, int H, uint8_t *out, int outW) {
+  int ks = swo_lanczos_ksize(inW, outW);
+  int *bounds = (int *)malloc(sizeof(int) * 2 * (size_t)outW);
+  int32_t *kk = (int32_t *)malloc(sizeof(int32_t) * (size_t)ks * outW);
+  swo_lanczos_coeffs(inW, outW, bounds, kk);
+  for (int y = 0; y < H; y++) {
+    const uint8_t *line = in + (size_t)y * inW * 3;
+    for (int xx = 0; xx < outW; xx++) {
+      int xmin = bounds[xx * 2], cnt = bounds[xx * 2 + 1];
+      const int32_t *k = kk + (size_t)xx * ks;
+      int s0 = 1 << (SWO_PRECISION_BITS - 1), s1 = s0, s2 = s0;
+      for (int x = 0; x < cnt; x++) {
+        const uint8_t *p = line + (size_t)(x + xmin) * 3;
+        s0 += p[0] * k[x];
+        s1 += p[1] * k[x];
+        s2 += p[2] * k[x];
+      }
+      uint8_t *o = out + ((size_t)y * outW + xx) * 3;
+      o[0] = clip8(s0); o[1] = clip8(s1); o[2] = clip8(s2);
+    }
+  }
+  free(bounds);
+  free(kk);
+}
+
+static void vpass(const uint8_t *in, int W, int inH, uint8_t *out, int outH) {
+  int ks = swo_lanczos_ksize(inH, outH);
+  int *bounds = (int *)malloc(sizeof(int) * 2 * (size_t)outH);
+  int32_t *kk = (int32_t *)malloc(sizeof(int32_t) * (size_t)ks * outH);
+  swo_lanczos_coeffs(inH, outH, bounds, kk);
+  for (int yy = 0; yy < outH; yy++) {
+    int ymin = bounds[yy * 2], cnt = bounds[yy * 2 + 1];
+    const int32_t *k = kk + (size_t)yy * ks;
+    for (int xx = 0; xx < W; xx++) {
+      int s0 = 1 << (SWO_PRECISION_BITS - 1), s1 = s0, s2 = s0;
+      for (int y = 0; y < cnt; y++) {
+        const uint8_t *p = in + ((size_t)(y + ymin) * W + xx) * 3;
+        s0 += p[0] * k[y];
+        s1 += p[1] * k[y];
+        s2 += p[2] * k[y];
+      }
+      uint8_t *o = out + ((size_t)yy * W + xx) * 3;
+      o[0] = clip8(s0); o[1] = clip8(s1); o[2] = clip8(s2);
+    }
+  }
+  free(bounds);
+  free(kk);
+}
+
 /*
- * in: inH x inW x 3, out: outH x outW x 3 (RGB row-major).  Horizontal pass into a
- * uint8 image, then vertical pass (ImagingResample; both passes needed when both
- * sizes change).  If the sizes are equal Image.resize returns a plain copy.
- * tmp_h (optional, may be NULL): receives the inH x outW x 3 horizontal-pass image.
+ * in: inH x inW x 3, out: outH x outW x 3 (RGB row-major).  Image.resize: a plain copy if the
+ * sizes are equal; otherwise ImagingResample, one pass per axis whose size changes, each into a
+ * uint8 image.  The horizontal pass comes first, except that Image.resize (Pillow 12.2.0)
+ * resizes an image more than 100 times taller than wide vertically first when it shrinks its
+ * height (`self.size[1] > self.size[0] * 100 and size[1] < self.size[1]`).
+ * tmp (optional, may be NULL): receives the first pass's image when both axes change, inH x outW
+ * x 3 (horizontal first) or outH x inW x 3 (vertical first) -- the same number of bytes when
+ * both sizes shrink by the same factor.
  */
+static int vertical_first(int inW, int inH, int outH) {
+  return (int64_t)inH > (int64_t)inW * 100 && outH < inH;
+}
+
 SWO_API void swo_lanczos_resize(const uint8_t *in, int inW, int inH, uint8_t *out, int outW,
-                                int outH, uint8_t *tmp_h) {
+                                int outH, uint8_t *tmp) {
   if (inW == outW && inH == outH) {
     memcpy(out, in, (size_t)inW * inH * 3);
     return;
   }
-  const uint8_t *src = in;
-  uint8_t *hbuf = NULL;
-  int curW = inW;
-  if (inW != outW) {
-    int ks = swo_lanczos_ksize(inW, outW);
-    int *bounds = (int *)malloc(sizeof(int) * 2 * (size_t)outW);
-    int32_t *kk = (int32_t *)malloc(sizeof(int32_t) * (size_t)ks * outW);
-    swo_lanczos_coeffs(inW, outW, bounds, kk);
-    hbuf = tmp_h ? tmp_h : (uint8_t *)malloc((size_t)inH * outW * 3);
-    for (int y = 0; y < inH; y++) {
-      const uint8_t *line = in + (size_t)y * inW * 3;
-      for (int xx = 0; xx < outW; xx++) {
-        int xmin = bounds[xx * 2], cnt = bounds[xx * 2 + 1];
-        const int32_t *k = kk + (size_t)xx * ks;
-        int s0 = 1 << (SWO_PRECISION_BITS - 1), s1 = s0, s2 = s0;
-        for (int x = 0; x < cnt; x++) {
-          const uint8_t *p = line + (size_t)(x + xmin) * 3;
-          s0 += p[0] * k[x];
-          s1 += p[1] * k[x];
-          s2 += p[2] * k[x];
-        }
-        uint8_t *o = hbuf + ((size_t)y * outW + xx) * 3;
-        o[0] = clip8(s0); o[1] = clip8(s1); o[2] = clip8(s2);
-      }
-    }
-    free(bounds);
-    free(kk);
-    src = hbuf;
-    curW = outW;
+  if (inW == outW) {
+    vpass(in, inW, inH, out, outH);
+    return;
   }
-  if (inH != outH) {
-    int ks = swo_lanczos_ksize(inH, outH);
-    int *bounds = (int *)malloc(sizeof(int) * 2 * (size_t)outH);
-    int32_t *kk = (int32_t *)malloc(sizeof(int32_t) * (size_t)ks * outH);
-    swo_lanczos_coeffs(inH, outH, bounds, kk);
-    for (int yy = 0; yy < outH; yy++) {
-      int ymin = bounds[yy * 2], cnt = bounds[yy * 2 + 1];
-      const int32_t *k = kk + (size_t)yy * ks;
-      for (int xx = 0; xx < curW; xx++) {
-        int s0 = 1 << (SWO_PRECISION_BITS - 1), s1 = s0, s2 = s0;
-        for (int y = 0; y < cnt; y++) {
-          const uint8_t *p = src + ((size_t)(y + ymin) * curW + xx) * 3;
-          s0 += p[0] * k[y];
-          s1 += p[1] * k[y];
-          s2 += p[2] * k[y];
-        }
-        uint8_t *o = out + ((size_t)yy * curW + xx) * 3;
-        o[0] = clip8(s0); o[1] = clip8(s1); o[2] = clip8(s2);
-      }
-    }
-    free(bounds);
-    free(kk);
+  if (inH == outH) {
+    hpass(in, inW, inH, out, outW);
+    return;
+  }
+  const int vfirst = vertical_first(inW, inH, outH);
+  const size_t mid_bytes = vfirst ? (size_t)outH * inW * 3 : (size_t)inH * outW * 3;
+  uint8_t *mid = tmp ? tmp : (uint8_t *)malloc(mid_bytes);
+  if (vfirst) {
+    vpass(in, inW, inH, mid, outH);
+    hpass(mid, inW, outH, out, outW);
   } else {
-    memcpy(out, src, (size_t)inH * curW * 3);
+    hpass(in, inW, inH, mid, outW);
+    vpass(mid, outW, inH, out, outH);
   }
-  if (hbuf && hbuf != tmp_h) free(hbuf);
+  if (mid != tmp) free(mid);
 }

@@ -403,6 +403,12 @@ int swb_raster_create(swb_engine *eng, int32_t width, int32_t height, int32_t aa
   if (aa < 1) return fail("anti_aliasing must be >= 1");
   if ((int64_t)width * aa > 4095 || (int64_t)height * aa > 4095)
     return fail("canvas %dx%d exceeds 4095 pixels per side", width * aa, height * aa);
+  // Image.resize shrinks a canvas more than 100 times taller than wide vertically first
+  // (Pillow 12.2.0), which rounds differently from the kernel's horizontal-then-vertical passes
+  if (aa > 1 && height > (int64_t)width * 100)
+    return fail("image %dx%d is more than 100 times taller than wide; with anti_aliasing > 1 "
+                "Pillow resizes such frames vertically first, which the render kernel does not",
+                width, height);
   CUDA_TRY(cudaSetDevice(eng->device));
   swb_raster *r = new swb_raster();
   r->eng = eng;
@@ -470,13 +476,17 @@ static int launch_render_targets(swb_engine *eng, swb_raster *r, const RenderTar
   if (r->eng != eng) return fail("raster belongs to another engine");
   RasterDev rd = r->rd;
   rd.max_spans = eng->max_spans;
-  const RenderLayout L(eng->st.S, r->smem_rows, rd.max_spans, rd.band_rows, rd.W, rd.aa, rd.ncls_x,
-                       rd.ncls_y);
+  int max_smem = 0;
+  CUDA_TRY(cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, eng->device));
+  RenderLayout L(eng->st.S, r->smem_rows, rd.max_spans, rd.band_rows, rd.W, rd.aa, rd.ncls_x, rd.ncls_y);
+  // many convex slots on a wide raster: rather than refuse the raster, keep 16 visible segments
+  // per canvas row as with concave shapes (a row with more is flagged, see RenderLayout)
+  if (L.total > max_smem && L.segcap > 16)
+    L = RenderLayout(eng->st.S, r->smem_rows, rd.max_spans, rd.band_rows, rd.W, rd.aa, rd.ncls_x,
+                     rd.ncls_y, false);
   if ((L.cap + rd.max_spans) * 4 * r->smem_rows > L.scratch_bytes)
     return fail("render scratch (%d B) cannot hold one sprite spanning %d canvas rows", L.scratch_bytes,
                 r->smem_rows);
-  int max_smem = 0;
-  CUDA_TRY(cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, eng->device));
   if (L.total > max_smem)
     return fail("render needs %d B of shared memory per CTA (limit %d): too many sprite slots / too large a canvas",
                 L.total, max_smem);

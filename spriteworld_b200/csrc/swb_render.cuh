@@ -75,8 +75,10 @@ struct RenderLayout {
   int off_meta, off_edge_i, off_edge_f, off_edge_yr, off_hl, off_region;
   int off_nseg, off_segs, off_prefix, off_xwin, off_ywin, off_scratch, off_frame, total;
   int scratch_bytes, segcap;
+  // exact_segs: with convex shapes only, size the segment table for every row a scene can
+  // produce (2S-1 pieces); false caps it at 16 like the concave case
   __host__ __device__ RenderLayout(int S_, int rows_, int M_, int band_rows_, int W_, int aa_,
-                                   int ncx_, int ncy_)
+                                   int ncx_, int ncy_, bool exact_segs = true)
       : S(S_), rows(rows_), M(M_), band_rows(band_rows_), W(W_), aa(aa_), ncx(ncx_), ncy(ncy_) {
     int o = 0;
     auto take = [&](int bytes) { int r = o; o += (bytes + 15) & ~15; return r; };
@@ -87,8 +89,12 @@ struct RenderLayout {
     off_edge_yr = take(S * EV * 4);        // ymin | ymax<<16 of non-horizontal edges, empty otherwise
     off_hl = take(S * EV * 3 * 2);         // horizontal edges: y, xmin, xmax (int16)
     off_region = take(S * 4 * 2);
-    // visible segments kept per canvas row: n one-span sprites leave at most 2n-1 pieces
-    segcap = M > 1 ? 16 : (2 * S - 1 < 3 ? 3 : (2 * S - 1 > 16 ? 16 : 2 * S - 1));
+    // visible segments kept per canvas row: n one-span sprites leave at most 2n-1 pieces, so
+    // with convex shapes only (M == 1) the exact table never overflows.  With several spans
+    // per sprite row, or where the exact table does not fit, it is capped at 16: a row with
+    // more visible pieces sets SWB_ENV_SPAN_OVERFLOW (DESIGN §8)
+    segcap = M > 1 ? 16 : (2 * S - 1 < 3 ? 3 : 2 * S - 1);
+    if (!exact_segs && segcap > 16) segcap = 16;
     off_nseg = take(((rows + 3) & ~3) + 8);  // +: quads of the H pass may end past the last row
     off_segs = take(rows * segcap * 4);
     off_prefix = take(ncx * 33 * 4);
@@ -944,7 +950,12 @@ render_kernel(DevState st, RasterDev rd, const RenderLayout L, const RenderTarge
   // the frame and costs it one instruction per rank ----------------------------------------
   const int n_bytes = n_yo * row_bytes;
   const size_t band_off = (size_t)(targets.env_offset + e) * rd.H * row_bytes + (size_t)(rd.H - yo_b1) * row_bytes;
-  if ((n_bytes & 15) == 0 && (band_off & 15) == 0) {
+  // the bulk copy needs a 16-byte aligned size and destination address in every target; the
+  // caller's buffers may start anywhere (a view at an odd offset), so test the address itself
+  bool bulk = (n_bytes & 15) == 0;
+  for (int i = 0; i < (kPeers ? targets.n : 1); ++i)
+    bulk &= (((uintptr_t)(kPeers ? s_dst[i] : targets.dst[0]) + band_off) & 15) == 0;
+  if (bulk) {
     if (tid == 0) {
       const uint32_t src = (uint32_t)__cvta_generic_to_shared(s_frame);
       // peers in an order rotated by rank and frame, so that at any moment the ranks' copies are

@@ -247,6 +247,17 @@ class Engine(object):
       return _native.DTYPE_F64
     raise ValueError('actions must be float32 or float64')
 
+  def _check_frames(self, frames, raster, n_frames):
+    """The render kernel writes n_frames * H * W * 3 bytes from frames.data_ptr(): anything but
+    a contiguous uint8 tensor of exactly that shape on this device would be written out of
+    bounds or scrambled."""
+    shape = (n_frames, raster.height, raster.width, 3)
+    if (not isinstance(frames, torch.Tensor) or frames.dtype != torch.uint8 or
+        frames.device != self.device or tuple(frames.shape) != shape or
+        not frames.is_contiguous()):
+      raise ValueError('frames must be a contiguous uint8 tensor of shape %s on %s, got %s' % (
+          shape, self.device, _describe(frames)))
+
   def step(self, actions, raster=None, frames=None):
     """One Environment.step for every env.  `actions`: device tensor."""
     if actions.device != self.device or not actions.is_contiguous():
@@ -258,6 +269,7 @@ class Engine(object):
     else:
       if frames is None:
         frames = raster.new_frames()
+      self._check_frames(frames, raster, self.n_envs)
       _native.check(self._lib.swb_step_render(
           self._h, raster._h, ctypes.c_void_p(actions.data_ptr()), dt, ctypes.byref(self._out),
           ctypes.c_void_p(frames.data_ptr()), self._stream()))
@@ -272,6 +284,7 @@ class Engine(object):
       raise ValueError('actions must be a contiguous tensor on %s' % self.device)
     dt = self._action_dtype(actions)
     ptrs, n, env_offset, local = targets
+    self._check_frames(local, raster, int(n) * self.n_envs)
     _native.check(self._lib.swb_step_render_gather(
         self._h, raster._h, ctypes.c_void_p(actions.data_ptr()), dt, ctypes.byref(self._out),
         ptrs, n, env_offset, self._stream()))
@@ -280,6 +293,7 @@ class Engine(object):
   def render(self, raster, frames=None):
     if frames is None:
       frames = raster.new_frames()
+    self._check_frames(frames, raster, self.n_envs)
     _native.check(self._lib.swb_render(self._h, raster._h, ctypes.c_void_p(frames.data_ptr()),
                                        self._stream()))
     return frames
@@ -298,7 +312,9 @@ class Engine(object):
     wrong).  Synchronises."""
     if int(self.render_status().max().item()) & _native.ENV_SPAN_OVERFLOW:
       raise _native.NativeError(
-          'render: more visible segments / spans per canvas row than the engine was sized for')
+          'render: a canvas row has more crossings, spans or visible segments than the engine '
+          'was sized for (once a star or spoke shape is uploaded, at most 16 visible segments '
+          'per canvas row; see DESIGN.md section 8)')
 
   def step_host(self, actions, raster=None, want_frames=True, out=None):
     """Whole call with HOST buffers (numpy in, numpy out): H2D, step, render, D2H, sync.
@@ -370,6 +386,13 @@ class Engine(object):
 
   def launch_count(self):
     return int(self._lib.swb_launch_count(self._h))
+
+
+def _describe(t):
+  if not isinstance(t, torch.Tensor):
+    return type(t).__name__
+  return '%s %s on %s%s' % (t.dtype, tuple(t.shape), t.device,
+                            '' if t.is_contiguous() else ' (not contiguous)')
 
 
 def fill_task_nodes(cfg, nodes):

@@ -12,6 +12,16 @@ import pytest
 from oracle import oracle
 from tests import fixtures
 
+# (output width, output height, anti_aliasing) of tests/test_gpu_render_geometry.py's sweep:
+# frames with short bands, partial blocks, column tails and canvas sides of 4095 pixels
+SWEEP_GEOMETRIES = ((33, 17, 3), (50, 50, 5), (64, 65, 5), (64, 100, 5), (36, 70, 3),
+                    (7, 130, 4), (101, 30, 2), (1, 1, 1), (1, 1, 5), (2, 3, 5), (819, 8, 5),
+                    (8, 819, 5))
+# Image.resize shrinks an image more than 100 times taller than wide vertically first: the
+# oracle follows that rule on both sides of the H = 100 W boundary
+TALL_GEOMETRIES = ((8, 819, 5), (8, 1023, 4), (8, 1300, 3), (1, 101, 2), (1, 150, 3),
+                   (2, 250, 2), (3, 400, 5), (4, 401, 3), (1, 200, 5), (1, 100, 3), (8, 800, 5))
+
 PIL = pytest.importorskip('PIL')
 from PIL import Image, ImageDraw  # noqa: E402
 
@@ -53,6 +63,17 @@ def test_lanczos_matches_pillow():
         img[y0:y0 + rng.randint(1, h), x0:x0 + rng.randint(1, w)] = rng.randint(0, 256, 3)
     ref = np.array(Image.fromarray(img).resize((o, oh), Image.LANCZOS))
     assert np.array_equal(oracle.lanczos_resize(img, o, oh), ref)
+  for t, (o, oh, aa) in enumerate((SWEEP_GEOMETRIES + TALL_GEOMETRIES) * 2):
+    w, h = o * aa, oh * aa
+    if t % 2:
+      img = rng.randint(0, 256, (h, w, 3)).astype(np.uint8)
+    else:   # saturated rectangles: the LANCZOS overshoot clips at both ends
+      img = np.full((h, w, 3), 255 * (t % 4 == 0), np.uint8)
+      for _ in range(6):
+        x0, y0 = rng.randint(0, w), rng.randint(0, h)
+        img[y0:y0 + rng.randint(1, h + 1), x0:x0 + rng.randint(1, w + 1)] = 255 * rng.randint(0, 2, 3)
+    ref = np.array(Image.fromarray(img).resize((o, oh), Image.LANCZOS))
+    assert np.array_equal(oracle.lanczos_resize(img, o, oh), ref), (o, oh, aa)
 
 
 def test_polygon_fill_matches_pillow_spriteworld_shapes():
@@ -74,6 +95,18 @@ def test_polygon_fill_matches_pillow_spriteworld_shapes():
       plain = oracle.polygon_fill(np.zeros((h, w, 3), np.uint8), xy, (9, 200, 77),
                                   corner_join=0)
       n_without += not np.array_equal(plain, ref)
+    # the canvases of the render sweep, angles on multiples of 45 degrees half of the time
+    for o, oh, aa in SWEEP_GEOMETRIES:
+      w, h = o * aa, oh * aa
+      for _ in range(4):
+        s = float(np.exp(rng.uniform(np.log(0.001), np.log(2.0))))
+        ang = 45.0 * rng.randint(8) if rng.rand() < 0.5 else rng.uniform(0, 360)
+        c, sn = math.cos(math.radians(ang)), math.sin(math.radians(ang))
+        pos = rng.uniform(-0.2, 1.2, 2)
+        xy = ((verts * s) @ np.array([[c, sn], [-sn, c]]) + pos) * np.array([w, h])
+        ref = _pil_polygon(w, h, xy, (255, 0, 255))
+        got = oracle.polygon_fill(np.zeros((h, w, 3), np.uint8), xy, (255, 0, 255))
+        assert np.array_equal(got, ref), (name, w, h, s, ang, pos)
   # the corner-joining refinement is not optional: some instances need it
   assert n_without > 0
 
@@ -82,8 +115,11 @@ def test_polygon_fill_matches_pillow_random_polygons():
   rng = np.random.RandomState(9)
   bad = 0
   n = 4000
-  for _ in range(n):
+  sweep = [d * aa for o, oh, aa in SWEEP_GEOMETRIES for d in (o, oh)]
+  for i in range(n):
     w, h = int(rng.choice([16, 64, 320])), int(rng.choice([16, 64, 320]))
+    if i % 8 == 7:   # every eighth polygon on a canvas of the render sweep
+      w, h = int(rng.choice(sweep)), int(rng.choice(sweep))
     kind, nv = rng.randint(3), rng.randint(3, 10)
     if kind == 0:  # convex, float coordinates, partly off canvas
       ang = np.sort(rng.uniform(0, 2 * np.pi, nv))
