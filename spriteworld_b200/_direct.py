@@ -9,6 +9,7 @@ positions back into the `Sprite` objects.  Engines are cached per configuration.
 There is deliberately no CPU implementation of this math in the package.
 """
 import collections
+import ctypes
 import json
 
 import numpy as np
@@ -109,18 +110,9 @@ def action_step(action_space, action, sprites, keep_in_frame):
       raise IndexError('list index out of range')   # sprites[-1] in the reference
   eng = _engine(max(1, len(sprites)), cfg, _NO_TASK, keep_in_frame)
   _load(eng, sprites)
-  a = np.asarray(action)
-  if cfg['kind'] == 'embodied':
-    t = torch.from_numpy(np.ascontiguousarray(a, dtype=np.int32).reshape(1, 2))
-    dtype = _native.DTYPE_I32
-  elif a.dtype == np.float32:
-    t = torch.from_numpy(np.ascontiguousarray(a).reshape(1, 4))
-    dtype = _native.DTYPE_F32
-  else:
-    t = torch.from_numpy(np.ascontiguousarray(a, dtype=np.float64).reshape(1, 4))
-    dtype = _native.DTYPE_F64
-  t = t.to(eng.device)
-  import ctypes
+  a = engine_lib.host_actions(cfg['kind'], np.reshape(action, (1, -1)))
+  dtype = engine_lib.action_dtype(eng.action_kind, 1, a)
+  t = torch.from_numpy(a).to(eng.device)
   _native.check(eng._lib.swb_apply_action(eng._h, ctypes.c_void_p(t.data_ptr()), dtype, eng._out,
                                           eng._stream()))
   state = eng.download_state()
@@ -131,7 +123,7 @@ def action_step(action_space, action, sprites, keep_in_frame):
     s._position[0] = state['pos_x'][0, k]
     s._position[1] = state['pos_y'][0, k]
   cost = float(eng._reward[0].item())
-  if cfg['kind'] != 'embodied' and a.dtype == np.float32:
+  if dtype == _native.DTYPE_F32:
     return np.float32(cost)
   return cost
 

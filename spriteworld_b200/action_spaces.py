@@ -98,8 +98,7 @@ class Embodied(object):
     if action[1] not in self.action_to_motion:
       raise KeyError(action[1])
     from spriteworld_b200 import _direct
-    return _direct.action_step(self, np.array([int(bool(action[0])), int(action[1])], np.int32),
-                               sprites, keep_in_frame)
+    return _direct.action_step(self, action, sprites, keep_in_frame)
 
   def sample(self):
     return [np.random.randint(0, 2), np.random.randint(0, 4)]

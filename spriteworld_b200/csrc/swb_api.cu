@@ -3,6 +3,7 @@
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
+#include <optional>
 #include <string>
 #include <vector>
 
@@ -350,50 +351,74 @@ int swb_request_reset(swb_engine *eng, const uint8_t *mask, void *stream_) {
   return 0;
 }
 
-int swb_step(swb_engine *eng, const void *actions, int32_t action_dtype, const swb_step_out *out,
-             void *stream_) {
-  if (!eng || !actions || !out) return fail("swb_step: null argument");
+enum { STEP_WHOLE = 0, STEP_TASK = 1, STEP_ACTION = 2 };  // step_kernel modes
+
+// What a step_kernel launch reads from its caller: the engine, every output pointer and, unless
+// it evaluates the task only, actions of a dtype the engine's action kind takes.
+static int check_step(const swb_engine *eng, const void *actions, int32_t action_dtype,
+                      const swb_step_out *out, int mode) {
+  if (!eng || !out || (mode != STEP_TASK && !actions)) return fail("step: null argument");
   if (!out->reward || !out->step_type || !out->success || !out->status)
-    return fail("swb_step: every swb_step_out pointer must be set");
+    return fail("step: every swb_step_out pointer must be set");
+  if (mode == STEP_TASK) return 0;
   const bool emb = eng->cfg.action_kind == SWB_ACT_EMBODIED;
   if (emb && action_dtype != SWB_DTYPE_I32) return fail("Embodied actions must be int32 [E][2]");
   if (!emb && action_dtype != SWB_DTYPE_F32 && action_dtype != SWB_DTYPE_F64)
     return fail("SelectMove/DragAndDrop actions must be float32 or float64 [E][4]");
+  return 0;
+}
+
+// Enqueues step_kernel over every env, after check_step has passed.
+static int launch_step(swb_engine *eng, const void *actions, int32_t action_dtype,
+                       const swb_step_out &out, cudaStream_t stream, int mode) {
   CUDA_TRY(cudaSetDevice(eng->device));
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   const int blocks = (eng->st.E + STEP_WARPS - 1) / STEP_WARPS;
-  step_kernel<<<blocks, STEP_WARPS * 32, 0, stream>>>(eng->st, eng->d_step_cfg, actions, action_dtype, *out, 0);
+  step_kernel<<<blocks, STEP_WARPS * 32, 0, stream>>>(eng->st, eng->d_step_cfg, actions, action_dtype, out, mode);
   eng->launches++;
   CUDA_TRY(cudaGetLastError());
   return 0;
 }
 
-static int launch_partial(swb_engine *eng, const void *actions, int32_t action_dtype,
-                          const swb_step_out *out, void *stream_, int mode) {
-  if (!eng || !out) return fail("null argument");
-  if (!out->reward || !out->step_type || !out->success || !out->status)
-    return fail("every swb_step_out pointer must be set");
-  CUDA_TRY(cudaSetDevice(eng->device));
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  const int blocks = (eng->st.E + STEP_WARPS - 1) / STEP_WARPS;
-  step_kernel<<<blocks, STEP_WARPS * 32, 0, stream>>>(eng->st, eng->d_step_cfg, actions, action_dtype, *out, mode);
-  eng->launches++;
-  CUDA_TRY(cudaGetLastError());
-  return 0;
+int swb_step(swb_engine *eng, const void *actions, int32_t action_dtype, const swb_step_out *out,
+             void *stream) {
+  if (check_step(eng, actions, action_dtype, out, STEP_WHOLE)) return 1;
+  return launch_step(eng, actions, action_dtype, *out, static_cast<cudaStream_t>(stream), STEP_WHOLE);
 }
 
 int swb_eval_task(swb_engine *eng, const swb_step_out *out, void *stream) {
-  return launch_partial(eng, nullptr, SWB_DTYPE_F32, out, stream, 1);
+  if (check_step(eng, nullptr, SWB_DTYPE_F32, out, STEP_TASK)) return 1;
+  return launch_step(eng, nullptr, SWB_DTYPE_F32, *out, static_cast<cudaStream_t>(stream), STEP_TASK);
 }
 
 int swb_apply_action(swb_engine *eng, const void *actions, int32_t action_dtype,
                      const swb_step_out *out, void *stream) {
-  if (!actions) return fail("swb_apply_action: null actions");
-  const bool emb = eng && eng->cfg.action_kind == SWB_ACT_EMBODIED;
-  if (emb && action_dtype != SWB_DTYPE_I32) return fail("Embodied actions must be int32 [E][2]");
-  if (!emb && action_dtype != SWB_DTYPE_F32 && action_dtype != SWB_DTYPE_F64)
-    return fail("SelectMove/DragAndDrop actions must be float32 or float64 [E][4]");
-  return launch_partial(eng, actions, action_dtype, out, stream, 2);
+  if (check_step(eng, actions, action_dtype, out, STEP_ACTION)) return 1;
+  return launch_step(eng, actions, action_dtype, *out, static_cast<cudaStream_t>(stream), STEP_ACTION);
+}
+
+// The checks of a render launch of raster `r` by `eng` with `max_spans` spans per sprite row;
+// on success *plan is the shared-memory layout the launch needs.  Every entry point that renders
+// runs them before it enqueues anything; swb_raster_create runs them for a convex-only pool.
+static int check_render(const swb_engine *eng, const swb_raster *r, int max_spans,
+                        std::optional<RenderLayout> *plan) {
+  if (r->eng != eng) return fail("raster belongs to another engine");
+  const RasterDev &rd = r->rd;
+  int max_smem = 0;
+  CUDA_TRY(cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, eng->device));
+  RenderLayout L(eng->st.S, r->smem_rows, max_spans, rd.band_rows, rd.W, rd.aa, rd.ncls_x, rd.ncls_y);
+  // many convex slots on a wide raster: rather than refuse the raster, keep 16 visible segments
+  // per canvas row as with concave shapes (a row with more is flagged, see RenderLayout)
+  if (L.total > max_smem && L.segcap > 16)
+    L = RenderLayout(eng->st.S, r->smem_rows, max_spans, rd.band_rows, rd.W, rd.aa, rd.ncls_x,
+                     rd.ncls_y, false);
+  if ((L.cap + max_spans) * 4 * r->smem_rows > L.scratch_bytes)
+    return fail("render scratch (%d B) cannot hold one sprite spanning %d canvas rows", L.scratch_bytes,
+                r->smem_rows);
+  if (L.total > max_smem)
+    return fail("render needs %d B of shared memory per CTA (limit %d): too many sprite slots / too large a canvas",
+                L.total, max_smem);
+  plan->emplace(L);
+  return 0;
 }
 
 int swb_raster_create(swb_engine *eng, int32_t width, int32_t height, int32_t aa,
@@ -442,6 +467,12 @@ int swb_raster_create(swb_engine *eng, int32_t width, int32_t height, int32_t aa
     }
   }
   r->smem_rows = rows;
+  // refuse a raster that cannot render even convex shapes (a star or spoke may still fail later)
+  std::optional<RenderLayout> plan;
+  if (check_render(eng, r, 1, &plan)) {
+    delete r;
+    return 1;
+  }
   VFragHost vf;
   if (!build_vfrag(r->ay, &vf, &err)) {
     delete r;
@@ -465,37 +496,21 @@ void swb_raster_destroy(swb_raster *r) {
   delete r;
 }
 
-// after_step: the launch follows this step's step_kernel on the stream.  It is then made a
-// programmatic dependent launch: the render CTAs may become resident and load their tables while
-// the step kernel's last CTAs run (step_kernel signals griddepcontrol.launch_dependents at once),
-// and wait (griddepcontrol.wait, after their set-up) until the step grid has completed and its
-// writes are visible.
-static int launch_render_targets(swb_engine *eng, swb_raster *r, const RenderTargets &targets,
-                                 uint8_t *status, cudaStream_t stream, int env_base = 0,
-                                 int env_count = -1, bool after_step = false) {
-  if (r->eng != eng) return fail("raster belongs to another engine");
+// Enqueues render_kernel for envs [env_base, env_base + env_count) with a layout check_render
+// returned.  after_step: the launch follows this step's step_kernel on the stream.  It is then
+// made a programmatic dependent launch: the render CTAs may become resident and load their tables
+// while the step kernel's last CTAs run (step_kernel signals griddepcontrol.launch_dependents at
+// once), and wait (griddepcontrol.wait, after their set-up) until the step grid has completed and
+// its writes are visible.
+static int enqueue_render(swb_engine *eng, const swb_raster *r, const RenderLayout &L,
+                          const RenderTargets &targets, uint8_t *status, cudaStream_t stream,
+                          int env_base, int env_count, bool after_step) {
   RasterDev rd = r->rd;
-  rd.max_spans = eng->max_spans;
-  int max_smem = 0;
-  CUDA_TRY(cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, eng->device));
-  RenderLayout L(eng->st.S, r->smem_rows, rd.max_spans, rd.band_rows, rd.W, rd.aa, rd.ncls_x, rd.ncls_y);
-  // many convex slots on a wide raster: rather than refuse the raster, keep 16 visible segments
-  // per canvas row as with concave shapes (a row with more is flagged, see RenderLayout)
-  if (L.total > max_smem && L.segcap > 16)
-    L = RenderLayout(eng->st.S, r->smem_rows, rd.max_spans, rd.band_rows, rd.W, rd.aa, rd.ncls_x,
-                     rd.ncls_y, false);
-  if ((L.cap + rd.max_spans) * 4 * r->smem_rows > L.scratch_bytes)
-    return fail("render scratch (%d B) cannot hold one sprite spanning %d canvas rows", L.scratch_bytes,
-                r->smem_rows);
-  if (L.total > max_smem)
-    return fail("render needs %d B of shared memory per CTA (limit %d): too many sprite slots / too large a canvas",
-                L.total, max_smem);
+  rd.max_spans = L.M;
   auto kernel = targets.n > 1 ? render_kernel<true> : render_kernel<false>;
   CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, L.total));
   DevState st = eng->st;
   st.render_status = status;
-  if (env_count < 0) env_count = eng->st.E - env_base;
-  if (env_count <= 0) return 0;
   // persistent CTAs: one per resident slot (or per item if there are fewer), claiming
   // (env, band) items from the engine's counter; see render_kernel
   const int n_items = env_count * rd.n_bands;
@@ -517,50 +532,44 @@ static int launch_render_targets(swb_engine *eng, swb_raster *r, const RenderTar
   return 0;
 }
 
-static int launch_render(swb_engine *eng, swb_raster *r, uint8_t *frames, uint8_t *status,
-                         cudaStream_t stream, int env_base = 0, int env_count = -1,
-                         bool after_step = false) {
-  RenderTargets targets{};
-  targets.dst[0] = frames;
-  targets.n = 1;
-  targets.env_offset = 0;
-  targets.self = 0;
-  return launch_render_targets(eng, r, targets, status, stream, env_base, env_count, after_step);
-}
-
 int swb_render(swb_engine *eng, swb_raster *r, uint8_t *frames, void *stream_) {
   if (!eng || !r || !frames) return fail("swb_render: null argument");
+  std::optional<RenderLayout> plan;
+  if (check_render(eng, r, eng->max_spans, &plan)) return 1;
   CUDA_TRY(cudaSetDevice(eng->device));
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   CUDA_TRY(cudaMemsetAsync(eng->st.render_status, 0, eng->st.E, stream));
-  return launch_render(eng, r, frames, eng->st.render_status, stream);
+  return enqueue_render(eng, r, *plan, RenderTargets{{frames}, 1, 0, 0}, eng->st.render_status, stream,
+                        0, eng->st.E, false);
 }
 
 int swb_step_render(swb_engine *eng, swb_raster *r, const void *actions, int32_t action_dtype,
-                    const swb_step_out *out, uint8_t *frames, void *stream_) {
-  if (!r || !frames) return fail("swb_step_render: null argument");
-  if (swb_step(eng, actions, action_dtype, out, stream_)) return 1;
-  return launch_render(eng, r, frames, out->status, static_cast<cudaStream_t>(stream_), 0, -1, true);
+                    const swb_step_out *out, uint8_t *frames, void *stream) {
+  if (!eng || !r || !frames) return fail("swb_step_render: null argument");
+  uint8_t *const dst[1] = {frames};  // one target at env offset 0: the frames of this engine alone
+  return swb_step_render_gather(eng, r, actions, action_dtype, out, dst, 1, 0, stream);
 }
 
 int swb_step_render_gather(swb_engine *eng, swb_raster *r, const void *actions,
                            int32_t action_dtype, const swb_step_out *out, uint8_t *const *dst,
                            int32_t n_dst, int64_t env_offset, void *stream_) {
-  if (!r || !dst) return fail("swb_step_render_gather: null argument");
+  if (!eng || !r || !dst) return fail("swb_step_render_gather: null argument");
   if (n_dst < 1 || n_dst > SWB_MAX_PEERS)
     return fail("swb_step_render_gather: n_dst = %d, expected 1..%d", n_dst, SWB_MAX_PEERS);
-  if (env_offset < 0 || env_offset > INT32_MAX - (eng ? eng->st.E : 0))
+  if (env_offset < 0 || env_offset > INT32_MAX - eng->st.E)
     return fail("swb_step_render_gather: env_offset out of range");
-  RenderTargets targets{};
+  RenderTargets targets{{}, n_dst, (int)env_offset, (int)((env_offset / eng->st.E) % n_dst)};
   for (int i = 0; i < n_dst; ++i) {
     if (!dst[i]) return fail("swb_step_render_gather: dst[%d] is null", i);
     targets.dst[i] = dst[i];
   }
-  targets.n = n_dst;
-  targets.env_offset = (int)env_offset;
-  targets.self = (int)((env_offset / (eng ? eng->st.E : 1)) % n_dst);
-  if (swb_step(eng, actions, action_dtype, out, stream_)) return 1;
-  return launch_render_targets(eng, r, targets, out->status, static_cast<cudaStream_t>(stream_), 0, -1, true);
+  std::optional<RenderLayout> plan;
+  if (check_step(eng, actions, action_dtype, out, STEP_WHOLE) ||
+      check_render(eng, r, eng->max_spans, &plan))
+    return 1;
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (launch_step(eng, actions, action_dtype, *out, stream, STEP_WHOLE)) return 1;
+  return enqueue_render(eng, r, *plan, targets, out->status, stream, 0, eng->st.E, true);
 }
 
 int swb_ipc_alloc(int32_t device, uint64_t bytes, void **ptr, uint8_t *handle) {
@@ -610,7 +619,7 @@ int swb_ipc_close(void *ptr) {
 int swb_step_host(swb_engine *eng, swb_raster *r, const void *actions, int32_t action_dtype,
                   double *reward, int8_t *step_type, uint8_t *success, uint8_t *status,
                   uint8_t *frames, void *stream_) {
-  if (!eng || !actions) return fail("swb_step_host: null argument");
+  if (!eng) return fail("swb_step_host: null argument");
   CUDA_TRY(cudaSetDevice(eng->device));
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   const int E = eng->st.E;
@@ -621,24 +630,29 @@ int swb_step_host(swb_engine *eng, swb_raster *r, const void *actions, int32_t a
     CUDA_TRY(cudaMalloc(&eng->h_out.success, E + 4));
     CUDA_TRY(cudaMalloc(&eng->h_out.status, E + 4));
   }
-  const size_t abytes = action_dtype == SWB_DTYPE_I32 ? (size_t)E * 2 * 4
-                        : (action_dtype == SWB_DTYPE_F32 ? (size_t)E * 16 : (size_t)E * 32);
+  std::optional<RenderLayout> plan;
+  if (check_step(eng, actions, action_dtype, &eng->h_out, STEP_WHOLE) ||
+      (r && check_render(eng, r, eng->max_spans, &plan)))
+    return 1;
+  // [E][2] int32 or [E][4] float32 / float64, as checked
+  const size_t abytes = (size_t)E * (action_dtype == SWB_DTYPE_I32 ? 8 : action_dtype == SWB_DTYPE_F32 ? 16 : 32);
   CUDA_TRY(cudaMemcpyAsync(eng->h_actions, actions, abytes, cudaMemcpyHostToDevice, stream));
+  const size_t fbytes = r ? (size_t)E * r->rd.H * r->rd.W * 3 : 0;
+  if (fbytes > eng->h_frames_bytes) {
+    CUDA_TRY(cudaStreamSynchronize(stream));
+    cudaFree(eng->h_frames);
+    eng->h_frames_bytes = 0;
+    CUDA_TRY(cudaMalloc(&eng->h_frames, fbytes));
+    // written only by the render kernel's bulk copies, which initcheck does not track: zero
+    // it once so that the tool sees every byte the D2H copies read as initialised
+    CUDA_TRY(cudaMemsetAsync(eng->h_frames, 0, fbytes, stream));
+    eng->h_frames_bytes = fbytes;
+  }
+  if (launch_step(eng, eng->h_actions, action_dtype, eng->h_out, stream, STEP_WHOLE)) return 1;
   if (r) {
-    const size_t fbytes = (size_t)E * r->rd.H * r->rd.W * 3;
-    if (fbytes > eng->h_frames_bytes) {
-      CUDA_TRY(cudaStreamSynchronize(stream));
-      cudaFree(eng->h_frames);
-      eng->h_frames_bytes = 0;
-      CUDA_TRY(cudaMalloc(&eng->h_frames, fbytes));
-      // written only by the render kernel's bulk copies, which initcheck does not track: zero
-      // it once so that the tool sees every byte the D2H copies read as initialised
-      CUDA_TRY(cudaMemsetAsync(eng->h_frames, 0, fbytes, stream));
-      eng->h_frames_bytes = fbytes;
-    }
-    if (swb_step(eng, eng->h_actions, action_dtype, &eng->h_out, stream)) return 1;
+    const RenderTargets targets{{eng->h_frames}, 1, 0, 0};
     if (!frames) {
-      if (launch_render(eng, r, eng->h_frames, eng->h_out.status, stream, 0, -1, true)) return 1;
+      if (enqueue_render(eng, r, *plan, targets, eng->h_out.status, stream, 0, E, true)) return 1;
     } else {
       // render in env chunks; each chunk's frames go to the host on a second stream while
       // the next chunk renders
@@ -651,7 +665,7 @@ int swb_step_host(swb_engine *eng, swb_raster *r, const void *actions, int32_t a
       const int n_chunks = E >= 1024 ? 8 : (E >= 64 ? 2 : 1);
       for (int c = 0; c < n_chunks; ++c) {
         const int e0 = (int)((int64_t)E * c / n_chunks), e1 = (int)((int64_t)E * (c + 1) / n_chunks);
-        if (launch_render(eng, r, eng->h_frames, eng->h_out.status, stream, e0, e1 - e0, c == 0)) return 1;
+        if (enqueue_render(eng, r, *plan, targets, eng->h_out.status, stream, e0, e1 - e0, c == 0)) return 1;
         CUDA_TRY(cudaEventRecord(eng->chunk_done[c], stream));
         CUDA_TRY(cudaStreamWaitEvent(eng->copy_stream, eng->chunk_done[c], 0));
         CUDA_TRY(cudaMemcpyAsync(frames + per_env * e0, eng->h_frames + per_env * e0, per_env * (e1 - e0),
@@ -660,8 +674,6 @@ int swb_step_host(swb_engine *eng, swb_raster *r, const void *actions, int32_t a
       CUDA_TRY(cudaEventRecord(eng->copies_done, eng->copy_stream));
       CUDA_TRY(cudaStreamWaitEvent(stream, eng->copies_done, 0));
     }
-  } else {
-    if (swb_step(eng, eng->h_actions, action_dtype, &eng->h_out, stream)) return 1;
   }
   if (reward) CUDA_TRY(cudaMemcpyAsync(reward, eng->h_out.reward, (size_t)E * sizeof(double), cudaMemcpyDeviceToHost, stream));
   if (step_type) CUDA_TRY(cudaMemcpyAsync(step_type, eng->h_out.step_type, E, cudaMemcpyDeviceToHost, stream));

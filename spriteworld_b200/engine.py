@@ -4,6 +4,7 @@ PyTorch is used only for device memory and streams: action, reward, flag and fra
 buffers are torch tensors whose `data_ptr()` is handed to the C-ABI
 (include/spriteworld_b200.h).  All compute happens in the CUDA library.
 """
+import collections
 import ctypes
 
 import numpy as np
@@ -40,13 +41,63 @@ OUT_BYTES_PER_ENV = 8 + 1 + 1 + 1
 
 def split_outputs(buf, n_envs):
   """Views (reward f64, step_type i8, success u8, status u8) of a packed output buffer of
-  n_envs * OUT_BYTES_PER_ENV bytes (layout: all rewards, then all step types, ...)."""
+  n_envs * OUT_BYTES_PER_ENV bytes (layout: all rewards, then all step types, ...); of a
+  (n, n_envs * OUT_BYTES_PER_ENV) buffer, n such buffers, copies of n * n_envs outputs each."""
   E = int(n_envs)
-  reward = buf[:8 * E].view(torch.float64)
-  step_type = buf[8 * E:9 * E].view(torch.int8)
-  success = buf[9 * E:10 * E]
-  status = buf[10 * E:11 * E]
+  reward = buf[..., :8 * E].contiguous().view(torch.float64).reshape(-1)
+  step_type = buf[..., 8 * E:9 * E].reshape(-1).view(torch.int8)
+  success = buf[..., 9 * E:10 * E].reshape(-1)
+  status = buf[..., 10 * E:11 * E].reshape(-1)
   return reward, step_type, success, status
+
+
+ActionSpec = collections.namedtuple('ActionSpec', ['kind', 'columns', 'dtypes'])
+
+# What the engine accepts per action kind: (E, columns) actions of one of `dtypes` (dtype name ->
+# swb action dtype), as device tensors (step, step_gather) or host arrays (step_host)
+_FLOATS = {'float32': _native.DTYPE_F32, 'float64': _native.DTYPE_F64}
+ACTIONS = {'select_move': ActionSpec(_native.ACT_SELECT_MOVE, 4, _FLOATS),
+           'drag_and_drop': ActionSpec(_native.ACT_DRAG_AND_DROP, 4, _FLOATS),
+           'embodied': ActionSpec(_native.ACT_EMBODIED, 2, {'int32': _native.DTYPE_I32})}
+_SPECS = {spec.kind: spec for spec in ACTIONS.values()}   # the same table by swb action kind
+
+
+def action_dtype(action_kind, n_envs, actions, device=None):
+  """The swb action dtype of `actions` (tensor or array) for `n_envs` envs of swb `action_kind`;
+  with `device`, a contiguous tensor on it.  ValueError otherwise: nothing is converted."""
+  if device is not None and not (isinstance(actions, torch.Tensor) and actions.device == device
+                                 and actions.is_contiguous()):
+    raise ValueError('actions must be a contiguous tensor on %s, got %s'
+                     % (device, _describe(actions)))
+  spec = _SPECS[action_kind]
+  name = str(actions.dtype).replace('torch.', '')
+  shape = (int(n_envs), spec.columns)
+  if tuple(actions.shape) != shape or name not in spec.dtypes:
+    raise ValueError('actions must have shape %s and dtype %s, got %s %s' % (
+        shape, ' or '.join(spec.dtypes), name, tuple(actions.shape)))
+  return spec.dtypes[name]
+
+
+def host_actions(kind, actions):
+  """Host actions (array-like, one row per env) as a contiguous array the engine accepts.
+  SelectMove / DragAndDrop: float32 stays float32, anything else becomes float64.  Embodied: int32
+  (carry != 0, direction); a direction that is not an integer in 0..3 becomes -1, so the step
+  reports ENV_BAD_ACTION (the reference's KeyError) rather than a wrapped or truncated move."""
+  a = np.asarray(actions)
+  if kind != 'embodied':
+    return np.ascontiguousarray(a if a.dtype == np.float32 else a.astype(np.float64))
+  if a.ndim == 0 or a.shape[-1] != 2:
+    raise ValueError('Embodied actions must be (carry, direction) rows, got shape %s' % (a.shape,))
+  valid = np.isin(a[..., 1], (0, 1, 2, 3))
+  out = np.full(a.shape, -1, np.int32)
+  out[..., 0] = a[..., 0] != 0
+  out[..., 1][valid] = a[..., 1][valid]
+  return out
+
+
+def zero_actions(kind, n_envs):
+  """All-zero host actions, for a step that resets every env (and so ignores them)."""
+  return host_actions(kind, np.zeros((int(n_envs), ACTIONS[kind].columns), np.float32))
 
 
 class SerialSnapshot(object):
@@ -107,9 +158,7 @@ class Engine(object):
     self._lib = _native.load()
     self.n_envs, self.n_slots, self.pool_depth = int(n_envs), int(n_slots), int(pool_depth)
     self.device = torch.device('cuda', device)
-    self.action_kind = {'select_move': _native.ACT_SELECT_MOVE,
-                        'drag_and_drop': _native.ACT_DRAG_AND_DROP,
-                        'embodied': _native.ACT_EMBODIED}[action['kind']]
+    self.action_kind = ACTIONS[action['kind']].kind
     cfg = _native.Config()
     cfg.device = device
     cfg.n_envs, cfg.n_slots, cfg.pool_depth = self.n_envs, self.n_slots, self.pool_depth
@@ -234,19 +283,6 @@ class Engine(object):
     _native.check(self._lib.swb_request_reset(self._h, ptr, self._stream()))
 
   # -- stepping ---------------------------------------------------------------------
-  def _action_dtype(self, actions):
-    if self.action_kind == _native.ACT_EMBODIED:
-      if actions.dtype != torch.int32 or tuple(actions.shape) != (self.n_envs, 2):
-        raise ValueError('Embodied actions must be an int32 tensor of shape (E, 2)')
-      return _native.DTYPE_I32
-    if tuple(actions.shape) != (self.n_envs, 4):
-      raise ValueError('actions must have shape (E, 4)')
-    if actions.dtype == torch.float32:
-      return _native.DTYPE_F32
-    if actions.dtype == torch.float64:
-      return _native.DTYPE_F64
-    raise ValueError('actions must be float32 or float64')
-
   def _check_frames(self, frames, raster, n_frames):
     """The render kernel writes n_frames * H * W * 3 bytes from frames.data_ptr(): anything but
     a contiguous uint8 tensor of exactly that shape on this device would be written out of
@@ -260,9 +296,7 @@ class Engine(object):
 
   def step(self, actions, raster=None, frames=None):
     """One Environment.step for every env.  `actions`: device tensor."""
-    if actions.device != self.device or not actions.is_contiguous():
-      raise ValueError('actions must be a contiguous tensor on %s' % self.device)
-    dt = self._action_dtype(actions)
+    dt = action_dtype(self.action_kind, self.n_envs, actions, self.device)
     if raster is None:
       _native.check(self._lib.swb_step(self._h, ctypes.c_void_p(actions.data_ptr()), dt,
                                        ctypes.byref(self._out), self._stream()))
@@ -280,9 +314,7 @@ class Engine(object):
     each finished frame is stored into every rank's gathered buffer (`targets`, a
     distributed.PeerFrames slot) over NVLink peer memory.  Returns the StepResult with the
     local rank's gathered tensor as `frames`; it is whole after `targets.barrier()`."""
-    if actions.device != self.device or not actions.is_contiguous():
-      raise ValueError('actions must be a contiguous tensor on %s' % self.device)
-    dt = self._action_dtype(actions)
+    dt = action_dtype(self.action_kind, self.n_envs, actions, self.device)
     ptrs, n, env_offset, local = targets
     self._check_frames(local, raster, int(n) * self.n_envs)
     _native.check(self._lib.swb_step_render_gather(
@@ -324,20 +356,7 @@ class Engine(object):
     """
     # swb_step_host reads E rows of 2 int32 or 4 floats from the buffer: check what step() checks
     a = np.ascontiguousarray(actions)
-    if self.action_kind == _native.ACT_EMBODIED:
-      if a.dtype != np.int32 or a.shape != (self.n_envs, 2):
-        raise ValueError('Embodied actions must be an int32 array of shape (E, 2), got %s %s'
-                         % (a.dtype, a.shape))
-      dt = _native.DTYPE_I32
-    else:
-      if a.shape != (self.n_envs, 4):
-        raise ValueError('actions must have shape (E, 4), got %s' % (a.shape,))
-      if a.dtype == np.float32:
-        dt = _native.DTYPE_F32
-      elif a.dtype == np.float64:
-        dt = _native.DTYPE_F64
-      else:
-        raise ValueError('actions must be float32 or float64, got %s' % a.dtype)
+    dt = action_dtype(self.action_kind, self.n_envs, a)
     E = self.n_envs
     out = out or {}
     reward = out.get('reward') if 'reward' in out else np.empty(E, np.float64)

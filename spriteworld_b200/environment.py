@@ -113,8 +113,8 @@ class Environment(dm_env.Environment):
       self._engine.close()
     self._engine = engine_lib.Engine(
         1, slots, 2, self._action_space.compile(), self._nodes, constants.SHAPES,
-        keep_in_frame=self._keep_in_frame,
-        max_episode_length=int(min(self._max_episode_length, 2 ** 31 - 1)), device=self._device)
+        keep_in_frame=self._keep_in_frame, max_episode_length=self._max_episode_length,
+        device=self._device)
     self._rasters = {
         name: engine_lib.Raster(self._engine, r.width, r.height, r.anti_aliasing, r.bg_color)
         for name, r in self._pil.items()}
@@ -149,13 +149,10 @@ class Environment(dm_env.Environment):
     if kind == 'embodied':
       if action[1] not in (0, 1, 2, 3):
         raise KeyError(action[1])
-      a = np.array([[int(bool(action[0])), int(action[1])]], np.int32)
     else:
-      a = np.asarray(self._action_space.apply_noise_to_action(np.asarray(action)))
-      a = a.reshape(1, 4)
-      if a.dtype != np.float32:
-        a = a.astype(np.float64)
-    return torch.from_numpy(np.ascontiguousarray(a)).to(self._engine.device)
+      action = self._action_space.apply_noise_to_action(np.asarray(action))
+    a = engine_lib.host_actions(kind, np.reshape(action, (1, -1)))
+    return torch.from_numpy(a).to(self._engine.device)
 
   def _run_step(self, action_tensor):
     eng = self._engine
@@ -175,11 +172,6 @@ class Environment(dm_env.Environment):
     self._sync_sprites()
     return {name: f[0].cpu().numpy() for name, f in frames.items()}
 
-  def _dummy_action(self):
-    if self._action_space.compile()['kind'] == 'embodied':
-      return torch.zeros((1, 2), dtype=torch.int32, device=self._engine.device)
-    return torch.zeros((1, 4), dtype=torch.float32, device=self._engine.device)
-
   # -- dm_env API ----------------------------------------------------------------------
   def reset(self):
     self._sprites = self._init_sprites()            # environment.py:75
@@ -187,7 +179,8 @@ class Environment(dm_env.Environment):
     self._reset_next_step = False
     self._load_scene()
     self._engine.request_reset()
-    images = self._run_step(self._dummy_action())
+    zero = engine_lib.zero_actions(self._action_space.compile()['kind'], 1)
+    images = self._run_step(torch.from_numpy(zero).to(self._engine.device))
     return dm_env.restart(self._observation(images))
 
   def success(self):
@@ -319,8 +312,7 @@ class BatchedEnvironment(object):
     slots = max(1, int(slots))
     self._engine = engine_lib.Engine(
         E, slots, K, action_space.compile(), self._nodes, constants.SHAPES,
-        keep_in_frame=keep_in_frame,
-        max_episode_length=int(min(max_episode_length, 2 ** 31 - 1)), device=device)
+        keep_in_frame=keep_in_frame, max_episode_length=max_episode_length, device=device)
     self._rasters = collections.OrderedDict(
         (name, engine_lib.Raster(self._engine, r.width, r.height, r.anti_aliasing, r.bg_color))
         for name, r in self._pil.items())
@@ -557,19 +549,14 @@ class BatchedEnvironment(object):
     return self._engine
 
   def _to_device(self, actions):
+    """Host actions through engine.host_actions; tensors are moved, not converted."""
     dev = self._engine.device
-    if isinstance(actions, torch.Tensor):
-      t = actions
-    else:
-      a = np.asarray(actions)
-      if self._action_space.compile()['kind'] == 'embodied':
-        a = a.astype(np.int32)
-      elif a.dtype != np.float32:
-        a = a.astype(np.float64)
-      t = torch.from_numpy(np.ascontiguousarray(a))
-    t = t.to(dev)
+    kind = self._action_space.compile()['kind']
+    if not isinstance(actions, torch.Tensor):
+      actions = torch.from_numpy(engine_lib.host_actions(kind, actions))
+    t = actions.to(dev)
     noise_scale = getattr(self._action_space, '_noise_scale', None)
-    if noise_scale and self._action_space.compile()['kind'] != 'embodied':
+    if noise_scale and kind != 'embodied':
       # SelectMove.apply_noise_to_action (action_spaces.py:69-75), one draw per env; like
       # there, float32 actions become float64 by the addition
       noise = self._rng.normal(loc=0.0, scale=noise_scale, size=(self.n_envs, 4))
@@ -605,10 +592,7 @@ class BatchedEnvironment(object):
     """Restarts every env from its next pooled scene; returns the FIRST timestep."""
     self._resets += 1
     self._engine.request_reset()
-    kind = self._action_space.compile()['kind']
-    shape, dtype = ((self.n_envs, 2), torch.int32) if kind == 'embodied' else (
-        (self.n_envs, 4), torch.float32)
-    return self.step(torch.zeros(shape, dtype=dtype, device=self._engine.device))
+    return self.step(engine_lib.zero_actions(self._action_space.compile()['kind'], self.n_envs))
 
   def observation_spec(self):
     """Per-env specs (the leading n_envs axis of the batched observations is not included)."""
@@ -721,11 +705,7 @@ class ShardedBatchedEnvironment(object):
       # render kernel (and with it its peer stores) has
       dist.all_gather_into_tensor(self._out_all, eng.out_bytes, group=self.group)
     self._t += 1
-    per_rank = self._out_all.view(W, engine_lib.OUT_BYTES_PER_ENV * E)
-    reward = per_rank[:, :8 * E].contiguous().view(torch.float64).reshape(W * E)
-    step_type = per_rank[:, 8 * E:9 * E].reshape(W * E).view(torch.int8)
-    success = per_rank[:, 9 * E:10 * E].reshape(W * E)
-    status = per_rank[:, 10 * E:11 * E].reshape(W * E)
+    reward, step_type, success, status = engine_lib.split_outputs(self._out_all.view(W, -1), E)
     discount = (step_type != _native.STEP_LAST).to(torch.float32)
     obs = collections.OrderedDict([(self._image, res.frames)])
     return BatchedTimeStep(step_type, reward, discount, obs, success, status)
@@ -734,10 +714,7 @@ class ShardedBatchedEnvironment(object):
     env = self.local
     env._resets += 1
     env.engine.request_reset()
-    kind = env._action_space.compile()['kind']
-    shape, dtype = ((self.n_local, 2), torch.int32) if kind == 'embodied' else (
-        (self.n_local, 4), torch.float32)
-    return self.step(torch.zeros(shape, dtype=dtype, device=env.engine.device))
+    return self.step(engine_lib.zero_actions(env._action_space.compile()['kind'], self.n_local))
 
   def observation_spec(self):
     return self.local.observation_spec()

@@ -69,9 +69,7 @@ class OracleEngine(object):
                max_episode_length=1000, device=0):
     self.n_envs, self.n_slots, self.pool_depth = int(n_envs), int(n_slots), int(pool_depth)
     self.device = torch.device('cpu')
-    self.action_kind = {'select_move': _native.ACT_SELECT_MOVE,
-                        'drag_and_drop': _native.ACT_DRAG_AND_DROP,
-                        'embodied': _native.ACT_EMBODIED}[action['kind']]
+    self.action_kind = engine_lib.ACTIONS[action['kind']].kind
     # the engine's FindGoalPosition distance: the correctly rounded sqrt
     self._cfg = oracle.with_device_sqrt(fixtures.env_cfg_from_meta(dict(
         action=dict(kind=action['kind'], scale=float(action['scale']),
@@ -129,6 +127,7 @@ class OracleEngine(object):
       self._bo.reset_next[np.asarray(mask, bool)] = 1
 
   def step(self, actions, raster=None, frames=None):
+    engine_lib.action_dtype(self.action_kind, self.n_envs, actions)   # what Engine.step accepts
     a = np.ascontiguousarray(actions.numpy())
     self._bo.step(a)   # a bad Embodied direction sets ENV_BAD_ACTION, like the engine
     self._launches += 1

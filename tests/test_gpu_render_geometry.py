@@ -9,7 +9,7 @@ unwritten band or a stray store shows up instead of matching a background by cha
 guard bytes on both sides must come back untouched.  Frames are compared bit-exact.
 
 CASES is the sweep; test_case_table_covers_render_paths recomputes, from the host formulas of
-swb_raster_create and launch_render_targets, which kernel paths each case reaches and fails if
+swb_raster_create and check_render, which kernel paths each case reaches and fails if
 the table stops covering one of them.
 """
 import ctypes
@@ -90,7 +90,7 @@ def _n_envs(case, n_sms):
 
 
 # ---------------------------------------------------------------------------------------
-# host formulas of swb_raster_create / launch_render_targets / render_kernel phase D
+# host formulas of swb_raster_create / check_render / enqueue_render / render_kernel phase D
 # ---------------------------------------------------------------------------------------
 
 def render_plan(W, H, S, E, n_sms=H100_SMS, base=0):
