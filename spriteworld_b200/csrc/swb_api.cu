@@ -405,12 +405,13 @@ static int check_render(const swb_engine *eng, const swb_raster *r, int max_span
   const RasterDev &rd = r->rd;
   int max_smem = 0;
   CUDA_TRY(cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, eng->device));
-  RenderLayout L(eng->st.S, r->smem_rows, max_spans, rd.band_rows, rd.W, rd.aa, rd.ncls_x, rd.ncls_y);
+  RenderLayout L(eng->st.S, r->smem_rows, max_spans, rd.band_rows, rd.W, rd.aa, rd.ncls_x, rd.ncls_y,
+                 rd.prefix_stride, rd.v_nks);
   // many convex slots on a wide raster: rather than refuse the raster, keep 16 visible segments
   // per canvas row as with concave shapes (a row with more is flagged, see RenderLayout)
   if (L.total > max_smem && L.segcap > 16)
     L = RenderLayout(eng->st.S, r->smem_rows, max_spans, rd.band_rows, rd.W, rd.aa, rd.ncls_x,
-                     rd.ncls_y, false);
+                     rd.ncls_y, rd.prefix_stride, rd.v_nks, false);
   if ((L.cap + max_spans) * 4 * r->smem_rows > L.scratch_bytes)
     return fail("render scratch (%d B) cannot hold one sprite spanning %d canvas rows", L.scratch_bytes,
                 r->smem_rows);
@@ -450,35 +451,39 @@ int swb_raster_create(swb_engine *eng, int32_t width, int32_t height, int32_t aa
   rd.max_spans = 1;
   rd.ncls_x = r->ax.n_cls;
   rd.ncls_y = r->ay.n_cls;
+  rd.prefix_stride = r->ax.prefix_stride;
   int rows = 0;
   for (int b = 0; b < rd.n_bands; ++b) {
     const int y0 = b * rd.band_rows, y1 = std::min(y0 + rd.band_rows, height) - 1;
     // the kernel counts a band's canvas rows from a multiple of four
     rows = std::max(rows, r->ay.win_min[y1] + r->ay.win_len[y1] - (r->ay.win_min[y0] & ~3));
-    // a tile of TILE_BLOCKS blocks of eight output rows must fit the H tile's row length
-    for (int t0 = y0; t0 <= y1; t0 += 8) {
-      const int t1 = std::min(t0 + 8 * TILE_BLOCKS - 1, y1);
-      const int span = r->ay.win_min[t1] + r->ay.win_len[t1] - (r->ay.win_min[t0] & ~3);
-      if (span > 4 * HT_ROWW) {
-        delete r;
-        return fail("vertical tap windows of %d output rows span %d canvas rows (limit %d)",
-                    8 * TILE_BLOCKS, span, 4 * HT_ROWW);
-      }
-    }
   }
   r->smem_rows = rows;
-  // refuse a raster that cannot render even convex shapes (a star or spoke may still fail later)
-  std::optional<RenderLayout> plan;
-  if (check_render(eng, r, 1, &plan)) {
+  // a tile's canvas rows must fit the H tile's row length: as many blocks per tile as fit
+  rd.tile_blocks = choose_tile_blocks(r->ay, rd.band_rows, TILE_BLOCKS, 4 * HT_ROWW);
+  if (rd.tile_blocks == 0) {
+    const int span = tile_span(r->ay, rd.band_rows, 1);
     delete r;
-    return 1;
+    return fail("vertical tap windows of 8 output rows span %d canvas rows, more than the %d of the "
+                "render kernel's H tile (anti_aliasing %d is too large for a frame %d rows high)",
+                span, 4 * HT_ROWW, aa, height);
   }
   VFragHost vf;
   if (!build_vfrag(r->ay, &vf, &err)) {
     delete r;
     return fail("%s", err.c_str());
   }
+  if (vf.nks > V_KS_WIDE) {  // cannot happen: one block's windows fit 4 * HT_ROWW canvas rows
+    delete r;
+    return fail("vertical pass needs %d k-steps (limit %d)", vf.nks, V_KS_WIDE);
+  }
   rd.v_nks = vf.nks;
+  // refuse a raster that cannot render even convex shapes (a star or spoke may still fail later)
+  std::optional<RenderLayout> plan;
+  if (check_render(eng, r, 1, &plan)) {
+    delete r;
+    return 1;
+  }
   const uint32_t *d_frag = nullptr;
   if (upload_axis(r, r->ax, &rd.ax) || upload_axis(r, r->ay, &rd.ay) ||
       upload_vec(r, vf.blk_cls, &rd.v_blk_cls) || upload_vec(r, vf.frag, &d_frag)) {
@@ -507,14 +512,17 @@ static int enqueue_render(swb_engine *eng, const swb_raster *r, const RenderLayo
                           int env_base, int env_count, bool after_step) {
   RasterDev rd = r->rd;
   rd.max_spans = L.M;
-  auto kernel = targets.n > 1 ? render_kernel<true> : render_kernel<false>;
+  // the wide instantiation only for rasters whose tables the narrow one was not compiled for
+  const bool wide = render_wide(rd);
+  auto kernel = targets.n > 1 ? (wide ? render_kernel<true, true> : render_kernel<true, false>)
+                              : (wide ? render_kernel<false, true> : render_kernel<false, false>);
   CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, L.total));
   DevState st = eng->st;
   st.render_status = status;
   // persistent CTAs: one per resident slot (or per item if there are fewer), claiming
   // (env, band) items from the engine's counter; see render_kernel
   const int n_items = env_count * rd.n_bands;
-  const int grid = std::min(n_items, eng->n_sms * R_CTAS_PER_SM);
+  const int grid = std::min(n_items, eng->n_sms * (wide ? R_CTAS_PER_SM_WIDE : R_CTAS_PER_SM));
   cudaLaunchConfig_t lc = {};
   lc.gridDim = dim3(grid);
   lc.blockDim = dim3(R_THREADS);

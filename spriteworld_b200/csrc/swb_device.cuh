@@ -47,12 +47,16 @@ struct StepCfg {
   swb_task_node nodes[SWB_MAX_NODES];
 };
 
+// Prefix-table stride of windows up to 32 taps (anti_aliasing <= 5), the stride the render
+// kernel's narrow instantiation is compiled for; longer windows take their length + 1.
+constexpr int kNarrowPrefixStride = 33;
+
 // Resampling tables for one axis (Pillow precompute_coeffs / normalize_coeffs_8bpc).
 struct AxisTables {
   const int16_t *win_min;    // [n_out]  first input index of the tap window
-  const uint8_t *win_len;    // [n_out]  taps (<= 32)
+  const uint8_t *win_len;    // [n_out]  taps (6 * anti_aliasing at most, <= 255)
   const uint8_t *win_cls;    // [n_out]  class = distinct tap vector
-  const int32_t *prefix;     // [n_cls][33] prefix sums of the tap vector, prefix[len] = total
+  const int32_t *prefix;     // [n_cls][RasterDev::prefix_stride] prefix sums of the tap vector, prefix[len] = total
   const int16_t *first_out;  // [n_in] first output whose window contains input index i
   const int16_t *last_out;   // [n_in] last  output whose window contains input index i
 };
@@ -64,10 +68,13 @@ struct RasterDev {
   int n_bands;
   int max_spans;  // spans kept per (sprite, canvas row)
   int ncls_x, ncls_y;  // distinct tap vectors per axis
+  int prefix_stride;   // entries per class of ax.prefix: the longest horizontal window + 1, >= 33
+  int tile_blocks;     // blocks of eight output rows per phase-C tile (3, 2 or 1): the most whose
+                       // vertical windows fit the H tile's 4 * HT_ROWW canvas rows in every band
   // vertical pass on the integer tensor pipe (mma.sync m16n8k32 u8 x s8 -> s32): per block of
   // eight output rows the 22-bit tap matrix, cut into three signed 8-bit limbs and laid out as
   // the instruction's B fragments (see swb_tables.h build_vfrag)
-  int v_nks;                 // k-steps (32 canvas rows each) a block's taps span
+  int v_nks;                 // k-steps (32 canvas rows each) a block's taps span (1..6)
   const uint8_t *v_blk_cls;  // [ceil(H/8)] class (distinct coefficient matrix) of each block
   const uint2 *v_frag;       // [n_cls][v_nks][3 limbs][32 lanes] {b0, b1}
   AxisTables ax, ay;

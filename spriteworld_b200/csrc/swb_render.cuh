@@ -15,7 +15,8 @@
 //                 the row's list of VISIBLE segments (x range + sprite), i.e. the painter's
 //                 algorithm resolved once per canvas row.
 //   C  per sprite region (the outputs whose 2-D tap window can see the sprite), in tiles of
-//      up to three blocks of eight output rows x 20 columns:
+//      up to rd.tile_blocks (3; 2 or 1 where the vertical windows are too long for three)
+//      blocks of eight output rows x 20 columns:
 //        H  horizontal LANCZOS pass of the canvas rows the tile needs.  A canvas row is
 //           piecewise constant, so an output is bg*K + sum_segments (colour-bg) * (P[b]-P[a])
 //           with P the prefix sums of the 22-bit tap vector and [a, b) the segment clamped
@@ -48,9 +49,13 @@ constexpr int R_THREADS = 256;
 #define SWB_RENDER_CTAS 5
 #endif
 constexpr int R_CTAS_PER_SM = SWB_RENDER_CTAS;  // resident CTAs per SM the register budget is set for
+constexpr int R_CTAS_PER_SM_WIDE = 2;            // the same for render_kernel<., true>
 constexpr int H_NC = 2;           // output columns one H-pass thread owns
 constexpr int TILE_X_MAX = 20;    // output columns per tile
-constexpr int TILE_BLOCKS = 3;    // blocks of eight output rows per tile
+constexpr int TILE_BLOCKS = 3;    // most blocks of eight output rows per tile (RasterDev::tile_blocks)
+constexpr int V_KS_NARROW = 3;    // most V-pass k-steps of render_kernel<., false>;
+                                  // render_kernel<., true> takes up to V_KS_WIDE
+constexpr int V_KS_WIDE = 6;      // a one-block tile spans at most 4 * HT_ROWW = 176 canvas rows: 6 k-steps
 constexpr int HT_N = 3 * TILE_X_MAX;  // (column, channel) rows of the H tile; the fourth MMA row tile of 16
                                   // reads four rows (and a k-step's tail) past it, into the staged frame
                                   // that follows in shared memory: values that are never stored
@@ -70,6 +75,11 @@ struct RenderTargets {
   int self;  // index of this rank's own buffer in dst
 };
 
+// Whether a raster needs render_kernel<., true>: tables beyond those of anti_aliasing <= 5
+inline bool render_wide(const RasterDev &rd) {
+  return rd.v_nks > V_KS_NARROW || rd.tile_blocks != TILE_BLOCKS || rd.prefix_stride != kNarrowPrefixStride;
+}
+
 struct RenderLayout {
   int S, rows, M, band_rows, W, aa, ncx, ncy, cap;
   int off_meta, off_edge_i, off_edge_f, off_edge_yr, off_hl, off_region;
@@ -77,8 +87,9 @@ struct RenderLayout {
   int scratch_bytes, segcap;
   // exact_segs: with convex shapes only, size the segment table for every row a scene can
   // produce (2S-1 pieces); false caps it at 16 like the concave case
+  // pstride: entries per class of the horizontal prefix table; nks: the raster's V-pass k-steps
   __host__ __device__ RenderLayout(int S_, int rows_, int M_, int band_rows_, int W_, int aa_,
-                                   int ncx_, int ncy_, bool exact_segs = true)
+                                   int ncx_, int ncy_, int pstride, int nks, bool exact_segs = true)
       : S(S_), rows(rows_), M(M_), band_rows(band_rows_), W(W_), aa(aa_), ncx(ncx_), ncy(ncy_) {
     int o = 0;
     auto take = [&](int bytes) { int r = o; o += (bytes + 15) & ~15; return r; };
@@ -97,7 +108,7 @@ struct RenderLayout {
     if (!exact_segs && segcap > 16) segcap = 16;
     off_nseg = take(((rows + 3) & ~3) + 8);  // +: quads of the H pass may end past the last row
     off_segs = take(rows * segcap * 4);
-    off_prefix = take(ncx * 33 * 4);
+    off_prefix = take(ncx * pstride * 4);
     off_xwin = take(W * 4);                // per output column: win_min | len<<16 | cls<<24
     off_ywin = take(band_rows * 4);
     cap = (M > 1) ? 16 : 8;                // crossings kept per (sprite, row)
@@ -110,8 +121,13 @@ struct RenderLayout {
     off_scratch = take(ht_bytes);
     off_frame = take(frame_bytes);
     scratch_bytes = o - off_scratch;
-    // the V pass may read up to row 63 of the H tile and 24 words past it (see HT_N)
-    if (o < off_scratch + (64 * HT_ROWW + 24) * 4) o = off_scratch + (64 * HT_ROWW + 24) * 4;
+    // The V pass reads, for H-tile row n <= 63 (see HT_N), the words kw + 8 ks + (lane & 3) + {0, 4},
+    // ks < nks, of that row: kw, the block's first word, is < HT_ROWW (the block's windows lie in
+    // the tile), so the last word read is below 63 * HT_ROWW + HT_ROWW + 8 nks.  Words past a
+    // block's window (the next H-tile row, the staged frame, this tail) meet zero taps: they
+    // must be addressable shared memory, nothing more
+    const int v_words = 64 * HT_ROWW + 8 * nks;
+    if (o < off_scratch + v_words * 4) o = off_scratch + v_words * 4;
     total = o;
   }
 };
@@ -242,8 +258,16 @@ __constant__ uint32_t c_prmt_insert[4] = {0x3214u, 0x3240u, 0x3410u, 0x4210u};  
 // Persistent: CTAs claim (env, band) items with atomicAdd(work_counter) - work_base until
 // none is left (the host advances work_base by n_items + gridDim.x per launch, so the
 // counter never needs a reset).
-template <bool kPeers>  // kPeers: also store the frame into the other ranks' buffers
-__global__ void __launch_bounds__(R_THREADS, R_CTAS_PER_SM)
+// kPeers: also store the frame into the other ranks' buffers.
+// kWide: the raster's tables go beyond those of anti_aliasing <= 5 (render_wide): the tile plan
+// takes rd.tile_blocks, the H pass the prefix stride rd.prefix_stride and the V pass up to
+// V_KS_WIDE k-steps.  The narrow instantiation has TILE_BLOCKS, kNarrowPrefixStride and
+// V_KS_NARROW compiled in: the code of the aa <= 5 path does not change with the wide one
+// (reading the stride and tile blocks at run time cost it 0.4 % at C2).  Wide rasters' staged
+// frames and segment tables leave room for few CTAs per SM anyway, so their register budget is
+// set for R_CTAS_PER_SM_WIDE
+template <bool kPeers, bool kWide>
+__global__ void __launch_bounds__(R_THREADS, kWide ? R_CTAS_PER_SM_WIDE : R_CTAS_PER_SM)
 render_kernel(DevState st, RasterDev rd, const RenderLayout L, const RenderTargets targets,
               int env_base, int n_items, unsigned *work_counter, unsigned work_base) {
   unsigned char *const smem = g_render_smem;
@@ -291,7 +315,8 @@ render_kernel(DevState st, RasterDev rd, const RenderLayout L, const RenderTarge
   // ---- once per CTA: the axis tables ------------------------------------------------------
   if (kPeers && tid < SWB_MAX_PEERS) s_dst[tid] = targets.dst[tid];
 #pragma unroll 1
-  for (int i = tid; i < rd.ncls_x * 33; i += R_THREADS) s_prefix[i] = rd.ax.prefix[i];
+  for (int i = tid; i < rd.ncls_x * (kWide ? rd.prefix_stride : kNarrowPrefixStride); i += R_THREADS)
+    s_prefix[i] = rd.ax.prefix[i];
 #pragma unroll 1
   for (int i = tid; i < rd.W; i += R_THREADS)
     s_xwin[i] = (uint32_t)(uint16_t)rd.ax.win_min[i] | ((uint32_t)rd.ax.win_len[i] << 16) |
@@ -483,11 +508,12 @@ render_kernel(DevState st, RasterDev rd, const RenderLayout L, const RenderTarge
       s_region[s * 4 + 0] = yo0; s_region[s * 4 + 1] = yo1;
       s_region[s * 4 + 2] = xo0; s_region[s * 4 + 3] = xo1;
       // tile plan: the blocks of eight output rows the region touches, in equal groups of at
-      // most TILE_BLOCKS; equal column blocks of at most TILE_X_MAX (columns need no halo)
+      // most rd.tile_blocks; equal column blocks of at most TILE_X_MAX (columns need no halo)
       int pny = 1, pnx = 1;
       if (yo1 >= yo0 && xo1 >= xo0) {
         const int nb = (yo1 >> 3) - (yo0 >> 3) + 1, rw = xo1 - xo0 + 1;  // nb <= 8: bands have <= 64 rows
-        const int nty = div20(nb + TILE_BLOCKS - 1, TILE_BLOCKS);
+        const int tb = kWide ? rd.tile_blocks : TILE_BLOCKS;
+        const int nty = div20(nb + tb - 1, tb);
         pny = div20(nb + nty - 1, nty);
         const int ntx = div20(rw + TILE_X_MAX - 1, TILE_X_MAX);  // rw <= 4096
         pnx = ntx <= 64 ? div20(rw + ntx - 1, ntx) : (rw + ntx - 1) / ntx;
@@ -686,7 +712,7 @@ render_kernel(DevState st, RasterDev rd, const RenderLayout L, const RenderTarge
   }
   SWB_MARK(7);
 
-  // ---- phase C: per sprite region, in tiles of <= TILE_BLOCKS blocks of eight output rows
+  // ---- phase C: per sprite region, in tiles of <= rd.tile_blocks blocks of eight output rows
   // x <= TILE_X_MAX columns.  Blocks are aligned to multiples of eight output rows of the
   // frame, so that a block's tap matrix is one of a few classes (rd.v_blk_cls); outputs of a
   // block outside the region are computed from whatever the H tile holds and not stored.
@@ -797,7 +823,7 @@ render_kernel(DevState st, RasterDev rd, const RenderLayout L, const RenderTarge
             for (int q = 0; q < H_NC; ++q) {
               const int c = c0 + q * cs;
               const uint32_t xw = s_xwin[tx0 + (c < nx ? c : c0)];
-              plo[q] = (int)(sm_prefix + (xw >> 24) * 33u * 4u);
+              plo[q] = (int)(sm_prefix + (xw >> 24) * (uint32_t)(kWide ? rd.prefix_stride : kNarrowPrefixStride) * 4u);
               phi[q] = plo[q] + (int)(((xw >> 16) & 0xFFu) << 2);
               poff[q] = plo[q] - ((int)(int16_t)(xw & 0xFFFFu) << 2);
               kk[q] = lds_s32((uint32_t)phi[q]);  // sum of the window's taps
@@ -906,7 +932,7 @@ render_kernel(DevState st, RasterDev rd, const RenderLayout L, const RenderTarge
               const uint32_t a_addr = ht0 + v_aoff + (uint32_t)kw * 4u;
               int d0[4] = {1 << 21, 1 << 21, 1 << 21, 1 << 21}, d1[4] = {0, 0, 0, 0}, d2[4] = {0, 0, 0, 0};
 #pragma unroll
-              for (int ks = 0; ks < 3; ++ks) {  // v_nks <= 3
+              for (int ks = 0; ks < (kWide ? V_KS_WIDE : V_KS_NARROW); ++ks) {  // v_nks <= this
                 if (ks < nks) {
                   uint32_t a[4];
                   a[0] = lds_u32(a_addr + 32u * ks);

@@ -5,7 +5,8 @@
 // renderers/pil_renderer.py:84): support 3*scale, window [int(c-s+.5), int(c+s+.5)),
 // taps normalised in double and quantised to 22-bit fixed point.  On top of the raw taps
 // the kernel wants: a class id per output (outputs with identical tap vectors share one
-// table), prefix sums per class (horizontal pass over piecewise-constant rows), the
+// table), prefix sums per class (horizontal pass over piecewise-constant rows; one row of
+// max_len + 1 entries per class, at least 33: 33 up to 5x, 37 at 6x, 61 at 10x), the
 // inverse maps "input index -> first/last output whose window contains it" and, for the
 // vertical pass, the tap matrix of every block of eight outputs as tensor-core fragments.
 #pragma once
@@ -25,9 +26,10 @@ constexpr int kPrecisionBits = 32 - 8 - 2;  // Pillow PRECISION_BITS
 
 struct AxisHost {
   int n_in = 0, n_out = 0, n_cls = 0, max_len = 0;
+  int prefix_stride = 1;         // max(max_len + 1, kNarrowPrefixStride)
   std::vector<int16_t> win_min;
   std::vector<uint8_t> win_len, win_cls;
-  std::vector<int32_t> prefix;   // [n_cls][33]
+  std::vector<int32_t> prefix;   // [n_cls][prefix_stride]
   std::vector<int16_t> first_out, last_out;
   std::vector<std::vector<int32_t>> taps;  // per output, for tests
 };
@@ -78,9 +80,8 @@ inline bool build_axis(int n_in, int n_out, AxisHost *ax, std::string *err) {
       }
       for (int x = 0; x < xmax; ++x)
         if (ww != 0.0) k[x] /= ww;
-      if (xmax > 32) {
-        *err = "tap window of " + std::to_string(xmax) +
-               " > 32 (anti_aliasing > 5 is not supported by the render kernel)";
+      if (xmax > 255) {  // win_len and the kernel's packed windows hold 8 bits
+        *err = "tap window of " + std::to_string(xmax) + " > 255 taps";
         return false;
       }
       ax->win_min[xx] = (int16_t)xmin;
@@ -111,12 +112,13 @@ inline bool build_axis(int n_in, int n_out, AxisHost *ax, std::string *err) {
     ax->max_len = std::max<int>(ax->max_len, ax->win_len[xx]);
   }
   ax->n_cls = (int)cls.size();
-  ax->prefix.assign((size_t)ax->n_cls * 33, 0);
+  ax->prefix_stride = std::max(ax->max_len + 1, kNarrowPrefixStride);
+  ax->prefix.assign((size_t)ax->n_cls * ax->prefix_stride, 0);
   for (const auto &kv : cls) {
     const std::vector<int32_t> &t = kv.first;
-    int32_t *P = ax->prefix.data() + (size_t)kv.second * 33;
+    int32_t *P = ax->prefix.data() + (size_t)kv.second * ax->prefix_stride;
     int32_t run = 0;
-    for (int i = 0; i <= 32; ++i) {
+    for (int i = 0; i < ax->prefix_stride; ++i) {
       P[i] = run;
       if (i < (int)t.size()) run += t[i];
     }
@@ -144,6 +146,30 @@ inline bool build_axis(int n_in, int n_out, AxisHost *ax, std::string *err) {
       ax->last_out[i] = 0;
     }
   return true;
+}
+
+// Canvas rows the vertical tap windows of a phase-C tile of `tb` blocks of eight output rows span
+// at most.  Bands are `band_rows` output rows; a tile may start at any block of a band and never
+// crosses into the next one, and its rows are counted from a multiple of four (the H tile packs
+// four canvas rows into a word).
+inline int tile_span(const AxisHost &ay, int band_rows, int tb) {
+  int span = 0;
+  for (int y0 = 0; y0 < ay.n_out; y0 += band_rows) {
+    const int y1 = std::min(y0 + band_rows, ay.n_out) - 1;
+    for (int t0 = y0; t0 <= y1; t0 += 8) {
+      const int t1 = std::min(t0 + 8 * tb - 1, y1);
+      span = std::max(span, ay.win_min[t1] + ay.win_len[t1] - (ay.win_min[t0] & ~3));
+    }
+  }
+  return span;
+}
+
+// Blocks per phase-C tile: the largest tb <= max_blocks whose tiles span at most max_rows canvas
+// rows, or 0 if not even one block fits.
+inline int choose_tile_blocks(const AxisHost &ay, int band_rows, int max_blocks, int max_rows) {
+  int tb = max_blocks;
+  while (tb > 0 && tile_span(ay, band_rows, tb) > max_rows) --tb;
+  return tb;
 }
 
 // Vertical pass as a banded integer contraction on the tensor pipe.
