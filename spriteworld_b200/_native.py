@@ -115,6 +115,11 @@ def load():
   L.swb_render_status_pointer.argtypes = [vp, ctypes.POINTER(vp)]
   L.swb_download_state.argtypes = [vp, vp, vp, vp, vp, vp, vp]
   L.swb_upload_state.argtypes = [vp, vp, vp, vp, vp, vp, vp]
+  L.swb_env_record_bytes.argtypes = [vp]
+  L.swb_env_record_bytes.restype = ctypes.c_int64
+  L.swb_save_envs.argtypes = [vp, vp, ci, vp, ctypes.c_uint64, ctypes.POINTER(ci), vp]
+  L.swb_load_envs.argtypes = [vp, vp, ci, vp, ctypes.c_uint64, ci, vp]
+  L.swb_copy_envs.argtypes = [vp, vp, vp, ci, vp]
   L.swb_launch_count.argtypes = [vp]
   L.swb_launch_count.restype = ctypes.c_int64
   if L.swb_sizeof_config() != ctypes.sizeof(Config):
@@ -132,7 +137,7 @@ EXPORTS = (
     'swb_step', 'swb_eval_task', 'swb_apply_action', 'swb_raster_create', 'swb_raster_destroy', 'swb_render', 'swb_step_render',
     'swb_step_render_gather', 'swb_ipc_alloc', 'swb_ipc_free', 'swb_ipc_open', 'swb_ipc_close', 'swb_peer_copy',
     'swb_step_host', 'swb_state_pointers', 'swb_scene_serial_pointer', 'swb_render_status_pointer', 'swb_download_state', 'swb_upload_state',
-    'swb_launch_count')
+    'swb_env_record_bytes', 'swb_save_envs', 'swb_load_envs', 'swb_copy_envs', 'swb_launch_count')
 
 
 def check(rc):

@@ -12,7 +12,7 @@ import sys
 CSRC = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'csrc')
 LIB = os.path.join(CSRC, 'libspriteworld_b200.so')
 SOURCES = ['swb_api.cu']
-HEADERS = ['swb_device.cuh', 'swb_render.cuh', 'swb_step.cuh', 'swb_tables.h',
+HEADERS = ['swb_device.cuh', 'swb_render.cuh', 'swb_states.cuh', 'swb_step.cuh', 'swb_tables.h',
            os.path.join('..', '..', 'include', 'spriteworld_b200.h')]
 
 NVCC_FLAGS = [

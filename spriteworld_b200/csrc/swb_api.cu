@@ -9,6 +9,7 @@
 
 #include "swb_device.cuh"
 #include "swb_render.cuh"
+#include "swb_states.cuh"
 #include "swb_step.cuh"
 #include "swb_tables.h"
 
@@ -55,6 +56,15 @@ struct UploadSlot {
   bool in_flight = false;
 };
 
+// Pinned staging of the env ids of swb_save_envs / swb_load_envs / swb_copy_envs and its device
+// twin, `cap` int32 each; two alternate, so the host stages call i+1 while call i's copy is queued.
+struct IdSlot {
+  size_t cap = 0;
+  int32_t *host = nullptr, *dev = nullptr;
+  cudaEvent_t done = nullptr;  // recorded after the kernels that read `dev`
+  bool in_flight = false;
+};
+
 struct swb_engine {
   swb_config cfg;
   StepCfg step_cfg;
@@ -69,6 +79,11 @@ struct swb_engine {
   // staging for scene uploads (pinned host + device), grown on demand, double-buffered
   UploadSlot upload_slots[2];
   int upload_next = 0;
+  // env records: id staging, and the records of an overlapping swb_copy_envs (grown on demand)
+  IdSlot id_slots[2];
+  int id_next = 0;
+  unsigned char *d_records = nullptr;
+  size_t records_bytes = 0;
   std::vector<void *> owned;
   // buffers of swb_step_host
   void *h_actions = nullptr;
@@ -141,7 +156,7 @@ int upload_axis(swb_raster *r, const AxisHost &h, AxisTables *d) {
 extern "C" {
 
 const char *swb_last_error(void) { return g_error.c_str(); }
-int swb_version(void) { return 1; }
+int swb_version(void) { return 2; }
 int swb_sizeof_config(void) { return (int)sizeof(swb_config); }
 int swb_sizeof_task_node(void) { return (int)sizeof(swb_task_node); }
 
@@ -244,6 +259,13 @@ void swb_engine_destroy(swb_engine *eng) {
     if (slot.dev) cudaFree(slot.dev);
     if (slot.done) cudaEventDestroy(slot.done);
   }
+  for (auto &slot : eng->id_slots) {
+    if (slot.in_flight) cudaEventSynchronize(slot.done);
+    if (slot.host) cudaFreeHost(slot.host);
+    if (slot.dev) cudaFree(slot.dev);
+    if (slot.done) cudaEventDestroy(slot.done);
+  }
+  cudaFree(eng->d_records);
   cudaFree(eng->h_actions); cudaFree(eng->h_out.reward); cudaFree(eng->h_out.step_type);
   cudaFree(eng->h_out.success); cudaFree(eng->h_out.status); cudaFree(eng->h_frames);
   if (eng->copy_stream) cudaStreamDestroy(eng->copy_stream);
@@ -742,6 +764,178 @@ int swb_upload_state(swb_engine *eng, const double *pos_x, const double *pos_y, 
   if (reset_next) CUDA_TRY(cudaMemcpyAsync(eng->st.reset_next, reset_next, eng->st.E, cudaMemcpyHostToDevice, stream));
   CUDA_TRY(cudaStreamSynchronize(stream));
   return 0;
+}
+
+}  // extern "C"
+
+// Env ids of a record call: every id in [0, E); with `mark`, no id twice (destinations), and each
+// id is marked in it.
+static int check_env_ids(const swb_engine *eng, const char *fn, const int32_t *ids, int32_t n,
+                         std::vector<uint8_t> *mark) {
+  for (int32_t i = 0; i < n; ++i) {
+    if (ids[i] < 0 || ids[i] >= eng->st.E)
+      return fail("%s: env id %d out of range [0, %d)", fn, ids[i], eng->st.E);
+    if (mark) {
+      if ((*mark)[ids[i]]) return fail("%s: destination env id %d appears twice", fn, ids[i]);
+      (*mark)[ids[i]] = 1;
+    }
+  }
+  return 0;
+}
+
+// Moves `n` ids from `a` (and `n` from `b`, if given) into a staging slot and enqueues one copy of
+// them to its device twin; the caller enqueues the kernels that read them, then finish_ids.
+static int stage_ids(swb_engine *eng, const int32_t *a, const int32_t *b, int32_t n, cudaStream_t stream,
+                     IdSlot **out) {
+  IdSlot &slot = eng->id_slots[eng->id_next];
+  eng->id_next ^= 1;
+  if (slot.in_flight) {
+    CUDA_TRY(cudaEventSynchronize(slot.done));
+    slot.in_flight = false;
+  }
+  const size_t need = 2 * (size_t)n;
+  if (need > slot.cap) {
+    if (slot.host) cudaFreeHost(slot.host);
+    if (slot.dev) cudaFree(slot.dev);
+    slot.host = slot.dev = nullptr;
+    slot.cap = 0;
+    const size_t cap = std::max<size_t>(need, 1024);
+    CUDA_TRY(cudaMallocHost(reinterpret_cast<void **>(&slot.host), cap * sizeof(int32_t)));
+    CUDA_TRY(cudaMalloc(reinterpret_cast<void **>(&slot.dev), cap * sizeof(int32_t)));
+    if (!slot.done) CUDA_TRY(cudaEventCreateWithFlags(&slot.done, cudaEventDisableTiming));
+    slot.cap = cap;
+  }
+  memcpy(slot.host, a, n * sizeof(int32_t));
+  if (b) memcpy(slot.host + n, b, n * sizeof(int32_t));
+  CUDA_TRY(cudaMemcpyAsync(slot.dev, slot.host, (b ? 2 : 1) * n * sizeof(int32_t), cudaMemcpyHostToDevice,
+                           stream));
+  *out = &slot;
+  return 0;
+}
+
+static int finish_ids(IdSlot *slot, cudaStream_t stream) {
+  CUDA_TRY(cudaEventRecord(slot->done, stream));
+  slot->in_flight = true;
+  return 0;
+}
+
+static int launch_save(swb_engine *eng, const int32_t *d_ids, int32_t n, void *dst, cudaStream_t stream) {
+  const int threads = 256, blocks = (int)(((size_t)n * eng->st.S + threads - 1) / threads);
+  save_envs_kernel<<<blocks, threads, 0, stream>>>(eng->st, n, d_ids, static_cast<unsigned char *>(dst),
+                                                   RecordLayout(eng->st.S).bytes());
+  eng->launches++;
+  CUDA_TRY(cudaGetLastError());
+  return 0;
+}
+
+static int launch_load(swb_engine *eng, const int32_t *d_ids, int32_t n, const void *src,
+                       cudaStream_t stream) {
+  const int threads = 256, blocks = (int)(((size_t)n * eng->st.S + threads - 1) / threads);
+  load_envs_kernel<<<blocks, threads, 0, stream>>>(eng->st, n, d_ids, static_cast<const unsigned char *>(src),
+                                                   RecordLayout(eng->st.S).bytes());
+  eng->launches++;
+  CUDA_TRY(cudaGetLastError());
+  return 0;
+}
+
+extern "C" {
+
+int64_t swb_env_record_bytes(const swb_engine *eng) {
+  if (!eng) {
+    fail("swb_env_record_bytes: null engine");
+    return -1;
+  }
+  return (int64_t)RecordLayout(eng->st.S).bytes();
+}
+
+int swb_save_envs(swb_engine *eng, const int32_t *env_ids, int32_t n, void *dst, uint64_t dst_bytes,
+                  int32_t *span_class, void *stream_) {
+  if (!eng || !span_class) return fail("swb_save_envs: null argument");
+  if (n < 0) return fail("swb_save_envs: n = %d", n);
+  if (n == 0) {
+    *span_class = eng->max_spans;
+    return 0;
+  }
+  if (!env_ids || !dst) return fail("swb_save_envs: null argument");
+  if (reinterpret_cast<uintptr_t>(dst) % 16) return fail("swb_save_envs: dst is not 16-byte aligned");
+  const uint64_t need = (uint64_t)n * RecordLayout(eng->st.S).bytes();
+  if (dst_bytes < need)
+    return fail("swb_save_envs: %d records need %llu bytes, the buffer has %llu", n,
+                (unsigned long long)need, (unsigned long long)dst_bytes);
+  if (check_env_ids(eng, "swb_save_envs", env_ids, n, nullptr)) return 1;
+  CUDA_TRY(cudaSetDevice(eng->device));
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  IdSlot *slot = nullptr;
+  if (stage_ids(eng, env_ids, nullptr, n, stream, &slot) || launch_save(eng, slot->dev, n, dst, stream))
+    return 1;
+  *span_class = eng->max_spans;
+  return finish_ids(slot, stream);
+}
+
+int swb_load_envs(swb_engine *eng, const int32_t *env_ids, int32_t n, const void *src, uint64_t src_bytes,
+                  int32_t span_class, void *stream_) {
+  if (!eng) return fail("swb_load_envs: null engine");
+  if (n < 0) return fail("swb_load_envs: n = %d", n);
+  if (span_class != 1 && span_class != 4)
+    return fail("swb_load_envs: span_class must be 1 or 4, got %d", span_class);
+  if (n == 0) return 0;
+  if (!env_ids || !src) return fail("swb_load_envs: null argument");
+  if (reinterpret_cast<uintptr_t>(src) % 16) return fail("swb_load_envs: src is not 16-byte aligned");
+  const uint64_t need = (uint64_t)n * RecordLayout(eng->st.S).bytes();
+  if (src_bytes < need)
+    return fail("swb_load_envs: %d records need %llu bytes, the buffer has %llu", n,
+                (unsigned long long)need, (unsigned long long)src_bytes);
+  std::vector<uint8_t> mark(eng->st.E, 0);
+  if (check_env_ids(eng, "swb_load_envs", env_ids, n, &mark)) return 1;
+  CUDA_TRY(cudaSetDevice(eng->device));
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  // records of stars or spokes need the concave span tables, as if their scenes were uploaded
+  eng->max_spans = std::max(eng->max_spans, (int)span_class);
+  IdSlot *slot = nullptr;
+  if (stage_ids(eng, env_ids, nullptr, n, stream, &slot) || launch_load(eng, slot->dev, n, src, stream))
+    return 1;
+  return finish_ids(slot, stream);
+}
+
+int swb_copy_envs(swb_engine *eng, const int32_t *src_ids, const int32_t *dst_ids, int32_t n, void *stream_) {
+  if (!eng) return fail("swb_copy_envs: null engine");
+  if (n < 0) return fail("swb_copy_envs: n = %d", n);
+  if (n == 0) return 0;
+  if (!src_ids || !dst_ids) return fail("swb_copy_envs: null argument");
+  std::vector<uint8_t> mark(eng->st.E, 0);
+  if (check_env_ids(eng, "swb_copy_envs", dst_ids, n, &mark) ||
+      check_env_ids(eng, "swb_copy_envs", src_ids, n, nullptr))
+    return 1;
+  bool overlap = false;
+  for (int32_t i = 0; i < n && !overlap; ++i) overlap = mark[src_ids[i]] != 0;
+  CUDA_TRY(cudaSetDevice(eng->device));
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  // an env both read and written: every source is saved to engine scratch before any destination
+  // is written, so every read sees the state from before the call
+  const size_t need = overlap ? (size_t)n * RecordLayout(eng->st.S).bytes() : 0;
+  if (need > eng->records_bytes) {
+    if (eng->d_records) {
+      CUDA_TRY(cudaDeviceSynchronize());  // an earlier copy on any stream may still read it
+      cudaFree(eng->d_records);
+      eng->d_records = nullptr;
+      eng->records_bytes = 0;
+    }
+    CUDA_TRY(cudaMalloc(reinterpret_cast<void **>(&eng->d_records), need));
+    eng->records_bytes = need;
+  }
+  IdSlot *slot = nullptr;
+  if (stage_ids(eng, src_ids, dst_ids, n, stream, &slot)) return 1;
+  if (!overlap) {
+    const int threads = 256, blocks = (int)(((size_t)n * eng->st.S + threads - 1) / threads);
+    copy_envs_kernel<<<blocks, threads, 0, stream>>>(eng->st, n, slot->dev, slot->dev + n);
+    eng->launches++;
+    CUDA_TRY(cudaGetLastError());
+    return finish_ids(slot, stream);
+  }
+  if (launch_save(eng, slot->dev, n, eng->d_records, stream) ||
+      launch_load(eng, slot->dev + n, n, eng->d_records, stream))
+    return 1;
+  return finish_ids(slot, stream);
 }
 
 #ifdef SWB_PHASE_CLOCKS

@@ -159,16 +159,9 @@ class Engine(object):
     self.n_envs, self.n_slots, self.pool_depth = int(n_envs), int(n_slots), int(pool_depth)
     self.device = torch.device('cuda', device)
     self.action_kind = ACTIONS[action['kind']].kind
-    cfg = _native.Config()
-    cfg.device = device
-    cfg.n_envs, cfg.n_slots, cfg.pool_depth = self.n_envs, self.n_slots, self.pool_depth
-    cfg.action_kind = self.action_kind
-    cfg.action_scale = float(action['scale'])
-    cfg.motion_cost = float(action.get('motion_cost', 0.0))
-    cfg.keep_in_frame = int(bool(keep_in_frame))
-    cfg.max_episode_length = int(min(max_episode_length, 2 ** 31 - 1))
-    fill_task_nodes(cfg, nodes)
-    fill_shapes(cfg, shapes)
+    cfg = make_config(n_envs, n_slots, pool_depth, action, nodes, shapes, keep_in_frame,
+                      max_episode_length, device)
+    self.signature = config_signature(cfg)
     h = ctypes.c_void_p()
     _native.check(self._lib.swb_engine_create(ctypes.byref(cfg), ctypes.byref(h)))
     self._h = h
@@ -410,8 +403,180 @@ class Engine(object):
       out[name] = torch.as_tensor(_DevicePointer(ptr.value, shape, typestr), device=self.device)
     return out
 
+  # -- env records ------------------------------------------------------------------
+  # Ids are lists, ndarrays or tensors; the library checks them on the host, so a CUDA tensor of
+  # ids costs a device-to-host copy (env_ids_array).  The work goes to the current stream.
+  @property
+  def record_bytes(self):
+    """Bytes of one env record (include/spriteworld_b200.h)."""
+    return int(self._lib.swb_env_record_bytes(self._h))
+
+  def _all_or(self, env_ids):
+    return np.arange(self.n_envs, dtype=np.int32) if env_ids is None else env_ids_array(env_ids)
+
+  def save_envs(self, env_ids=None):
+    """EnvStates of envs `env_ids` (default: all, in order), on this engine's device."""
+    ids = self._all_or(env_ids)
+    rb = self.record_bytes
+    data = torch.empty((len(ids), rb), dtype=torch.uint8, device=self.device)
+    span = ctypes.c_int32()
+    _native.check(self._lib.swb_save_envs(self._h, _as_ptr(ids), len(ids), ctypes.c_void_p(data.data_ptr()),
+                                          data.numel(), ctypes.byref(span), self._stream()))
+    return EnvStates(data, span.value, self.signature, self.n_slots)
+
+  def check_states(self, states, n):
+    """ValueError unless `states` holds n records that this engine can load."""
+    if not isinstance(states, EnvStates):
+      raise ValueError('expected EnvStates, got %s' % type(states).__name__)
+    if states.signature != self.signature:
+      raise ValueError('EnvStates were saved by an engine of another configuration (slot count, '
+                       'action space, task tree, shape table, keep_in_frame or max_episode_length)')
+    d = states.data
+    if (d.dtype != torch.uint8 or d.device != self.device or tuple(d.shape) != (n, self.record_bytes)
+        or not d.is_contiguous() or d.data_ptr() % 16):
+      raise ValueError('EnvStates must hold a contiguous, 16-byte aligned uint8 (%d, %d) tensor on '
+                       '%s, got %s' % (n, self.record_bytes, self.device, _describe(d)))
+
+  def load_envs(self, states, env_ids=None):
+    """Env env_ids[i] <- record i of `states` (default ids: all envs, in order; distinct)."""
+    ids = self._all_or(env_ids)
+    self.check_states(states, len(ids))
+    _native.check(self._lib.swb_load_envs(self._h, _as_ptr(ids), len(ids),
+                                          ctypes.c_void_p(states.data.data_ptr()), states.data.numel(),
+                                          states.span_class, self._stream()))
+
+  def copy_envs(self, src_ids, dst_ids):
+    """Env dst_ids[i] <- env src_ids[i]; every read sees the state from before the call."""
+    src, dst = env_ids_array(src_ids), env_ids_array(dst_ids)
+    if len(src) != len(dst):
+      raise ValueError('copy_envs: %d sources, %d destinations' % (len(src), len(dst)))
+    _native.check(self._lib.swb_copy_envs(self._h, _as_ptr(src), _as_ptr(dst), len(src), self._stream()))
+
   def launch_count(self):
     return int(self._lib.swb_launch_count(self._h))
+
+
+def make_config(n_envs, n_slots, pool_depth, action, nodes, shapes, keep_in_frame=True,
+                max_episode_length=1000, device=0):
+  """The swb_config of an engine (see Engine)."""
+  cfg = _native.Config()
+  cfg.device = device
+  cfg.n_envs, cfg.n_slots, cfg.pool_depth = int(n_envs), int(n_slots), int(pool_depth)
+  cfg.action_kind = ACTIONS[action['kind']].kind
+  cfg.action_scale = float(action['scale'])
+  cfg.motion_cost = float(action.get('motion_cost', 0.0))
+  cfg.keep_in_frame = int(bool(keep_in_frame))
+  cfg.max_episode_length = int(min(max_episode_length, 2 ** 31 - 1))
+  fill_task_nodes(cfg, nodes)
+  fill_shapes(cfg, shapes)
+  return cfg
+
+
+def config_signature(cfg):
+  """The bytes of `cfg` with n_envs, pool_depth and device zeroed: engines with equal signatures
+  step and render an env record alike, so records of one load into the other."""
+  sig = _native.Config()
+  ctypes.memmove(ctypes.byref(sig), ctypes.byref(cfg), ctypes.sizeof(_native.Config))
+  sig.n_envs = sig.pool_depth = sig.device = 0
+  return bytes(sig)
+
+
+def record_layout(n_slots):
+  """(fields, record bytes) of an env record of an engine with n_slots slots: fields is a list of
+  (name, byte offset, NumPy dtype, shape within one record).  The table of
+  include/spriteworld_b200.h; `factors` is (5, S) there: scale, angle, c0, c1, c2."""
+  S = int(n_slots)
+  fields, off = [], 0
+  for name in ('x0', 'y0', 'm00', 'm01', 'm10', 'm11', 'vx', 'vy', 'pos_x', 'pos_y'):
+    fields.append((name, off, np.dtype('<f8'), (S,)))
+    off += 8 * S
+  for name, dtype, shape in (('member', '<u4', (S,)), ('rgb', '<u4', (S,)), ('factors', '<f4', (5, S)),
+                             ('step_count', '<i4', ()), ('reset_next', 'u1', ()),
+                             ('shape', 'u1', (S,)), ('pos_f32', 'u1', (S,))):
+    dtype = np.dtype(dtype)
+    fields.append((name, off, dtype, shape))
+    off += dtype.itemsize * int(np.prod(shape, dtype=np.int64))
+  return fields, (off + 15) // 16 * 16
+
+
+_TORCH_DTYPES = {np.dtype('<f8'): torch.float64, np.dtype('<f4'): torch.float32,
+                 np.dtype('<i4'): torch.int32, np.dtype('<u4'): torch.int32, np.dtype('u1'): torch.uint8}
+
+
+def env_ids_array(ids):
+  """Host int32 array of env ids from a list, ndarray or tensor.  A CUDA tensor costs a
+  device-to-host copy, which waits for the work enqueued on its stream."""
+  if isinstance(ids, torch.Tensor):
+    ids = ids.detach().cpu().numpy()
+  a = np.asarray(ids)
+  if a.ndim != 1:
+    raise ValueError('env ids must be one-dimensional, got shape %s' % (a.shape,))
+  if a.size and not np.issubdtype(a.dtype, np.integer):
+    raise ValueError('env ids must be integers, got %s' % a.dtype)
+  if a.size and (a.min() < -2 ** 31 or a.max() >= 2 ** 31):
+    raise ValueError('env id out of range')
+  return np.ascontiguousarray(a, np.int32)
+
+
+class EnvStates(object):
+  """Env records saved on the device (Engine.save_envs): a (n, record_bytes) uint8 tensor, the
+  span class the records need (1: convex shapes only, 4: stars or spokes) and the signature of
+  the engine configuration they belong to (config_signature).
+
+  len(), indexing and slicing (a device gather; an int keeps one record), `to(device)`,
+  EnvStates.cat() and torch.save / torch.load; to_host() decodes the records into NumPy arrays."""
+
+  def __init__(self, data, span_class, signature, n_slots):
+    self.data, self.span_class = data, int(span_class)
+    self.signature, self.n_slots = bytes(signature), int(n_slots)
+
+  @property
+  def record_bytes(self):
+    return int(self.data.shape[1])
+
+  def __len__(self):
+    return int(self.data.shape[0])
+
+  def __getitem__(self, idx):
+    if isinstance(idx, (int, np.integer)):
+      idx = slice(idx, idx + 1 if idx != -1 else None)
+    elif not isinstance(idx, slice):
+      idx = torch.as_tensor(env_ids_array(idx).astype(np.int64), device=self.data.device)
+    return EnvStates(self.data[idx].contiguous(), self.span_class, self.signature, self.n_slots)
+
+  def to(self, device):
+    return EnvStates(self.data.to(device), self.span_class, self.signature, self.n_slots)
+
+  @staticmethod
+  def cat(states):
+    """One EnvStates of the records of `states` (a sequence of EnvStates of one configuration)."""
+    states = list(states)
+    if not states or any(s.signature != states[0].signature for s in states):
+      raise ValueError('EnvStates.cat needs at least one EnvStates, all of one engine configuration')
+    return EnvStates(torch.cat([s.data for s in states]), max(s.span_class for s in states),
+                     states[0].signature, states[0].n_slots)
+
+  def fields(self):
+    """dict name -> device tensor view (n,) + shape of every field (uint32 fields as int32)."""
+    layout, _ = record_layout(self.n_slots)
+    n, out = len(self), {}
+    for name, off, dtype, shape in layout:
+      nbytes = dtype.itemsize * int(np.prod(shape, dtype=np.int64))
+      out[name] = self.data[:, off:off + nbytes].view(_TORCH_DTYPES[dtype]).reshape((n,) + shape)
+    return out
+
+  def to_host(self):
+    """dict of NumPy arrays, one per field: x0 .. vy, pos_x, pos_y (n, S) float64, member (n, S)
+    uint32, rgb (n, S, 3) uint8, factors (n, S, 5) float32, shape and pos_f32 (n, S) uint8,
+    step_count (n,) int32, reset_next (n,) uint8."""
+    out = {name: t.cpu().numpy().copy() for name, t in self.fields().items()}
+    out['member'] = out['member'].view(np.uint32)
+    out['rgb'] = out['rgb'].view(np.uint32)[..., None].view(np.uint8)[..., :3].copy()
+    out['factors'] = np.ascontiguousarray(out['factors'].transpose(0, 2, 1))
+    return out
+
+
+torch.serialization.add_safe_globals([EnvStates])   # torch.load(..., weights_only=True)
 
 
 def _describe(t):

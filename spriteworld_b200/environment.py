@@ -336,8 +336,10 @@ class BatchedEnvironment(object):
     # explicit resets so far _safe_resets) and step t an env can have started at most
     # ceil((t - _safe_step) / 2) + (resets since) scenes: an auto-reset takes a LAST and a
     # FIRST step, an explicit reset() one step.  K - 1 fresh scenes were there at the snapshot.
+    # A load or copy counts as an explicit reset: a record saved about to reset (reset_next = 1)
+    # makes the env start its next ring scene on the next step, as reset() does.
     self._t = 0                    # steps enqueued
-    self._resets = 0               # explicit reset() calls
+    self._resets = 0               # explicit reset() calls, load_envs and copy_envs calls
     self._safe_step, self._safe_resets = 0, 0
     self._period = max(1, (K - 2) // 2 if refill == 'async' else 2 * (K - 2))
     self._inflight = None          # async: dict(snapshot step/resets, future)
@@ -593,6 +595,54 @@ class BatchedEnvironment(object):
     self._resets += 1
     self._engine.request_reset()
     return self.step(engine_lib.zero_actions(self._action_space.compile()['kind'], self.n_envs))
+
+  # -- env records -------------------------------------------------------------------------
+  # On the step stream, after everything enqueued so far.  A record holds an env's current scene
+  # and episode counters, not its place in the scene ring: a loaded env plays the saved episode
+  # out, then starts the next scene of its own ring.  A record with reset_next = 1 starts that
+  # scene on the next step, as reset() does, so every load or copy counts as a reset against the
+  # ring's underflow guard (_risk): with loads before every step the ring is refilled more often
+  # rather than an env running onto a ring slot that has not been refilled.
+  # Ids: lists, ndarrays or tensors (a CUDA tensor costs a device-to-host copy).
+  def save_envs(self, env_ids=None):
+    """engine.EnvStates of envs `env_ids` (default: all, in order)."""
+    return self._engine.save_envs(env_ids)
+
+  def load_envs(self, states, env_ids=None):
+    """Env env_ids[i] <- record i of `states` (default ids: all envs, in order)."""
+    self._engine.load_envs(states, env_ids)
+    self._resets += 1
+    if getattr(self, '_pool_static', None) is not None:
+      f = states.fields()
+      static = torch.cat([f['shape'][..., None].float(), f['factors'].transpose(1, 2),
+                          f['vx'][..., None].float(), f['vy'][..., None].float()], -1)
+      self._set_static(np.arange(self.n_envs) if env_ids is None else env_ids, static)
+
+  def copy_envs(self, src_ids, dst_ids):
+    """Env dst_ids[i] <- env src_ids[i]; every read sees the state from before the call."""
+    self._engine.copy_envs(src_ids, dst_ids)
+    self._resets += 1
+    if getattr(self, '_pool_static', None) is not None:
+      cursor = self._engine.state_tensors()['cursor'].long()
+      src = self._device_ids(src_ids)
+      self._set_static(dst_ids, self._pool_static[src, cursor[src]])
+
+  def _device_ids(self, ids):
+    return torch.as_tensor(engine_lib.env_ids_array(ids).astype(np.int64), device=self._engine.device)
+
+  def _set_static(self, env_ids, static):
+    """Factor observations of envs `env_ids` follow a load or copy: their current pool entry."""
+    e = self._device_ids(env_ids)
+    cursor = self._engine.state_tensors()['cursor'].long()
+    self._pool_static[e, cursor[e]] = static
+
+  def render(self):
+    """Re-renders every PILRenderer observation of the current state (a loaded one, say) into
+    this environment's frame buffers, and returns them: dict name -> uint8 (n_envs, H, W, 3)."""
+    out = collections.OrderedDict()
+    for name, r in self._rasters.items():
+      out[name] = self._engine.render(r, self._frames[name])
+    return out
 
   def observation_spec(self):
     """Per-env specs (the leading n_envs axis of the batched observations is not included)."""
