@@ -14,12 +14,14 @@ MAX_SLOTS = 32
 MAX_FILTERS = 32
 
 ACT_SELECT_MOVE, ACT_DRAG_AND_DROP, ACT_EMBODIED = 0, 1, 2
-DTYPE_F32, DTYPE_F64, DTYPE_I32 = 0, 1, 2
+DTYPE_F32, DTYPE_F64, DTYPE_I32, DTYPE_I64 = 0, 1, 2, 3
 TASK_NO_REWARD, TASK_FIND_GOAL, TASK_CLUSTERING, TASK_META = 0, 1, 2, 3
 AGG = {'sum': 0, 'max': 1, 'min': 2, 'mean': 3}
 CRIT = {'all': 0, 'any': 1}
 STEP_FIRST, STEP_MID, STEP_LAST = 0, 1, 2
 ENV_OK, ENV_CLUSTER_LABELS, ENV_CLUSTER_ZERODIV, ENV_BAD_ACTION, ENV_SPAN_OVERFLOW = 0, 1, 2, 4, 8
+IDS_CALL_SAVE, IDS_CALL_LOAD, IDS_CALL_COPY = 0, 1, 2
+IDS_OUT_OF_RANGE, IDS_REPEATED = 1, 2
 
 _c32, _f64, _u8p = ctypes.c_int32, ctypes.c_double, ctypes.POINTER(ctypes.c_uint8)
 
@@ -120,6 +122,10 @@ def load():
   L.swb_save_envs.argtypes = [vp, vp, ci, vp, ctypes.c_uint64, ctypes.POINTER(ci), vp]
   L.swb_load_envs.argtypes = [vp, vp, ci, vp, ctypes.c_uint64, ci, vp]
   L.swb_copy_envs.argtypes = [vp, vp, vp, ci, vp]
+  L.swb_save_envs_dev.argtypes = [vp, vp, ci, ci, vp, ctypes.c_uint64, ctypes.POINTER(ci), vp]
+  L.swb_load_envs_dev.argtypes = [vp, vp, ci, ci, vp, ctypes.c_uint64, ci, vp]
+  L.swb_copy_envs_dev.argtypes = [vp, vp, vp, ci, ci, vp]
+  L.swb_env_ids_status_pointer.argtypes = [vp, ctypes.POINTER(vp)]
   L.swb_launch_count.argtypes = [vp]
   L.swb_launch_count.restype = ctypes.c_int64
   if L.swb_sizeof_config() != ctypes.sizeof(Config):
@@ -137,7 +143,8 @@ EXPORTS = (
     'swb_step', 'swb_eval_task', 'swb_apply_action', 'swb_raster_create', 'swb_raster_destroy', 'swb_render', 'swb_step_render',
     'swb_step_render_gather', 'swb_ipc_alloc', 'swb_ipc_free', 'swb_ipc_open', 'swb_ipc_close', 'swb_peer_copy',
     'swb_step_host', 'swb_state_pointers', 'swb_scene_serial_pointer', 'swb_render_status_pointer', 'swb_download_state', 'swb_upload_state',
-    'swb_env_record_bytes', 'swb_save_envs', 'swb_load_envs', 'swb_copy_envs', 'swb_launch_count')
+    'swb_env_record_bytes', 'swb_save_envs', 'swb_load_envs', 'swb_copy_envs', 'swb_save_envs_dev',
+    'swb_load_envs_dev', 'swb_copy_envs_dev', 'swb_env_ids_status_pointer', 'swb_launch_count')
 
 
 def check(rc):

@@ -84,6 +84,10 @@ struct swb_engine {
   int id_next = 0;
   unsigned char *d_records = nullptr;
   size_t records_bytes = 0;
+  // device-checked id lists (IdCall in swb_states.cuh): claims, the failure word, the status record
+  unsigned long long *d_id_claim = nullptr, *d_id_fail = nullptr;
+  swb_ids_status *d_id_status = nullptr;
+  uint32_t id_seq = 0;
   std::vector<void *> owned;
   // buffers of swb_step_host
   void *h_actions = nullptr;
@@ -156,7 +160,7 @@ int upload_axis(swb_raster *r, const AxisHost &h, AxisTables *d) {
 extern "C" {
 
 const char *swb_last_error(void) { return g_error.c_str(); }
-int swb_version(void) { return 2; }
+int swb_version(void) { return 3; }
 int swb_sizeof_config(void) { return (int)sizeof(swb_config); }
 int swb_sizeof_task_node(void) { return (int)sizeof(swb_task_node); }
 
@@ -229,6 +233,7 @@ int swb_engine_create(const swb_config *cfg, swb_engine **out) {
   A(&st.scene_serial, st.E);
   A(&d_verts, (size_t)SWB_NUM_SHAPES * SWB_MAX_VERTS * 2);
   A(&d_nv, SWB_NUM_SHAPES);
+  A(&eng->d_id_claim, st.E); A(&eng->d_id_fail, 1); A(&eng->d_id_status, 1);
   if (!ok) {
     swb_engine_destroy(eng);
     return fail("device allocation failed: %s", cudaGetErrorString(cudaGetLastError()));
@@ -245,6 +250,8 @@ int swb_engine_create(const swb_config *cfg, swb_engine **out) {
   st.shape_n = d_nv;
   // every env starts "about to reset" (environment.py:70)
   CUDA_TRY(cudaMemset(st.reset_next, 1, st.E));
+  CUDA_TRY(cudaMemset(eng->d_id_claim, 0xFF, (size_t)st.E * sizeof(unsigned long long)));
+  CUDA_TRY(cudaMemset(eng->d_id_fail, 0xFF, sizeof(unsigned long long)));
   *out = eng;
   return 0;
 }
@@ -838,6 +845,94 @@ static int launch_load(swb_engine *eng, const int32_t *d_ids, int32_t n, const v
   return 0;
 }
 
+// Engine scratch of at least `need` bytes for the records of a copy.
+static int grow_records(swb_engine *eng, size_t need) {
+  if (need <= eng->records_bytes) return 0;
+  if (eng->d_records) {
+    CUDA_TRY(cudaDeviceSynchronize());  // an earlier copy on any stream may still read it
+    cudaFree(eng->d_records);
+    eng->d_records = nullptr;
+    eng->records_bytes = 0;
+  }
+  CUDA_TRY(cudaMalloc(reinterpret_cast<void **>(&eng->d_records), need));
+  eng->records_bytes = need;
+  return 0;
+}
+
+// Host checks of a device id list: everything the host sees without reading device memory.
+static int check_dev_ids(const swb_engine *eng, const char *fn, const void *ids, int32_t id_dtype) {
+  if (!ids) return fail("%s: null argument", fn);
+  if (id_dtype != SWB_DTYPE_I32 && id_dtype != SWB_DTYPE_I64)
+    return fail("%s: id_dtype must be SWB_DTYPE_I32 or SWB_DTYPE_I64, got %d", fn, id_dtype);
+  if (reinterpret_cast<uintptr_t>(ids) % (id_dtype == SWB_DTYPE_I64 ? 8 : 4))
+    return fail("%s: ids are not aligned to their type", fn);
+  cudaPointerAttributes at;
+  if (cudaPointerGetAttributes(&at, ids) != cudaSuccess) {
+    cudaGetLastError();
+    return fail("%s: ids are not device memory", fn);
+  }
+  if ((at.type != cudaMemoryTypeDevice && at.type != cudaMemoryTypeManaged) || at.device != eng->device)
+    return fail("%s: ids must be device memory of device %d", fn, eng->device);
+  return 0;
+}
+
+// The IdCall of the next device-checked call; enqueues nothing but, once every 2^32 - 2 calls,
+// the reset of the claims and the failure word that lets the sequence number start over.
+static int begin_id_call(swb_engine *eng, int call, const void *a, const void *b, int dst_arg, int32_t n,
+                         cudaStream_t stream, IdCall *c) {
+  if (++eng->id_seq == 0xFFFFFFFFu) {
+    CUDA_TRY(cudaMemsetAsync(eng->d_id_claim, 0xFF, (size_t)eng->st.E * sizeof(unsigned long long), stream));
+    CUDA_TRY(cudaMemsetAsync(eng->d_id_fail, 0xFF, sizeof(unsigned long long), stream));
+    eng->id_seq = 1;
+  }
+  c->ids[0] = a;
+  c->ids[1] = b;
+  c->n = n;
+  c->dst_arg = dst_arg;
+  c->call = call;
+  c->hi = (unsigned long long)(~eng->id_seq) << 32;
+  c->claim = eng->d_id_claim;
+  c->fail = eng->d_id_fail;
+  c->status = eng->d_id_status;
+  return 0;
+}
+
+static unsigned grid_of(size_t threads) { return (unsigned)((threads + 255) / 256); }
+
+template <typename T>
+static int enqueue_save_dev(swb_engine *eng, const IdCall &c, void *dst, cudaStream_t stream) {
+  const size_t rb = RecordLayout(eng->st.S).bytes();
+  check_ids_kernel<T><<<grid_of(c.n), 256, 0, stream>>>(c, eng->st.E);
+  save_envs_dev_kernel<T><<<grid_of((size_t)c.n * eng->st.S), 256, 0, stream>>>(
+      eng->st, c, static_cast<unsigned char *>(dst), rb);
+  eng->launches += 2;
+  CUDA_TRY(cudaGetLastError());
+  return 0;
+}
+
+template <typename T>
+static int enqueue_load_dev(swb_engine *eng, const IdCall &c, const void *src, cudaStream_t stream) {
+  const size_t rb = RecordLayout(eng->st.S).bytes();
+  check_ids_kernel<T><<<grid_of(c.n), 256, 0, stream>>>(c, eng->st.E);
+  repeat_ids_kernel<T><<<grid_of(c.n), 256, 0, stream>>>(c, eng->st.E);
+  load_envs_dev_kernel<T><<<grid_of((size_t)c.n * eng->st.S), 256, 0, stream>>>(
+      eng->st, c, static_cast<const unsigned char *>(src), rb);
+  eng->launches += 3;
+  CUDA_TRY(cudaGetLastError());
+  return 0;
+}
+
+template <typename T>
+static int enqueue_copy_dev(swb_engine *eng, const IdCall &c, cudaStream_t stream) {
+  const size_t rb = RecordLayout(eng->st.S).bytes();
+  check_ids_kernel<T><<<grid_of(2 * (size_t)c.n), 256, 0, stream>>>(c, eng->st.E);
+  stage_copy_dev_kernel<T><<<grid_of((size_t)c.n * eng->st.S), 256, 0, stream>>>(eng->st, c, eng->d_records, rb);
+  load_envs_dev_kernel<T><<<grid_of((size_t)c.n * eng->st.S), 256, 0, stream>>>(eng->st, c, eng->d_records, rb);
+  eng->launches += 3;
+  CUDA_TRY(cudaGetLastError());
+  return 0;
+}
+
 extern "C" {
 
 int64_t swb_env_record_bytes(const swb_engine *eng) {
@@ -912,17 +1007,7 @@ int swb_copy_envs(swb_engine *eng, const int32_t *src_ids, const int32_t *dst_id
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   // an env both read and written: every source is saved to engine scratch before any destination
   // is written, so every read sees the state from before the call
-  const size_t need = overlap ? (size_t)n * RecordLayout(eng->st.S).bytes() : 0;
-  if (need > eng->records_bytes) {
-    if (eng->d_records) {
-      CUDA_TRY(cudaDeviceSynchronize());  // an earlier copy on any stream may still read it
-      cudaFree(eng->d_records);
-      eng->d_records = nullptr;
-      eng->records_bytes = 0;
-    }
-    CUDA_TRY(cudaMalloc(reinterpret_cast<void **>(&eng->d_records), need));
-    eng->records_bytes = need;
-  }
+  if (grow_records(eng, overlap ? (size_t)n * RecordLayout(eng->st.S).bytes() : 0)) return 1;
   IdSlot *slot = nullptr;
   if (stage_ids(eng, src_ids, dst_ids, n, stream, &slot)) return 1;
   if (!overlap) {
@@ -936,6 +1021,78 @@ int swb_copy_envs(swb_engine *eng, const int32_t *src_ids, const int32_t *dst_id
       launch_load(eng, slot->dev + n, n, eng->d_records, stream))
     return 1;
   return finish_ids(slot, stream);
+}
+
+int swb_save_envs_dev(swb_engine *eng, const void *env_ids, int32_t id_dtype, int32_t n, void *dst,
+                      uint64_t dst_bytes, int32_t *span_class, void *stream_) {
+  if (!eng || !span_class) return fail("swb_save_envs_dev: null argument");
+  if (n < 0) return fail("swb_save_envs_dev: n = %d", n);
+  if (n == 0) {
+    *span_class = eng->max_spans;
+    return 0;
+  }
+  if (!dst) return fail("swb_save_envs_dev: null argument");
+  if (check_dev_ids(eng, "swb_save_envs_dev", env_ids, id_dtype)) return 1;
+  if (reinterpret_cast<uintptr_t>(dst) % 16) return fail("swb_save_envs_dev: dst is not 16-byte aligned");
+  const uint64_t need = (uint64_t)n * RecordLayout(eng->st.S).bytes();
+  if (dst_bytes < need)
+    return fail("swb_save_envs_dev: %d records need %llu bytes, the buffer has %llu", n,
+                (unsigned long long)need, (unsigned long long)dst_bytes);
+  CUDA_TRY(cudaSetDevice(eng->device));
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  IdCall c;
+  if (begin_id_call(eng, SWB_IDS_CALL_SAVE, env_ids, nullptr, -1, n, stream, &c)) return 1;
+  if (id_dtype == SWB_DTYPE_I64 ? enqueue_save_dev<int64_t>(eng, c, dst, stream)
+                                : enqueue_save_dev<int32_t>(eng, c, dst, stream))
+    return 1;
+  *span_class = eng->max_spans;
+  return 0;
+}
+
+int swb_load_envs_dev(swb_engine *eng, const void *env_ids, int32_t id_dtype, int32_t n, const void *src,
+                      uint64_t src_bytes, int32_t span_class, void *stream_) {
+  if (!eng) return fail("swb_load_envs_dev: null engine");
+  if (n < 0) return fail("swb_load_envs_dev: n = %d", n);
+  if (span_class != 1 && span_class != 4)
+    return fail("swb_load_envs_dev: span_class must be 1 or 4, got %d", span_class);
+  if (n == 0) return 0;
+  if (!src) return fail("swb_load_envs_dev: null argument");
+  if (check_dev_ids(eng, "swb_load_envs_dev", env_ids, id_dtype)) return 1;
+  if (reinterpret_cast<uintptr_t>(src) % 16) return fail("swb_load_envs_dev: src is not 16-byte aligned");
+  const uint64_t need = (uint64_t)n * RecordLayout(eng->st.S).bytes();
+  if (src_bytes < need)
+    return fail("swb_load_envs_dev: %d records need %llu bytes, the buffer has %llu", n,
+                (unsigned long long)need, (unsigned long long)src_bytes);
+  CUDA_TRY(cudaSetDevice(eng->device));
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  eng->max_spans = std::max(eng->max_spans, (int)span_class);
+  IdCall c;
+  if (begin_id_call(eng, SWB_IDS_CALL_LOAD, env_ids, nullptr, 0, n, stream, &c)) return 1;
+  return id_dtype == SWB_DTYPE_I64 ? enqueue_load_dev<int64_t>(eng, c, src, stream)
+                                   : enqueue_load_dev<int32_t>(eng, c, src, stream);
+}
+
+int swb_copy_envs_dev(swb_engine *eng, const void *src_ids, const void *dst_ids, int32_t id_dtype, int32_t n,
+                      void *stream_) {
+  if (!eng) return fail("swb_copy_envs_dev: null engine");
+  if (n < 0) return fail("swb_copy_envs_dev: n = %d", n);
+  if (n == 0) return 0;
+  if (check_dev_ids(eng, "swb_copy_envs_dev", src_ids, id_dtype) ||
+      check_dev_ids(eng, "swb_copy_envs_dev", dst_ids, id_dtype))
+    return 1;
+  CUDA_TRY(cudaSetDevice(eng->device));
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (grow_records(eng, (size_t)n * RecordLayout(eng->st.S).bytes())) return 1;
+  IdCall c;
+  if (begin_id_call(eng, SWB_IDS_CALL_COPY, src_ids, dst_ids, 1, n, stream, &c)) return 1;
+  return id_dtype == SWB_DTYPE_I64 ? enqueue_copy_dev<int64_t>(eng, c, stream)
+                                   : enqueue_copy_dev<int32_t>(eng, c, stream);
+}
+
+int swb_env_ids_status_pointer(swb_engine *eng, swb_ids_status **status) {
+  if (!eng || !status) return fail("swb_env_ids_status_pointer: null argument");
+  *status = eng->d_id_status;
+  return 0;
 }
 
 #ifdef SWB_PHASE_CLOCKS

@@ -153,4 +153,123 @@ __global__ void copy_envs_kernel(DevState st, int n, const int32_t *__restrict__
   write_state(st, dst[r], s, read_state(st, src[r], s));
 }
 
+// Device-checked id lists (swb_save_envs_dev / swb_load_envs_dev / swb_copy_envs_dev).
+//
+// Every call k of an engine gets a sequence number seq (1 .. 2^32 - 2, so that hi = ~seq never
+// equals the all-ones initial value) and keys hi << 32 | low: a later call's keys are smaller.
+// Failing positions atomicMin the key hi | (position << 1 | argument) into one engine word, so
+// that word holds a key of call k exactly when call k failed, and then the lowest failing position
+// of it.  A destination id claims its env with atomicMin(claim[id], hi | position); after that
+// pass a destination whose claim is not its own key repeats an id at a lower position.  Neither
+// word needs clearing between calls: the next call's keys replace the last one's.
+struct IdCall {
+  const void *ids[2];          // id arguments 0 and 1 (copy: src, dst; else ids[1] is null)
+  int n;
+  int dst_arg;                 // the argument whose ids must be distinct, or -1 (save)
+  int call;                    // SWB_IDS_CALL_*
+  unsigned long long hi;       // ~seq << 32
+  unsigned long long *claim;   // [E]
+  unsigned long long *fail;    // [1]
+  swb_ids_status *status;
+};
+
+template <typename T>
+__device__ __forceinline__ bool id_in_range(T id, int E) {
+  return id >= 0 && id < static_cast<T>(E);   // in T's width: an int64 2^32 + 1 does not wrap
+}
+
+// Argument a's ids (a select, not an index: an indexed kernel parameter array goes to the stack)
+template <typename T>
+__device__ __forceinline__ const T *ids_of(const IdCall &c, int a) {
+  return static_cast<const T *>(a ? c.ids[1] : c.ids[0]);
+}
+
+__device__ __forceinline__ bool call_refused(const IdCall &c) {
+  return (*c.fail >> 32) == (c.hi >> 32);
+}
+
+// Thread 0 of a call's last kernel: the ok word, and the call's first failure if none is recorded.
+template <typename T>
+__device__ void report_ids(const IdCall &c, int E) {
+  const unsigned long long f = *c.fail;
+  const bool bad = (f >> 32) == (c.hi >> 32);
+  swb_ids_status *s = c.status;
+  s->ok = bad ? 0u : 1u;
+  if (!bad || s->failed) return;
+  const unsigned low = (unsigned)f;
+  const int a = (int)(low & 1u), p = (int)(low >> 1);
+  const T id = ids_of<T>(c, a)[p];
+  s->call = c.call;
+  s->arg = a;
+  s->reason = id_in_range(id, E) ? SWB_IDS_REPEATED : SWB_IDS_OUT_OF_RANGE;
+  s->position = p;
+  s->value = (int64_t)id;
+  s->failed = 1u;
+}
+
+// One thread per (argument, position): range check, and the claims of destination ids.
+template <typename T>
+__global__ void check_ids_kernel(IdCall c, int E) {
+  const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int n_args = c.ids[1] ? 2 : 1;
+  if (t >= (size_t)n_args * c.n) return;
+  const int a = (int)(t / c.n), p = (int)(t - (size_t)a * c.n);
+  const T id = ids_of<T>(c, a)[p];
+  if (!id_in_range(id, E))
+    atomicMin(c.fail, c.hi | ((unsigned long long)p << 1 | (unsigned)a));
+  else if (a == c.dst_arg)
+    atomicMin(c.claim + id, c.hi | (unsigned)p);
+}
+
+// After check_ids_kernel: a destination whose claim is another position's repeats an id.
+template <typename T>
+__device__ __forceinline__ void check_repeat(const IdCall &c, int E, int p) {
+  const T id = ids_of<T>(c, c.dst_arg)[p];
+  if (id_in_range(id, E) && c.claim[id] != (c.hi | (unsigned)p))
+    atomicMin(c.fail, c.hi | ((unsigned long long)p << 1 | (unsigned)c.dst_arg));
+}
+
+template <typename T>
+__global__ void repeat_ids_kernel(IdCall c, int E) {
+  const size_t p = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p < (size_t)c.n) check_repeat<T>(c, E, (int)p);
+}
+
+// record i <- env ids[i], or zeros in every record of a refused call
+template <typename T>
+__global__ void save_envs_dev_kernel(DevState st, IdCall c, unsigned char *__restrict__ rec,
+                                     size_t record_bytes) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i == 0) report_ids<T>(c, st.E);
+  if (i >= (size_t)c.n * st.S) return;
+  const int r = (int)(i / st.S), s = (int)(i - (size_t)r * st.S);
+  const int id = (int)ids_of<T>(c, 0)[r];
+  write_record(rec + (size_t)r * record_bytes, st.S, s, call_refused(c) ? SlotRecord{} : read_state(st, id, s));
+}
+
+// Copy, first half: the repeat check of the destinations, and record i <- env src[i] in engine
+// scratch for every source in range (the load below reads none of it if the call is refused).
+template <typename T>
+__global__ void stage_copy_dev_kernel(DevState st, IdCall c, unsigned char *__restrict__ rec,
+                                      size_t record_bytes) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (size_t)c.n * st.S) return;
+  const int r = (int)(i / st.S), s = (int)(i - (size_t)r * st.S);
+  if (s == 0) check_repeat<T>(c, st.E, r);
+  const T id = ids_of<T>(c, 0)[r];
+  if (id_in_range(id, st.E)) write_record(rec + (size_t)r * record_bytes, st.S, s, read_state(st, (int)id, s));
+}
+
+// env ids[dst_arg][i] <- record i, unless the call is refused
+template <typename T>
+__global__ void load_envs_dev_kernel(DevState st, IdCall c, const unsigned char *__restrict__ rec,
+                                     size_t record_bytes) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i == 0) report_ids<T>(c, st.E);
+  if (i >= (size_t)c.n * st.S || call_refused(c)) return;
+  const int r = (int)(i / st.S), s = (int)(i - (size_t)r * st.S);
+  const int id = (int)ids_of<T>(c, c.dst_arg)[r];
+  write_state(st, id, s, read_record(st, rec + (size_t)r * record_bytes, s));
+}
+
 }  // namespace swb

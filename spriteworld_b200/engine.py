@@ -404,8 +404,11 @@ class Engine(object):
     return out
 
   # -- env records ------------------------------------------------------------------
-  # Ids are lists, ndarrays or tensors; the library checks them on the host, so a CUDA tensor of
-  # ids costs a device-to-host copy (env_ids_array).  The work goes to the current stream.
+  # Ids are lists, ndarrays or tensors; with check='host' (the default) the library checks them on
+  # the host, so a CUDA tensor of ids costs a device-to-host copy (env_ids_array).  With
+  # check='device' the ids are an int32 or int64 tensor on this engine's device, checked by kernels
+  # without the host waiting for them: a refused call changes nothing, and check_env_ids() reports
+  # it.  The work goes to the current stream.
   @property
   def record_bytes(self):
     """Bytes of one env record (include/spriteworld_b200.h)."""
@@ -414,12 +417,20 @@ class Engine(object):
   def _all_or(self, env_ids):
     return np.arange(self.n_envs, dtype=np.int32) if env_ids is None else env_ids_array(env_ids)
 
-  def save_envs(self, env_ids=None):
-    """EnvStates of envs `env_ids` (default: all, in order), on this engine's device."""
-    ids = self._all_or(env_ids)
+  def save_envs(self, env_ids=None, check='host'):
+    """EnvStates of envs `env_ids` (default: all, in order), on this engine's device.  With
+    check='device', a save refused on the device returns zero records."""
     rb = self.record_bytes
-    data = torch.empty((len(ids), rb), dtype=torch.uint8, device=self.device)
     span = ctypes.c_int32()
+    if device_checked(check, env_ids):
+      ids, dt = self._dev_ids(env_ids, 'save_envs')
+      data = torch.empty((ids.numel(), rb), dtype=torch.uint8, device=self.device)
+      _native.check(self._lib.swb_save_envs_dev(self._h, ctypes.c_void_p(ids.data_ptr()), dt, ids.numel(),
+                                                ctypes.c_void_p(data.data_ptr()), data.numel(),
+                                                ctypes.byref(span), self._stream()))
+      return EnvStates(data, span.value, self.signature, self.n_slots)
+    ids = self._all_or(env_ids)
+    data = torch.empty((len(ids), rb), dtype=torch.uint8, device=self.device)
     _native.check(self._lib.swb_save_envs(self._h, _as_ptr(ids), len(ids), ctypes.c_void_p(data.data_ptr()),
                                           data.numel(), ctypes.byref(span), self._stream()))
     return EnvStates(data, span.value, self.signature, self.n_slots)
@@ -437,20 +448,76 @@ class Engine(object):
       raise ValueError('EnvStates must hold a contiguous, 16-byte aligned uint8 (%d, %d) tensor on '
                        '%s, got %s' % (n, self.record_bytes, self.device, _describe(d)))
 
-  def load_envs(self, states, env_ids=None):
+  def load_envs(self, states, env_ids=None, check='host'):
     """Env env_ids[i] <- record i of `states` (default ids: all envs, in order; distinct)."""
+    if device_checked(check, env_ids):
+      ids, dt = self._dev_ids(env_ids, 'load_envs')
+      self.check_states(states, ids.numel())
+      _native.check(self._lib.swb_load_envs_dev(self._h, ctypes.c_void_p(ids.data_ptr()), dt, ids.numel(),
+                                                ctypes.c_void_p(states.data.data_ptr()), states.data.numel(),
+                                                states.span_class, self._stream()))
+      return
     ids = self._all_or(env_ids)
     self.check_states(states, len(ids))
     _native.check(self._lib.swb_load_envs(self._h, _as_ptr(ids), len(ids),
                                           ctypes.c_void_p(states.data.data_ptr()), states.data.numel(),
                                           states.span_class, self._stream()))
 
-  def copy_envs(self, src_ids, dst_ids):
+  def copy_envs(self, src_ids, dst_ids, check='host'):
     """Env dst_ids[i] <- env src_ids[i]; every read sees the state from before the call."""
+    if device_checked(check, src_ids):
+      src, dt = self._dev_ids(src_ids, 'copy_envs')
+      dst, dt_dst = self._dev_ids(dst_ids, 'copy_envs')
+      if src.numel() != dst.numel():
+        raise ValueError('copy_envs: %d sources, %d destinations' % (src.numel(), dst.numel()))
+      if dt != dt_dst:    # one id type per call: widen the int32 side on the device
+        src, dst, dt = src.long(), dst.long(), _native.DTYPE_I64
+      _native.check(self._lib.swb_copy_envs_dev(self._h, ctypes.c_void_p(src.data_ptr()),
+                                                ctypes.c_void_p(dst.data_ptr()), dt, src.numel(),
+                                                self._stream()))
+      return
     src, dst = env_ids_array(src_ids), env_ids_array(dst_ids)
     if len(src) != len(dst):
       raise ValueError('copy_envs: %d sources, %d destinations' % (len(src), len(dst)))
     _native.check(self._lib.swb_copy_envs(self._h, _as_ptr(src), _as_ptr(dst), len(src), self._stream()))
+
+  def _dev_ids(self, ids, fn):
+    """(contiguous ids, swb id dtype) of a device-checked call.  Nothing here reads the ids or
+    waits for the device; a non-contiguous tensor is made contiguous on the device."""
+    if not (isinstance(ids, torch.Tensor) and ids.device == self.device and ids.dtype in _ID_DTYPES
+            and ids.dim() == 1):
+      raise ValueError("%s with check='device' takes one-dimensional int32 or int64 ids on %s, got %s"
+                       % (fn, self.device, _describe(ids)))
+    return ids.contiguous(), _ID_DTYPES[ids.dtype]
+
+  def env_ids_status(self):
+    """Zero-copy uint8 (32,) view of the engine's swb_ids_status record (include/spriteworld_b200.h)."""
+    if getattr(self, '_ids_status_view', None) is None:
+      p = ctypes.c_void_p()
+      _native.check(self._lib.swb_env_ids_status_pointer(self._h, ctypes.byref(p)))
+      self._ids_status_view = torch.as_tensor(_DevicePointer(p.value, (_IDS_STATUS.itemsize,), '|u1'),
+                                              device=self.device)
+    return self._ids_status_view
+
+  def env_ids_ok(self):
+    """0-dim bool device tensor: True if the last device-checked record call passed its id checks.
+    Read in stream order, it masks work that follows a call without waiting for it."""
+    return self.env_ids_status()[:4].view(torch.int32)[0] != 0
+
+  def check_env_ids(self):
+    """Raises ValueError naming the call, the argument, the position, the id and the reason if a
+    device-checked save_envs / load_envs / copy_envs has been refused since the last check (the
+    first such), and clears the record.  Synchronises."""
+    view = self.env_ids_status()
+    rec = view.cpu().numpy().view(_IDS_STATUS)[0]
+    if not rec['failed']:
+      return
+    view[4:].zero_()
+    fn = _IDS_CALLS[int(rec['call'])]
+    arg = ('src_ids', 'dst_ids')[int(rec['arg'])] if fn == 'copy_envs' else 'env_ids'
+    why = ('is out of range [0, %d)' % self.n_envs if rec['reason'] == _native.IDS_OUT_OF_RANGE
+           else 'repeats a destination at a lower position')
+    raise ValueError('%s: %s[%d] = %d %s' % (fn, arg, int(rec['position']), int(rec['value']), why))
 
   def launch_count(self):
     return int(self._lib.swb_launch_count(self._h))
@@ -497,6 +564,22 @@ def record_layout(n_slots):
     fields.append((name, off, dtype, shape))
     off += dtype.itemsize * int(np.prod(shape, dtype=np.int64))
   return fields, (off + 15) // 16 * 16
+
+
+_ID_DTYPES = {torch.int32: _native.DTYPE_I32, torch.int64: _native.DTYPE_I64}
+# swb_ids_status
+_IDS_STATUS = np.dtype([('ok', '<u4'), ('failed', '<u4'), ('call', '<i4'), ('arg', '<i4'), ('reason', '<i4'),
+                        ('position', '<i4'), ('value', '<i8')])
+_IDS_CALLS = {_native.IDS_CALL_SAVE: 'save_envs', _native.IDS_CALL_LOAD: 'load_envs',
+              _native.IDS_CALL_COPY: 'copy_envs'}
+
+
+def device_checked(check, env_ids):
+  """True for a record call that takes device ids checked on the device: check='device' with ids
+  given (env_ids=None, all envs, takes the host path).  ValueError for another `check`."""
+  if check not in ('host', 'device'):
+    raise ValueError("check must be 'host' or 'device', got %r" % (check,))
+  return check == 'device' and env_ids is not None
 
 
 _TORCH_DTYPES = {np.dtype('<f8'): torch.float64, np.dtype('<f4'): torch.float32,

@@ -603,27 +603,47 @@ class BatchedEnvironment(object):
   # scene on the next step, as reset() does, so every load or copy counts as a reset against the
   # ring's underflow guard (_risk): with loads before every step the ring is refilled more often
   # rather than an env running onto a ring slot that has not been refilled.
-  # Ids: lists, ndarrays or tensors (a CUDA tensor costs a device-to-host copy).
-  def save_envs(self, env_ids=None):
+  # Ids: lists, ndarrays or tensors (a CUDA tensor costs a device-to-host copy), or with
+  # check='device' int32 / int64 tensors on the engine's device, checked there without a wait
+  # (Engine.check_env_ids reports a refused call).  A device-checked load or copy counts as a
+  # reset whether or not the device refuses it.
+  def save_envs(self, env_ids=None, check='host'):
     """engine.EnvStates of envs `env_ids` (default: all, in order)."""
+    if engine_lib.device_checked(check, env_ids):
+      return self._engine.save_envs(env_ids, check='device')
     return self._engine.save_envs(env_ids)
 
-  def load_envs(self, states, env_ids=None):
+  def load_envs(self, states, env_ids=None, check='host'):
     """Env env_ids[i] <- record i of `states` (default ids: all envs, in order)."""
-    self._engine.load_envs(states, env_ids)
+    checked = engine_lib.device_checked(check, env_ids)
+    if checked:
+      self._engine.load_envs(states, env_ids, check='device')
+    else:
+      self._engine.load_envs(states, env_ids)
     self._resets += 1
     if getattr(self, '_pool_static', None) is not None:
       f = states.fields()
       static = torch.cat([f['shape'][..., None].float(), f['factors'].transpose(1, 2),
                           f['vx'][..., None].float(), f['vy'][..., None].float()], -1)
-      self._set_static(np.arange(self.n_envs) if env_ids is None else env_ids, static)
+      if checked:
+        self._set_static_checked(env_ids, static)
+      else:
+        self._set_static(np.arange(self.n_envs) if env_ids is None else env_ids, static)
 
-  def copy_envs(self, src_ids, dst_ids):
+  def copy_envs(self, src_ids, dst_ids, check='host'):
     """Env dst_ids[i] <- env src_ids[i]; every read sees the state from before the call."""
-    self._engine.copy_envs(src_ids, dst_ids)
+    checked = engine_lib.device_checked(check, src_ids)
+    if checked:
+      self._engine.copy_envs(src_ids, dst_ids, check='device')
+    else:
+      self._engine.copy_envs(src_ids, dst_ids)
     self._resets += 1
     if getattr(self, '_pool_static', None) is not None:
       cursor = self._engine.state_tensors()['cursor'].long()
+      if checked:
+        src = self._clamped(src_ids)
+        self._set_static_checked(dst_ids, self._pool_static[src, cursor[src]])
+        return
       src = self._device_ids(src_ids)
       self._set_static(dst_ids, self._pool_static[src, cursor[src]])
 
@@ -635,6 +655,19 @@ class BatchedEnvironment(object):
     e = self._device_ids(env_ids)
     cursor = self._engine.state_tensors()['cursor'].long()
     self._pool_static[e, cursor[e]] = static
+
+  def _clamped(self, ids):
+    """Device ids of a device-checked call as indices into [0, n_envs): unchecked ids must not
+    index a tensor (an out-of-range index is a device-side assert)."""
+    return ids.long().clamp(0, self.n_envs - 1)
+
+  def _set_static_checked(self, env_ids, static):
+    """_set_static after a device-checked call, without a wait: ids clamped, and the entries
+    written back as they were unless the call passed its checks, so a refused call changes
+    nothing (a refused call's repeated ids all write the same old value)."""
+    e = self._clamped(env_ids)
+    k = self._engine.state_tensors()['cursor'].long()[e]
+    self._pool_static[e, k] = torch.where(self._engine.env_ids_ok(), static, self._pool_static[e, k])
 
   def render(self):
     """Re-renders every PILRenderer observation of the current state (a loaded one, say) into

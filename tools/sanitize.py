@@ -13,6 +13,10 @@ frame to the bulk-copy engine while the next frame's set-up runs: what racecheck
 The last run renders 70-row frames (bands of 64 and 6 rows) for three times as many (env, band)
 items as there are resident render CTAs, so every CTA claims several items of unequal bands,
 some written out by the bulk copy and some by the per-byte loop, one after the other.
+
+Between those, device-checked env records: saves, loads and copies with int32 and int64 device
+ids, valid and refused (out of range either way, 2^32 + 1, repeated destinations), so that memcheck
+sees that a refused id never indexes engine memory.
 """
 import ctypes
 import os
@@ -49,7 +53,40 @@ def main():
     print('%s: %d envs, %d kernel launches' % (wl.name, E, eng.launch_count()), flush=True)
     raster.close()
     eng.close()
+  device_checked_records(torch)
   persistent_mixed(torch)
+
+
+def device_checked_records(torch):
+  from spriteworld_b200 import workloads
+  wl = workloads.WORKLOADS['c2']()
+  E = 40
+  eng, raster, _ = workloads.build_engine(wl, E, 4, device=0, seed=4, max_episode_length=3)
+  eng.step(torch.from_numpy(wl.sample_actions(np.random.RandomState(2), 1, E)[0]).cuda(), raster)
+  ids = torch.arange(E, device='cuda')
+  refused = 0
+  for dt in (torch.int32, torch.int64):
+    good = ids.flip(0).to(dt)
+    s = eng.save_envs(good, check='device')
+    eng.load_envs(s, ids.to(dt), check='device')
+    eng.copy_envs(good, torch.roll(ids, 3).to(dt), check='device')
+    for bad in ([-1, 3], [E, 3], [5, 5]) + (([2 ** 32 + 1, 3],) if dt == torch.int64 else ()):
+      b = torch.tensor(bad, device='cuda', dtype=dt)
+      for call in (lambda: eng.save_envs(b, check='device'), lambda: eng.load_envs(s[:2], b, check='device'),
+                   lambda: eng.copy_envs(b, ids[:2].to(dt), check='device'),
+                   lambda: eng.copy_envs(ids[:2].to(dt), b, check='device')):
+        call()
+        try:
+          eng.check_env_ids()
+        except ValueError:
+          refused += 1
+  torch.cuda.synchronize()
+  eng.check_env_ids()
+  assert refused == 24, refused   # every call but a save or a copy source with a repeat
+  print('device-checked records: %d envs, %d refused reports, %d kernel launches'
+        % (E, refused, eng.launch_count()), flush=True)
+  raster.close()
+  eng.close()
 
 
 def persistent_mixed(torch):

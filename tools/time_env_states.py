@@ -11,11 +11,19 @@ Per workload, each between CUDA events, warmed up and repeated for at least --se
                 engine scratch
   copy_half     copy_envs(first half, second half): disjoint sets, one kernel
   save_load     save_envs() then load_envs() of all envs
+  *_dev         the same three calls with check='device': int64 id tensors on the device,
+                checked there (a copy always goes through engine scratch: three kernels)
 The calls include their host work (id checks, pinned staging), as a user pays it; the events
 measure the stream, so a call that the host cannot enqueue as fast as the device runs it shows
 its host time.  GB/s counts the record bytes read and written on the device: 2 x records for a
-direct copy, 4 x for a copy through scratch and for a save plus a load.  Prints one JSON line
-per workload, headed by the card's name and power limit read in the same run.
+direct copy, 4 x for a copy through scratch and for a save plus a load.
+
+Then a branching loop, timed on the host clock and ending in a synchronise: per step one
+Engine.step with the render and a torch.multinomial resample of all envs (weights drawn on the
+device), copied into place with copy_envs.  `resample_host` passes the draw as host-checked ids,
+which copies it to the host and so waits for the step; `resample_dev` passes it with
+check='device'.  Both in env-steps/s.  Prints one JSON line per workload, headed by the card's
+name and power limit read in the same run.
 """
 import argparse
 import json
@@ -91,7 +99,54 @@ def run(key, seconds):
     out[name + '_us'] = us
     out[name + '_GBps'] = moved / us / 1e3
     out[name + '_share_of_step'] = us / step_us
+  dev = torch.arange(E, device=eng.device)
+  dev_shifted, dev_lo, dev_hi = torch.roll(dev, 1), dev[:half].clone(), dev[half:2 * half].clone()
+
+  def save_load_dev():
+    eng.load_envs(eng.save_envs(dev, check='device'), dev, check='device')
+
+  for name, fn, moved in (('copy_shift_dev', lambda: eng.copy_envs(dev, dev_shifted, check='device'), 4 * E * rb),
+                          ('copy_half_dev', lambda: eng.copy_envs(dev_lo, dev_hi, check='device'), 4 * half * rb),
+                          ('save_load_dev', save_load_dev, 4 * E * rb)):
+    us = _time(fn, seconds)
+    out[name + '_us'] = us
+    out[name + '_GBps'] = moved / us / 1e3
+    out[name + '_share_of_step'] = us / step_us
+  eng.check_env_ids()
+  gen = torch.Generator(device=eng.device)
+  gen.manual_seed(0)
+
+  def resample(check):
+    eng.step(acts[next(it) % len(acts)], raster, frames)
+    src = torch.multinomial(torch.rand(E, device=eng.device, generator=gen), E, replacement=True, generator=gen)
+    if check == 'device':
+      eng.copy_envs(src, dev, check='device')
+    else:
+      eng.copy_envs(src, np.arange(E))
+
+  for check in ('host', 'device'):
+    out['resample_%s_env_steps_per_s' % check] = E / _loop_seconds(lambda: resample(check), seconds)
+  eng.check_env_ids()
   return out
+
+
+def _loop_seconds(fn, seconds):
+  """Seconds per call of fn(), host clock around calls that end in a synchronise."""
+  import time
+  import torch
+  for _ in range(5):
+    fn()
+  torch.cuda.synchronize()
+  n = 10
+  while True:
+    t0 = time.perf_counter()
+    for _ in range(n):
+      fn()
+    torch.cuda.synchronize()
+    dt = time.perf_counter() - t0
+    if dt >= seconds:
+      return dt / n
+    n = max(2 * n, int(n * seconds / max(dt, 1e-6)) + 1)
 
 
 def main():
