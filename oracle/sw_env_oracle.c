@@ -272,7 +272,9 @@ SWO_API int swo_action_step(const swo_env_cfg *cfg, const swo_shape_table *tab, 
       my = (a[3] - a[1]) * cfg->action_scale;
     }
     px = a[0]; py = a[1];
-    norm = sqrt(mx * mx + my * my);
+    /* np.linalg.norm = sqrt(x.dot(x)); OpenBLAS ddot of two elements is fma(m1, m1, m0 * m0).
+     * This file builds with -ffp-contract=off, so the fusion is spelled out. */
+    norm = sqrt(fma(my, my, mx * mx));
   }
   for (int s = S - 1; s >= 0; s--) { /* :77-81 top-most first */
     if (!sp[s].shape) continue;

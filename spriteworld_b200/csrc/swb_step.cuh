@@ -456,7 +456,9 @@ step_kernel(DevState st, const StepCfg *__restrict__ step_cfg, const void *__res
           my = __dmul_rn(__dsub_rn(a[3], a[1]), c_step.action_scale);
         }
         px = a[0]; py = a[1];
-        norm = __dsqrt_rn(__dadd_rn(__dmul_rn(mx, mx), __dmul_rn(my, my)));
+        // np.linalg.norm of a float64 2-vector is sqrt(x.dot(x)), and OpenBLAS ddot fuses the
+        // second product into the first: fma(my, my, mx * mx) (DESIGN.md section 5)
+        norm = __dsqrt_rn(__fma_rn(my, my, __dmul_rn(mx, mx)));
       }
       for (int s = S - 1; s >= 0; s--) {  // :77-81 top-most first
         if (!ws.shape[s]) continue;

@@ -4,8 +4,9 @@ Each case of CASES builds seeded scenes and actions and runs T steps through Eng
 Engine.step_host.  After every step it compares with oracle.BatchOracle in its sqrt-distance
 mode (oracle.with_device_sqrt, the engine's FindGoalPosition distance): positions of the
 occupied slots, cursor, step_count, reset_next, scene_serial, step type, success, status and
-reward (NaN-aware).  Action-only cases also run through swb_apply_action (mode 2) and
-swb_eval_task (mode 1) the way _direct.py calls them.
+reward (positions and rewards NaN-aware).  Action-only cases also run through swb_apply_action (mode 2) and
+swb_eval_task (mode 1) the way _direct.py calls them.  Clicks are in [0, 1], or (case_actions)
+far outside it with a float64 motion cost, or carry NaN and +-inf components.
 
 A bad Embodied direction follows the reference's state after its KeyError
 (environment.py:93-95): the step is counted, nothing moves (no velocity update either), the
@@ -33,12 +34,13 @@ AGGS = ('sum', 'mean', 'max', 'min')
 
 def _case(name, S, E, action, dtype, T=12, K=2, nodes='goal', pos='f32', keep=True, mel=50,
           empty='front', vel=0.0, reset_mask=(), edge_pos=False, filter_sizes=(), direct=False,
-          expect=()):
-  """expect: events (see _count) the case must produce at least once, besides FIRST steps."""
+          expect=(), actions='unit', scale=None, motion_cost=None):
+  """expect: events (see _count) the case must produce at least once, besides FIRST steps.
+  actions: see case_actions.  scale, motion_cost: the action space's, instead of drawn ones."""
   return dict(name=name, S=S, E=E, action=action, dtype=dtype, T=T, K=K, nodes=nodes, pos=pos,
               keep=keep, mel=mel, empty=empty, vel=vel, reset_mask=tuple(reset_mask),
               edge_pos=edge_pos, filter_sizes=tuple(filter_sizes), direct=direct,
-              expect=tuple(expect))
+              expect=tuple(expect), actions=actions, scale=scale, motion_cost=motion_cost)
 
 
 CASES = [
@@ -71,6 +73,15 @@ CASES = [
           expect=('last', 'bad')),
     _case('reset_mask', 6, 41, 'select_move', 'f64', mel=5, K=3, T=14, vel=0.02,
           reset_mask=(3, 4, 9), expect=('last', 'reset_on_last', 'reset_mid')),
+    # clicks far outside [0, 1] and non-finite components, with a float64 motion cost
+    _case('wide_f64_cost', 9, 65, 'select_move', 'f64', pos='mixed', keep=False, actions='wide',
+          scale=3.0, motion_cost=0.7, direct=True, expect=('last',)),
+    _case('nonfinite_f32', 5, 65, 'drag_and_drop', 'f32', pos='mixed', keep=False,
+          actions='nonfinite', scale=3.0, motion_cost=0.7, direct=True, expect=('last',)),
+    _case('nonfinite_f64_s32', 32, 129, 'select_move', 'f64', pos='mixed', keep=False,
+          actions='nonfinite', scale=3.0, motion_cost=0.7, expect=('last',)),
+    _case('nonfinite_f64_keep', 5, 33, 'drag_and_drop', 'f64', pos='mixed', actions='nonfinite',
+          motion_cost=0.0),
 ]
 
 
@@ -186,7 +197,11 @@ def case_nodes(case, rng):
 
 def case_actions(case, arrs, rng, T):
   """(T, E, 4) float clicks -- half of them on a sprite of the env's first scene -- or (T, E, 2)
-  int32 Embodied actions with carry 0, 1, 2, -1 and, mid-episode, bad directions."""
+  int32 Embodied actions with carry 0, 1, 2, -1 and, mid-episode, bad directions.
+
+  case['actions'] of clicks: 'unit' in [0, 1]; 'wide' with every component in [-3, 4] (the
+  click position too, when it is not on a sprite); 'nonfinite' as 'unit', with NaN, +inf or
+  -inf in a random subset of the components of a third of the actions."""
   E = case['E']
   if case['action'] == 'embodied':
     a = np.zeros((T, E, 2), np.int32)
@@ -197,6 +212,8 @@ def case_actions(case, arrs, rng, T):
     a[..., 1][bad] = rng.choice([-1, 4, INT32_MIN], bad.sum())
     return a
   a = rng.uniform(0, 1, (T, E, 4))
+  if case['actions'] == 'wide':
+    a = rng.uniform(-3, 4, (T, E, 4))
   occ = arrs['shape'][:, 0] > 0
   for t in range(T):
     for e in range(E):
@@ -204,6 +221,11 @@ def case_actions(case, arrs, rng, T):
         s = rng.choice(np.nonzero(occ[e])[0])
         a[t, e, 0] = arrs['x'][e, 0, s] + rng.normal(0, 0.01)
         a[t, e, 1] = arrs['y'][e, 0, s] + rng.normal(0, 0.01)
+  if case['actions'] == 'nonfinite':
+    hit = rng.rand(T, E) < 1 / 3.
+    comp = rng.rand(T, E, 4) < 0.4
+    vals = np.array([np.nan, np.inf, -np.inf])[rng.randint(0, 3, (T, E, 4))]
+    a = np.where(hit[..., None] & comp, vals, a)
   return a.astype(np.float32 if case['dtype'] == 'f32' else np.float64)
 
 
@@ -280,6 +302,10 @@ def _setup(case):
                 motion_cost=float(rng.choice([0.0, 0.25])))
   if case['action'] == 'embodied':
     action['scale'] = 0.05
+  if case['scale'] is not None:
+    action['scale'] = case['scale']
+  if case['motion_cost'] is not None:
+    action['motion_cost'] = case['motion_cost']
   acts = case_actions(case, arrs, rng, case['T'])
   return arrs, nodes, action, acts
 
@@ -318,8 +344,8 @@ def test_step_matches_oracle(case, host):
     assert np.array_equal(st['step_count'], bo.step_count), where
     assert np.array_equal(st['reset_next'], bo.reset_next), where
     occ = bo.cur['shape'] > 0
-    assert np.array_equal(st['pos_x'][occ], bo.cur['x'][occ]), where
-    assert np.array_equal(st['pos_y'][occ], bo.cur['y'][occ]), where
+    assert np.array_equal(st['pos_x'][occ], bo.cur['x'][occ], equal_nan=True), where
+    assert np.array_equal(st['pos_y'][occ], bo.cur['y'][occ], equal_nan=True), where
     n_first += bo.step_type == oracle.STEP_FIRST
     assert np.array_equal(eng.download_state_serial() - serial0, n_first), where
     _count(seen, bo)
@@ -355,12 +381,13 @@ def test_apply_action_and_eval_task_match_oracle(case):
     for e in range(E):
       try:
         want_cost, _ = oracle.action_step(bo.cfg, bo.tab, cur[e], acts[t][e], case['dtype'] == 'f32')
-        assert status[e] == 0 and cost[e] == want_cost, (case['name'], t, e)
+        assert status[e] == 0 and np.array_equal(cost[e], want_cost, equal_nan=True), (
+            case['name'], t, e)
       except KeyError:
         assert status[e] == _native.ENV_BAD_ACTION and cost[e] == 0.0, (case['name'], t, e)
     occ = cur['shape'] > 0
-    assert np.array_equal(st['pos_x'][occ], cur['x'][occ]), (case['name'], t)
-    assert np.array_equal(st['pos_y'][occ], cur['y'][occ]), (case['name'], t)
+    assert np.array_equal(st['pos_x'][occ], cur['x'][occ], equal_nan=True), (case['name'], t)
+    assert np.array_equal(st['pos_y'][occ], cur['y'][occ], equal_nan=True), (case['name'], t)
     _native.check(eng._lib.swb_eval_task(eng._h, eng._out, eng._stream()))
     got_r, got_s, got_e = (a.cpu().numpy() for a in (eng._reward, eng._success, eng._status))
     for e in range(E):
@@ -567,6 +594,21 @@ def test_case_table_covers_the_step_paths():
   assert {-1, 4, INT32_MIN} <= set(np.unique(a[..., 1]).tolist())
   assert any(c['direct'] for c in CASES if c['action'] == 'embodied')
   assert {c['dtype'] for c in CASES if c['direct']} == {'f32', 'f64', 'i32'}
+  # a float64 cost with a nonzero motion cost (np.linalg.norm's fused dot), clicks outside
+  # [0, 1] and non-finite action components, with keep_in_frame off and on
+  f64_cost, nonfinite, wide = set(), set(), set()
+  for c in CASES:
+    if c['action'] == 'embodied':
+      continue
+    _, _, action, acts = _setup(c)
+    if c['dtype'] == 'f64' and action['motion_cost'] > 0:
+      f64_cost.add(c['name'])
+    if not np.isfinite(acts).all():
+      nonfinite.add((c['dtype'], c['keep']))
+    if ((acts < 0) | (acts > 1)).any() and action['motion_cost'] > 0 and action['scale'] > 1:
+      wide.add(c['dtype'])
+  assert f64_cost and 'f64' in wide
+  assert {('f32', False), ('f64', False), ('f64', True)} <= nonfinite
   # the events the step path must meet somewhere in the table, checked on the oracle
   expected = {e for c in CASES for e in c['expect']}
   assert expected >= {'bad', 'labels', 'zerodiv', 'last', 'success_and_oof', 'reset_on_last',
