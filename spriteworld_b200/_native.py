@@ -128,6 +128,11 @@ def load():
   L.swb_env_ids_status_pointer.argtypes = [vp, ctypes.POINTER(vp)]
   L.swb_launch_count.argtypes = [vp]
   L.swb_launch_count.restype = ctypes.c_int64
+  L.swb_sampler_load.argtypes = [vp, vp, ctypes.c_uint64, ctypes.c_int64]
+  L.swb_sample_scenes.argtypes = [vp, vp, vp, ci, vp, vp]
+  L.swb_refill_device.argtypes = [vp, vp, vp]
+  L.swb_pool_pointers.argtypes = [vp, vp] + [ctypes.POINTER(vp)] * 5
+  L.swb_sampler_pointers.argtypes = [vp, ctypes.POINTER(vp), ctypes.POINTER(vp)]
   if L.swb_sizeof_config() != ctypes.sizeof(Config):
     raise NativeError('ABI mismatch: swb_config is %d bytes in the library, %d in the binding'
                       % (L.swb_sizeof_config(), ctypes.sizeof(Config)))
@@ -144,7 +149,9 @@ EXPORTS = (
     'swb_step_render_gather', 'swb_ipc_alloc', 'swb_ipc_free', 'swb_ipc_open', 'swb_ipc_close', 'swb_peer_copy',
     'swb_step_host', 'swb_state_pointers', 'swb_scene_serial_pointer', 'swb_render_status_pointer', 'swb_download_state', 'swb_upload_state',
     'swb_env_record_bytes', 'swb_save_envs', 'swb_load_envs', 'swb_copy_envs', 'swb_save_envs_dev',
-    'swb_load_envs_dev', 'swb_copy_envs_dev', 'swb_env_ids_status_pointer', 'swb_launch_count')
+    'swb_load_envs_dev', 'swb_copy_envs_dev', 'swb_env_ids_status_pointer', 'swb_launch_count',
+    'swb_sampler_sizeof_program', 'swb_sampler_load', 'swb_sample_scenes', 'swb_refill_device',
+    'swb_sampler_pointers', 'swb_pool_pointers')
 
 
 def check(rc):

@@ -12,7 +12,7 @@ import sys
 CSRC = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'csrc')
 LIB = os.path.join(CSRC, 'libspriteworld_b200.so')
 SOURCES = ['swb_api.cu']
-HEADERS = ['swb_device.cuh', 'swb_render.cuh', 'swb_states.cuh', 'swb_step.cuh', 'swb_tables.h',
+HEADERS = ['swb_device.cuh', 'swb_render.cuh', 'swb_sampler.cuh', 'swb_states.cuh', 'swb_step.cuh', 'swb_tables.h',
            os.path.join('..', '..', 'include', 'spriteworld_b200.h')]
 
 NVCC_FLAGS = [
@@ -62,8 +62,34 @@ def build_host(force=False):
   return HOST_LIB
 
 
+SAMPLER_HOST_LIB = os.path.join(CSRC, 'libswb_sampler_host.so')
+SAMPLER_HOST_SRC = os.path.join(CSRC, 'swb_sampler_host.cpp')
+SAMPLER_HOST_INPUTS = [SAMPLER_HOST_SRC, os.path.join(CSRC, 'swb_sampler.cuh'),
+                       os.path.join(CSRC, '..', '..', 'include', 'spriteworld_b200.h')]
+# the same arithmetic as the kernels built with -fmad=false: no contraction
+SAMPLER_HOST_FLAGS = ['-O2', '-std=c++17', '-ffp-contract=off', '-fPIC', '-shared', '-Wall', '-Wextra']
+
+
+def build_sampler_host(force=False):
+  """libswb_sampler_host.so (g++): the device scene sampler built for the CPU
+  (scene_program.sample_on_host), the restatement the kernels are tested against."""
+  if not force and os.path.exists(SAMPLER_HOST_LIB) and os.path.getmtime(SAMPLER_HOST_LIB) >= max(
+      [os.path.getmtime(f) for f in SAMPLER_HOST_INPUTS] + [os.path.getmtime(os.path.abspath(__file__))]):
+    return SAMPLER_HOST_LIB
+  cxx = shutil.which('g++') or shutil.which('c++')
+  if not cxx:
+    raise RuntimeError('no C++ compiler for libswb_sampler_host.so')
+  proc = subprocess.run([cxx] + SAMPLER_HOST_FLAGS + ['-o', SAMPLER_HOST_LIB, SAMPLER_HOST_SRC],
+                        stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
+  if proc.returncode:
+    sys.stderr.write(proc.stdout)
+    raise RuntimeError('building libswb_sampler_host.so failed (%d)' % proc.returncode)
+  return SAMPLER_HOST_LIB
+
+
 def build(force=False, verbose=False):
   build_host(force)
+  build_sampler_host(force)
   if not force and not is_stale():
     return LIB
   cmd = [_nvcc()] + NVCC_FLAGS + (['-Xptxas', '-v'] if verbose else []) + ['-o', LIB] + SOURCES

@@ -1,6 +1,5 @@
 """Task-free exploration: 1-6 random sprites, no reward, 10-step episodes
 (reference: configs/cobra/exploration.py)."""
-import numpy as np
 
 from spriteworld_b200 import factor_distributions as distribs
 from spriteworld_b200 import sprite_generators as gen
@@ -19,5 +18,5 @@ def get_config(mode=None):
       distribs.Continuous('c1', 0.3, 1.),
       distribs.Continuous('c2', 0.9, 1.),
   ])
-  sprite_gen = gen.generate_sprites(factors, num_sprites=lambda: np.random.randint(1, 7))
+  sprite_gen = gen.generate_sprites(factors, num_sprites=gen.uniform_count(1, 7))
   return common.config(tasks.NoReward(), sprite_gen, 10, __file__, None)

@@ -2,8 +2,6 @@
 rotated stars and spokes (reference: configs/examples/goal_finding_clustering.py)."""
 import os
 
-import numpy as np
-
 from spriteworld_b200 import action_spaces
 from spriteworld_b200 import factor_distributions as distribs
 from spriteworld_b200 import renderers as sw_renderers
@@ -45,14 +43,14 @@ def get_config(mode='train'):
   for colors in goal_colors:
     factors = distribs.Product([pose, goal_scale, goal_shapes, colors])
     generators.append(gen.generate_sprites(factors,
-                                           num_sprites=lambda: np.random.randint(1, 3)))
+                                           num_sprites=gen.uniform_count(1, 3)))
 
   distractor = distribs.Product([
       pose, distribs.Discrete('shape', ['circle']), _int('c0', 64, 256, 'uint8'),
       _int('c1', 64, 256, 'uint8'), _int('c2', 64, 256, 'uint8'),
       distribs.Continuous('scale', 0.08, 0.12)])
   generators.append(gen.generate_sprites(distractor,
-                                         num_sprites=lambda: np.random.randint(0, 3)))
+                                         num_sprites=gen.uniform_count(0, 3)))
   sprite_gen = gen.shuffle(gen.chain_generators(*generators))
 
   subtasks = [tasks.Clustering(cluster_shapes, terminate_bonus=0., reward_range=10.)]

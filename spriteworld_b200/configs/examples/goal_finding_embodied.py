@@ -3,8 +3,6 @@ plus the agent's body (a small white circle) always in front
 (reference: configs/examples/goal_finding_embodied.py)."""
 import os
 
-import numpy as np
-
 from spriteworld_b200 import action_spaces
 from spriteworld_b200 import factor_distributions as distribs
 from spriteworld_b200 import renderers as sw_renderers
@@ -12,8 +10,8 @@ from spriteworld_b200 import sprite_generators as gen
 from spriteworld_b200 import tasks
 
 TERMINATE_DISTANCE = 0.075
-NUM_TARGETS = lambda: np.random.randint(1, 4)
-NUM_DISTRACTORS = lambda: np.random.randint(1, 4)
+NUM_TARGETS = gen.uniform_count(1, 4)
+NUM_DISTRACTORS = gen.uniform_count(1, 4)
 
 
 def get_config(mode=None):

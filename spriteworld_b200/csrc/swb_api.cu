@@ -9,6 +9,7 @@
 
 #include "swb_device.cuh"
 #include "swb_render.cuh"
+#include "swb_sampler.cuh"
 #include "swb_states.cuh"
 #include "swb_step.cuh"
 #include "swb_tables.h"
@@ -88,6 +89,12 @@ struct swb_engine {
   unsigned long long *d_id_claim = nullptr, *d_id_fail = nullptr;
   swb_ids_status *d_id_status = nullptr;
   uint32_t id_seq = 0;
+  // device scene sampler (swb_sampler_load): program, refill bookkeeping, first failure
+  swb_scene_program *d_prog = nullptr;
+  uint64_t seed = 0;
+  int64_t env_offset = 0;
+  int64_t *d_refilled_upto = nullptr;
+  swb_sampler_status *d_sampler_status = nullptr;
   std::vector<void *> owned;
   // buffers of swb_step_host
   void *h_actions = nullptr;
@@ -160,7 +167,7 @@ int upload_axis(swb_raster *r, const AxisHost &h, AxisTables *d) {
 extern "C" {
 
 const char *swb_last_error(void) { return g_error.c_str(); }
-int swb_version(void) { return 3; }
+int swb_version(void) { return 4; }
 int swb_sizeof_config(void) { return (int)sizeof(swb_config); }
 int swb_sizeof_task_node(void) { return (int)sizeof(swb_task_node); }
 
@@ -273,6 +280,7 @@ void swb_engine_destroy(swb_engine *eng) {
     if (slot.done) cudaEventDestroy(slot.done);
   }
   cudaFree(eng->d_records);
+  cudaFree(eng->d_prog); cudaFree(eng->d_refilled_upto); cudaFree(eng->d_sampler_status);
   cudaFree(eng->h_actions); cudaFree(eng->h_out.reward); cudaFree(eng->h_out.step_type);
   cudaFree(eng->h_out.success); cudaFree(eng->h_out.status); cudaFree(eng->h_frames);
   if (eng->copy_stream) cudaStreamDestroy(eng->copy_stream);
@@ -1092,6 +1100,205 @@ int swb_copy_envs_dev(swb_engine *eng, const void *src_ids, const void *dst_ids,
 int swb_env_ids_status_pointer(swb_engine *eng, swb_ids_status **status) {
   if (!eng || !status) return fail("swb_env_ids_status_pointer: null argument");
   *status = eng->d_id_status;
+  return 0;
+}
+
+}  // extern "C"
+
+namespace {
+
+// Records a rejection loop that ran out of tries, unless an earlier one is recorded.
+__device__ void sampler_fail(swb_sampler_status *st, int op, int64_t g, int64_t a) {
+  if (atomicCAS(&st->failed, 0u, 1u) == 0u) {
+    st->op = op;
+    st->env = g;
+    st->scene = a;
+  }
+}
+
+// swb_sample_scenes: one thread per requested scene.
+__global__ void sample_scenes_kernel(const swb_scene_program *__restrict__ prog, uint64_t seed, int S,
+                                     const int64_t *__restrict__ env_ids,
+                                     const int64_t *__restrict__ scene_idx, int n, swb_sample_out out,
+                                     swb_sampler_status *status) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int64_t g = env_ids[i], a = scene_idx[i];
+  swb_sampler::Scene sc;
+  const int bad = swb_sampler::sample_and_pack(
+      *prog, seed, (uint64_t)g, (uint64_t)a, S, sc,
+      [&](int slot, const swb_sampler::Packed &o, const swb_sampler::Sprite *s) {
+        const size_t d = (size_t)i * S + slot;
+        out.x[d] = o.x; out.y[d] = o.y;
+        out.m00[d] = o.m00; out.m01[d] = o.m01; out.m10[d] = o.m10; out.m11[d] = o.m11;
+        out.vx[d] = o.vx; out.vy[d] = o.vy;
+        out.member[d] = o.member; out.shape[d] = o.shape; out.pos_f32[d] = o.pos_f32;
+        for (int c = 0; c < 3; ++c) out.rgb[d * 3 + c] = o.rgb[c];
+        for (int f = 0; f < 5; ++f) out.factors[d * 5 + f] = o.factors[f];
+        for (int f = 0; f < swb_sampler::kFactors; ++f) {
+          out.factor_value[d * swb_sampler::kFactors + f] = s ? s->val[f] : 0.0;
+          out.factor_kind[d * swb_sampler::kFactors + f] = s ? s->kind[f] : (uint8_t)SWB_FT_NONE;
+        }
+      });
+  if (bad >= 0) sampler_fail(status, bad, g, a);
+}
+
+// swb_refill_device: one thread per env, scenes refilled_upto + 1 .. scene_serial + K - 1 into the
+// ring.  The scene the env is on (ring slot serial % K) is never among them.
+__global__ void refill_device_kernel(const swb_scene_program *__restrict__ prog, uint64_t seed,
+                                     int64_t env_offset, DevState st, int64_t *refilled_upto,
+                                     swb_sampler_status *status, float *static_rows) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= st.E) return;
+  const int64_t serial = st.scene_serial[e], want = serial + st.K - 1;
+  const int64_t g = env_offset + e;
+  // from the first scene not sampled yet, never below the one after the current scene (scene 0
+  // itself is sampled by the first refill after swb_sampler_load)
+  const int64_t lo = refilled_upto[e] < 0 ? serial : serial + 1;
+  int64_t a = refilled_upto[e] + 1;
+  if (a < lo) a = lo;
+  for (; a <= want; ++a) {
+    const size_t base = ((size_t)e * st.K + (size_t)(a % st.K)) * st.S;
+    swb_sampler::Scene sc;
+    const int bad = swb_sampler::sample_and_pack(
+        *prog, seed, (uint64_t)g, (uint64_t)a, st.S, sc,
+        [&](int slot, const swb_sampler::Packed &o, const swb_sampler::Sprite *) {
+          const size_t d = base + slot;
+          st.p_x[d] = o.x; st.p_y[d] = o.y;
+          st.p_m00[d] = o.m00; st.p_m01[d] = o.m01; st.p_m10[d] = o.m10; st.p_m11[d] = o.m11;
+          st.p_vx[d] = o.vx; st.p_vy[d] = o.vy;
+          st.p_member[d] = o.member; st.p_shape[d] = o.shape; st.p_pos_f32[d] = o.pos_f32;
+          st.p_rgb[d] = (uint32_t)o.rgb[0] | ((uint32_t)o.rgb[1] << 8) | ((uint32_t)o.rgb[2] << 16);
+          for (int f = 0; f < 5; ++f) st.p_factors[d * 5 + f] = o.factors[f];
+          if (static_rows) {   // shape, scale, angle, c0, c1, c2, vx, vy as float32
+            float *r = static_rows + d * 8;
+            r[0] = (float)o.shape;
+            for (int f = 0; f < 5; ++f) r[1 + f] = o.factors[f];
+            r[6] = (float)o.vx;
+            r[7] = (float)o.vy;
+          }
+        });
+    if (bad >= 0) sampler_fail(status, bad, g, a);
+  }
+  if (want > refilled_upto[e]) refilled_upto[e] = want;
+}
+
+// What the kernels rely on: every op, jump, constant and angle index inside the program.
+int check_program(const swb_scene_program &p, int S) {
+  if (p.n_ops < 1 || p.n_ops > SWB_PROG_MAX_OPS) return fail("program: n_ops %d out of range", p.n_ops);
+  if (p.n_consts < 0 || p.n_consts > SWB_PROG_MAX_CONSTS) return fail("program: n_consts out of range");
+  if (p.n_angles < 1 || p.n_angles > SWB_PROG_MAX_ANGLES) return fail("program: n_angles out of range");
+  if (p.n_filters < 0 || p.n_filters > SWB_MAX_FILTERS) return fail("program: n_filters out of range");
+  if (p.max_sprites < 0 || p.max_sprites > S)
+    return fail("program: scenes of up to %d sprites do not fit %d slots", p.max_sprites, S);
+  auto pc_ok = [&](int pc) { return pc >= 0 && pc < p.n_ops; };
+  auto consts_ok = [&](int off, int n) { return n >= 1 && off >= 0 && off + n <= p.n_consts; };
+  for (int f = 0; f < p.n_filters; ++f)
+    if (!pc_ok(p.filter_pc[f])) return fail("program: filter %d has no code", f);
+  for (int i = 0; i < p.n_ops; ++i) {
+    const swb_prog_op &o = p.ops[i];
+    const bool key_ok = o.key >= 0 && o.key < swb_sampler::kFactors;
+    bool ok = true;
+    switch (o.op) {
+      case SWB_OP_G_END: case SWB_OP_G_MARK: case SWB_OP_G_SHUFFLE: case SWB_OP_D_RET:
+      case SWB_OP_D_REJ_BEGIN: case SWB_OP_P_RET: case SWB_OP_P_NOT: break;
+      case SWB_OP_G_SPRITES: ok = pc_ok(o.a) && o.b >= 0 && (o.dtype == 0 || o.c > o.b); break;
+      case SWB_OP_G_CHOOSE: case SWB_OP_D_MIX: ok = consts_ok(o.c, o.b) && i + o.b < p.n_ops; break;
+      case SWB_OP_G_JUMP: case SWB_OP_D_JUMP: ok = pc_ok(o.a); break;
+      case SWB_OP_D_CONT: ok = key_ok; break;
+      case SWB_OP_D_DISC: ok = key_ok && consts_ok(o.a, o.b) && (o.c < 0 || consts_ok(o.c, o.b)); break;
+      case SWB_OP_D_REJ_END: ok = pc_ok(o.a); break;
+      case SWB_OP_P_CONT: ok = key_ok; break;
+      case SWB_OP_P_DISC: ok = key_ok && consts_ok(o.a, o.b); break;
+      case SWB_OP_P_AND: case SWB_OP_P_OR: ok = o.b >= 1 && o.b <= SWB_PROG_MAX_STACK; break;
+      default: ok = false;
+    }
+    if (!ok) return fail("program: op %d (code %d) is malformed", i, o.op);
+  }
+  return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int swb_sampler_sizeof_program(void) { return (int)sizeof(swb_scene_program); }
+
+int swb_sampler_load(swb_engine *eng, const swb_scene_program *prog, uint64_t seed, int64_t env_offset) {
+  if (!eng || !prog) return fail("swb_sampler_load: null argument");
+  if (env_offset < 0) return fail("swb_sampler_load: env_offset must be >= 0");
+  if (check_program(*prog, eng->st.S)) return 1;
+  CUDA_TRY(cudaSetDevice(eng->device));
+  if (!eng->d_prog) {  // all three or none: the other calls test d_prog alone
+    swb_scene_program *prog_d = nullptr;
+    int64_t *upto_d = nullptr;
+    swb_sampler_status *status_d = nullptr;
+    if (dev_alloc(&prog_d, 1) != cudaSuccess || dev_alloc(&upto_d, eng->st.E) != cudaSuccess ||
+        dev_alloc(&status_d, 1) != cudaSuccess) {
+      cudaFree(prog_d); cudaFree(upto_d); cudaFree(status_d);
+      return fail("swb_sampler_load: device allocation failed");
+    }
+    eng->d_prog = prog_d;
+    eng->d_refilled_upto = upto_d;
+    eng->d_sampler_status = status_d;
+  }
+  CUDA_TRY(cudaDeviceSynchronize());
+  CUDA_TRY(cudaMemcpy(eng->d_prog, prog, sizeof(swb_scene_program), cudaMemcpyHostToDevice));
+  CUDA_TRY(cudaMemset(eng->d_refilled_upto, 0xFF, (size_t)eng->st.E * sizeof(int64_t)));
+  eng->seed = seed;
+  eng->env_offset = env_offset;
+  return 0;
+}
+
+int swb_sample_scenes(swb_engine *eng, const int64_t *env_ids, const int64_t *scene_idx, int32_t n,
+                      const swb_sample_out *out, void *stream_) {
+  if (!eng || !out) return fail("swb_sample_scenes: null argument");
+  if (!eng->d_prog) return fail("swb_sample_scenes: no program (swb_sampler_load)");
+  if (n < 0) return fail("swb_sample_scenes: n < 0");
+  if (n == 0) return 0;
+  if (!env_ids || !scene_idx || !out->x || !out->y || !out->m00 || !out->m01 || !out->m10 || !out->m11 ||
+      !out->vx || !out->vy || !out->member || !out->shape || !out->pos_f32 || !out->rgb || !out->factors ||
+      !out->factor_value || !out->factor_kind)
+    return fail("swb_sample_scenes: every pointer must be set");
+  CUDA_TRY(cudaSetDevice(eng->device));
+  const int threads = 128;
+  sample_scenes_kernel<<<(n + threads - 1) / threads, threads, 0, static_cast<cudaStream_t>(stream_)>>>(
+      eng->d_prog, eng->seed, eng->st.S, env_ids, scene_idx, n, *out, eng->d_sampler_status);
+  eng->launches++;
+  CUDA_TRY(cudaGetLastError());
+  return 0;
+}
+
+int swb_refill_device(swb_engine *eng, float *static_rows, void *stream_) {
+  if (!eng) return fail("swb_refill_device: null engine");
+  if (!eng->d_prog) return fail("swb_refill_device: no program (swb_sampler_load)");
+  CUDA_TRY(cudaSetDevice(eng->device));
+  const int threads = 64;
+  refill_device_kernel<<<(eng->st.E + threads - 1) / threads, threads, 0, static_cast<cudaStream_t>(stream_)>>>(
+      eng->d_prog, eng->seed, eng->env_offset, eng->st, eng->d_refilled_upto, eng->d_sampler_status,
+      static_rows);
+  eng->launches++;
+  CUDA_TRY(cudaGetLastError());
+  return 0;
+}
+
+int swb_sampler_pointers(swb_engine *eng, int64_t **refilled_upto, swb_sampler_status **status) {
+  if (!eng) return fail("swb_sampler_pointers: null engine");
+  if (!eng->d_prog) return fail("swb_sampler_pointers: no program (swb_sampler_load)");
+  if (refilled_upto) *refilled_upto = eng->d_refilled_upto;
+  if (status) *status = eng->d_sampler_status;
+  return 0;
+}
+
+int swb_pool_pointers(swb_engine *eng, double **f64, uint32_t **member, uint8_t **shape, uint8_t **pos_f32,
+                      uint32_t **rgb, float **factors) {
+  if (!eng || !f64 || !member || !shape || !pos_f32 || !rgb || !factors)
+    return fail("swb_pool_pointers: null argument");
+  const DevState &st = eng->st;
+  double *p[8] = {st.p_x, st.p_y, st.p_m00, st.p_m01, st.p_m10, st.p_m11, st.p_vx, st.p_vy};
+  for (int i = 0; i < 8; ++i) f64[i] = p[i];
+  *member = st.p_member; *shape = st.p_shape; *pos_f32 = st.p_pos_f32; *rgb = st.p_rgb;
+  *factors = st.p_factors;
   return 0;
 }
 

@@ -519,6 +519,104 @@ class Engine(object):
            else 'repeats a destination at a lower position')
     raise ValueError('%s: %s[%d] = %d %s' % (fn, arg, int(rec['position']), int(rec['value']), why))
 
+  # -- device scene sampler ---------------------------------------------------------------
+  def load_sampler(self, program, seed, env_offset=0):
+    """Gives the engine a scene_program.SceneProgram and a seed; env e is global env
+    env_offset + e.  Synchronises; no scene is sampled until refill_device() or sample_scenes()."""
+    from spriteworld_b200 import scene_program
+    if self._lib.swb_sampler_sizeof_program() != ctypes.sizeof(scene_program.Program):
+      raise _native.NativeError('ABI mismatch: swb_scene_program')
+    _native.check(self._lib.swb_sampler_load(self._h, ctypes.byref(program.struct),
+                                             int(seed) & (2 ** 64 - 1), int(env_offset)))
+    self._program = program
+    self._refilled_view = self._sampler_status_view = None
+
+  def sample_scenes(self, env_ids, scene_idx):
+    """Scenes (env_ids[i], scene_idx[i]) (global env ids, absolute scene indices) as device
+    tensors: the fields of a scene batch shaped (n, S[, ...]) plus 'factor_value' float64 and
+    'factor_kind' uint8 (n, S, 10).  The pool is not touched."""
+    from spriteworld_b200 import scene_program
+    ids = torch.as_tensor(env_ids, dtype=torch.int64, device=self.device).contiguous()
+    idx = torch.as_tensor(scene_idx, dtype=torch.int64, device=self.device).contiguous()
+    if ids.dim() != 1 or ids.shape != idx.shape:
+      raise ValueError('env_ids and scene_idx must be one-dimensional and of one length')
+    n, S = ids.numel(), self.n_slots
+    f64 = dict(dtype=torch.float64, device=self.device)
+    out = {f: torch.zeros((n, S), **f64) for f in SCENE_FIELDS_F64}
+    out['member'] = torch.zeros((n, S), dtype=torch.int32, device=self.device)
+    for f in ('shape', 'pos_f32'):
+      out[f] = torch.zeros((n, S), dtype=torch.uint8, device=self.device)
+    out['rgb'] = torch.zeros((n, S, 3), dtype=torch.uint8, device=self.device)
+    out['factors'] = torch.zeros((n, S, 5), dtype=torch.float32, device=self.device)
+    out['factor_value'] = torch.zeros((n, S, 10), **f64)
+    out['factor_kind'] = torch.zeros((n, S, 10), dtype=torch.uint8, device=self.device)
+    st = scene_program.sample_out_struct(out, lambda t: t.data_ptr())
+    _native.check(self._lib.swb_sample_scenes(self._h, ctypes.c_void_p(ids.data_ptr()),
+                                              ctypes.c_void_p(idx.data_ptr()), n, ctypes.byref(st),
+                                              self._stream()))
+    return out
+
+  def refill_device(self, static_rows=None):
+    """Enqueues the device refill: every env's ring up to scene_serial + K - 1.  static_rows: an
+    optional float32 (E, K, S, 8) device tensor that gets the static factors of every slot written
+    (shape, scale, angle, c0, c1, c2, vx, vy)."""
+    ptr = None
+    if static_rows is not None:
+      E, K, S = self.n_envs, self.pool_depth, self.n_slots
+      if not (static_rows.dtype == torch.float32 and tuple(static_rows.shape) == (E, K, S, 8)
+              and static_rows.device == self.device and static_rows.is_contiguous()):
+        raise ValueError('static_rows must be a contiguous float32 (%d, %d, %d, 8) tensor on %s'
+                         % (E, K, S, self.device))
+      ptr = ctypes.c_void_p(static_rows.data_ptr())
+    _native.check(self._lib.swb_refill_device(self._h, ptr, self._stream()))
+
+  def pool_tensors(self):
+    """Zero-copy views of the scene pool, shaped (E, K, S[, ...]): x .. vy float64, member int32,
+    shape and pos_f32 uint8, rgb uint8 (E, K, S, 4) (r, g, b, 0), factors float32 (E, K, S, 5)."""
+    vp = ctypes.c_void_p
+    f64 = (vp * 8)()
+    ptrs = [vp() for _ in range(5)]
+    _native.check(self._lib.swb_pool_pointers(self._h, f64, *[ctypes.byref(p) for p in ptrs]))
+    E, K, S = self.n_envs, self.pool_depth, self.n_slots
+
+    def view(p, typestr, tail=()):
+      return torch.as_tensor(_DevicePointer(p, (E, K, S) + tail, typestr), device=self.device)
+
+    out = {f: view(f64[i], '<f8') for i, f in enumerate(SCENE_FIELDS_F64)}
+    out['member'] = view(ptrs[0].value, '<i4')
+    out['shape'] = view(ptrs[1].value, '|u1')
+    out['pos_f32'] = view(ptrs[2].value, '|u1')
+    out['rgb'] = view(ptrs[3].value, '|u1', (4,))
+    out['factors'] = view(ptrs[4].value, '<f4', (5,))
+    return out
+
+  def _sampler_views(self):
+    if getattr(self, '_refilled_view', None) is None:
+      p, q = ctypes.c_void_p(), ctypes.c_void_p()
+      _native.check(self._lib.swb_sampler_pointers(self._h, ctypes.byref(p), ctypes.byref(q)))
+      self._refilled_view = torch.as_tensor(_DevicePointer(p.value, (self.n_envs,), '<i8'),
+                                            device=self.device)
+      self._sampler_status_view = torch.as_tensor(_DevicePointer(q.value, (3,), '<i8'),
+                                                  device=self.device)
+    return self._refilled_view, self._sampler_status_view
+
+  def refilled_upto(self):
+    """Zero-copy int64 (E,) view: the newest scene each env's ring holds (-1: none yet)."""
+    return self._sampler_views()[0]
+
+  def check_sampler(self):
+    """Raises the reference's ValueError if a rejection loop of the device sampler ran out of
+    tries since the last check (the first such; its scene was left empty), and clears the record.
+    Synchronises."""
+    view = self._sampler_views()[1]
+    rec = view.cpu().numpy()
+    if not rec[0] & 0xFFFFFFFF:
+      return
+    view.zero_()
+    op = int(rec[0] >> 32)
+    err = self._program.error(op)
+    raise ValueError('%s (env %d, scene %d)' % (err.args[0], int(rec[1]), int(rec[2])))
+
   def launch_count(self):
     return int(self._lib.swb_launch_count(self._h))
 

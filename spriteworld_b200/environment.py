@@ -271,7 +271,8 @@ class BatchedEnvironment(object):
 
   def __init__(self, task, action_space, renderers, init_sprites, keep_in_frame=True,
                max_episode_length=1000, metadata=None, n_envs=1, n_slots=None, pool_depth=8,
-               device=0, rng=None, refill=None, refill_threads=1, refill_procs=0):
+               device=0, rng=None, refill=None, refill_threads=1, refill_procs=0, sampler='host',
+               seed=None, env_offset=0):
     """Args beyond the reference's Environment:
       n_envs: environments advanced in lockstep.
       n_slots: sprite slots per env; default: the generator's own bound (`max_sprites`), or,
@@ -285,6 +286,14 @@ class BatchedEnvironment(object):
         (_sampler_pool; NumPy sampling is GIL-bound, threads do not scale it).  0 (default): the
         refill thread samples block after block.  Opt-in: next to a stepping process the
         workers have been seen running one after the other (DESIGN.md section 4).
+      sampler: 'host' (default: scenes drawn by init_sprites' NumPy sampler, as the reference
+        draws them for a given seed) or 'device': init_sprites compiled to a program
+        (scene_program.compile_program) that the GPU runs.  Scene a of env e is then a pure
+        function of (seed, env_offset + e, a): the same distribution as the host's, drawn from
+        its own stream, independent of timing; refills are kernels on the step stream, with no
+        host thread.  `refill`, `refill_threads` and `refill_procs` do not apply.
+      seed: the device sampler's seed (default: drawn from `rng`).
+      env_offset: the global id of env 0 for the device sampler (a shard's first env).
     """
     self._task, self._action_space = task, action_space
     self._renderers = renderers
@@ -302,6 +311,12 @@ class BatchedEnvironment(object):
     task._filters_static()
     self._K = max(3, int(pool_depth))
     E, K = self.n_envs, self._K
+    if sampler not in ('host', 'device'):
+      raise ValueError("sampler must be 'host' or 'device'")
+    self._sampler = sampler
+    if sampler == 'device':
+      self._init_device_sampler(n_slots, keep_in_frame, max_episode_length, device, seed, env_offset)
+      return
     first = self._sample(E * K)
     slots = n_slots or getattr(init_sprites, 'max_sprites', None)
     if not slots:
@@ -367,6 +382,40 @@ class BatchedEnvironment(object):
         from spriteworld_b200 import _sampler_pool
         self._pool = _sampler_pool.SamplerPool(min(int(refill_procs), n_thr), init_sprites, slots,
                                                self._filters, self._color_to_rgb)
+
+  def _init_device_sampler(self, n_slots, keep_in_frame, max_episode_length, device, seed, env_offset):
+    from spriteworld_b200 import scene_program
+    self._program = scene_program.compile_program(self._init_sprites, self._filters, self._color_to_rgb)
+    E, K = self.n_envs, self._K
+    slots = max(1, int(n_slots or self._program.max_sprites))
+    self._engine = engine_lib.Engine(
+        E, slots, K, self._action_space.compile(), self._nodes, constants.SHAPES,
+        keep_in_frame=keep_in_frame, max_episode_length=max_episode_length, device=device)
+    self._rasters = collections.OrderedDict(
+        (name, engine_lib.Raster(self._engine, r.width, r.height, r.anti_aliasing, r.bg_color))
+        for name, r in self._pil.items())
+    self._frames = {name: r.new_frames() for name, r in self._rasters.items()}
+    self.seed = int(self._rng.randint(0, 2 ** 31 - 1)) if seed is None else int(seed)
+    self._engine.load_sampler(self._program, self.seed, env_offset)
+    if self._other:   # static factors of the pooled scenes, written by every refill
+      self._pool_static = torch.zeros((E, K, slots, 8), dtype=torch.float32, device=self._engine.device)
+    # every ring gets scenes 0 .. K-1; env e starts on its scene 0 and is about to reset
+    self._engine.refill_device(getattr(self, '_pool_static', None))
+    first = self._engine.sample_scenes(np.arange(E) + int(env_offset), np.zeros(E))
+    self._engine.upload_state(pos_x=first['x'].cpu().numpy(), pos_y=first['y'].cpu().numpy(),
+                              cursor=np.zeros(E), step_count=np.zeros(E), reset_next=np.ones(E))
+    self._refill_mode = 'device'
+    self._t, self._resets = 0, 0
+    self._safe_step, self._safe_resets = 0, 0
+    # a launch is stream-ordered before the next step: it covers everything up to that step
+    self._period = max(1, 2 * (K - 2))
+    self._worker = None
+    self._stats = dict(refills=0)
+
+  def check_sampler(self):
+    """sampler='device': raises the reference's ValueError if a rejection loop ran out of tries
+    (that scene was left empty) since the last check.  Synchronises."""
+    self._engine.check_sampler()
 
   # -- scenes ----------------------------------------------------------------------------
   def _sample(self, n):
@@ -518,6 +567,12 @@ class BatchedEnvironment(object):
   def _keep_ring_fresh(self):
     """Called before a step is enqueued."""
     K = self._K
+    if self._refill_mode == 'device':
+      if self._t - self._safe_step >= self._period or self._risk(self._t + 1) > K - 1:
+        self._engine.refill_device(getattr(self, '_pool_static', None))
+        self._stats['refills'] += 1
+        self._safe_step, self._safe_resets = self._t, self._resets
+      return
     if self._refill_mode == 'sync':
       if self._t - self._safe_step >= self._period or self._risk(self._t + 1) > K - 1:
         import time
@@ -541,6 +596,8 @@ class BatchedEnvironment(object):
   def refill_stats(self):
     """Counters of the scene-ring refill: refills, scenes sampled, host seconds spent sampling
     and packing, and how often / how long a step had to wait for scenes."""
+    if self._refill_mode == 'device':
+      return dict(mode='device', launches=self._stats['refills'], pool_depth=self._K, seed=self.seed)
     return dict(self._stats, mode=self._refill_mode, pool_depth=self._K,
                 threads=len(getattr(self, '_block_rngs', [None])),
                 procs=len(self._pool) if getattr(self, '_pool', None) is not None else 0)
@@ -742,6 +799,12 @@ class ShardedBatchedEnvironment(object):
     if device is None:
       device = torch.cuda.current_device()
     self.host_barrier = host_barrier
+    if config.get('sampler', 'host') == 'device':
+      # scenes are functions of (seed, global env id): every rank takes the common seed and the
+      # global id of its first env, so the run draws what a one-GPU run over all envs draws
+      config = dict(config, env_offset=self.env_start)
+      if config.get('seed') is None:
+        config['seed'] = int(seed)
     # every rank draws its own scenes: same seed, rank-specific stream
     self.local = BatchedEnvironment(n_envs=self.n_local, device=device,
                                     rng=np.random.RandomState((int(seed) + 7919 * self.rank) % (2 ** 31)),

@@ -92,9 +92,10 @@ class SpriteGenerator(object):
   `max_sprites` is an upper bound of the sprites in one scene, or None when a count is drawn
   by a user callable (the batched environment sizes its sprite slots from it)."""
 
-  def __init__(self, one, many, max_sprites=None):
+  def __init__(self, one, many, max_sprites=None, spec=None):
     self._one, self._many = one, many
     self.max_sprites = max_sprites
+    self._spec = spec   # what scene_program.compile_program flattens for the device sampler
 
   def __call__(self):
     return self._one()
@@ -130,6 +131,22 @@ def _column(values):
   return _as_column(values)
 
 
+class uniform_count(object):
+  """A sprite count drawn as np.random.randint(lo, hi): picklable, and compilable for the device
+  sampler (a lambda count runs on the host only)."""
+
+  def __init__(self, lo, hi):
+    self.lo, self.hi = int(lo), int(hi)
+    if self.hi <= self.lo:
+      raise ValueError('uniform_count needs lo < hi, got (%d, %d)' % (self.lo, self.hi))
+
+  def __call__(self):
+    return np.random.randint(self.lo, self.hi)
+
+  def __repr__(self):
+    return 'uniform_count(%d, %d)' % (self.lo, self.hi)
+
+
 def generate_sprites(factor_dist, num_sprites=1):
   """`num_sprites` (int or callable returning int) sprites drawn i.i.d. from `factor_dist`."""
 
@@ -155,7 +172,8 @@ def generate_sprites(factor_dist, num_sprites=1):
     ref_row = np.where(np.arange(width)[None, :] < count[:, None], ref_row, 0)
     return SceneLayout([SpriteTable(cols, total)], count, np.zeros_like(ref_row), ref_row)
 
-  return SpriteGenerator(one, many, None if callable(num_sprites) else int(num_sprites))
+  return SpriteGenerator(one, many, None if callable(num_sprites) else int(num_sprites),
+                         spec=('sprites', factor_dist, num_sprites))
 
 
 def _bounds(generators):
@@ -178,7 +196,8 @@ def chain_generators(*sprite_generators):
     return layout
 
   bounds = _bounds(sprite_generators)
-  return SpriteGenerator(one, many, None if None in bounds else sum(bounds))
+  return SpriteGenerator(one, many, None if None in bounds else sum(bounds),
+                         spec=('chain', sprite_generators))
 
 
 def sample_generator(sprite_generators, p=None):
@@ -198,7 +217,8 @@ def sample_generator(sprite_generators, p=None):
     return _stack_scenes(parts, where, n)
 
   bounds = _bounds(sprite_generators)
-  return SpriteGenerator(one, many, None if None in bounds else max(bounds))
+  return SpriteGenerator(one, many, None if None in bounds else max(bounds),
+                         spec=('sample', sprite_generators, p))
 
 
 def shuffle(sprite_generator):
@@ -219,4 +239,5 @@ def shuffle(sprite_generator):
     return SceneLayout(layout.tables, layout.count, layout.ref_table[rows, order],
                        layout.ref_row[rows, order])
 
-  return SpriteGenerator(one, many, getattr(sprite_generator, 'max_sprites', None))
+  return SpriteGenerator(one, many, getattr(sprite_generator, 'max_sprites', None),
+                         spec=('shuffle', sprite_generator))
