@@ -46,24 +46,18 @@ cudaError_t dev_alloc(T **p, size_t n) {
 
 }  // namespace
 
-// One staging slot of swb_upload_scenes: a pinned host block and its device twin, laid out
-// [8 x f64][member u32][rgb u32][factors 5 x f32][dst i32][shape u8][pos_f32 u8] for `cap`
-// scenes, moved with ONE cudaMemcpyAsync and scattered into the pool by one kernel.
-struct UploadSlot {
-  size_t cap = 0;          // scenes
+// A pinned host block and its device twin, grown on demand.  Two alternate (Staging::slots), so
+// the host fills call i+1 while call i's copy is queued; a slot is reused only after its event.
+struct StagingSlot {
   size_t bytes = 0;
   unsigned char *host = nullptr, *dev = nullptr;
-  cudaEvent_t done = nullptr;  // recorded after the scatter kernel that reads `dev`
+  cudaEvent_t done = nullptr;  // recorded after the kernels that read `dev`
   bool in_flight = false;
 };
 
-// Pinned staging of the env ids of swb_save_envs / swb_load_envs / swb_copy_envs and its device
-// twin, `cap` int32 each; two alternate, so the host stages call i+1 while call i's copy is queued.
-struct IdSlot {
-  size_t cap = 0;
-  int32_t *host = nullptr, *dev = nullptr;
-  cudaEvent_t done = nullptr;  // recorded after the kernels that read `dev`
-  bool in_flight = false;
+struct Staging {
+  StagingSlot slots[2];
+  int next = 0;
 };
 
 struct swb_engine {
@@ -77,12 +71,10 @@ struct swb_engine {
   int device = 0;
   int max_spans = 1;  // 1 while every uploaded shape is convex, else 4
   int64_t launches = 0;
-  // staging for scene uploads (pinned host + device), grown on demand, double-buffered
-  UploadSlot upload_slots[2];
-  int upload_next = 0;
-  // env records: id staging, and the records of an overlapping swb_copy_envs (grown on demand)
-  IdSlot id_slots[2];
-  int id_next = 0;
+  // scene uploads (from the refill thread, on its stream) and the ids of host-checked record
+  // calls (on the step stream) stage apart, so that neither waits for or overwrites the other
+  Staging upload_staging, id_staging;
+  // the records of a copy through engine scratch (grown on demand)
   unsigned char *d_records = nullptr;
   size_t records_bytes = 0;
   // device-checked id lists (IdCall in swb_states.cuh): claims, the failure word, the status record
@@ -267,18 +259,13 @@ void swb_engine_destroy(swb_engine *eng) {
   if (!eng) return;
   cudaSetDevice(eng->device);
   for (void *p : eng->owned) cudaFree(p);
-  for (auto &slot : eng->upload_slots) {
-    if (slot.in_flight) cudaEventSynchronize(slot.done);
-    if (slot.host) cudaFreeHost(slot.host);
-    if (slot.dev) cudaFree(slot.dev);
-    if (slot.done) cudaEventDestroy(slot.done);
-  }
-  for (auto &slot : eng->id_slots) {
-    if (slot.in_flight) cudaEventSynchronize(slot.done);
-    if (slot.host) cudaFreeHost(slot.host);
-    if (slot.dev) cudaFree(slot.dev);
-    if (slot.done) cudaEventDestroy(slot.done);
-  }
+  for (Staging *staging : {&eng->upload_staging, &eng->id_staging})
+    for (StagingSlot &slot : staging->slots) {
+      if (slot.in_flight) cudaEventSynchronize(slot.done);
+      if (slot.host) cudaFreeHost(slot.host);
+      if (slot.dev) cudaFree(slot.dev);
+      if (slot.done) cudaEventDestroy(slot.done);
+    }
   cudaFree(eng->d_records);
   cudaFree(eng->d_prog); cudaFree(eng->d_refilled_upto); cudaFree(eng->d_sampler_status);
   cudaFree(eng->h_actions); cudaFree(eng->h_out.reward); cudaFree(eng->h_out.step_type);
@@ -289,17 +276,50 @@ void swb_engine_destroy(swb_engine *eng) {
   delete eng;
 }
 
-static size_t upload_layout(size_t cap, int S, size_t off[7]) {
-  const size_t capS = cap * S;
+// The next slot of `staging`, of at least `need` bytes, once the kernels that last read it have
+// finished.  The caller enqueues the copy to `dev` and the kernels that read it, then release_slot.
+static int take_slot(Staging &staging, size_t need, StagingSlot **out) {
+  StagingSlot &slot = staging.slots[staging.next];
+  staging.next ^= 1;
+  if (slot.in_flight) {
+    CUDA_TRY(cudaEventSynchronize(slot.done));
+    slot.in_flight = false;
+  }
+  if (need > slot.bytes) {
+    if (slot.host) cudaFreeHost(slot.host);
+    if (slot.dev) cudaFree(slot.dev);
+    slot.host = slot.dev = nullptr;
+    slot.bytes = 0;
+    const size_t bytes = std::max<size_t>(need, 4096);
+    CUDA_TRY(cudaMallocHost(reinterpret_cast<void **>(&slot.host), bytes));
+    CUDA_TRY(cudaMalloc(reinterpret_cast<void **>(&slot.dev), bytes));
+    if (!slot.done) CUDA_TRY(cudaEventCreateWithFlags(&slot.done, cudaEventDisableTiming));
+    slot.bytes = bytes;
+  }
+  *out = &slot;
+  return 0;
+}
+
+static int release_slot(StagingSlot *slot, cudaStream_t stream) {
+  CUDA_TRY(cudaEventRecord(slot->done, stream));
+  slot->in_flight = true;
+  return 0;
+}
+
+// An upload of n scenes in its staging slot: [8 x f64][member u32][rgb u32][factors 5 x f32]
+// [dst i32][shape u8][pos_f32 u8], each array 256-byte aligned, moved with ONE cudaMemcpyAsync and
+// scattered into the pool by one kernel.
+static size_t upload_layout(size_t n, int S, size_t off[7]) {
+  const size_t nS = n * S;
   size_t o = 0;
   auto take = [&](size_t bytes) { size_t r = o; o += (bytes + 255) & ~(size_t)255; return r; };
-  off[0] = take(capS * 8 * sizeof(double));   // f64 x 8
-  off[1] = take(capS * sizeof(uint32_t));     // member
-  off[2] = take(capS * sizeof(uint32_t));     // rgb
-  off[3] = take(capS * 5 * sizeof(float));    // factors
-  off[4] = take(cap * sizeof(int32_t));       // dst
-  off[5] = take(capS);                        // shape
-  off[6] = take(capS);                        // pos_f32
+  off[0] = take(nS * 8 * sizeof(double));   // f64 x 8
+  off[1] = take(nS * sizeof(uint32_t));     // member
+  off[2] = take(nS * sizeof(uint32_t));     // rgb
+  off[3] = take(nS * 5 * sizeof(float));    // factors
+  off[4] = take(n * sizeof(int32_t));       // dst
+  off[5] = take(nS);                        // shape
+  off[6] = take(nS);                        // pos_f32
   return o;
 }
 
@@ -325,34 +345,12 @@ int swb_upload_scenes(swb_engine *eng, const swb_scene_soa *sc, const int32_t *e
     if (sh > 6) eng->max_spans = 4;  // stars / spokes: several spans per canvas row
     if (sh && eng->cfg.shape_n_verts[sh] < 3) return fail("shape %d has no vertex table", sh);
   }
-  // two staging slots alternate, so the host packs upload i+1 while upload i is in flight; a
-  // slot is reused only after the scatter kernel that read it has finished (its event)
-  UploadSlot &slot = eng->upload_slots[eng->upload_next];
-  eng->upload_next ^= 1;
-  if (slot.in_flight) {
-    CUDA_TRY(cudaEventSynchronize(slot.done));
-    slot.in_flight = false;
-  }
-  if ((size_t)n > slot.cap) {
-    if (slot.host) cudaFreeHost(slot.host);
-    if (slot.dev) cudaFree(slot.dev);
-    slot.host = slot.dev = nullptr;
-    slot.cap = 0;
-    size_t off[7];
-    const size_t cap = std::max<size_t>((size_t)n, 256);
-    const size_t bytes = upload_layout(cap, S, off);
-    CUDA_TRY(cudaMallocHost(reinterpret_cast<void **>(&slot.host), bytes));
-    CUDA_TRY(cudaMalloc(reinterpret_cast<void **>(&slot.dev), bytes));
-    if (!slot.done) CUDA_TRY(cudaEventCreateWithFlags(&slot.done, cudaEventDisableTiming));
-    slot.cap = cap;
-    slot.bytes = bytes;
-  }
   size_t off[7];
-  upload_layout(slot.cap, S, off);
-  const size_t stride = slot.cap * S;
-  unsigned char *h = slot.host;
+  StagingSlot *slot = nullptr;
+  if (take_slot(eng->upload_staging, upload_layout(n, S, off), &slot)) return 1;
+  unsigned char *h = slot->host;
   for (int a = 0; a < 8; ++a)
-    memcpy(h + off[0] + a * stride * sizeof(double), f64_src[a], nS * sizeof(double));
+    memcpy(h + off[0] + a * nS * sizeof(double), f64_src[a], nS * sizeof(double));
   memcpy(h + off[1], sc->member, nS * sizeof(uint32_t));
   uint32_t *rgb = reinterpret_cast<uint32_t *>(h + off[2]);
   for (size_t i = 0; i < nS; ++i)
@@ -364,18 +362,16 @@ int swb_upload_scenes(swb_engine *eng, const swb_scene_soa *sc, const int32_t *e
   memcpy(h + off[5], sc->shape, nS);
   memcpy(h + off[6], sc->pos_f32, nS);
   // everything up to the end of the last used array, in one copy
-  CUDA_TRY(cudaMemcpyAsync(slot.dev, slot.host, off[6] + nS, cudaMemcpyHostToDevice, stream));
+  CUDA_TRY(cudaMemcpyAsync(slot->dev, slot->host, off[6] + nS, cudaMemcpyHostToDevice, stream));
   const int threads = 256, blocks = (int)((nS + threads - 1) / threads);
-  unsigned char *d = slot.dev;
+  unsigned char *d = slot->dev;
   scatter_scenes_kernel<<<blocks, threads, 0, stream>>>(
       eng->st, n, reinterpret_cast<const int32_t *>(d + off[4]), reinterpret_cast<const double *>(d + off[0]),
-      stride, reinterpret_cast<const uint32_t *>(d + off[1]), d + off[5], d + off[6],
+      nS, reinterpret_cast<const uint32_t *>(d + off[1]), d + off[5], d + off[6],
       reinterpret_cast<const uint32_t *>(d + off[2]), reinterpret_cast<const float *>(d + off[3]));
   eng->launches++;
   CUDA_TRY(cudaGetLastError());
-  CUDA_TRY(cudaEventRecord(slot.done, stream));
-  slot.in_flight = true;
-  return 0;
+  return release_slot(slot, stream);
 }
 
 int swb_request_reset(swb_engine *eng, const uint8_t *mask, void *stream_) {
@@ -783,7 +779,28 @@ int swb_upload_state(swb_engine *eng, const double *pos_x, const double *pos_y, 
 
 }  // extern "C"
 
-// Env ids of a record call: every id in [0, E); with `mark`, no id twice (destinations), and each
+// The argument checks every record call makes before it checks its ids: the engine, n, a load's
+// span class and, for n > 0, the id pointers and the record buffer of a save (dst) or a load (src):
+// set, 16-byte aligned and n records long.  `call` is SWB_IDS_CALL_*; `fn` names the entry point.
+static int check_record_args(const swb_engine *eng, const char *fn, int call, int32_t n, const void *ids0,
+                             const void *ids1, const void *rec, uint64_t rec_bytes, int32_t span_class) {
+  if (!eng) return fail("%s: null engine", fn);
+  if (n < 0) return fail("%s: n = %d", fn, n);
+  if (call == SWB_IDS_CALL_LOAD && span_class != 1 && span_class != 4)
+    return fail("%s: span_class must be 1 or 4, got %d", fn, span_class);
+  if (n == 0) return 0;
+  if (!ids0 || (call == SWB_IDS_CALL_COPY ? !ids1 : !rec)) return fail("%s: null argument", fn);
+  if (call == SWB_IDS_CALL_COPY) return 0;
+  if (reinterpret_cast<uintptr_t>(rec) % 16)
+    return fail("%s: %s is not 16-byte aligned", fn, call == SWB_IDS_CALL_SAVE ? "dst" : "src");
+  const uint64_t need = (uint64_t)n * RecordLayout(eng->st.S).bytes();
+  if (rec_bytes < need)
+    return fail("%s: %d records need %llu bytes, the buffer has %llu", fn, n, (unsigned long long)need,
+                (unsigned long long)rec_bytes);
+  return 0;
+}
+
+// Host ids of a record call: every id in [0, E); with `mark`, no id twice (destinations), and each
 // id is marked in it.
 static int check_env_ids(const swb_engine *eng, const char *fn, const int32_t *ids, int32_t n,
                          std::vector<uint8_t> *mark) {
@@ -798,58 +815,19 @@ static int check_env_ids(const swb_engine *eng, const char *fn, const int32_t *i
   return 0;
 }
 
-// Moves `n` ids from `a` (and `n` from `b`, if given) into a staging slot and enqueues one copy of
-// them to its device twin; the caller enqueues the kernels that read them, then finish_ids.
-static int stage_ids(swb_engine *eng, const int32_t *a, const int32_t *b, int32_t n, cudaStream_t stream,
-                     IdSlot **out) {
-  IdSlot &slot = eng->id_slots[eng->id_next];
-  eng->id_next ^= 1;
-  if (slot.in_flight) {
-    CUDA_TRY(cudaEventSynchronize(slot.done));
-    slot.in_flight = false;
-  }
-  const size_t need = 2 * (size_t)n;
-  if (need > slot.cap) {
-    if (slot.host) cudaFreeHost(slot.host);
-    if (slot.dev) cudaFree(slot.dev);
-    slot.host = slot.dev = nullptr;
-    slot.cap = 0;
-    const size_t cap = std::max<size_t>(need, 1024);
-    CUDA_TRY(cudaMallocHost(reinterpret_cast<void **>(&slot.host), cap * sizeof(int32_t)));
-    CUDA_TRY(cudaMalloc(reinterpret_cast<void **>(&slot.dev), cap * sizeof(int32_t)));
-    if (!slot.done) CUDA_TRY(cudaEventCreateWithFlags(&slot.done, cudaEventDisableTiming));
-    slot.cap = cap;
-  }
-  memcpy(slot.host, a, n * sizeof(int32_t));
-  if (b) memcpy(slot.host + n, b, n * sizeof(int32_t));
-  CUDA_TRY(cudaMemcpyAsync(slot.dev, slot.host, (b ? 2 : 1) * n * sizeof(int32_t), cudaMemcpyHostToDevice,
-                           stream));
-  *out = &slot;
-  return 0;
-}
-
-static int finish_ids(IdSlot *slot, cudaStream_t stream) {
-  CUDA_TRY(cudaEventRecord(slot->done, stream));
-  slot->in_flight = true;
-  return 0;
-}
-
-static int launch_save(swb_engine *eng, const int32_t *d_ids, int32_t n, void *dst, cudaStream_t stream) {
-  const int threads = 256, blocks = (int)(((size_t)n * eng->st.S + threads - 1) / threads);
-  save_envs_kernel<<<blocks, threads, 0, stream>>>(eng->st, n, d_ids, static_cast<unsigned char *>(dst),
-                                                   RecordLayout(eng->st.S).bytes());
-  eng->launches++;
-  CUDA_TRY(cudaGetLastError());
-  return 0;
-}
-
-static int launch_load(swb_engine *eng, const int32_t *d_ids, int32_t n, const void *src,
-                       cudaStream_t stream) {
-  const int threads = 256, blocks = (int)(((size_t)n * eng->st.S + threads - 1) / threads);
-  load_envs_kernel<<<blocks, threads, 0, stream>>>(eng->st, n, d_ids, static_cast<const unsigned char *>(src),
-                                                   RecordLayout(eng->st.S).bytes());
-  eng->launches++;
-  CUDA_TRY(cudaGetLastError());
+// Copies `n` host ids from `a` (and `n` from `b`, if given) into an id staging slot, enqueues their
+// copy to its device twin, and makes *c the IdCall of them, checked on the host.  After the kernels
+// that read them, release_slot(*slot).
+static int stage_ids(swb_engine *eng, const int32_t *a, const int32_t *b, int32_t n, int dst_arg,
+                     cudaStream_t stream, IdCall *c, StagingSlot **slot) {
+  const size_t bytes = (b ? 2 : 1) * (size_t)n * sizeof(int32_t);
+  if (take_slot(eng->id_staging, bytes, slot)) return 1;
+  int32_t *h = reinterpret_cast<int32_t *>((*slot)->host);
+  memcpy(h, a, n * sizeof(int32_t));
+  if (b) memcpy(h + n, b, n * sizeof(int32_t));
+  CUDA_TRY(cudaMemcpyAsync((*slot)->dev, h, bytes, cudaMemcpyHostToDevice, stream));
+  const int32_t *d = reinterpret_cast<const int32_t *>((*slot)->dev);
+  *c = IdCall{{d, b ? d + n : nullptr}, n, dst_arg, true};
   return 0;
 }
 
@@ -869,7 +847,6 @@ static int grow_records(swb_engine *eng, size_t need) {
 
 // Host checks of a device id list: everything the host sees without reading device memory.
 static int check_dev_ids(const swb_engine *eng, const char *fn, const void *ids, int32_t id_dtype) {
-  if (!ids) return fail("%s: null argument", fn);
   if (id_dtype != SWB_DTYPE_I32 && id_dtype != SWB_DTYPE_I64)
     return fail("%s: id_dtype must be SWB_DTYPE_I32 or SWB_DTYPE_I64, got %d", fn, id_dtype);
   if (reinterpret_cast<uintptr_t>(ids) % (id_dtype == SWB_DTYPE_I64 ? 8 : 4))
@@ -893,50 +870,63 @@ static int begin_id_call(swb_engine *eng, int call, const void *a, const void *b
     CUDA_TRY(cudaMemsetAsync(eng->d_id_fail, 0xFF, sizeof(unsigned long long), stream));
     eng->id_seq = 1;
   }
-  c->ids[0] = a;
-  c->ids[1] = b;
-  c->n = n;
-  c->dst_arg = dst_arg;
-  c->call = call;
-  c->hi = (unsigned long long)(~eng->id_seq) << 32;
-  c->claim = eng->d_id_claim;
-  c->fail = eng->d_id_fail;
-  c->status = eng->d_id_status;
+  *c = IdCall{{a, b}, n, dst_arg, false, call, (unsigned long long)(~eng->id_seq) << 32, eng->d_id_claim,
+              eng->d_id_fail, eng->d_id_status};
   return 0;
 }
 
 static unsigned grid_of(size_t threads) { return (unsigned)((threads + 255) / 256); }
 
+// The kernels of a save, load or copy of the ids `c`, checked on the host or, by the check kernels
+// enqueued first, on the device.
 template <typename T>
-static int enqueue_save_dev(swb_engine *eng, const IdCall &c, void *dst, cudaStream_t stream) {
-  const size_t rb = RecordLayout(eng->st.S).bytes();
-  check_ids_kernel<T><<<grid_of(c.n), 256, 0, stream>>>(c, eng->st.E);
-  save_envs_dev_kernel<T><<<grid_of((size_t)c.n * eng->st.S), 256, 0, stream>>>(
-      eng->st, c, static_cast<unsigned char *>(dst), rb);
-  eng->launches += 2;
+static int enqueue_save(swb_engine *eng, const IdCall &c, void *dst, cudaStream_t stream) {
+  if (!c.host_checked) {
+    check_ids_kernel<T><<<grid_of(c.n), 256, 0, stream>>>(c, eng->st.E);
+    eng->launches++;
+  }
+  save_envs_kernel<T><<<grid_of((size_t)c.n * eng->st.S), 256, 0, stream>>>(
+      eng->st, c, static_cast<unsigned char *>(dst), RecordLayout(eng->st.S).bytes());
+  eng->launches++;
   CUDA_TRY(cudaGetLastError());
   return 0;
 }
 
 template <typename T>
-static int enqueue_load_dev(swb_engine *eng, const IdCall &c, const void *src, cudaStream_t stream) {
-  const size_t rb = RecordLayout(eng->st.S).bytes();
-  check_ids_kernel<T><<<grid_of(c.n), 256, 0, stream>>>(c, eng->st.E);
-  repeat_ids_kernel<T><<<grid_of(c.n), 256, 0, stream>>>(c, eng->st.E);
-  load_envs_dev_kernel<T><<<grid_of((size_t)c.n * eng->st.S), 256, 0, stream>>>(
-      eng->st, c, static_cast<const unsigned char *>(src), rb);
-  eng->launches += 3;
+static int enqueue_load(swb_engine *eng, const IdCall &c, const void *src, cudaStream_t stream) {
+  if (!c.host_checked) {
+    check_ids_kernel<T><<<grid_of(c.n), 256, 0, stream>>>(c, eng->st.E);
+    repeat_ids_kernel<T><<<grid_of(c.n), 256, 0, stream>>>(c, eng->st.E);
+    eng->launches += 2;
+  }
+  load_envs_kernel<T><<<grid_of((size_t)c.n * eng->st.S), 256, 0, stream>>>(
+      eng->st, c, static_cast<const unsigned char *>(src), RecordLayout(eng->st.S).bytes());
+  eng->launches++;
   CUDA_TRY(cudaGetLastError());
   return 0;
 }
 
+// `disjoint`: the host found no env among both sources and destinations, so one kernel copies.
+// Otherwise every source is saved to engine scratch before any destination is written, so every
+// read sees the state from before the call.
 template <typename T>
-static int enqueue_copy_dev(swb_engine *eng, const IdCall &c, cudaStream_t stream) {
-  const size_t rb = RecordLayout(eng->st.S).bytes();
-  check_ids_kernel<T><<<grid_of(2 * (size_t)c.n), 256, 0, stream>>>(c, eng->st.E);
-  stage_copy_dev_kernel<T><<<grid_of((size_t)c.n * eng->st.S), 256, 0, stream>>>(eng->st, c, eng->d_records, rb);
-  load_envs_dev_kernel<T><<<grid_of((size_t)c.n * eng->st.S), 256, 0, stream>>>(eng->st, c, eng->d_records, rb);
-  eng->launches += 3;
+static int enqueue_copy(swb_engine *eng, const IdCall &c, bool disjoint, cudaStream_t stream) {
+  const size_t threads = (size_t)c.n * eng->st.S, rb = RecordLayout(eng->st.S).bytes();
+  if (disjoint) {
+    copy_envs_kernel<<<grid_of(threads), 256, 0, stream>>>(eng->st, c);
+    eng->launches++;
+  } else {
+    if (grow_records(eng, c.n * rb)) return 1;
+    if (c.host_checked) {
+      save_envs_kernel<T><<<grid_of(threads), 256, 0, stream>>>(eng->st, c, eng->d_records, rb);
+    } else {
+      check_ids_kernel<T><<<grid_of(2 * (size_t)c.n), 256, 0, stream>>>(c, eng->st.E);
+      stage_copy_dev_kernel<T><<<grid_of(threads), 256, 0, stream>>>(eng->st, c, eng->d_records, rb);
+      eng->launches++;
+    }
+    load_envs_kernel<T><<<grid_of(threads), 256, 0, stream>>>(eng->st, c, eng->d_records, rb);
+    eng->launches += 2;
+  }
   CUDA_TRY(cudaGetLastError());
   return 0;
 }
@@ -954,147 +944,104 @@ int64_t swb_env_record_bytes(const swb_engine *eng) {
 int swb_save_envs(swb_engine *eng, const int32_t *env_ids, int32_t n, void *dst, uint64_t dst_bytes,
                   int32_t *span_class, void *stream_) {
   if (!eng || !span_class) return fail("swb_save_envs: null argument");
-  if (n < 0) return fail("swb_save_envs: n = %d", n);
-  if (n == 0) {
-    *span_class = eng->max_spans;
-    return 0;
-  }
-  if (!env_ids || !dst) return fail("swb_save_envs: null argument");
-  if (reinterpret_cast<uintptr_t>(dst) % 16) return fail("swb_save_envs: dst is not 16-byte aligned");
-  const uint64_t need = (uint64_t)n * RecordLayout(eng->st.S).bytes();
-  if (dst_bytes < need)
-    return fail("swb_save_envs: %d records need %llu bytes, the buffer has %llu", n,
-                (unsigned long long)need, (unsigned long long)dst_bytes);
+  if (check_record_args(eng, "swb_save_envs", SWB_IDS_CALL_SAVE, n, env_ids, nullptr, dst, dst_bytes, 0))
+    return 1;
+  *span_class = eng->max_spans;
+  if (n == 0) return 0;
   if (check_env_ids(eng, "swb_save_envs", env_ids, n, nullptr)) return 1;
   CUDA_TRY(cudaSetDevice(eng->device));
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  IdSlot *slot = nullptr;
-  if (stage_ids(eng, env_ids, nullptr, n, stream, &slot) || launch_save(eng, slot->dev, n, dst, stream))
+  IdCall c;
+  StagingSlot *slot = nullptr;
+  if (stage_ids(eng, env_ids, nullptr, n, -1, stream, &c, &slot) || enqueue_save<int32_t>(eng, c, dst, stream))
+    return 1;
+  return release_slot(slot, stream);
+}
+
+int swb_save_envs_dev(swb_engine *eng, const void *env_ids, int32_t id_dtype, int32_t n, void *dst,
+                      uint64_t dst_bytes, int32_t *span_class, void *stream_) {
+  if (!eng || !span_class) return fail("swb_save_envs_dev: null argument");
+  if (check_record_args(eng, "swb_save_envs_dev", SWB_IDS_CALL_SAVE, n, env_ids, nullptr, dst, dst_bytes, 0))
     return 1;
   *span_class = eng->max_spans;
-  return finish_ids(slot, stream);
+  if (n == 0) return 0;
+  if (check_dev_ids(eng, "swb_save_envs_dev", env_ids, id_dtype)) return 1;
+  CUDA_TRY(cudaSetDevice(eng->device));
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  IdCall c;
+  if (begin_id_call(eng, SWB_IDS_CALL_SAVE, env_ids, nullptr, -1, n, stream, &c)) return 1;
+  return id_dtype == SWB_DTYPE_I64 ? enqueue_save<int64_t>(eng, c, dst, stream)
+                                   : enqueue_save<int32_t>(eng, c, dst, stream);
 }
 
 int swb_load_envs(swb_engine *eng, const int32_t *env_ids, int32_t n, const void *src, uint64_t src_bytes,
                   int32_t span_class, void *stream_) {
-  if (!eng) return fail("swb_load_envs: null engine");
-  if (n < 0) return fail("swb_load_envs: n = %d", n);
-  if (span_class != 1 && span_class != 4)
-    return fail("swb_load_envs: span_class must be 1 or 4, got %d", span_class);
+  if (check_record_args(eng, "swb_load_envs", SWB_IDS_CALL_LOAD, n, env_ids, nullptr, src, src_bytes,
+                        span_class))
+    return 1;
   if (n == 0) return 0;
-  if (!env_ids || !src) return fail("swb_load_envs: null argument");
-  if (reinterpret_cast<uintptr_t>(src) % 16) return fail("swb_load_envs: src is not 16-byte aligned");
-  const uint64_t need = (uint64_t)n * RecordLayout(eng->st.S).bytes();
-  if (src_bytes < need)
-    return fail("swb_load_envs: %d records need %llu bytes, the buffer has %llu", n,
-                (unsigned long long)need, (unsigned long long)src_bytes);
   std::vector<uint8_t> mark(eng->st.E, 0);
   if (check_env_ids(eng, "swb_load_envs", env_ids, n, &mark)) return 1;
   CUDA_TRY(cudaSetDevice(eng->device));
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   // records of stars or spokes need the concave span tables, as if their scenes were uploaded
   eng->max_spans = std::max(eng->max_spans, (int)span_class);
-  IdSlot *slot = nullptr;
-  if (stage_ids(eng, env_ids, nullptr, n, stream, &slot) || launch_load(eng, slot->dev, n, src, stream))
-    return 1;
-  return finish_ids(slot, stream);
-}
-
-int swb_copy_envs(swb_engine *eng, const int32_t *src_ids, const int32_t *dst_ids, int32_t n, void *stream_) {
-  if (!eng) return fail("swb_copy_envs: null engine");
-  if (n < 0) return fail("swb_copy_envs: n = %d", n);
-  if (n == 0) return 0;
-  if (!src_ids || !dst_ids) return fail("swb_copy_envs: null argument");
-  std::vector<uint8_t> mark(eng->st.E, 0);
-  if (check_env_ids(eng, "swb_copy_envs", dst_ids, n, &mark) ||
-      check_env_ids(eng, "swb_copy_envs", src_ids, n, nullptr))
-    return 1;
-  bool overlap = false;
-  for (int32_t i = 0; i < n && !overlap; ++i) overlap = mark[src_ids[i]] != 0;
-  CUDA_TRY(cudaSetDevice(eng->device));
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  // an env both read and written: every source is saved to engine scratch before any destination
-  // is written, so every read sees the state from before the call
-  if (grow_records(eng, overlap ? (size_t)n * RecordLayout(eng->st.S).bytes() : 0)) return 1;
-  IdSlot *slot = nullptr;
-  if (stage_ids(eng, src_ids, dst_ids, n, stream, &slot)) return 1;
-  if (!overlap) {
-    const int threads = 256, blocks = (int)(((size_t)n * eng->st.S + threads - 1) / threads);
-    copy_envs_kernel<<<blocks, threads, 0, stream>>>(eng->st, n, slot->dev, slot->dev + n);
-    eng->launches++;
-    CUDA_TRY(cudaGetLastError());
-    return finish_ids(slot, stream);
-  }
-  if (launch_save(eng, slot->dev, n, eng->d_records, stream) ||
-      launch_load(eng, slot->dev + n, n, eng->d_records, stream))
-    return 1;
-  return finish_ids(slot, stream);
-}
-
-int swb_save_envs_dev(swb_engine *eng, const void *env_ids, int32_t id_dtype, int32_t n, void *dst,
-                      uint64_t dst_bytes, int32_t *span_class, void *stream_) {
-  if (!eng || !span_class) return fail("swb_save_envs_dev: null argument");
-  if (n < 0) return fail("swb_save_envs_dev: n = %d", n);
-  if (n == 0) {
-    *span_class = eng->max_spans;
-    return 0;
-  }
-  if (!dst) return fail("swb_save_envs_dev: null argument");
-  if (check_dev_ids(eng, "swb_save_envs_dev", env_ids, id_dtype)) return 1;
-  if (reinterpret_cast<uintptr_t>(dst) % 16) return fail("swb_save_envs_dev: dst is not 16-byte aligned");
-  const uint64_t need = (uint64_t)n * RecordLayout(eng->st.S).bytes();
-  if (dst_bytes < need)
-    return fail("swb_save_envs_dev: %d records need %llu bytes, the buffer has %llu", n,
-                (unsigned long long)need, (unsigned long long)dst_bytes);
-  CUDA_TRY(cudaSetDevice(eng->device));
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   IdCall c;
-  if (begin_id_call(eng, SWB_IDS_CALL_SAVE, env_ids, nullptr, -1, n, stream, &c)) return 1;
-  if (id_dtype == SWB_DTYPE_I64 ? enqueue_save_dev<int64_t>(eng, c, dst, stream)
-                                : enqueue_save_dev<int32_t>(eng, c, dst, stream))
+  StagingSlot *slot = nullptr;
+  if (stage_ids(eng, env_ids, nullptr, n, 0, stream, &c, &slot) || enqueue_load<int32_t>(eng, c, src, stream))
     return 1;
-  *span_class = eng->max_spans;
-  return 0;
+  return release_slot(slot, stream);
 }
 
 int swb_load_envs_dev(swb_engine *eng, const void *env_ids, int32_t id_dtype, int32_t n, const void *src,
                       uint64_t src_bytes, int32_t span_class, void *stream_) {
-  if (!eng) return fail("swb_load_envs_dev: null engine");
-  if (n < 0) return fail("swb_load_envs_dev: n = %d", n);
-  if (span_class != 1 && span_class != 4)
-    return fail("swb_load_envs_dev: span_class must be 1 or 4, got %d", span_class);
+  if (check_record_args(eng, "swb_load_envs_dev", SWB_IDS_CALL_LOAD, n, env_ids, nullptr, src, src_bytes,
+                        span_class))
+    return 1;
   if (n == 0) return 0;
-  if (!src) return fail("swb_load_envs_dev: null argument");
   if (check_dev_ids(eng, "swb_load_envs_dev", env_ids, id_dtype)) return 1;
-  if (reinterpret_cast<uintptr_t>(src) % 16) return fail("swb_load_envs_dev: src is not 16-byte aligned");
-  const uint64_t need = (uint64_t)n * RecordLayout(eng->st.S).bytes();
-  if (src_bytes < need)
-    return fail("swb_load_envs_dev: %d records need %llu bytes, the buffer has %llu", n,
-                (unsigned long long)need, (unsigned long long)src_bytes);
   CUDA_TRY(cudaSetDevice(eng->device));
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   eng->max_spans = std::max(eng->max_spans, (int)span_class);
   IdCall c;
   if (begin_id_call(eng, SWB_IDS_CALL_LOAD, env_ids, nullptr, 0, n, stream, &c)) return 1;
-  return id_dtype == SWB_DTYPE_I64 ? enqueue_load_dev<int64_t>(eng, c, src, stream)
-                                   : enqueue_load_dev<int32_t>(eng, c, src, stream);
+  return id_dtype == SWB_DTYPE_I64 ? enqueue_load<int64_t>(eng, c, src, stream)
+                                   : enqueue_load<int32_t>(eng, c, src, stream);
+}
+
+int swb_copy_envs(swb_engine *eng, const int32_t *src_ids, const int32_t *dst_ids, int32_t n, void *stream_) {
+  if (check_record_args(eng, "swb_copy_envs", SWB_IDS_CALL_COPY, n, src_ids, dst_ids, nullptr, 0, 0)) return 1;
+  if (n == 0) return 0;
+  std::vector<uint8_t> mark(eng->st.E, 0);
+  if (check_env_ids(eng, "swb_copy_envs", dst_ids, n, &mark) ||
+      check_env_ids(eng, "swb_copy_envs", src_ids, n, nullptr))
+    return 1;
+  bool disjoint = true;
+  for (int32_t i = 0; i < n && disjoint; ++i) disjoint = !mark[src_ids[i]];
+  CUDA_TRY(cudaSetDevice(eng->device));
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  IdCall c;
+  StagingSlot *slot = nullptr;
+  if (stage_ids(eng, src_ids, dst_ids, n, 1, stream, &c, &slot) ||
+      enqueue_copy<int32_t>(eng, c, disjoint, stream))
+    return 1;
+  return release_slot(slot, stream);
 }
 
 int swb_copy_envs_dev(swb_engine *eng, const void *src_ids, const void *dst_ids, int32_t id_dtype, int32_t n,
                       void *stream_) {
-  if (!eng) return fail("swb_copy_envs_dev: null engine");
-  if (n < 0) return fail("swb_copy_envs_dev: n = %d", n);
+  if (check_record_args(eng, "swb_copy_envs_dev", SWB_IDS_CALL_COPY, n, src_ids, dst_ids, nullptr, 0, 0))
+    return 1;
   if (n == 0) return 0;
   if (check_dev_ids(eng, "swb_copy_envs_dev", src_ids, id_dtype) ||
       check_dev_ids(eng, "swb_copy_envs_dev", dst_ids, id_dtype))
     return 1;
   CUDA_TRY(cudaSetDevice(eng->device));
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  if (grow_records(eng, (size_t)n * RecordLayout(eng->st.S).bytes())) return 1;
   IdCall c;
   if (begin_id_call(eng, SWB_IDS_CALL_COPY, src_ids, dst_ids, 1, n, stream, &c)) return 1;
-  return id_dtype == SWB_DTYPE_I64 ? enqueue_copy_dev<int64_t>(eng, c, stream)
-                                   : enqueue_copy_dev<int32_t>(eng, c, stream);
+  return id_dtype == SWB_DTYPE_I64 ? enqueue_copy<int64_t>(eng, c, false, stream)
+                                   : enqueue_copy<int32_t>(eng, c, false, stream);
 }
 
 int swb_env_ids_status_pointer(swb_engine *eng, swb_ids_status **status) {

@@ -1,4 +1,7 @@
-// Env records: the save / load / copy kernels of swb_save_envs, swb_load_envs and swb_copy_envs.
+// Env records: the kernels of swb_save_envs, swb_load_envs and swb_copy_envs and of their _dev
+// variants.  save_envs_kernel<T> and load_envs_kernel<T> serve both; copy_envs_kernel copies
+// host-checked ids that do not overlap; device-checked ids add check_ids_kernel<T>,
+// repeat_ids_kernel<T> and stage_copy_dev_kernel<T>.
 //
 // An env record is everything that decides an env's future steps and frames within its current
 // episode: the sprite records of its current scene (the pool entry at (e, cursor[e])), its live
@@ -126,46 +129,23 @@ __device__ __forceinline__ void write_record(unsigned char *rec, int S, int s, c
   }
 }
 
-// One thread per (record, slot), as scatter_scenes_kernel.  record i <- env ids[i]
-__global__ void save_envs_kernel(DevState st, int n, const int32_t *__restrict__ ids,
-                                 unsigned char *__restrict__ rec, size_t record_bytes) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n * st.S) return;
-  const int r = i / st.S, s = i - r * st.S;
-  write_record(rec + (size_t)r * record_bytes, st.S, s, read_state(st, ids[r], s));
-}
-
-// env ids[i] <- record i (ids distinct)
-__global__ void load_envs_kernel(DevState st, int n, const int32_t *__restrict__ ids,
-                                 const unsigned char *__restrict__ rec, size_t record_bytes) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n * st.S) return;
-  const int r = i / st.S, s = i - r * st.S;
-  write_state(st, ids[r], s, read_record(st, rec + (size_t)r * record_bytes, s));
-}
-
-// env dst[i] <- env src[i], for id sets that do not overlap (no thread reads what another writes)
-__global__ void copy_envs_kernel(DevState st, int n, const int32_t *__restrict__ src,
-                                 const int32_t *__restrict__ dst) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n * st.S) return;
-  const int r = i / st.S, s = i - r * st.S;
-  write_state(st, dst[r], s, read_state(st, src[r], s));
-}
-
-// Device-checked id lists (swb_save_envs_dev / swb_load_envs_dev / swb_copy_envs_dev).
+// The id lists of a record call (swb_save_envs / swb_load_envs / swb_copy_envs and their _dev
+// variants).  Ids checked on the host (host_checked) are int32 and all valid: no check kernel runs
+// before the call's kernels, the call is never refused and reports nothing.
 //
-// Every call k of an engine gets a sequence number seq (1 .. 2^32 - 2, so that hi = ~seq never
-// equals the all-ones initial value) and keys hi << 32 | low: a later call's keys are smaller.
-// Failing positions atomicMin the key hi | (position << 1 | argument) into one engine word, so
-// that word holds a key of call k exactly when call k failed, and then the lowest failing position
-// of it.  A destination id claims its env with atomicMin(claim[id], hi | position); after that
-// pass a destination whose claim is not its own key repeats an id at a lower position.  Neither
-// word needs clearing between calls: the next call's keys replace the last one's.
+// Device-checked ids: every call k of an engine gets a sequence number seq (1 .. 2^32 - 2, so that
+// hi = ~seq never equals the all-ones initial value) and keys hi << 32 | low: a later call's keys
+// are smaller.  Failing positions atomicMin the key hi | (position << 1 | argument) into one engine
+// word, so that word holds a key of call k exactly when call k failed, and then the lowest failing
+// position of it.  A destination id claims its env with atomicMin(claim[id], hi | position); after
+// that pass a destination whose claim is not its own key repeats an id at a lower position.
+// Neither word needs clearing between calls: the next call's keys replace the last one's.
 struct IdCall {
   const void *ids[2];          // id arguments 0 and 1 (copy: src, dst; else ids[1] is null)
   int n;
   int dst_arg;                 // the argument whose ids must be distinct, or -1 (save)
+  bool host_checked;
+  // device-checked ids only
   int call;                    // SWB_IDS_CALL_*
   unsigned long long hi;       // ~seq << 32
   unsigned long long *claim;   // [E]
@@ -185,12 +165,14 @@ __device__ __forceinline__ const T *ids_of(const IdCall &c, int a) {
 }
 
 __device__ __forceinline__ bool call_refused(const IdCall &c) {
-  return (*c.fail >> 32) == (c.hi >> 32);
+  return !c.host_checked && (*c.fail >> 32) == (c.hi >> 32);
 }
 
-// Thread 0 of a call's last kernel: the ok word, and the call's first failure if none is recorded.
+// Thread 0 of a device-checked call's last kernel: the ok word, and the call's first failure if
+// none is recorded.
 template <typename T>
 __device__ void report_ids(const IdCall &c, int E) {
+  if (c.host_checked) return;
   const unsigned long long f = *c.fail;
   const bool bad = (f >> 32) == (c.hi >> 32);
   swb_ids_status *s = c.status;
@@ -235,10 +217,11 @@ __global__ void repeat_ids_kernel(IdCall c, int E) {
   if (p < (size_t)c.n) check_repeat<T>(c, E, (int)p);
 }
 
-// record i <- env ids[i], or zeros in every record of a refused call
+// One thread per (record, slot), as scatter_scenes_kernel.  record i <- env ids[0][i], or zeros
+// in every record of a refused call
 template <typename T>
-__global__ void save_envs_dev_kernel(DevState st, IdCall c, unsigned char *__restrict__ rec,
-                                     size_t record_bytes) {
+__global__ void save_envs_kernel(DevState st, IdCall c, unsigned char *__restrict__ rec,
+                                 size_t record_bytes) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i == 0) report_ids<T>(c, st.E);
   if (i >= (size_t)c.n * st.S) return;
@@ -247,8 +230,9 @@ __global__ void save_envs_dev_kernel(DevState st, IdCall c, unsigned char *__res
   write_record(rec + (size_t)r * record_bytes, st.S, s, call_refused(c) ? SlotRecord{} : read_state(st, id, s));
 }
 
-// Copy, first half: the repeat check of the destinations, and record i <- env src[i] in engine
-// scratch for every source in range (the load below reads none of it if the call is refused).
+// Device-checked copy, first half: the repeat check of the destinations, and record i <- env
+// src[i] in engine scratch for every source in range (the load below reads none of it if the call
+// is refused).
 template <typename T>
 __global__ void stage_copy_dev_kernel(DevState st, IdCall c, unsigned char *__restrict__ rec,
                                       size_t record_bytes) {
@@ -260,16 +244,25 @@ __global__ void stage_copy_dev_kernel(DevState st, IdCall c, unsigned char *__re
   if (id_in_range(id, st.E)) write_record(rec + (size_t)r * record_bytes, st.S, s, read_state(st, (int)id, s));
 }
 
-// env ids[dst_arg][i] <- record i, unless the call is refused
+// env ids[dst_arg][i] <- record i (ids distinct), unless the call is refused
 template <typename T>
-__global__ void load_envs_dev_kernel(DevState st, IdCall c, const unsigned char *__restrict__ rec,
-                                     size_t record_bytes) {
+__global__ void load_envs_kernel(DevState st, IdCall c, const unsigned char *__restrict__ rec,
+                                 size_t record_bytes) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i == 0) report_ids<T>(c, st.E);
   if (i >= (size_t)c.n * st.S || call_refused(c)) return;
   const int r = (int)(i / st.S), s = (int)(i - (size_t)r * st.S);
   const int id = (int)ids_of<T>(c, c.dst_arg)[r];
   write_state(st, id, s, read_record(st, rec + (size_t)r * record_bytes, s));
+}
+
+// Host-checked copy of id sets that do not overlap (no thread reads what another writes):
+// env dst[i] <- env src[i] in one pass, without scratch
+__global__ void copy_envs_kernel(DevState st, IdCall c) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= c.n * st.S) return;
+  const int r = i / st.S, s = i - r * st.S;
+  write_state(st, ids_of<int32_t>(c, 1)[r], s, read_state(st, ids_of<int32_t>(c, 0)[r], s));
 }
 
 }  // namespace swb

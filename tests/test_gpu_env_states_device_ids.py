@@ -196,8 +196,11 @@ def test_refused_ids_change_nothing_and_are_reported():
       eng.copy_envs(t, _dev(good, eng, dt), check='device')
     else:
       eng.copy_envs(_dev(src_ok, eng, dt), t, check='device')
+    status = eng.env_ids_status().clone()                # ok = 0, failed = 1
+    assert status[0] == 0 and status[4] == 1, name
     assert torch.equal(eng.save_envs().data, before), name
     assert torch.equal(eng.render(raster), frames), name
+    assert torch.equal(eng.env_ids_status(), status), name   # host-checked calls never write it
     with pytest.raises(ValueError, match=re.escape(msg)):
       eng.check_env_ids()
     eng.check_env_ids()                                 # cleared
@@ -207,7 +210,11 @@ def test_refused_ids_change_nothing_and_are_reported():
     g = torch.as_tensor(good, device=eng.device)
     assert torch.equal(after[g], before[torch.as_tensor(src_ok, device=eng.device)]), name
     eng.check_env_ids()
+    status = eng.env_ids_status().clone()                # ok = 1, failed = 0
+    assert status[0] == 1 and status[4] == 0, name
+    eng.copy_envs(src_ok, good)
     eng.load_envs(engine_states(eng, before), check='host')
+    assert torch.equal(eng.env_ids_status(), status), name
   # the first refused call since the last check is the one reported
   bad = torch.tensor([0, E], device=eng.device)
   eng.save_envs(bad, check='device')

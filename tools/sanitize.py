@@ -14,9 +14,10 @@ The last run renders 70-row frames (bands of 64 and 6 rows) for three times as m
 items as there are resident render CTAs, so every CTA claims several items of unequal bands,
 some written out by the bulk copy and some by the per-byte loop, one after the other.
 
-Between those, device-checked env records: saves, loads and copies with int32 and int64 device
-ids, valid and refused (out of range either way, 2^32 + 1, repeated destinations), so that memcheck
-sees that a refused id never indexes engine memory.
+Between those, env records: host-checked saves, loads and copies (disjoint and overlapping), which
+run the device-checked calls' save and load kernels on int32 ids, and device-checked ones with int32
+and int64 device ids, valid and refused (out of range either way, 2^32 + 1, repeated destinations),
+so that memcheck sees that a refused id never indexes engine memory.
 """
 import ctypes
 import os
@@ -63,6 +64,10 @@ def device_checked_records(torch):
   E = 40
   eng, raster, _ = workloads.build_engine(wl, E, 4, device=0, seed=4, max_episode_length=3)
   eng.step(torch.from_numpy(wl.sample_actions(np.random.RandomState(2), 1, E)[0]).cuda(), raster)
+  host = np.arange(E)
+  eng.load_envs(eng.save_envs(host[::-1].copy()), host)
+  eng.copy_envs(host, np.roll(host, 3))          # overlapping: through engine scratch
+  eng.copy_envs(host[:10], host[20:30])          # disjoint: one kernel
   ids = torch.arange(E, device='cuda')
   refused = 0
   for dt in (torch.int32, torch.int64):
