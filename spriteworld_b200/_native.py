@@ -19,6 +19,7 @@ TASK_NO_REWARD, TASK_FIND_GOAL, TASK_CLUSTERING, TASK_META = 0, 1, 2, 3
 AGG = {'sum': 0, 'max': 1, 'min': 2, 'mean': 3}
 CRIT = {'all': 0, 'any': 1}
 STEP_FIRST, STEP_MID, STEP_LAST = 0, 1, 2
+STEP_NONE = -1   # padding of a rollout: no step
 ENV_OK, ENV_CLUSTER_LABELS, ENV_CLUSTER_ZERODIV, ENV_BAD_ACTION, ENV_SPAN_OVERFLOW = 0, 1, 2, 4, 8
 IDS_CALL_SAVE, IDS_CALL_LOAD, IDS_CALL_COPY = 0, 1, 2
 IDS_OUT_OF_RANGE, IDS_REPEATED = 1, 2
@@ -99,6 +100,7 @@ def load():
   L.swb_step.argtypes = [vp, vp, ci, ctypes.POINTER(StepOut), vp]
   L.swb_eval_task.argtypes = [vp, ctypes.POINTER(StepOut), vp]
   L.swb_apply_action.argtypes = [vp, vp, ci, ctypes.POINTER(StepOut), vp]
+  L.swb_rollout.argtypes = [vp, vp, ci, ci, ci, ctypes.POINTER(StepOut), vp]
   L.swb_raster_create.argtypes = [vp, ci, ci, ci, vp, ctypes.POINTER(vp)]
   L.swb_raster_destroy.argtypes = [vp]
   L.swb_raster_destroy.restype = None
@@ -145,7 +147,7 @@ def load():
 EXPORTS = (
     'swb_last_error', 'swb_version', 'swb_sizeof_config', 'swb_sizeof_task_node',
     'swb_engine_create', 'swb_engine_destroy', 'swb_upload_scenes', 'swb_request_reset',
-    'swb_step', 'swb_eval_task', 'swb_apply_action', 'swb_raster_create', 'swb_raster_destroy', 'swb_render', 'swb_step_render',
+    'swb_step', 'swb_eval_task', 'swb_apply_action', 'swb_rollout', 'swb_raster_create', 'swb_raster_destroy', 'swb_render', 'swb_step_render',
     'swb_step_render_gather', 'swb_ipc_alloc', 'swb_ipc_free', 'swb_ipc_open', 'swb_ipc_close', 'swb_peer_copy',
     'swb_step_host', 'swb_state_pointers', 'swb_scene_serial_pointer', 'swb_render_status_pointer', 'swb_download_state', 'swb_upload_state',
     'swb_env_record_bytes', 'swb_save_envs', 'swb_load_envs', 'swb_copy_envs', 'swb_save_envs_dev',

@@ -9,6 +9,7 @@
 
 #include "swb_device.cuh"
 #include "swb_render.cuh"
+#include "swb_rollout.cuh"
 #include "swb_sampler.cuh"
 #include "swb_states.cuh"
 #include "swb_step.cuh"
@@ -159,7 +160,7 @@ int upload_axis(swb_raster *r, const AxisHost &h, AxisTables *d) {
 extern "C" {
 
 const char *swb_last_error(void) { return g_error.c_str(); }
-int swb_version(void) { return 5; }
+int swb_version(void) { return 6; }
 int swb_sizeof_config(void) { return (int)sizeof(swb_config); }
 int swb_sizeof_task_node(void) { return (int)sizeof(swb_task_node); }
 
@@ -427,6 +428,24 @@ int swb_apply_action(swb_engine *eng, const void *actions, int32_t action_dtype,
                      const swb_step_out *out, void *stream) {
   if (check_step(eng, actions, action_dtype, out, STEP_ACTION)) return 1;
   return launch_step(eng, actions, action_dtype, *out, static_cast<cudaStream_t>(stream), STEP_ACTION);
+}
+
+int swb_rollout(swb_engine *eng, const void *actions, int32_t action_dtype, int32_t n_steps,
+                int32_t n_candidates, const swb_step_out *out, void *stream) {
+  if (check_step(eng, actions, action_dtype, out, STEP_WHOLE)) return 1;
+  if (n_steps < 1 || n_candidates < 1)
+    return fail("swb_rollout: n_steps = %d and n_candidates = %d must both be >= 1", n_steps, n_candidates);
+  const int64_t plans = (int64_t)eng->st.E * n_candidates;
+  if (plans > SWB_ROLLOUT_MAX_ENTRIES / n_steps)
+    return fail("swb_rollout: %d steps x %d envs x %d candidates exceed %d entries per call", n_steps,
+                eng->st.E, n_candidates, SWB_ROLLOUT_MAX_ENTRIES);
+  CUDA_TRY(cudaSetDevice(eng->device));
+  const unsigned blocks = (unsigned)((plans + ROLLOUT_WARPS - 1) / ROLLOUT_WARPS);
+  rollout_kernel<<<blocks, ROLLOUT_WARPS * 32, 0, static_cast<cudaStream_t>(stream)>>>(
+      eng->st, eng->d_step_cfg, actions, action_dtype, n_steps, n_candidates, *out);
+  eng->launches++;
+  CUDA_TRY(cudaGetLastError());
+  return 0;
 }
 
 // The checks of a render launch of raster `r` by `eng` with `max_spans` spans per sprite row;

@@ -360,6 +360,172 @@ __device__ void task_eval(const StepCfg &c_step, const WarpSprites &ws, int S, d
   *success = val[nn - 1].success;
 }
 
+// One env's row of `actions` in registers, as raw 32-bit words: 2 of an int32 row, 4 of a float32
+// row, 8 of a float64 row.
+struct ActionRow {
+  uint32_t w[8];
+};
+
+__device__ __forceinline__ ActionRow load_action(const void *__restrict__ actions, int action_dtype,
+                                                 size_t row) {
+  ActionRow r = {};
+  if (action_dtype == SWB_DTYPE_I32) {
+    const int32_t *a = reinterpret_cast<const int32_t *>(actions) + 2 * row;
+    r.w[0] = (uint32_t)a[0]; r.w[1] = (uint32_t)a[1];
+  } else if (action_dtype == SWB_DTYPE_F32) {
+    const float *a = reinterpret_cast<const float *>(actions) + 4 * row;
+    for (int i = 0; i < 4; i++) r.w[i] = __float_as_uint(a[i]);
+  } else {
+    const double *a = reinterpret_cast<const double *>(actions) + 4 * row;
+    for (int i = 0; i < 4; i++) {
+      r.w[2 * i] = (uint32_t)__double2loint(a[i]);
+      r.w[2 * i + 1] = (uint32_t)__double2hiint(a[i]);
+    }
+  }
+  return r;
+}
+
+// action_space.step of one action on the warp's sprites (every lane calls it): moves the clicked /
+// carried / body sprite, returns the action's cost; a bad Embodied direction sets
+// SWB_ENV_BAD_ACTION in *status and moves nothing.  The warp is synchronised on return.
+__device__ __forceinline__ double apply_action(const DevState &st, const StepCfg &c_step, WarpSprites &ws,
+                                               int S, const ActionRow &row, int action_dtype, int lane,
+                                               int *status) {
+  double cost = 0.;
+  const bool keep = c_step.keep_in_frame != 0;
+  if (c_step.action_kind == SWB_ACT_EMBODIED) {  // action_spaces.py:187-214
+    const bool carry = row.w[0] != 0;
+    const int dir = (int)row.w[1];
+    const double step = c_step.action_scale;
+    double mx = 0., my = 0.;
+    if (dir == 0) my = step;
+    else if (dir == 1) mx = -step;
+    else if (dir == 2) my = -step;
+    else if (dir == 3) mx = step;
+    else *status |= SWB_ENV_BAD_ACTION;
+    if (!(*status & SWB_ENV_BAD_ACTION)) {
+      const int body = S - 1;
+      if (carry) {  // :180-185
+        for (int s = body - 1; s >= 0; s--) {
+          if (!ws.shape[s]) continue;
+          const double tx = offset_component(ws.x[body], ws.f32[body], ws.x[s], ws.f32[s]);
+          const double ty = offset_component(ws.y[body], ws.f32[body], ws.y[s], ws.f32[s]);
+          if (warp_contains(st, ws, s, tx, ty, lane)) {
+            __syncwarp();  // every lane is done reading the pose lane 0 overwrites
+            if (lane == 0) sprite_move(ws, s, mx, my, keep);
+            break;
+          }
+        }
+        __syncwarp();
+      }
+      if (lane == 0) sprite_move(ws, body, mx, my, keep);
+      cost = __dmul_rn(-c_step.motion_cost, c_step.action_scale);
+    }
+  } else {  // SelectMove :83-104 / DragAndDrop :133-137
+    double px, py, mx, my, norm;
+    const bool af32 = action_dtype == SWB_DTYPE_F32;
+    if (af32) {
+      float a[4];
+      for (int i = 0; i < 4; i++) a[i] = __uint_as_float(row.w[i]);
+      const float fsc = (float)c_step.action_scale;
+      float d0, d1;
+      if (c_step.action_kind == SWB_ACT_SELECT_MOVE) {
+        d0 = __fsub_rn(a[2], 0.5f); d1 = __fsub_rn(a[3], 0.5f);
+      } else {
+        d0 = __fsub_rn(a[2], a[0]); d1 = __fsub_rn(a[3], a[1]);
+      }
+      const float m0 = __fmul_rn(d0, fsc), m1 = __fmul_rn(d1, fsc);
+      px = a[0]; py = a[1]; mx = m0; my = m1;
+      norm = (double)__fsqrt_rn(__fadd_rn(__fmul_rn(m0, m0), __fmul_rn(m1, m1)));
+    } else {
+      double a[4];
+      for (int i = 0; i < 4; i++) a[i] = __hiloint2double((int)row.w[2 * i + 1], (int)row.w[2 * i]);
+      if (c_step.action_kind == SWB_ACT_SELECT_MOVE) {
+        mx = __dmul_rn(__dsub_rn(a[2], 0.5), c_step.action_scale);
+        my = __dmul_rn(__dsub_rn(a[3], 0.5), c_step.action_scale);
+      } else {
+        mx = __dmul_rn(__dsub_rn(a[2], a[0]), c_step.action_scale);
+        my = __dmul_rn(__dsub_rn(a[3], a[1]), c_step.action_scale);
+      }
+      px = a[0]; py = a[1];
+      // np.linalg.norm of a float64 2-vector is sqrt(x.dot(x)), and OpenBLAS ddot fuses the
+      // second product into the first: fma(my, my, mx * mx) (DESIGN.md section 5)
+      norm = __dsqrt_rn(__fma_rn(my, my, __dmul_rn(mx, mx)));
+    }
+    for (int s = S - 1; s >= 0; s--) {  // :77-81 top-most first
+      if (!ws.shape[s]) continue;
+      const double tx = offset_component(px, af32, ws.x[s], ws.f32[s]);
+      const double ty = offset_component(py, af32, ws.y[s], ws.f32[s]);
+      if (warp_contains(st, ws, s, tx, ty, lane)) {
+        __syncwarp();
+        if (lane == 0) sprite_move(ws, s, mx, my, keep);
+        break;
+      }
+    }
+    if (af32) cost = (double)__fmul_rn((float)(-c_step.motion_cost), (float)norm);
+    else cost = __dmul_rn(-c_step.motion_cost, norm);
+  }
+  __syncwarp();
+  return cost;
+}
+
+// velocity update of every sprite (environment.py:98-99), slot-parallel; the reference's KeyError
+// skips it.  The warp is synchronised on return.
+__device__ __forceinline__ void velocity_update(const StepCfg &c_step, WarpSprites &ws, int S, int lane,
+                                                double vx, double vy, int status) {
+  if (!(status & SWB_ENV_BAD_ACTION) && lane < S && ws.shape[lane])
+    sprite_move(ws, lane, vx, vy, c_step.keep_in_frame != 0);
+  __syncwarp();
+}
+
+// The end of Environment.step for one env (one lane calls it) after its action, velocity update
+// and task: counts the step in *count, returns the step type and sets *reward.
+__device__ __forceinline__ int finish_step(const StepCfg &c_step, const WarpSprites &ws, int S,
+                                           int action_dtype, double cost, double tr, int succ,
+                                           int status, int *count, double *reward) {
+  *count += 1;  // :93
+  if (status & SWB_ENV_BAD_ACTION) {
+    // the reference's state after the KeyError: the step is counted (:93), nothing moved
+    *reward = nan("");
+    return SWB_STEP_MID;
+  }
+  bool oof = false;
+  for (int s = 0; s < S; s++) {
+    if (!ws.shape[s]) continue;
+    if (!((ws.x[s] >= 0.0 && ws.y[s] >= 0.0) && (ws.x[s] <= 1.0 && ws.y[s] <= 1.0))) oof = true;
+  }
+  const bool timeout = *count >= c_step.max_episode_length;  // :84
+  // :101.  A float32 click costs an np.float32; Clustering's reward is a Python float, so
+  // NumPy 2 adds the two in float32.  Every other root returns np.float64 (or 0.0, which
+  // leaves the float32 cost unchanged either way).
+  const bool f32_sum = action_dtype == SWB_DTYPE_F32 && c_step.action_kind != SWB_ACT_EMBODIED &&
+                       c_step.nodes[c_step.n_nodes - 1].kind == SWB_TASK_CLUSTERING;
+  *reward = f32_sum ? (double)__fadd_rn((float)cost, (float)tr) : __dadd_rn(cost, tr);
+  return (succ || oof || timeout) ? SWB_STEP_LAST : SWB_STEP_MID;
+}
+
+// The env's current scene -- the pool entry at `scene0` -- in the warp's WarpSprites, with the
+// pool's initial positions (`from_pool`) or the live ones; *vx, *vy: lane s holds slot s's velocity.
+__device__ __forceinline__ void stage_sprites(const DevState &st, WarpSprites &ws, int S, int e, int scene0,
+                                              bool from_pool, int lane, double *vx, double *vy) {
+  *vx = 0.; *vy = 0.;
+  if (lane < S) {
+    const int sc = scene0 + lane;
+    ws.shape[lane] = st.p_shape[sc];
+    ws.f32[lane] = st.p_pos_f32[sc];
+    ws.member[lane] = st.p_member[sc];
+    ws.m00[lane] = st.p_m00[sc]; ws.m01[lane] = st.p_m01[sc];
+    ws.m10[lane] = st.p_m10[sc]; ws.m11[lane] = st.p_m11[sc];
+    if (from_pool) {
+      ws.x[lane] = st.p_x[sc]; ws.y[lane] = st.p_y[sc];
+    } else {
+      ws.x[lane] = st.pos_x[e * S + lane]; ws.y[lane] = st.pos_y[e * S + lane];
+      *vx = st.p_vx[sc]; *vy = st.p_vy[sc];
+    }
+  }
+  __syncwarp();
+}
+
 __global__ void __launch_bounds__(STEP_WARPS * 32)
 step_kernel(DevState st, const StepCfg *__restrict__ step_cfg, const void *__restrict__ actions,
             int action_dtype, swb_step_out out, int mode) {
@@ -380,104 +546,15 @@ step_kernel(DevState st, const StepCfg *__restrict__ step_cfg, const void *__res
   const bool resetting = mode == 0 && st.reset_next[e] != 0;
   int cursor = st.cursor[e];
   if (resetting) cursor = (cursor + 1) % st.K;  // environment.py:90-91 -> reset() :74-78
-  const int scene0 = (e * st.K + cursor) * S;
-  double vx = 0., vy = 0.;
-  if (lane < S) {
-    const int sc = scene0 + lane;
-    ws.shape[lane] = st.p_shape[sc];
-    ws.f32[lane] = st.p_pos_f32[sc];
-    ws.member[lane] = st.p_member[sc];
-    ws.m00[lane] = st.p_m00[sc]; ws.m01[lane] = st.p_m01[sc];
-    ws.m10[lane] = st.p_m10[sc]; ws.m11[lane] = st.p_m11[sc];
-    if (resetting) {
-      ws.x[lane] = st.p_x[sc]; ws.y[lane] = st.p_y[sc];
-    } else {
-      ws.x[lane] = st.pos_x[e * S + lane]; ws.y[lane] = st.pos_y[e * S + lane];
-      vx = st.p_vx[sc]; vy = st.p_vy[sc];
-    }
-  }
-  __syncwarp();
+  double vx, vy;
+  stage_sprites(st, ws, S, e, (e * st.K + cursor) * S, resetting, lane, &vx, &vy);
 
   double cost = 0.;
   int status = 0;
-  const bool keep = c_step.keep_in_frame != 0;
   if (!resetting && mode != 1) {
-    if (c_step.action_kind == SWB_ACT_EMBODIED) {  // action_spaces.py:187-214
-      const int32_t *a = reinterpret_cast<const int32_t *>(actions) + 2 * (size_t)e;
-      const bool carry = a[0] != 0;
-      const int dir = a[1];
-      const double step = c_step.action_scale;
-      double mx = 0., my = 0.;
-      if (dir == 0) my = step;
-      else if (dir == 1) mx = -step;
-      else if (dir == 2) my = -step;
-      else if (dir == 3) mx = step;
-      else status |= SWB_ENV_BAD_ACTION;
-      if (!(status & SWB_ENV_BAD_ACTION)) {
-        const int body = S - 1;
-        if (carry) {  // :180-185
-          for (int s = body - 1; s >= 0; s--) {
-            if (!ws.shape[s]) continue;
-            const double tx = offset_component(ws.x[body], ws.f32[body], ws.x[s], ws.f32[s]);
-            const double ty = offset_component(ws.y[body], ws.f32[body], ws.y[s], ws.f32[s]);
-            if (warp_contains(st, ws, s, tx, ty, lane)) {
-              __syncwarp();  // every lane is done reading the pose lane 0 overwrites
-              if (lane == 0) sprite_move(ws, s, mx, my, keep);
-              break;
-            }
-          }
-          __syncwarp();
-        }
-        if (lane == 0) sprite_move(ws, body, mx, my, keep);
-        cost = __dmul_rn(-c_step.motion_cost, c_step.action_scale);
-      }
-    } else {  // SelectMove :83-104 / DragAndDrop :133-137
-      double px, py, mx, my, norm;
-      const bool af32 = action_dtype == SWB_DTYPE_F32;
-      if (af32) {
-        const float *a = reinterpret_cast<const float *>(actions) + 4 * (size_t)e;
-        const float fsc = (float)c_step.action_scale;
-        float d0, d1;
-        if (c_step.action_kind == SWB_ACT_SELECT_MOVE) {
-          d0 = __fsub_rn(a[2], 0.5f); d1 = __fsub_rn(a[3], 0.5f);
-        } else {
-          d0 = __fsub_rn(a[2], a[0]); d1 = __fsub_rn(a[3], a[1]);
-        }
-        const float m0 = __fmul_rn(d0, fsc), m1 = __fmul_rn(d1, fsc);
-        px = a[0]; py = a[1]; mx = m0; my = m1;
-        norm = (double)__fsqrt_rn(__fadd_rn(__fmul_rn(m0, m0), __fmul_rn(m1, m1)));
-      } else {
-        const double *a = reinterpret_cast<const double *>(actions) + 4 * (size_t)e;
-        if (c_step.action_kind == SWB_ACT_SELECT_MOVE) {
-          mx = __dmul_rn(__dsub_rn(a[2], 0.5), c_step.action_scale);
-          my = __dmul_rn(__dsub_rn(a[3], 0.5), c_step.action_scale);
-        } else {
-          mx = __dmul_rn(__dsub_rn(a[2], a[0]), c_step.action_scale);
-          my = __dmul_rn(__dsub_rn(a[3], a[1]), c_step.action_scale);
-        }
-        px = a[0]; py = a[1];
-        // np.linalg.norm of a float64 2-vector is sqrt(x.dot(x)), and OpenBLAS ddot fuses the
-        // second product into the first: fma(my, my, mx * mx) (DESIGN.md section 5)
-        norm = __dsqrt_rn(__fma_rn(my, my, __dmul_rn(mx, mx)));
-      }
-      for (int s = S - 1; s >= 0; s--) {  // :77-81 top-most first
-        if (!ws.shape[s]) continue;
-        const double tx = offset_component(px, af32, ws.x[s], ws.f32[s]);
-        const double ty = offset_component(py, af32, ws.y[s], ws.f32[s]);
-        if (warp_contains(st, ws, s, tx, ty, lane)) {
-          __syncwarp();
-          if (lane == 0) sprite_move(ws, s, mx, my, keep);
-          break;
-        }
-      }
-      if (af32) cost = (double)__fmul_rn((float)(-c_step.motion_cost), (float)norm);
-      else cost = __dmul_rn(-c_step.motion_cost, norm);
-    }
-    __syncwarp();
-    // velocity update of every sprite (environment.py:98-99); the reference's KeyError skips it
-    if (mode == 0 && !(status & SWB_ENV_BAD_ACTION) && lane < S && ws.shape[lane])
-      sprite_move(ws, lane, vx, vy, keep);
-    __syncwarp();
+    cost = apply_action(st, c_step, ws, S, load_action(actions, action_dtype, (size_t)e), action_dtype,
+                        lane, &status);
+    if (mode == 0) velocity_update(c_step, ws, S, lane, vx, vy, status);
   }
 
   if (mode != 1 && lane < S) {
@@ -504,33 +581,14 @@ step_kernel(DevState st, const StepCfg *__restrict__ step_cfg, const void *__res
       out.status[e] = (uint8_t)status;
       return;
     }
-    int step_type;
-    int count = st.step_count[e];
-    if (resetting) {
-      count = 0;
-      step_type = SWB_STEP_FIRST;
-      out.reward[e] = 0.0;
-    } else if (status & SWB_ENV_BAD_ACTION) {
-      // the reference's state after the KeyError: the step is counted (:93), nothing moved
-      count += 1;
-      step_type = SWB_STEP_MID;
-      out.reward[e] = nan("");
-    } else {
-      count += 1;  // :93
-      bool oof = false;
-      for (int s = 0; s < S; s++) {
-        if (!ws.shape[s]) continue;
-        if (!((ws.x[s] >= 0.0 && ws.y[s] >= 0.0) && (ws.x[s] <= 1.0 && ws.y[s] <= 1.0))) oof = true;
-      }
-      const bool timeout = count >= c_step.max_episode_length;  // :84
-      step_type = (succ || oof || timeout) ? SWB_STEP_LAST : SWB_STEP_MID;
-      // :101.  A float32 click costs an np.float32; Clustering's reward is a Python float, so
-      // NumPy 2 adds the two in float32.  Every other root returns np.float64 (or 0.0, which
-      // leaves the float32 cost unchanged either way).
-      const bool f32_sum = action_dtype == SWB_DTYPE_F32 && c_step.action_kind != SWB_ACT_EMBODIED &&
-                           c_step.nodes[c_step.n_nodes - 1].kind == SWB_TASK_CLUSTERING;
-      out.reward[e] = f32_sum ? (double)__fadd_rn((float)cost, (float)tr) : __dadd_rn(cost, tr);
+    int step_type = SWB_STEP_FIRST;
+    int count = 0;
+    double reward = 0.0;
+    if (!resetting) {
+      count = st.step_count[e];
+      step_type = finish_step(c_step, ws, S, action_dtype, cost, tr, succ, status, &count, &reward);
     }
+    out.reward[e] = reward;
     st.cursor[e] = cursor;
     if (resetting) st.scene_serial[e] += 1;  // monotonic: the host's refill bookkeeping reads it
     st.step_count[e] = count;

@@ -36,6 +36,16 @@ class StepResult(object):
     self.status, self.frames = status, frames
 
 
+class RolloutResult(object):
+  """Outputs of a rollout, (T, n_envs, C) each: reward float64, step_type int8 (STEP_MID, STEP_LAST
+  or, after a plan's first LAST and for an env about to reset, STEP_NONE with reward 0), success
+  and status uint8.  The caller's own tensors: no later call overwrites them."""
+  __slots__ = ('reward', 'step_type', 'success', 'status')
+
+  def __init__(self, reward, step_type, success, status):
+    self.reward, self.step_type, self.success, self.status = reward, step_type, success, status
+
+
 OUT_BYTES_PER_ENV = 8 + 1 + 1 + 1
 
 
@@ -62,20 +72,41 @@ ACTIONS = {'select_move': ActionSpec(_native.ACT_SELECT_MOVE, 4, _FLOATS),
 _SPECS = {spec.kind: spec for spec in ACTIONS.values()}   # the same table by swb action kind
 
 
-def action_dtype(action_kind, n_envs, actions, device=None):
+def action_dtype(action_kind, n_envs, actions, device=None, plans=False):
   """The swb action dtype of `actions` (tensor or array) for `n_envs` envs of swb `action_kind`;
-  with `device`, a contiguous tensor on it.  ValueError otherwise: nothing is converted."""
+  with `device`, a contiguous tensor on it; with `plans`, the (T, n_envs, C, columns) actions of a
+  rollout, T and C at least 1.  ValueError otherwise: nothing is converted."""
   if device is not None and not (isinstance(actions, torch.Tensor) and actions.device == device
                                  and actions.is_contiguous()):
     raise ValueError('actions must be a contiguous tensor on %s, got %s'
                      % (device, _describe(actions)))
   spec = _SPECS[action_kind]
   name = str(actions.dtype).replace('torch.', '')
-  shape = (int(n_envs), spec.columns)
-  if tuple(actions.shape) != shape or name not in spec.dtypes:
+  shape, got = (int(n_envs), spec.columns), tuple(actions.shape)
+  if plans:
+    ok = len(got) == 4 and got[1::2] == shape and got[0] >= 1 and got[2] >= 1
+    shape = ('T >= 1', shape[0], 'C >= 1', shape[1])
+  else:
+    ok = got == shape
+  if not ok or name not in spec.dtypes:
     raise ValueError('actions must have shape %s and dtype %s, got %s %s' % (
-        shape, ' or '.join(spec.dtypes), name, tuple(actions.shape)))
+        shape, ' or '.join(spec.dtypes), name, got))
   return spec.dtypes[name]
+
+
+def rollout_outputs(out, n_steps, n_envs, n_candidates, device):
+  """(packed buffer, RolloutResult of its views) for a rollout of that size: `out`, or if it is None
+  a new uint8 tensor, of n_steps * n_envs * n_candidates * OUT_BYTES_PER_ENV bytes on `device`, laid
+  out as split_outputs reads it."""
+  shape = (int(n_steps), int(n_envs), int(n_candidates))
+  n = shape[0] * shape[1] * shape[2]
+  if out is None:
+    out = torch.empty(n * OUT_BYTES_PER_ENV, dtype=torch.uint8, device=device)
+  elif (not isinstance(out, torch.Tensor) or out.dtype != torch.uint8 or out.device != device or
+        tuple(out.shape) != (n * OUT_BYTES_PER_ENV,) or not out.is_contiguous() or out.data_ptr() % 8):
+    raise ValueError('out must be a contiguous, 8-byte aligned uint8 tensor of %d bytes on %s, got %s'
+                     % (n * OUT_BYTES_PER_ENV, device, _describe(out)))
+  return out, RolloutResult(*[v.view(shape) for v in split_outputs(out, n)])
 
 
 def host_actions(kind, actions):
@@ -301,6 +332,20 @@ class Engine(object):
           self._h, raster._h, ctypes.c_void_p(actions.data_ptr()), dt, ctypes.byref(self._out),
           ctypes.c_void_p(frames.data_ptr()), self._stream()))
     return StepResult(self._reward, self._step_type, self._success, self._status, frames)
+
+  def rollout(self, actions, out=None):
+    """What each of C candidate action sequences of T steps would earn from the state every env is
+    in now, in one launch that changes nothing (swb_rollout).  `actions`: device tensor
+    (T, n_envs, C, columns) of a dtype step() takes.  Returns a RolloutResult; with `out`, a packed
+    uint8 tensor of T * n_envs * C * OUT_BYTES_PER_ENV bytes, its tensors are views of that."""
+    dt = action_dtype(self.action_kind, self.n_envs, actions, self.device, plans=True)
+    T, _, C, _ = actions.shape
+    out, res = rollout_outputs(out, T, self.n_envs, C, self.device)
+    ptrs = _native.StepOut(res.reward.data_ptr(), res.step_type.data_ptr(), res.success.data_ptr(),
+                           res.status.data_ptr())
+    _native.check(self._lib.swb_rollout(self._h, ctypes.c_void_p(actions.data_ptr()), dt, T, C,
+                                        ctypes.byref(ptrs), self._stream()))
+    return res
 
   def step_gather(self, actions, raster, targets):
     """Environment.step for every env with the frame gather fused into the render kernel:

@@ -259,6 +259,10 @@ BatchedTimeStep = collections.namedtuple(
     'BatchedTimeStep', ['step_type', 'reward', 'discount', 'observation', 'success', 'status'])
 
 
+BatchedRollout = collections.namedtuple(
+    'BatchedRollout', ['step_type', 'reward', 'discount', 'success', 'status'])
+
+
 class BatchedEnvironment(object):
   """`n_envs` Spriteworld environments advanced in lockstep on one GPU.
 
@@ -267,6 +271,10 @@ class BatchedEnvironment(object):
   reward float64 (0 on FIRST), discount float32 (1 MID/FIRST, 0 LAST), observation dict
   name -> uint8 (n_envs, H, W, 3), success uint8, status uint8 (per-env task errors the
   reference would raise: _native.ENV_*).
+
+  rollout(actions) scores plans without stepping: for (T, n_envs, C, 4) or (T, n_envs, C, 2)
+  actions it returns a BatchedRollout of (T, n_envs, C) device tensors, entry [t, e, c] being what
+  step t of candidate c would report for env e from the state it is in now.  No env changes.
   """
 
   def __init__(self, task, action_space, renderers, init_sprites, keep_in_frame=True,
@@ -675,6 +683,31 @@ class BatchedEnvironment(object):
     else:
       self._engine.copy_envs(src_ids, dst_ids)
     self._resets += 1
+
+  def rollout(self, actions):
+    """Scores C candidate action sequences of T steps per env from the state every env is in now,
+    in one kernel launch, and leaves every env as it is: no position, counter, scene ring or
+    frame changes, so nothing here counts against the ring's refill.
+
+    `actions`: (T, n_envs, C, 4) float32 / float64 or (T, n_envs, C, 2) int32, array or tensor, as
+    step() takes them per env.  Returns a BatchedRollout of (T, n_envs, C) device tensors the
+    caller owns.  Entry [t, e, c] is, bit for bit, what step(actions[t, :, c]) would report for env
+    e after the steps before it: step_type int8, reward float64, success and status uint8, and
+    discount float32 (1 on MID, 0 on LAST and on padding).  A plan ends with its first LAST (the
+    task solved, a sprite out of frame, or max_episode_length counted from the env's own step
+    count); the entries after it are padding -- step_type _native.STEP_NONE, reward 0 -- so
+    reward.sum(0) is each plan's return.  An env that is about to reset (before the first reset(),
+    or after a LAST) has no episode to plan in: all its entries are padding.
+
+    A rollout evaluates the noiseless model: the action space's `noise_scale` is not applied and
+    nothing is drawn from `rng`, so the timesteps of a run are bit-identical with and without
+    rollouts between its steps."""
+    kind = self._action_space.compile()['kind']
+    if not isinstance(actions, torch.Tensor):
+      actions = torch.from_numpy(engine_lib.host_actions(kind, actions))
+    res = self._engine.rollout(actions.to(self._engine.device).contiguous())
+    discount = (res.step_type == _native.STEP_MID).to(torch.float32)
+    return BatchedRollout(res.step_type, res.reward, discount, res.success, res.status)
 
   def render(self):
     """Re-renders every PILRenderer observation of the current state (a loaded one, say) into
