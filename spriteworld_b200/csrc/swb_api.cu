@@ -160,7 +160,7 @@ int upload_axis(swb_raster *r, const AxisHost &h, AxisTables *d) {
 extern "C" {
 
 const char *swb_last_error(void) { return g_error.c_str(); }
-int swb_version(void) { return 6; }
+int swb_version(void) { return 7; }
 int swb_sizeof_config(void) { return (int)sizeof(swb_config); }
 int swb_sizeof_task_node(void) { return (int)sizeof(swb_task_node); }
 
@@ -430,22 +430,47 @@ int swb_apply_action(swb_engine *eng, const void *actions, int32_t action_dtype,
   return launch_step(eng, actions, action_dtype, *out, static_cast<cudaStream_t>(stream), STEP_ACTION);
 }
 
-int swb_rollout(swb_engine *eng, const void *actions, int32_t action_dtype, int32_t n_steps,
-                int32_t n_candidates, const swb_step_out *out, void *stream) {
+// The checks of a rollout from n_roots roots (`what`: "envs" for the live envs, else "roots") that
+// every rollout entry point makes.  T * n_roots * C <= SWB_ROLLOUT_MAX_ENTRIES also keeps the
+// kernel's warp index n_roots * C within an int32.
+static_assert(SWB_ROLLOUT_MAX_ENTRIES <= 2147483647, "rollout indices are int32");
+static int check_rollout(const swb_engine *eng, const char *fn, const char *what, const void *actions,
+                         int32_t action_dtype, int32_t n_steps, int32_t n_candidates, int32_t n_roots,
+                         const swb_step_out *out) {
   if (check_step(eng, actions, action_dtype, out, STEP_WHOLE)) return 1;
   if (n_steps < 1 || n_candidates < 1)
-    return fail("swb_rollout: n_steps = %d and n_candidates = %d must both be >= 1", n_steps, n_candidates);
-  const int64_t plans = (int64_t)eng->st.E * n_candidates;
+    return fail("%s: n_steps = %d and n_candidates = %d must both be >= 1", fn, n_steps, n_candidates);
+  const int64_t plans = (int64_t)n_roots * n_candidates;
   if (plans > SWB_ROLLOUT_MAX_ENTRIES / n_steps)
-    return fail("swb_rollout: %d steps x %d envs x %d candidates exceed %d entries per call", n_steps,
-                eng->st.E, n_candidates, SWB_ROLLOUT_MAX_ENTRIES);
+    return fail("%s: %d steps x %d %s x %d candidates exceed %d entries per call", fn, n_steps, n_roots,
+                what, n_candidates, SWB_ROLLOUT_MAX_ENTRIES);
+  return 0;
+}
+
+// Enqueues the one rollout_kernel launch of a checked call: roots from io.roots unless it is null
+// (the live envs), leaves into io.leaves unless it is null.
+static int enqueue_rollout(swb_engine *eng, const void *actions, int32_t action_dtype, int32_t n_steps,
+                           int32_t n_candidates, const swb_step_out &out, RolloutRecords io,
+                           cudaStream_t stream) {
   CUDA_TRY(cudaSetDevice(eng->device));
+  const int64_t plans = (int64_t)(io.roots ? io.n_roots : eng->st.E) * n_candidates;
   const unsigned blocks = (unsigned)((plans + ROLLOUT_WARPS - 1) / ROLLOUT_WARPS);
-  rollout_kernel<<<blocks, ROLLOUT_WARPS * 32, 0, static_cast<cudaStream_t>(stream)>>>(
-      eng->st, eng->d_step_cfg, actions, action_dtype, n_steps, n_candidates, *out);
+  auto kernel = io.roots ? (io.leaves ? rollout_kernel<true, true> : rollout_kernel<true, false>)
+                         : (io.leaves ? rollout_kernel<false, true> : rollout_kernel<false, false>);
+  kernel<<<blocks, ROLLOUT_WARPS * 32, 0, stream>>>(eng->st, eng->d_step_cfg, actions, action_dtype, n_steps,
+                                                    n_candidates, out, io);
   eng->launches++;
   CUDA_TRY(cudaGetLastError());
   return 0;
+}
+
+int swb_rollout(swb_engine *eng, const void *actions, int32_t action_dtype, int32_t n_steps,
+                int32_t n_candidates, const swb_step_out *out, void *stream) {
+  if (check_rollout(eng, "swb_rollout", "envs", actions, action_dtype, n_steps, n_candidates,
+                    eng ? eng->st.E : 0, out))
+    return 1;
+  return enqueue_rollout(eng, actions, action_dtype, n_steps, n_candidates, *out, RolloutRecords{},
+                         static_cast<cudaStream_t>(stream));
 }
 
 // The checks of a render launch of raster `r` by `eng` with `max_spans` spans per sprite row;
@@ -801,6 +826,17 @@ int swb_upload_state(swb_engine *eng, const double *pos_x, const double *pos_y, 
 // The argument checks every record call makes before it checks its ids: the engine, n, a load's
 // span class and, for n > 0, the id pointers and the record buffer of a save (dst) or a load (src):
 // set, 16-byte aligned and n records long.  `call` is SWB_IDS_CALL_*; `fn` names the entry point.
+// A record buffer `name` of fn that must hold n records: 16-byte aligned and large enough.
+static int check_record_buffer(const swb_engine *eng, const char *fn, const char *name, const void *rec,
+                               uint64_t rec_bytes, int64_t n) {
+  if (reinterpret_cast<uintptr_t>(rec) % 16) return fail("%s: %s is not 16-byte aligned", fn, name);
+  const uint64_t need = (uint64_t)n * RecordLayout(eng->st.S).bytes();
+  if (rec_bytes < need)
+    return fail("%s: %lld records need %llu bytes, the buffer has %llu", fn, (long long)n,
+                (unsigned long long)need, (unsigned long long)rec_bytes);
+  return 0;
+}
+
 static int check_record_args(const swb_engine *eng, const char *fn, int call, int32_t n, const void *ids0,
                              const void *ids1, const void *rec, uint64_t rec_bytes, int32_t span_class) {
   if (!eng) return fail("%s: null engine", fn);
@@ -810,13 +846,7 @@ static int check_record_args(const swb_engine *eng, const char *fn, int call, in
   if (n == 0) return 0;
   if (!ids0 || (call == SWB_IDS_CALL_COPY ? !ids1 : !rec)) return fail("%s: null argument", fn);
   if (call == SWB_IDS_CALL_COPY) return 0;
-  if (reinterpret_cast<uintptr_t>(rec) % 16)
-    return fail("%s: %s is not 16-byte aligned", fn, call == SWB_IDS_CALL_SAVE ? "dst" : "src");
-  const uint64_t need = (uint64_t)n * RecordLayout(eng->st.S).bytes();
-  if (rec_bytes < need)
-    return fail("%s: %d records need %llu bytes, the buffer has %llu", fn, n, (unsigned long long)need,
-                (unsigned long long)rec_bytes);
-  return 0;
+  return check_record_buffer(eng, fn, call == SWB_IDS_CALL_SAVE ? "dst" : "src", rec, rec_bytes, n);
 }
 
 // Host ids of a record call: every id in [0, E); with `mark`, no id twice (destinations), and each
@@ -1061,6 +1091,35 @@ int swb_copy_envs_dev(swb_engine *eng, const void *src_ids, const void *dst_ids,
   if (begin_id_call(eng, SWB_IDS_CALL_COPY, src_ids, dst_ids, 1, n, stream, &c)) return 1;
   return id_dtype == SWB_DTYPE_I64 ? enqueue_copy<int64_t>(eng, c, false, stream)
                                    : enqueue_copy<int32_t>(eng, c, false, stream);
+}
+
+int swb_rollout_states(swb_engine *eng, const void *roots, int32_t n_roots, uint64_t roots_bytes,
+                       const void *actions, int32_t action_dtype, int32_t n_steps, int32_t n_candidates,
+                       const swb_step_out *out, void *leaves, uint64_t leaves_bytes, int32_t *span_class,
+                       void *stream) {
+  static const char fn[] = "swb_rollout_states";
+  if (!eng) return fail("%s: null engine", fn);
+  if (roots ? n_roots < 1 : n_roots != eng->st.E)
+    return roots ? fail("%s: n_roots = %d must be >= 1", fn, n_roots)
+                 : fail("%s: n_roots = %d must be E = %d when the roots are the live envs", fn, n_roots,
+                        eng->st.E);
+  if (check_rollout(eng, fn, roots ? "roots" : "envs", actions, action_dtype, n_steps, n_candidates, n_roots,
+                    out))
+    return 1;
+  const uint64_t rb = RecordLayout(eng->st.S).bytes();
+  const uint64_t plans = (uint64_t)n_roots * n_candidates;
+  if (roots && check_record_buffer(eng, fn, "roots", roots, roots_bytes, n_roots)) return 1;
+  if (leaves && check_record_buffer(eng, fn, "leaves", leaves, leaves_bytes, (int64_t)plans)) return 1;
+  if (roots && leaves) {
+    const uintptr_t r0 = reinterpret_cast<uintptr_t>(roots), l0 = reinterpret_cast<uintptr_t>(leaves);
+    if (r0 < l0 + plans * rb && l0 < r0 + (uint64_t)n_roots * rb)
+      return fail("%s: the leaves overlap the roots", fn);
+  }
+  if (!roots && span_class) *span_class = eng->max_spans;
+  return enqueue_rollout(eng, actions, action_dtype, n_steps, n_candidates, *out,
+                         RolloutRecords{static_cast<const unsigned char *>(roots),
+                                        static_cast<unsigned char *>(leaves), (size_t)rb, n_roots},
+                         static_cast<cudaStream_t>(stream));
 }
 
 int swb_env_ids_status_pointer(swb_engine *eng, swb_ids_status **status) {

@@ -1,40 +1,89 @@
-// Rollout kernel: what C candidate action sequences of T steps would earn from the state every
-// env is in now, without changing that state.
+// Rollout kernel: what C candidate action sequences of T steps would earn from a set of root
+// states, without changing any env, and optionally the state each plan ends in.
 //
-// One warp per (env, candidate), warp index w = e * C + c.  The warp stages the env's current
-// scene -- the pool entry at (e, cursor) with the live positions -- into shared memory once and
-// runs T steps of step_kernel's own action, velocity, task and termination code
-// (swb_step.cuh) on that copy.  Entry [t][e][c] of the outputs is what Environment.step would
-// report at step t; after the plan's first LAST, and for an env about to reset, the entries are
-// padding (SWB_STEP_NONE, reward 0, success 0, status 0).  The kernel writes the outputs only.
+// One warp per (root, candidate), warp index w = r * C + c.  A root is either live env r -- its
+// current scene, the pool entry at (r, cursor), with the live positions (swb_rollout) -- or record
+// r of a device buffer of env records (swb_rollout_states).  The warp stages the root's scene into
+// shared memory once and runs T steps of step_kernel's own action, velocity, task and termination
+// code (swb_step.cuh) on that copy.  Entry [t][r][c] of the outputs is what Environment.step would
+// report at step t; after the plan's first LAST, and for a root about to reset, the entries are
+// padding (SWB_STEP_NONE, reward 0, success 0, status 0).
 //
-// Actions are [T][E][C][A]: at a step the warps of a CTA read consecutive rows, every lane the
+// Leaves: when a warp is done (after step T, after the plan's first LAST, or at once for a root
+// about to reset) lanes < S write record w: the record swb_save_envs would save of an env that
+// started in the root state and took the plan's live steps -- the root's scene, the final
+// positions, step_count after the counted steps and reset_next = 1 iff the last of them was LAST.
+// Leaves and roots share the record format, so one launch is one level of a search tree.
+//
+// Actions are [T][R][C][A]: at a step the warps of a CTA read consecutive rows, every lane the
 // row of its warp (one broadcast transaction), and the row of step t + 1 is loaded before step t
 // is evaluated, so its latency hides behind lane 0's task evaluation.
 #pragma once
+#include "swb_states.cuh"
 #include "swb_step.cuh"
 
 namespace swb {
 
 constexpr int ROLLOUT_WARPS = 4;
 
+// The record buffers of a rollout: roots (n_roots records) unless the roots are the live envs,
+// leaves (n_roots * C records) if asked for.  Each instantiation of rollout_kernel reads only
+// the members its template arguments use.
+struct RolloutRecords {
+  const unsigned char *roots;
+  unsigned char *leaves;
+  size_t record_bytes;
+  int n_roots;
+};
+
+// Root record `rec` in the warp's WarpSprites, as stage_sprites stages an env's pool entry with
+// its live positions (shape ids sanitised by read_record); *vx, *vy: lane s holds slot s's velocity.
+__device__ __forceinline__ void stage_record(const DevState &st, WarpSprites &ws, int S,
+                                             const unsigned char *rec, int lane, double *vx, double *vy) {
+  *vx = 0.; *vy = 0.;
+  if (lane < S) {
+    const SlotRecord r = read_record(st, rec, lane);
+    ws.shape[lane] = r.shape;
+    ws.f32[lane] = r.pos_f32;
+    ws.member[lane] = r.member;
+    ws.m00[lane] = r.f64[2]; ws.m01[lane] = r.f64[3];
+    ws.m10[lane] = r.f64[4]; ws.m11[lane] = r.f64[5];
+    ws.x[lane] = r.f64[8]; ws.y[lane] = r.f64[9];
+    *vx = r.f64[6]; *vy = r.f64[7];
+  }
+  __syncwarp();
+}
+
+// kRecordRoots: roots are io.roots (else the E live envs); kLeaves: write io.leaves.
+template <bool kRecordRoots, bool kLeaves>
 __global__ void __launch_bounds__(ROLLOUT_WARPS * 32)
 rollout_kernel(DevState st, const StepCfg *__restrict__ step_cfg, const void *__restrict__ actions,
-               int action_dtype, int T, int C, swb_step_out out) {
+               int action_dtype, int T, int C, swb_step_out out, RolloutRecords io) {
   const StepCfg &c_step = *step_cfg;
   __shared__ WarpSprites s_ws[ROLLOUT_WARPS];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int w = blockIdx.x * ROLLOUT_WARPS + warp;
-  const int EC = st.E * C;  // T * E * C fits an int32 (swb_rollout checks it)
+  // T * R * C fits an int32 (swb_rollout and swb_rollout_states check it)
+  const int EC = (kRecordRoots ? io.n_roots : st.E) * C;
   if (w >= EC) return;
   const int e = w / C;
   WarpSprites &ws = s_ws[warp];
   const int S = st.S;
-  int t = 0;
-  if (!st.reset_next[e]) {  // else the env's next step starts another scene: nothing to plan in
+  const RecordLayout L(S);
+  const unsigned char *root = kRecordRoots ? io.roots + (size_t)e * io.record_bytes : nullptr;
+  // else the env's next step starts another scene: nothing to plan in
+  const bool resetting = kRecordRoots ? root[L.reset_next()] != 0 : st.reset_next[e] != 0;
+  int t = 0, count = 0;
+  bool ended = false;
+  if (!resetting) {
     double vx, vy;
-    stage_sprites(st, ws, S, e, (e * st.K + st.cursor[e]) * S, false, lane, &vx, &vy);
-    int count = st.step_count[e];
+    if (kRecordRoots) {
+      stage_record(st, ws, S, root, lane, &vx, &vy);
+      count = *reinterpret_cast<const int32_t *>(root + L.step_count());
+    } else {
+      stage_sprites(st, ws, S, e, (e * st.K + st.cursor[e]) * S, false, lane, &vx, &vy);
+      count = st.step_count[e];
+    }
     ActionRow next = load_action(actions, action_dtype, (size_t)w);
     while (t < T) {
       const ActionRow row = next;
@@ -56,7 +105,10 @@ rollout_kernel(DevState st, const StepCfg *__restrict__ step_cfg, const void *__
       }
       step_type = __shfl_sync(0xFFFFFFFFu, step_type, 0);
       t++;
-      if (step_type == SWB_STEP_LAST) break;
+      if (step_type == SWB_STEP_LAST) {
+        ended = true;
+        break;
+      }
     }
   }
   for (int p = t + lane; p < T; p += 32) {
@@ -65,6 +117,16 @@ rollout_kernel(DevState st, const StepCfg *__restrict__ step_cfg, const void *__
     out.step_type[i] = (int8_t)SWB_STEP_NONE;
     out.success[i] = 0;
     out.status[i] = 0;
+  }
+  if (kLeaves && lane < S) {
+    SlotRecord leaf = kRecordRoots ? read_record(st, root, lane) : read_state(st, e, lane);
+    if (!resetting) {
+      leaf.f64[8] = ws.x[lane];
+      leaf.f64[9] = ws.y[lane];
+      leaf.step_count = count;   // lane 0 counted the steps; write_record stores slot 0's copy
+      leaf.reset_next = ended ? 1 : 0;
+    }
+    write_record(io.leaves + (size_t)w * io.record_bytes, S, lane, leaf);
   }
 }
 

@@ -39,11 +39,13 @@ class StepResult(object):
 class RolloutResult(object):
   """Outputs of a rollout, (T, n_envs, C) each: reward float64, step_type int8 (STEP_MID, STEP_LAST
   or, after a plan's first LAST and for an env about to reset, STEP_NONE with reward 0), success
-  and status uint8.  The caller's own tensors: no later call overwrites them."""
-  __slots__ = ('reward', 'step_type', 'success', 'status')
+  and status uint8.  The caller's own tensors: no later call overwrites them.  `leaves`: None, or
+  the EnvStates of the state each plan ends in (record r * C + c: root r's plan c)."""
+  __slots__ = ('reward', 'step_type', 'success', 'status', 'leaves')
 
-  def __init__(self, reward, step_type, success, status):
+  def __init__(self, reward, step_type, success, status, leaves=None):
     self.reward, self.step_type, self.success, self.status = reward, step_type, success, status
+    self.leaves = leaves
 
 
 OUT_BYTES_PER_ENV = 8 + 1 + 1 + 1
@@ -333,18 +335,46 @@ class Engine(object):
           ctypes.c_void_p(frames.data_ptr()), self._stream()))
     return StepResult(self._reward, self._step_type, self._success, self._status, frames)
 
-  def rollout(self, actions, out=None):
+  def rollout(self, actions, out=None, states=None, leaves=None):
     """What each of C candidate action sequences of T steps would earn from the state every env is
     in now, in one launch that changes nothing (swb_rollout).  `actions`: device tensor
     (T, n_envs, C, columns) of a dtype step() takes.  Returns a RolloutResult; with `out`, a packed
-    uint8 tensor of T * n_envs * C * OUT_BYTES_PER_ENV bytes, its tensors are views of that."""
-    dt = action_dtype(self.action_kind, self.n_envs, actions, self.device, plans=True)
+    uint8 tensor of T * n_envs * C * OUT_BYTES_PER_ENV bytes, its tensors are views of that.
+
+    `states`: EnvStates of n roots of this engine's configuration (any n >= 1) to plan from instead
+    of the live envs; actions and outputs are then (T, n, C, ...).  `leaves`: True for new
+    EnvStates of the n * C states the plans end in (RolloutResult.leaves), or EnvStates of n * C
+    records to fill in place; record r * C + c is what save_envs would return after loading root r
+    and stepping plan c's live steps.  Leaves carry the roots' span class.  Still one launch
+    (swb_rollout_states)."""
+    if states is not None and not isinstance(states, EnvStates):
+      raise ValueError('states must be EnvStates, got %s' % type(states).__name__)
+    n = self.n_envs if states is None else len(states)
+    dt = action_dtype(self.action_kind, n, actions, self.device, plans=True)
     T, _, C, _ = actions.shape
-    out, res = rollout_outputs(out, T, self.n_envs, C, self.device)
+    if states is not None:
+      self.check_states(states, n)
+    if leaves is True:
+      leaves = EnvStates(torch.empty((n * C, self.record_bytes), dtype=torch.uint8, device=self.device),
+                         1, self.signature, self.n_slots)
+    elif leaves is not None:
+      self.check_states(leaves, n * C)
+    out, res = rollout_outputs(out, T, n, C, self.device)
     ptrs = _native.StepOut(res.reward.data_ptr(), res.step_type.data_ptr(), res.success.data_ptr(),
                            res.status.data_ptr())
-    _native.check(self._lib.swb_rollout(self._h, ctypes.c_void_p(actions.data_ptr()), dt, T, C,
-                                        ctypes.byref(ptrs), self._stream()))
+    if states is None and leaves is None:
+      _native.check(self._lib.swb_rollout(self._h, ctypes.c_void_p(actions.data_ptr()), dt, T, C,
+                                          ctypes.byref(ptrs), self._stream()))
+      return res
+    span = ctypes.c_int32(1 if states is None else states.span_class)
+    roots = (None, 0) if states is None else (ctypes.c_void_p(states.data.data_ptr()), states.data.numel())
+    dst = (None, 0) if leaves is None else (ctypes.c_void_p(leaves.data.data_ptr()), leaves.data.numel())
+    _native.check(self._lib.swb_rollout_states(
+        self._h, roots[0], n, roots[1], ctypes.c_void_p(actions.data_ptr()), dt, T, C, ctypes.byref(ptrs),
+        dst[0], dst[1], ctypes.byref(span), self._stream()))
+    if leaves is not None:
+      leaves.span_class = span.value
+    res.leaves = leaves
     return res
 
   def step_gather(self, actions, raster, targets):
@@ -741,8 +771,9 @@ class EnvStates(object):
   span class the records need (1: convex shapes only, 4: stars or spokes) and the signature of
   the engine configuration they belong to (config_signature).
 
-  len(), indexing and slicing (a device gather; an int keeps one record), `to(device)`,
-  EnvStates.cat() and torch.save / torch.load; to_host() decodes the records into NumPy arrays."""
+  len(), indexing and slicing (a device gather; an int keeps one record), take() (a gather by a
+  device index tensor, without host synchronisation), `to(device)`, EnvStates.cat() and
+  torch.save / torch.load; to_host() decodes the records into NumPy arrays."""
 
   def __init__(self, data, span_class, signature, n_slots):
     self.data, self.span_class = data, int(span_class)
@@ -761,6 +792,25 @@ class EnvStates(object):
     elif not isinstance(idx, slice):
       idx = torch.as_tensor(env_ids_array(idx).astype(np.int64), device=self.data.device)
     return EnvStates(self.data[idx].contiguous(), self.span_class, self.signature, self.n_slots)
+
+  def take(self, index):
+    """EnvStates whose record i is record index[i]: a gather on the device that never waits for
+    it, for indices the device computes (a top-k over rollout returns, say).  `index`: a
+    one-dimensional int32 or int64 tensor on the records' device.  An entry outside [0, len(self))
+    gives a zero record, which loads as an env with only empty slots."""
+    if (not isinstance(index, torch.Tensor) or index.dim() != 1 or
+        index.dtype not in (torch.int32, torch.int64) or index.device != self.data.device):
+      raise ValueError('take needs a one-dimensional int32 or int64 tensor on %s, got %s'
+                       % (self.data.device, _describe(index)))
+    n = len(self)
+    if n == 0:
+      data = self.data.new_zeros((index.numel(), self.record_bytes))
+    else:
+      index = index.long()
+      inside = (index >= 0) & (index < n)
+      # clamped, so that no index outside the records reaches the gather
+      data = self.data.index_select(0, index.clamp(0, n - 1)).masked_fill_(~inside[:, None], 0)
+    return EnvStates(data, self.span_class, self.signature, self.n_slots)
 
   def to(self, device):
     return EnvStates(self.data.to(device), self.span_class, self.signature, self.n_slots)

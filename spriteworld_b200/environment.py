@@ -275,6 +275,8 @@ class BatchedEnvironment(object):
   rollout(actions) scores plans without stepping: for (T, n_envs, C, 4) or (T, n_envs, C, 2)
   actions it returns a BatchedRollout of (T, n_envs, C) device tensors, entry [t, e, c] being what
   step t of candidate c would report for env e from the state it is in now.  No env changes.
+  rollout(actions, states) plans from saved env records instead, and expand(actions, states) also
+  returns the state each plan ends in, as records: one level of a search tree.
   """
 
   def __init__(self, task, action_space, renderers, init_sprites, keep_in_frame=True,
@@ -684,10 +686,12 @@ class BatchedEnvironment(object):
       self._engine.copy_envs(src_ids, dst_ids)
     self._resets += 1
 
-  def rollout(self, actions):
+  def rollout(self, actions, states=None):
     """Scores C candidate action sequences of T steps per env from the state every env is in now,
     in one kernel launch, and leaves every env as it is: no position, counter, scene ring or
-    frame changes, so nothing here counts against the ring's refill.
+    frame changes, so nothing here counts against the ring's refill.  With `states` (EnvStates of
+    n roots saved by an environment of this configuration) the plans start from those records
+    instead, and actions and outputs are (T, n, C, ...).
 
     `actions`: (T, n_envs, C, 4) float32 / float64 or (T, n_envs, C, 2) int32, array or tensor, as
     step() takes them per env.  Returns a BatchedRollout of (T, n_envs, C) device tensors the
@@ -702,10 +706,33 @@ class BatchedEnvironment(object):
     A rollout evaluates the noiseless model: the action space's `noise_scale` is not applied and
     nothing is drawn from `rng`, so the timesteps of a run are bit-identical with and without
     rollouts between its steps."""
+    if states is None:
+      return self._batched_rollout(self._engine.rollout(self._plans(actions)))
+    return self._batched_rollout(self._engine.rollout(self._plans(actions), states=states))
+
+  def expand(self, actions, states=None):
+    """One level of a search tree: rollout(actions, states) that also returns the state every plan
+    ends in, as (BatchedRollout, EnvStates).  Leaf r * C + c is root r's plan c (the roots are the
+    live envs without `states`): what save_envs would return after loading the root and stepping
+    the plan's live steps -- its final positions and step count, and reset_next = 1 if the plan
+    ended on a LAST, so that a leaf's own rollouts are all padding.  Leaves go back in as `states`
+    (narrowed with EnvStates.take, say), with nothing on the host between levels.
+
+    As rollout(): no noise, no `rng` draw, and no env or scene ring changes; loading a leaf later
+    (load_envs) counts as a reset, as every load does."""
+    res = self._engine.rollout(self._plans(actions), states=states, leaves=True)
+    return self._batched_rollout(res), res.leaves
+
+  def _plans(self, actions):
+    """Rollout actions as a contiguous tensor on the engine's device (host actions through
+    engine.host_actions), without noise."""
     kind = self._action_space.compile()['kind']
     if not isinstance(actions, torch.Tensor):
       actions = torch.from_numpy(engine_lib.host_actions(kind, actions))
-    res = self._engine.rollout(actions.to(self._engine.device).contiguous())
+    return actions.to(self._engine.device).contiguous()
+
+  @staticmethod
+  def _batched_rollout(res):
     discount = (res.step_type == _native.STEP_MID).to(torch.float32)
     return BatchedRollout(res.step_type, res.reward, discount, res.success, res.status)
 

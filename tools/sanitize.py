@@ -17,7 +17,8 @@ some written out by the bulk copy and some by the per-byte loop, one after the o
 Between those, env records: host-checked saves, loads and copies (disjoint and overlapping), which
 run the device-checked calls' save and load kernels on int32 ids, and device-checked ones with int32
 and int64 device ids, valid and refused (out of range either way, 2^32 + 1, repeated destinations),
-so that memcheck sees that a refused id never indexes engine memory.
+so that memcheck sees that a refused id never indexes engine memory.  Then rollouts from records
+into leaves, from those leaves, and from the live envs into leaves.
 """
 import ctypes
 import os
@@ -90,6 +91,16 @@ def device_checked_records(torch):
   assert refused == 24, refused   # every call but a save or a copy source with a repeat
   print('device-checked records: %d envs, %d refused reports, %d kernel launches'
         % (E, refused, eng.launch_count()), flush=True)
+  # rollouts from records (an odd count, some about to reset) into leaves, and from the leaves
+  roots = eng.save_envs(np.arange(E - 3))
+  T, C = 4, 3
+  plans = torch.rand((T, len(roots), C, 4), device='cuda')
+  res = eng.rollout(plans, states=roots, leaves=True)
+  eng.rollout(torch.rand((T, len(res.leaves), 1, 4), device='cuda'), states=res.leaves, leaves=True)
+  eng.rollout(torch.rand((T, E, 2, 4), device='cuda'), leaves=True)
+  torch.cuda.synchronize()
+  print('record rollouts: %d roots, %d leaves, %d kernel launches'
+        % (len(roots), len(res.leaves), eng.launch_count()), flush=True)
   raster.close()
   eng.close()
 
