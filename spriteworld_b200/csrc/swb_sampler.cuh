@@ -80,22 +80,39 @@ struct Stream {
   SWB_HD int64_t below(int64_t n) { return (int64_t)mulhi64(next(), (uint64_t)n); }
 };
 
-SWB_HD bool is_int_kind(int k) { return k >= SWB_FT_I8 && k <= SWB_FT_U64; }
-SWB_HD bool is_int_like(int k) { return is_int_kind(k) || k == SWB_FT_PYINT; }
+// Float-to-integer conversions as NumPy's astype makes them on x86-64: truncation toward zero,
+// and INT32_MIN / INT64_MIN for a value out of range or NaN (what cvttsd2si returns).  C++ leaves
+// such conversions undefined and the device's cvt instructions saturate, so both builds convert
+// through these.
+SWB_HD int32_t trunc_i32(double v) {
+  return (v > -2147483649.0 && v < 2147483648.0) ? (int32_t)v : INT32_MIN;
+}
+SWB_HD int64_t trunc_i64(double v) {
+  return (v >= -9223372036854775808.0 && v < 9223372036854775808.0) ? (int64_t)v : INT64_MIN;
+}
+// astype(np.uint64): values from 2^63 up are converted less 2^63, and the top bit set again
+SWB_HD uint64_t trunc_u64(double v) {
+  return v >= 9223372036854775808.0
+             ? (uint64_t)trunc_i64(v - 9223372036854775808.0) ^ 0x8000000000000000ULL
+             : (uint64_t)trunc_i64(v);
+}
+// astype(np.uint8) of a float: through int32, so -153.2 gives 103 and anything beyond int32 gives 0
+SWB_HD uint8_t float_to_u8(double v) { return (uint8_t)trunc_i32(v); }
+
+SWB_HD bool small_int(int k) {
+  return k == SWB_FT_I8 || k == SWB_FT_U8 || k == SWB_FT_I16 || k == SWB_FT_U16;
+}
 
 // value (numpy scalar of kind `vk`) against a constant of kind `ck` (a Python float or int, or a
 // numpy scalar), as NumPy compares them: a Python float or int meeting a float32 value is cast to
-// float32 (NEP 50), integers compare exactly, anything else in float64.  Returns -1, 0 or 1;
-// 2 if the two do not compare (a shape name against a number).
+// float32 (NEP 50), anything else compares exactly -- in float64, which holds every value a draw
+// can have and every constant compile_program accepts (it refuses integers float64 cannot hold).
+// Returns -1, 0 or 1; 2 if the two do not compare (a shape name against a number).
 SWB_HD int compare(double v, int vk, double c, int ck) {
   if (vk == SWB_FT_SHAPE || ck == SWB_FT_SHAPE)
     return (vk == ck) ? (v == c ? 0 : (v < c ? -1 : 1)) : 2;
   if (vk == SWB_FT_F32 && (ck == SWB_FT_PYFLOAT || ck == SWB_FT_PYINT || ck == SWB_FT_F32)) {
     const float a = (float)v, b = (float)c;
-    return a == b ? 0 : (a < b ? -1 : 1);
-  }
-  if (is_int_like(vk) && is_int_like(ck)) {
-    const int64_t a = (int64_t)v, b = (int64_t)c;
     return a == b ? 0 : (a < b ? -1 : 1);
   }
   return v == c ? 0 : (v < c ? -1 : 1);
@@ -104,10 +121,14 @@ SWB_HD int compare(double v, int vk, double c, int ck) {
 // .astype(dtype) of a float64 draw: integer dtypes truncate (the program's ranges fit the type;
 // a draw that rounds up to `hi` wraps as the conversion through int64 does)
 SWB_HD double cast_draw(double v, int kind) {
-  const int64_t i = (int64_t)v;
   switch (kind) {
     case SWB_FT_F32: return (double)(float)v;
     case SWB_FT_F64: return v;
+    case SWB_FT_U64: return (double)trunc_u64(v);
+    default: break;
+  }
+  const int64_t i = trunc_i64(v);
+  switch (kind) {
     case SWB_FT_I8: return (double)(int8_t)i;
     case SWB_FT_I16: return (double)(int16_t)i;
     case SWB_FT_I32: return (double)(int32_t)i;
@@ -125,7 +146,7 @@ struct Sprite {
 
 SWB_HD void set_defaults(Sprite &s) {
   // Sprite.__init__ defaults (sprite.py), typed as scene._default_column types them
-  const double v[kFactors] = {0.5, 0.5, 1.0 /* square */, 0.0, 0.1, 0.0, 0.0, 0.0, 0.0, 0.0};
+  const double v[kFactors] = {0.5, 0.5, 2.0 /* ShapeType.square */, 0.0, 0.1, 0.0, 0.0, 0.0, 0.0, 0.0};
   const uint8_t k[kFactors] = {SWB_FT_F64, SWB_FT_F64, SWB_FT_SHAPE, SWB_FT_I64, SWB_FT_F64,
                                SWB_FT_I64, SWB_FT_I64, SWB_FT_I64, SWB_FT_F64, SWB_FT_F64};
   for (int f = 0; f < kFactors; ++f) { s.val[f] = v[f]; s.kind[f] = k[f]; }
@@ -289,7 +310,7 @@ SWB_HD void hsv_to_rgb(T h, T s, T v, uint8_t out[3]) {
   // colorsys.hsv_to_rgb, then (255 * rgb).astype(uint8) (color_maps.py, swb_host_pack.c)
   const T one = (T)1.0, six = (T)6.0, scale = (T)255;
   const T h6 = h * six;
-  const int64_t it = (int64_t)h6;
+  const int64_t it = trunc_i64((double)h6);
   const T f = h6 - (T)it;
   const T sf = s * f;
   const T pp = v * (one - s);
@@ -309,9 +330,9 @@ SWB_HD void hsv_to_rgb(T h, T s, T v, uint8_t out[3]) {
     default: r = v; g = pp; b = q; break;
   }
   if (s == (T)0) { r = v; g = v; b = v; }
-  out[0] = (uint8_t)(scale * r);
-  out[1] = (uint8_t)(scale * g);
-  out[2] = (uint8_t)(scale * b);
+  out[0] = float_to_u8((double)(scale * r));
+  out[1] = float_to_u8((double)(scale * g));
+  out[2] = float_to_u8((double)(scale * b));
 }
 
 // One packed slot, the fields of swb_scene_soa.
@@ -332,22 +353,26 @@ SWB_HD void pack_sprite(const swb_scene_program &p, const Sprite &s, Packed &o) 
   double c, sn;
   angle_cs(p, s.val[F_ANGLE], c, sn);
   o.m00 = c * scale; o.m01 = (-sn) * scale; o.m10 = sn * scale; o.m11 = c * scale;
-  // the filters see the columns scene._full_columns builds: x and y become float64 unless both
-  // are float32 (np.array([x, y]) promotes)
+  // the filters see the sprite's position, np.array([x, y]): float32 if one is float32 and the
+  // other float32 or an integer float32 holds (at most 16 bits), float64 (or an integer dtype,
+  // which compares alike) otherwise
+  const int kx = s.kind[F_X], ky = s.kind[F_Y];
+  const bool pos_f32 = (kx == SWB_FT_F32 && (ky == SWB_FT_F32 || small_int(ky))) ||
+                       (ky == SWB_FT_F32 && small_int(kx));
   Sprite t = s;
-  if (!(s.kind[F_X] == SWB_FT_F32 && s.kind[F_Y] == SWB_FT_F32)) t.kind[F_X] = t.kind[F_Y] = SWB_FT_F64;
+  t.kind[F_X] = t.kind[F_Y] = (uint8_t)(pos_f32 ? SWB_FT_F32 : SWB_FT_F64);
   uint32_t member = 0;
   for (int f = 0; f < p.n_filters; ++f)
     if (contains(p, p.filter_pc[f], t)) member |= 1u << f;
   o.member = member;
   o.shape = (uint8_t)s.val[F_SHAPE];
-  o.pos_f32 = s.kind[F_X] == SWB_FT_F32 && s.kind[F_Y] == SWB_FT_F32;
+  o.pos_f32 = pos_f32;
   const double c0 = s.val[F_C0], c1 = s.val[F_C1], c2 = s.val[F_C2];
   if (p.color_mode == SWB_COLOR_HSV) {
     if (s.kind[F_C0] == SWB_FT_F32) hsv_to_rgb<float>((float)c0, (float)c1, (float)c2, o.rgb);
     else hsv_to_rgb<double>(c0, c1, c2, o.rgb);
   } else {  // RGB values: through int64, then uint8 with wraparound
-    o.rgb[0] = (uint8_t)(int64_t)c0; o.rgb[1] = (uint8_t)(int64_t)c1; o.rgb[2] = (uint8_t)(int64_t)c2;
+    o.rgb[0] = (uint8_t)trunc_i64(c0); o.rgb[1] = (uint8_t)trunc_i64(c1); o.rgb[2] = (uint8_t)trunc_i64(c2);
   }
   o.factors[0] = (float)scale; o.factors[1] = (float)s.val[F_ANGLE];
   o.factors[2] = (float)c0; o.factors[3] = (float)c1; o.factors[4] = (float)c2;

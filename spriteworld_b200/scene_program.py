@@ -101,6 +101,9 @@ def _const_kind(v, what):
     kind = _NP_KINDS.get(v.dtype)
     if kind is None:
       _refuse('%s %r of dtype %s' % (what, v, v.dtype))
+    if kind in _INT_KINDS and int(float(v)) != int(v):
+      _refuse('%s %r: an integer float64 cannot hold exactly (the sampler compares in float64)'
+              % (what, v))
     return kind
   if isinstance(v, float):
     return FT_PYFLOAT
