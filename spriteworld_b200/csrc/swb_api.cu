@@ -160,7 +160,7 @@ int upload_axis(swb_raster *r, const AxisHost &h, AxisTables *d) {
 extern "C" {
 
 const char *swb_last_error(void) { return g_error.c_str(); }
-int swb_version(void) { return 7; }
+int swb_version(void) { return 8; }
 int swb_sizeof_config(void) { return (int)sizeof(swb_config); }
 int swb_sizeof_task_node(void) { return (int)sizeof(swb_task_node); }
 
@@ -583,16 +583,19 @@ void swb_raster_destroy(swb_raster *r) {
 // made a programmatic dependent launch: the render CTAs may become resident and load their tables
 // while the step kernel's last CTAs run (step_kernel signals griddepcontrol.launch_dependents at
 // once), and wait (griddepcontrol.wait, after their set-up) until the step grid has completed and
-// its writes are visible.
+// its writes are visible.  With recs.rec set, the items are records [0, env_count) of recs instead
+// of live envs (swb_render_states; one target, env_base 0, status [env_count]).
 static int enqueue_render(swb_engine *eng, const swb_raster *r, const RenderLayout &L,
                           const RenderTargets &targets, uint8_t *status, cudaStream_t stream,
-                          int env_base, int env_count, bool after_step) {
+                          int env_base, int env_count, bool after_step,
+                          const RenderRecords &recs = RenderRecords{nullptr, 0}) {
   RasterDev rd = r->rd;
   rd.max_spans = L.M;
   // the wide instantiation only for rasters whose tables the narrow one was not compiled for
   const bool wide = render_wide(rd);
-  auto kernel = targets.n > 1 ? (wide ? render_kernel<true, true> : render_kernel<true, false>)
-                              : (wide ? render_kernel<false, true> : render_kernel<false, false>);
+  auto kernel = recs.rec ? (wide ? render_kernel<false, true, true> : render_kernel<false, false, true>)
+                : targets.n > 1 ? (wide ? render_kernel<true, true, false> : render_kernel<true, false, false>)
+                                : (wide ? render_kernel<false, true, false> : render_kernel<false, false, false>);
   CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, L.total));
   DevState st = eng->st;
   st.render_status = status;
@@ -610,7 +613,8 @@ static int enqueue_render(swb_engine *eng, const swb_raster *r, const RenderLayo
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   lc.attrs = attr;
   lc.numAttrs = after_step ? 1 : 0;
-  CUDA_TRY(cudaLaunchKernelEx(&lc, kernel, st, rd, L, targets, env_base, n_items, eng->d_work, eng->work_base));
+  CUDA_TRY(cudaLaunchKernelEx(&lc, kernel, st, rd, L, targets, env_base, n_items, eng->d_work, eng->work_base,
+                              recs));
   eng->work_base += (unsigned)(n_items + grid);  // every CTA's last claim fails
   eng->launches++;
   CUDA_TRY(cudaGetLastError());
@@ -1120,6 +1124,35 @@ int swb_rollout_states(swb_engine *eng, const void *roots, int32_t n_roots, uint
                          RolloutRecords{static_cast<const unsigned char *>(roots),
                                         static_cast<unsigned char *>(leaves), (size_t)rb, n_roots},
                          static_cast<cudaStream_t>(stream));
+}
+
+int swb_render_states(swb_engine *eng, swb_raster *r, const void *records, int32_t n, uint64_t records_bytes,
+                      int32_t span_class, uint8_t *frames, uint8_t *status, void *stream_) {
+  static const char fn[] = "swb_render_states";
+  if (!eng || !r) return fail("%s: null engine or raster", fn);
+  if (n < 0) return fail("%s: n = %d", fn, n);
+  if (n == 0) return 0;
+  if (!records) return fail("%s: null records", fn);
+  if (check_record_buffer(eng, fn, "records", records, records_bytes, n)) return 1;
+  if (span_class != 1 && span_class != 4) return fail("%s: span_class must be 1 or 4, got %d", fn, span_class);
+  if (!frames || !status) return fail("%s: null frames or status", fn);
+  const RasterDev &rd = r->rd;
+  const uint64_t rb = RecordLayout(eng->st.S).bytes();
+  const uint64_t r0 = reinterpret_cast<uintptr_t>(records), r1 = r0 + (uint64_t)n * rb;
+  const uint64_t f0 = reinterpret_cast<uintptr_t>(frames), s0 = reinterpret_cast<uintptr_t>(status);
+  if (f0 < r1 && r0 < f0 + (uint64_t)n * rd.H * rd.W * 3) return fail("%s: the frames overlap the records", fn);
+  if (s0 < r1 && r0 < s0 + (uint64_t)n) return fail("%s: the status overlaps the records", fn);
+  // n_items and the kernel's item index are int
+  if ((int64_t)n * rd.n_bands > INT32_MAX)
+    return fail("%s: n = %d records of %d bands each exceed 2^31 - 1 render items", fn, n, rd.n_bands);
+  // read-only: records of stars or spokes get the concave span tables for this launch only
+  std::optional<RenderLayout> plan;
+  if (check_render(eng, r, std::max(eng->max_spans, (int)span_class), &plan)) return 1;
+  CUDA_TRY(cudaSetDevice(eng->device));
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  CUDA_TRY(cudaMemsetAsync(status, 0, (size_t)n, stream));
+  return enqueue_render(eng, r, *plan, RenderTargets{{frames}, 1, 0, 0}, status, stream, 0, n, false,
+                        RenderRecords{static_cast<const unsigned char *>(records), (size_t)rb});
 }
 
 int swb_env_ids_status_pointer(swb_engine *eng, swb_ids_status **status) {

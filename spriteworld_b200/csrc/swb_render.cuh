@@ -41,6 +41,7 @@
 #include <climits>
 
 #include "swb_device.cuh"
+#include "swb_states.cuh"
 
 namespace swb {
 
@@ -73,6 +74,13 @@ struct RenderTargets {
   int n;
   int env_offset;
   int self;  // index of this rank's own buffer in dst
+};
+
+// The env records render_kernel<., ., true> draws (swb_render_states): item e is record e, at
+// rec + e * record_bytes.  The live-env instantiations do not read it.
+struct RenderRecords {
+  const unsigned char *rec;
+  size_t record_bytes;
 };
 
 // Whether a raster needs render_kernel<., true>: tables beyond those of anti_aliasing <= 5
@@ -265,11 +273,17 @@ __constant__ uint32_t c_prmt_insert[4] = {0x3214u, 0x3240u, 0x3410u, 0x4210u};  
 // V_KS_NARROW compiled in: the code of the aa <= 5 path does not change with the wide one
 // (reading the stride and tile blocks at run time cost it 0.4 % at C2).  Wide rasters' staged
 // frames and segment tables leave room for few CTAs per SM anyway, so their register budget is
-// set for R_CTAS_PER_SM_WIDE
-template <bool kPeers, bool kWide>
+// set for R_CTAS_PER_SM_WIDE.
+// kRecords: item e is record e of recs (swb_render_states), not live env e: phase A reads the
+// record's pool-entry fields and live positions (RecordLayout) instead of the pool entry at
+// (e, cursor[e]), with shape ids sanitised as a load sanitises them; frame e and status byte e are
+// the record's.  Nothing indexed by env is read, so n may exceed E.  No peer variant.
+template <bool kPeers, bool kWide, bool kRecords>
 __global__ void __launch_bounds__(R_THREADS, kWide ? R_CTAS_PER_SM_WIDE : R_CTAS_PER_SM)
 render_kernel(DevState st, RasterDev rd, const RenderLayout L, const RenderTargets targets,
-              int env_base, int n_items, unsigned *work_counter, unsigned work_base) {
+              int env_base, int n_items, unsigned *work_counter, unsigned work_base,
+              const RenderRecords recs) {
+  static_assert(!(kPeers && kRecords), "records render into one buffer");
   unsigned char *const smem = g_render_smem;
   const int tid = threadIdx.x;
   const int S = st.S;
@@ -357,7 +371,8 @@ render_kernel(DevState st, RasterDev rd, const RenderLayout L, const RenderTarge
   // vertices come by shuffle, extents by warp reductions, "edges that share a start row" by
   // match_any; nothing leaves the warp until the barrier that ends the phase.
   if (tid == 0) s_overflow = 0;
-  const int cur = st.cursor[e];
+  const int cur = kRecords ? 0 : st.cursor[e];
+  const unsigned char *const rec = kRecords ? recs.rec + (size_t)e * recs.record_bytes : nullptr;
   // per-frame tables first: their loads overlap the sprite records' dependent loads below
 #pragma unroll 1
   for (int i = tid; i < (n_rows + 3) / 4; i += R_THREADS) reinterpret_cast<uint32_t *>(s_nseg)[i] = 0u;
@@ -369,13 +384,18 @@ render_kernel(DevState st, RasterDev rd, const RenderLayout L, const RenderTarge
     band_loaded = band;
   }
   for (int s = warp; s < S; s += NWARP) {
-    // sprite record of this env's current scene (warp-uniform loads)
+    // sprite record of this env's current scene, or slot s of record e (warp-uniform loads)
     const int scene = (e * st.K + cur) * S + s;
-    const int shape = st.p_shape[scene];
-    const uint32_t col = st.p_rgb[scene];
-    const double px = st.pos_x[e * S + s], py = st.pos_y[e * S + s];
-    const double m00 = st.p_m00[scene], m01 = st.p_m01[scene];
-    const double m10 = st.p_m10[scene], m11 = st.p_m11[scene];
+    const RecordLayout rl(S);
+    const double *const f64 = reinterpret_cast<const double *>(rec);  // [10][S], see RecordLayout
+    const int shape = kRecords ? sanitize_shape(st, rec[rl.shape() + s]) : st.p_shape[scene];
+    const uint32_t col = kRecords ? reinterpret_cast<const uint32_t *>(rec + rl.rgb())[s] : st.p_rgb[scene];
+    const double px = kRecords ? f64[8 * S + s] : st.pos_x[e * S + s];
+    const double py = kRecords ? f64[9 * S + s] : st.pos_y[e * S + s];
+    const double m00 = kRecords ? f64[2 * S + s] : st.p_m00[scene];
+    const double m01 = kRecords ? f64[3 * S + s] : st.p_m01[scene];
+    const double m10 = kRecords ? f64[4 * S + s] : st.p_m10[scene];
+    const double m11 = kRecords ? f64[5 * S + s] : st.p_m11[scene];
     const int nv = shape ? st.shape_n[shape] : 0;
     const int t = s * EV + lane;
     // integer canvas vertex of this lane

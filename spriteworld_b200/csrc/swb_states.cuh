@@ -90,8 +90,13 @@ __device__ __forceinline__ void write_state(const DevState &st, int e, int s, co
   }
 }
 
-// A shape id without a vertex table (a record that swb_save_envs did not write) loads as an empty
-// slot, so that no kernel indexes the shape table with it.
+// A shape id without a vertex table (a record that swb_save_envs did not write) is an empty slot
+// (0), so that no kernel indexes the shape table with it.  read_record and the record render path
+// (render_kernel<., ., true>) both take a record's shape ids through this.
+__device__ __forceinline__ int sanitize_shape(const DevState &st, int shape) {
+  return shape < SWB_NUM_SHAPES && st.shape_n[shape] >= 3 ? shape : 0;
+}
+
 __device__ __forceinline__ SlotRecord read_record(const DevState &st, const unsigned char *rec, int s) {
   const int S = st.S;
   const RecordLayout L(S);
@@ -103,8 +108,7 @@ __device__ __forceinline__ SlotRecord read_record(const DevState &st, const unsi
   r.rgb = reinterpret_cast<const uint32_t *>(rec + L.rgb())[s];
 #pragma unroll
   for (int f = 0; f < 5; ++f) r.factors[f] = reinterpret_cast<const float *>(rec + L.factors())[f * S + s];
-  const int shape = rec[L.shape() + s];
-  r.shape = shape < SWB_NUM_SHAPES && st.shape_n[shape] >= 3 ? shape : 0;
+  r.shape = sanitize_shape(st, rec[L.shape() + s]);
   r.pos_f32 = rec[L.pos_f32() + s];
   r.step_count = *reinterpret_cast<const int32_t *>(rec + L.step_count());
   r.reset_next = rec[L.reset_next()];

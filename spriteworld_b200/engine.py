@@ -398,6 +398,31 @@ class Engine(object):
                                        self._stream()))
     return frames
 
+  def render_states(self, raster, states, frames=None, status=None):
+    """The frames of env records without loading them (swb_render_states): frame i is what
+    render() would draw after load_envs of record i, status[i] its render status
+    (ENV_SPAN_OVERFLOW).  `states`: EnvStates of any n records of this engine's configuration.
+    Returns (frames (n, H, W, 3) uint8, status (n,) uint8) on this device, new unless given.  One
+    launch on the current stream; no env, frame buffer, render_status() or span class changes."""
+    if not isinstance(states, EnvStates):
+      raise ValueError('states must be EnvStates, got %s' % type(states).__name__)
+    n = len(states)
+    self.check_states(states, n)
+    if frames is None:
+      frames = torch.empty((n, raster.height, raster.width, 3), dtype=torch.uint8, device=self.device)
+    self._check_frames(frames, raster, n)
+    if status is None:
+      status = torch.empty(n, dtype=torch.uint8, device=self.device)
+    if (not isinstance(status, torch.Tensor) or status.dtype != torch.uint8 or status.device != self.device
+        or tuple(status.shape) != (n,) or not status.is_contiguous()):
+      raise ValueError('status must be a contiguous uint8 tensor of shape (%d,) on %s, got %s' % (
+          n, self.device, _describe(status)))
+    _native.check(self._lib.swb_render_states(
+        self._h, raster._h, ctypes.c_void_p(states.data.data_ptr()), n, states.data.numel(),
+        states.span_class, ctypes.c_void_p(frames.data_ptr()), ctypes.c_void_p(status.data_ptr()),
+        self._stream()))
+    return frames, status
+
   def render_status(self):
     """Zero-copy uint8 (E,) view of the per-env status of the last render() (ENV_SPAN_OVERFLOW)."""
     if getattr(self, '_render_status_view', None) is None:
@@ -903,6 +928,17 @@ SHAPE_IDS = {
     'triangle': 1, 'square': 2, 'pentagon': 3, 'hexagon': 4, 'octagon': 5, 'circle': 6,
     'star_4': 7, 'star_5': 8, 'star_6': 9, 'spoke_4': 10, 'spoke_5': 11, 'spoke_6': 12,
 }
+
+
+def shape_id_table(shapes):
+  """uint8 (256,) NumPy array: id -> the id an env record's shape id `id` loads as (swb_load_envs),
+  i.e. itself for a shape with a vertex table of at least 3 vertices in `shapes`, else 0 (an
+  empty slot)."""
+  table = np.zeros(256, np.uint8)
+  for name, sid in SHAPE_IDS.items():
+    if len(shapes[name]) >= 3:
+      table[sid] = sid
+  return table
 
 
 def fill_shapes(cfg, shapes):

@@ -433,9 +433,15 @@ class BatchedEnvironment(object):
 
   _FACTOR_COLUMNS = {'scale': 0, 'angle': 1, 'c0': 2, 'c1': 3, 'c2': 4}   # of the pool's `factors`
 
-  def factor_tensors(self, factors):
+  def factor_tensors(self, factors, states=None):
     """dict factor name -> float32 (n_envs, n_slots) tensor of the current scenes + 'mask': x and y
-    are the live positions, the rest is read from the pool entry each env is on."""
+    are the live positions, the rest is read from the pool entry each env is on.
+
+    With `states` (EnvStates of n records) the same dict of (n, n_slots) tensors is read from the
+    records on their device, without a host synchronisation: what factor_tensors() would return
+    after load_envs(states), shape ids sanitised as a load sanitises them."""
+    if states is not None:
+      return self._record_factor_tensors(factors, states)
     eng = self._engine
     live, pool, K = eng.state_tensors(), eng.pool_tensors(), eng.pool_depth
     entry = torch.arange(0, self.n_envs * K, K, device=eng.device) + live['cursor']   # env * K + cursor
@@ -455,6 +461,28 @@ class BatchedEnvironment(object):
       else:
         columns = at('factors') if columns is None else columns
         out[name] = columns[..., self._FACTOR_COLUMNS[name]]
+    out['mask'] = shape > 0
+    return out
+
+  def _record_factor_tensors(self, factors, states):
+    if not isinstance(states, engine_lib.EnvStates):
+      raise ValueError('states must be EnvStates, got %s' % type(states).__name__)
+    self._engine.check_states(states, len(states))
+    fields, dev = states.fields(), states.data.device
+    table = getattr(self, '_shape_ids', None)
+    if table is None or table.device != dev:
+      table = self._shape_ids = torch.from_numpy(engine_lib.shape_id_table(constants.SHAPES)).to(dev)
+    shape = table[fields['shape'].long()]
+    out = collections.OrderedDict()
+    for name in factors:
+      if name in ('x', 'y'):
+        out[name] = fields['pos_' + name].to(torch.float32)
+      elif name in ('x_vel', 'y_vel'):
+        out[name] = fields['v' + name[0]].to(torch.float32)
+      elif name == 'shape':
+        out[name] = shape.to(torch.float32)
+      else:
+        out[name] = fields['factors'][:, self._FACTOR_COLUMNS[name]].clone()
     out['mask'] = shape > 0
     return out
 
@@ -743,6 +771,35 @@ class BatchedEnvironment(object):
     for name, r in self._rasters.items():
       out[name] = self._engine.render(r, self._frames[name])
     return out
+
+  def observe(self, states):
+    """The observations of env records without loading them: (observation, status) for EnvStates
+    `states` of n records, observation an OrderedDict in renderer order of what step() would
+    observe for envs that load_envs(states) had loaded -- PILRenderer frames as new uint8
+    (n, H, W, 3) tensors (one render launch per raster; never this environment's own frame
+    buffers), SpriteFactors dicts of (n, n_slots) tensors -- and status uint8 (n,), the OR over the
+    rasters of their render status (_native.ENV_SPAN_OVERFLOW).
+
+    Enqueued on the current stream without a host synchronisation.  Read-only: no env, scene ring,
+    frame buffer or `rng` changes, and nothing counts against the ring's refill.  A renderer
+    without a record form (Success: success is a task evaluation, which rollout and expand
+    report) raises NotImplementedError before anything is enqueued."""
+    missing = [name for name, r in self._other.items() if not hasattr(r, 'render_states')]
+    if missing:
+      raise NotImplementedError('renderers %s have no record form: observe() cannot render them' % missing)
+    eng = self._engine
+    eng.check_states(states, len(states))
+    status, obs = None, collections.OrderedDict()
+    for name in self._renderers:
+      if name in self._rasters:
+        frames, st = eng.render_states(self._rasters[name], states)
+        obs[name] = frames
+        status = st if status is None else status.bitwise_or_(st)
+      else:
+        obs[name] = self._other[name].render_states(self, states)
+    if status is None:
+      status = torch.zeros(len(states), dtype=torch.uint8, device=eng.device)
+    return obs, status
 
   def observation_spec(self):
     """Per-env specs (the leading n_envs axis of the batched observations is not included)."""

@@ -57,6 +57,12 @@ class SpriteFactors(abstract_renderer.AbstractRenderer):
     (slot occupied).  Empty slots are padded at the front (the last slot is top-most)."""
     return env.factor_tensors(self._factors)
 
+  def render_states(self, env, states):
+    """render_batch of env records (EnvStates) instead of the live envs: dict factor -> float32
+    (n, n_slots) device tensor plus 'mask', what render_batch would return after
+    env.load_envs(states)."""
+    return env.factor_tensors(self._factors, states)
+
   def batch_observation_spec(self, env):
     n = env.engine.n_slots
     spec = {f: specs.Array(shape=(n,), dtype=np.float32) for f in self._factors}

@@ -101,6 +101,12 @@ def device_checked_records(torch):
   torch.cuda.synchronize()
   print('record rollouts: %d roots, %d leaves, %d kernel launches'
         % (len(roots), len(res.leaves), eng.launch_count()), flush=True)
+  # frames of those leaves (more records than envs) and of zero records
+  frames, status = eng.render_states(raster, res.leaves)
+  eng.render_states(raster, res.leaves.take(torch.tensor([-1, 0, len(res.leaves)], device='cuda')))
+  torch.cuda.synchronize()
+  print('record renders: %d frames, %d overflowed, %d kernel launches'
+        % (len(frames), int(status.bool().sum()), eng.launch_count()), flush=True)
   raster.close()
   eng.close()
 
