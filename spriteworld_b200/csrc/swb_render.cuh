@@ -613,13 +613,16 @@ render_kernel(DevState st, RasterDev rd, const RenderLayout L, const RenderTarge
       }
       uint32_t *dst = s_spans + ((size_t)(s - s_lo) * n_rows + (y - row_b0)) * M;
       const int nh = s_nh[s];
-      if (M == 1) {
+      bool several = M > 1;
+      if (!several) {
         // convex shapes: every span of the row merges into one [lo, hi] (kept in registers)
         int lo = 1, hi = 0;
+        // a second, disjoint span: recount the row with the list below, since a horizontal edge
+        // merged after the crossing spans can still join them (flat convex sprites on wide canvases)
         auto merge1 = [&](int xs, int xe) {
           if (lo > hi) { lo = xs; hi = xe; }
           else if (xs <= hi + 1 && lo <= xe + 1) { lo = min(lo, xs); hi = max(hi, xe); }
-          else ovf = true;  // a second, disjoint span: the engine was sized for convex shapes
+          else several = true;
         };
         int x_pos = 0;
         for (int i = 1; i < j; i += 2) {
@@ -638,7 +641,9 @@ render_kernel(DevState st, RasterDev rd, const RenderLayout L, const RenderTarge
           if (hl[0] == y) merge1(hl[1], hl[2]);
         }
         dst[0] = lo <= hi ? ((uint32_t)lo | ((uint32_t)hi << 16)) : 0x0000FFFFu;
-      } else {
+      }
+      if (several) {
+        // several spans per sprite row, merged in any order; more than M of them overflow
         int lxs[MAX_ROW_SPANS], lxe[MAX_ROW_SPANS];
         int n = 0;
         int x_pos = 0;

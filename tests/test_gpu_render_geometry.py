@@ -18,7 +18,7 @@ import numpy as np
 import pytest
 
 from oracle import oracle
-from tests import fixtures
+from tests import fixtures, span_overflow
 
 SENTINEL = 0xA5
 GUARD = 256                 # sentinel bytes on each side of a frame buffer; a multiple of 16
@@ -26,7 +26,6 @@ BAND_ROWS = 64              # swb_raster_create: output rows per band
 R_CTAS_PER_SM = 5           # render CTAs resident per SM (SWB_RENDER_CTAS)
 R_WARPS = 8                 # warps per render CTA: phase A gives each warp S / 8 sprites
 H100_SMS = 132
-SEGCAP_CONCAVE = 16         # visible segments per canvas row once a star / spoke is uploaded
 CONVEX = tuple(range(1, 7))         # triangle .. circle
 CONCAVE = tuple(range(7, 13))       # star_4 .. spoke_6
 
@@ -73,12 +72,8 @@ CASES = [
 REFUSED = {'w8h819a5', 'w1h101a2'}
 # cases whose segment table is capped at 16 although every shape is convex
 SEGCAP_16 = {'w550h64a5', 'w550h64a5_edges'}
-# known kernel defects the sweep has found and that are not fixed yet
-KNOWN_DEFECTS = {
-    'w550h64a5_edges': pytest.mark.xfail(strict=True, reason=(
-        'env 1 is flagged SWB_ENV_SPAN_OVERFLOW although no canvas row has more than 4 visible '
-        'pieces, no sprite row more than 6 crossings or 1 span: cause not found')),
-}
+# known kernel defects the sweep has found and that are not fixed yet (case id -> xfail mark)
+KNOWN_DEFECTS = {}
 
 
 def _n_envs(case, n_sms):
@@ -407,19 +402,23 @@ def _assert_guards(big, lo, n_bytes, where):
 
 
 class Sweep(object):
-  """One case: the engine with its scenes uploaded, and the oracle's frames of every env
-  (computed once, on first use)."""
+  """One case: the engine with its scenes uploaded, and the oracle's frames of every env and
+  the restated phase-B maxima (tests/span_overflow.py) that decide its status (each computed
+  once, on first use).  `arrs` and `shapes`: scenes and shape table other than the case's own."""
 
-  def __init__(self, case, n_sms):
+  def __init__(self, case, n_sms, arrs=None, shapes=None):
     import torch
     from spriteworld_b200 import constants, engine, scene
     self.case = case
     cid, self.W, self.H, self.aa, self.bg, self.S, _, concave, kind = case
     self.E = E = _n_envs(case, n_sms)
-    arrs = case_arrays(case, E)
-    self.segcap = SEGCAP_CONCAVE if concave or cid in SEGCAP_16 else 2 * self.S - 1
+    if arrs is None:
+      arrs = case_arrays(case, E)
+    shapes = constants.SHAPES if shapes is None else shapes
+    self.M = 4 if concave else 1
+    self.segcap = span_overflow.segcap(self.S, self.M, exact=cid not in SEGCAP_16)
     self.eng = engine.Engine(E, self.S, 1, dict(kind='select_move', scale=1.0),
-                             [dict(kind='no_reward')], constants.SHAPES, keep_in_frame=False)
+                             [dict(kind='no_reward')], shapes, keep_in_frame=False)
     b = scene.batch_from_factor_arrays(
         arrs['x'], arrs['y'], arrs['pos_f32'], arrs['shape'], arrs['angle'], arrs['scale'],
         arrs['c0'], arrs['c1'], arrs['c2'], arrs['vx'], arrs['vy'], arrs['member'], arrs['rgb'])
@@ -428,30 +427,41 @@ class Sweep(object):
                           reset_next=np.zeros(E))
     self.pos = (b['x'].copy(), b['y'].copy())
     self.rec = fixtures.records_from_arrays(arrs)
-    self.shapes = constants.SHAPES
-    self.tab = oracle.shape_table(constants.SHAPES)
+    self.shapes = shapes
+    self.tab = oracle.shape_table(shapes)
     self.rc = oracle.raster_cfg(self.W, self.H, self.aa, self.bg)
-    self._ref, self._pieces = {}, {}
+    self._ref, self._maxima = {}, {}
     self.actions = torch.full((E, 4), 0.5, dtype=torch.float32, device=self.eng.device)
 
   def ref(self, e):
+    """The oracle's frame of env e, and the restated maxima of phase B's capacities."""
     if e not in self._ref:
       self._ref[e] = oracle.render(self.rc, self.tab, self.rec[e])
-      self._pieces[e] = visible_pieces(self.W, self.H, self.aa, self.rec[e], self.shapes)
-    return self._ref[e], self._pieces[e]
+      self._maxima[e] = span_overflow.restate(self.W, self.H, self.aa, self.rec[e], self.shapes,
+                                              self.M)
+    return self._ref[e], self._maxima[e]
+
+  def overflow(self, e):
+    """The conditions that must flag env e under this sweep's span class and segment table."""
+    return span_overflow.conditions(self.ref(e)[1], self.M, self.segcap)
+
+  def within(self, e):
+    return not self.overflow(e)
 
   def check(self, frames, status, where):
-    """frames: (E, H, W, 3) uint8 numpy; status: (E,) uint8 numpy."""
+    """frames: (E, H, W, 3) uint8 numpy; status: (E,) uint8 numpy.  Every env is flagged
+    exactly when the restatement says so; every other env has status 0 and the oracle's frame."""
     from spriteworld_b200 import _native
     over = (status & _native.ENV_SPAN_OVERFLOW) != 0
     n_exact = 0
     for e in range(self.E):
-      ref, pieces = self.ref(int(e))
-      if pieces > self.segcap:
-        # beyond the segment table: the env must be flagged, its frame is not defined
-        assert over[e], (where, int(e), pieces, 'overflow not flagged')
-        continue
-      assert status[e] == 0, (where, int(e), int(status[e]), pieces)
+      ref, maxima = self.ref(int(e))
+      want = self.overflow(int(e))
+      assert over[e] == bool(want), (where, int(e), 'status %d' % status[e], 'restated %s' % (want,),
+                                     span_overflow.describe(maxima, self.M, self.segcap))
+      if want:
+        continue    # beyond phase B's tables: the frame is not defined
+      assert status[e] == 0, (where, int(e), int(status[e]), maxima)
       diff = frames[e] != ref
       assert not diff.any(), (where, int(e), int(diff.sum()), np.argwhere(diff)[:4].tolist())
       n_exact += 1
@@ -535,7 +545,7 @@ def test_geometry_sweep(case):
     assert case[0] not in REFUSED, (case[0], 'rendered, but the table says it is refused')
     # the sweep must not pass by flagging envs: at least 90 % of them are within the segment
     # table, and every write-out path renders every one of those exactly
-    n_within = sum(sw.ref(e)[1] <= sw.segcap for e in range(sw.E))
+    n_within = sum(sw.within(e) for e in range(sw.E))
     assert n_within >= 0.9 * sw.E and n_exact == [n_within] * 5, (case[0], n_exact, n_within, sw.E)
     raster.close()
   finally:
@@ -551,7 +561,7 @@ def test_frames_at_odd_addresses(cid):
   case = [c for c in CASES if c[0] == cid][0]
   sw = Sweep(case, _n_sms())
   raster = engine.Raster(sw.eng, sw.W, sw.H, sw.aa, sw.bg)
-  n_within = sum(sw.ref(e)[1] <= sw.segcap for e in range(sw.E))
+  n_within = sum(sw.within(e) for e in range(sw.E))
   assert n_within > 0 and _run_modes(sw, raster, skew=1) == [n_within] * 5
   raster.close()
   sw.close()

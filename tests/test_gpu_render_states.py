@@ -27,11 +27,13 @@ class _Permuted(object):
   """Sweep.check's view of records `perm` of a Sweep: frame i is env perm[i]'s."""
 
   def __init__(self, sw, perm):
-    self.sw, self.perm, self.E, self.segcap = sw, perm, len(perm), sw.segcap
+    self.sw, self.perm, self.E, self.M, self.segcap = sw, perm, len(perm), sw.M, sw.segcap
 
   def ref(self, i):
     return self.sw.ref(int(self.perm[i]))
 
+  overflow = geo.Sweep.overflow
+  within = geo.Sweep.within
   check = geo.Sweep.check
 
 
@@ -59,7 +61,7 @@ def _render_permuted(sw, raster):
     geo._assert_guards(sbig, slo, n, (sw.case[0], 'status', skew))
     n_exact.append(view.check(frames.cpu().numpy(), status.cpu().numpy(), (sw.case[0], 'records', skew)))
   assert sw.unmoved()
-  n_within = sum(view.ref(i)[1] <= view.segcap for i in range(n))
+  n_within = sum(view.within(i) for i in range(n))
   return n_exact, n_within
 
 

@@ -207,7 +207,7 @@ def test_wide_aa_sweep(case):
     sw.segcap = render_layout(W, H, aa, S, concave)[1]
     raster = engine.Raster(sw.eng, W, H, aa, bg)
     n_exact = geo._run_modes(sw, raster)
-    n_within = sum(sw.ref(e)[1] <= sw.segcap for e in range(sw.E))
+    n_within = sum(sw.within(e) for e in range(sw.E))
     assert n_within >= 0.9 * sw.E and n_exact == [n_within] * 5, (cid, n_exact, n_within, sw.E)
     raster.close()
   finally:
