@@ -138,6 +138,10 @@ def load():
   L.swb_refill_device.argtypes = [vp, vp]
   L.swb_pool_pointers.argtypes = [vp, vp] + [ctypes.POINTER(vp)] * 5
   L.swb_sampler_pointers.argtypes = [vp, ctypes.POINTER(vp), ctypes.POINTER(vp)]
+  L.swb_engine_state_bytes.argtypes = [vp]
+  L.swb_engine_state_bytes.restype = ctypes.c_int64
+  L.swb_save_engine.argtypes = [vp, vp, ctypes.c_uint64, vp]
+  L.swb_load_engine.argtypes = [vp, vp, ctypes.c_uint64, vp]
   if L.swb_sizeof_config() != ctypes.sizeof(Config):
     raise NativeError('ABI mismatch: swb_config is %d bytes in the library, %d in the binding'
                       % (L.swb_sizeof_config(), ctypes.sizeof(Config)))
@@ -156,7 +160,8 @@ EXPORTS = (
     'swb_env_record_bytes', 'swb_save_envs', 'swb_load_envs', 'swb_copy_envs', 'swb_rollout_states', 'swb_render_states', 'swb_save_envs_dev',
     'swb_load_envs_dev', 'swb_copy_envs_dev', 'swb_env_ids_status_pointer', 'swb_launch_count',
     'swb_sampler_sizeof_program', 'swb_sampler_load', 'swb_sample_scenes', 'swb_refill_device',
-    'swb_sampler_pointers', 'swb_pool_pointers')
+    'swb_sampler_pointers', 'swb_pool_pointers', 'swb_engine_state_bytes', 'swb_save_engine',
+    'swb_load_engine')
 
 
 def check(rc):

@@ -1,5 +1,6 @@
 // C-ABI of the engine (include/spriteworld_b200.h): engine/raster lifetime, scene upload,
 // kernel launches.  No torch types; plain CUDA runtime.
+#include <algorithm>
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
@@ -97,6 +98,12 @@ struct swb_engine {
   cudaStream_t copy_stream = nullptr;  // D2H of frame chunks overlaps the render of the next chunk
   cudaEvent_t chunk_done[8] = {};
   cudaEvent_t copies_done = nullptr;
+  // pinned staging of swb_save_engine / swb_load_engine (grown on demand); `ckpt_done` is recorded
+  // after the copies of the last load, which read it after the call has returned
+  unsigned char *h_ckpt = nullptr;
+  size_t h_ckpt_bytes = 0;
+  cudaEvent_t ckpt_done = nullptr;
+  bool ckpt_in_flight = false;
 };
 
 struct swb_raster {
@@ -160,7 +167,7 @@ int upload_axis(swb_raster *r, const AxisHost &h, AxisTables *d) {
 extern "C" {
 
 const char *swb_last_error(void) { return g_error.c_str(); }
-int swb_version(void) { return 8; }
+int swb_version(void) { return 9; }
 int swb_sizeof_config(void) { return (int)sizeof(swb_config); }
 int swb_sizeof_task_node(void) { return (int)sizeof(swb_task_node); }
 
@@ -274,6 +281,9 @@ void swb_engine_destroy(swb_engine *eng) {
   if (eng->copy_stream) cudaStreamDestroy(eng->copy_stream);
   for (auto &ev : eng->chunk_done) if (ev) cudaEventDestroy(ev);
   if (eng->copies_done) cudaEventDestroy(eng->copies_done);
+  if (eng->ckpt_in_flight) cudaEventSynchronize(eng->ckpt_done);
+  if (eng->h_ckpt) cudaFreeHost(eng->h_ckpt);
+  if (eng->ckpt_done) cudaEventDestroy(eng->ckpt_done);
   delete eng;
 }
 
@@ -1349,6 +1359,232 @@ int swb_pool_pointers(swb_engine *eng, double **f64, uint32_t **member, uint8_t 
   for (int i = 0; i < 8; ++i) f64[i] = p[i];
   *member = st.p_member; *shape = st.p_shape; *pos_f32 = st.p_pos_f32; *rgb = st.p_rgb;
   *factors = st.p_factors;
+  return 0;
+}
+
+}  // extern "C"
+
+// Engine checkpoints (swb_save_engine / swb_load_engine): the header, then every field of
+// CkptLayout from a 16-byte boundary, in the order of the table in include/spriteworld_b200.h.
+namespace {
+
+constexpr char kCkptMagic[8] = {'S', 'W', 'B', 'C', 'K', 'P', 'T', '\0'};
+constexpr uint32_t kCkptVersion = 1;
+constexpr size_t kCkptFixed = 56;  // header bytes before the config signature
+
+struct CkptHeader {
+  char magic[8];
+  uint32_t version;
+  int32_t E, K, S, span_class, sampler;
+  uint64_t seed;
+  int64_t env_offset;
+  uint32_t config_bytes, zero;
+};
+static_assert(sizeof(CkptHeader) == kCkptFixed, "checkpoint header layout");
+
+size_t align16(size_t n) { return (n + 15) & ~(size_t)15; }
+
+struct CkptField {
+  const char *name;
+  void *dev;      // the engine's array (refilled_upto: null without a sampler)
+  size_t elem;    // bytes per element
+  size_t count;
+  size_t off = 0;
+  size_t bytes() const { return elem * count; }
+};
+
+struct CkptLayout {
+  enum { POS_X, POS_Y, CURSOR, STEP_COUNT, SCENE_SERIAL, RESET_NEXT, P_X, P_Y, P_M00, P_M01, P_M10, P_M11,
+         P_VX, P_VY, MEMBER, RGB, FACTORS, SHAPE, POS_F32, REFILLED_UPTO, N };
+  CkptField f[N];
+  size_t header = 0, total = 0;
+
+  explicit CkptLayout(const swb_engine *eng) {
+    const DevState &st = eng->st;
+    const size_t E = st.E, ES = E * st.S, EKS = ES * st.K;
+    const CkptField init[N] = {
+        {"pos_x", st.pos_x, 8, ES}, {"pos_y", st.pos_y, 8, ES},
+        {"cursor", st.cursor, 4, E}, {"step_count", st.step_count, 4, E},
+        {"scene_serial", st.scene_serial, 4, E}, {"reset_next", st.reset_next, 1, E},
+        {"x", st.p_x, 8, EKS}, {"y", st.p_y, 8, EKS}, {"m00", st.p_m00, 8, EKS}, {"m01", st.p_m01, 8, EKS},
+        {"m10", st.p_m10, 8, EKS}, {"m11", st.p_m11, 8, EKS}, {"vx", st.p_vx, 8, EKS}, {"vy", st.p_vy, 8, EKS},
+        {"member", st.p_member, 4, EKS}, {"rgb", st.p_rgb, 4, EKS}, {"factors", st.p_factors, 4, EKS * 5},
+        {"shape", st.p_shape, 1, EKS}, {"pos_f32", st.p_pos_f32, 1, EKS},
+        {"refilled_upto", eng->d_refilled_upto, 8, E}};
+    header = align16(kCkptFixed + sizeof(swb_config));
+    size_t o = header;
+    for (int i = 0; i < N; ++i) {
+      f[i] = init[i];
+      f[i].off = o;
+      o = align16(o + f[i].bytes());
+    }
+    total = o;
+  }
+};
+
+// The config signature of an engine: its swb_config with n_envs, pool_depth and device zeroed
+// (engine.config_signature).
+swb_config signature_of(const swb_engine *eng) {
+  swb_config sig;
+  memcpy(&sig, &eng->cfg, sizeof sig);
+  sig.n_envs = sig.pool_depth = sig.device = 0;
+  return sig;
+}
+
+// The engine's pinned checkpoint staging, at least `need` bytes, once the last load's copies from
+// it have finished.
+int ckpt_staging(swb_engine *eng, size_t need) {
+  if (eng->ckpt_in_flight) {
+    CUDA_TRY(cudaEventSynchronize(eng->ckpt_done));
+    eng->ckpt_in_flight = false;
+  }
+  if (!eng->ckpt_done) CUDA_TRY(cudaEventCreateWithFlags(&eng->ckpt_done, cudaEventDisableTiming));
+  if (need > eng->h_ckpt_bytes) {
+    if (eng->h_ckpt) cudaFreeHost(eng->h_ckpt);
+    eng->h_ckpt = nullptr;
+    eng->h_ckpt_bytes = 0;
+    CUDA_TRY(cudaMallocHost(reinterpret_cast<void **>(&eng->h_ckpt), need));
+    eng->h_ckpt_bytes = need;
+  }
+  return 0;
+}
+
+template <typename T>
+const T *ckpt_array(const unsigned char *buf, const CkptField &f) {
+  return reinterpret_cast<const T *>(buf + f.off);
+}
+
+// Every check of swb_load_engine on a checkpoint `s` of n bytes (the staging copy, so that every
+// field is aligned), before anything is enqueued.  *stars <- some pool shape is a star or spoke.
+int check_checkpoint(const swb_engine *eng, const unsigned char *s, uint64_t n, const CkptLayout &L,
+                     bool *stars) {
+  static const char fn[] = "swb_load_engine";
+  const DevState &st = eng->st;
+  if (n < kCkptFixed) return fail("%s: %llu bytes are too few for the header", fn, (unsigned long long)n);
+  CkptHeader h;
+  memcpy(&h, s, sizeof h);
+  if (memcmp(h.magic, kCkptMagic, sizeof h.magic)) return fail("%s: magic: not an engine checkpoint", fn);
+  if (h.version != kCkptVersion)
+    return fail("%s: version = %u, this library reads version %u", fn, h.version, kCkptVersion);
+  if (h.E != st.E) return fail("%s: E = %d, the engine has n_envs = %d", fn, h.E, st.E);
+  if (h.K != st.K) return fail("%s: K = %d, the engine has pool_depth = %d", fn, h.K, st.K);
+  if (h.S != st.S) return fail("%s: S = %d, the engine has n_slots = %d", fn, h.S, st.S);
+  if (h.config_bytes != sizeof(swb_config))
+    return fail("%s: config_bytes = %u, sizeof(swb_config) is %zu", fn, h.config_bytes, sizeof(swb_config));
+  if (n != L.total)
+    return fail("%s: size = %llu bytes, a checkpoint of this engine has %llu", fn, (unsigned long long)n,
+                (unsigned long long)L.total);
+  const swb_config sig = signature_of(eng);
+  const unsigned char *a = s + kCkptFixed, *b = reinterpret_cast<const unsigned char *>(&sig);
+  for (size_t i = 0; i < sizeof sig; ++i)
+    if (a[i] != b[i])
+      return fail("%s: signature: the swb_config differs from the engine's at byte %zu (the engine's "
+                  "configuration is another)", fn, i);
+  if (h.span_class != 1 && h.span_class != 4)
+    return fail("%s: span_class = %d, expected 1 or 4", fn, h.span_class);
+  if (h.sampler != 0 && h.sampler != 1) return fail("%s: sampler = %d, expected 0 or 1", fn, h.sampler);
+  const bool has = eng->d_prog != nullptr;
+  if (h.sampler != (int)has)
+    return fail("%s: sampler: the checkpoint was saved %s a device sampler, the engine has %s", fn,
+                h.sampler ? "with" : "without", has ? "one (swb_sampler_load)" : "none");
+  if (has && h.seed != eng->seed)
+    return fail("%s: seed = %llu, the engine's sampler has seed %llu", fn, (unsigned long long)h.seed,
+                (unsigned long long)eng->seed);
+  if (has && h.env_offset != eng->env_offset)
+    return fail("%s: env_offset = %lld, the engine's sampler has env_offset %lld", fn,
+                (long long)h.env_offset, (long long)eng->env_offset);
+  const CkptField *f = L.f;
+  const int32_t *cursor = ckpt_array<int32_t>(s, f[CkptLayout::CURSOR]);
+  const int32_t *serial = ckpt_array<int32_t>(s, f[CkptLayout::SCENE_SERIAL]);
+  const uint8_t *reset_next = ckpt_array<uint8_t>(s, f[CkptLayout::RESET_NEXT]);
+  const int64_t *upto = ckpt_array<int64_t>(s, f[CkptLayout::REFILLED_UPTO]);
+  for (int e = 0; e < st.E; ++e) {
+    if (cursor[e] < 0 || cursor[e] >= st.K)
+      return fail("%s: cursor[%d] = %d is outside [0, %d)", fn, e, cursor[e], st.K);
+    if (serial[e] < 0) return fail("%s: scene_serial[%d] = %d is negative", fn, e, serial[e]);
+    if (reset_next[e] > 1) return fail("%s: reset_next[%d] = %d is not 0 or 1", fn, e, reset_next[e]);
+    if (upto[e] < -1) return fail("%s: refilled_upto[%d] = %lld is below -1", fn, e, (long long)upto[e]);
+  }
+  const uint8_t *shape = ckpt_array<uint8_t>(s, f[CkptLayout::SHAPE]);
+  *stars = false;
+  for (size_t i = 0; i < f[CkptLayout::SHAPE].count; ++i) {
+    const int sh = shape[i];
+    if (sh >= SWB_NUM_SHAPES || (sh && eng->cfg.shape_n_verts[sh] < 3))
+      return fail("%s: shape[%zu] = %d (env %zu, ring slot %zu, slot %zu) %s", fn, i, sh,
+                  i / st.S / st.K, i / st.S % st.K, i % st.S,
+                  sh >= SWB_NUM_SHAPES ? "is not a shape id" : "has no vertex table");
+    *stars = *stars || sh > 6;
+  }
+  return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int64_t swb_engine_state_bytes(const swb_engine *eng) {
+  if (!eng) {
+    fail("swb_engine_state_bytes: null engine");
+    return -1;
+  }
+  return (int64_t)CkptLayout(eng).total;
+}
+
+int swb_save_engine(swb_engine *eng, void *host_dst, uint64_t dst_bytes, void *stream_) {
+  static const char fn[] = "swb_save_engine";
+  if (!eng || !host_dst) return fail("%s: null argument", fn);
+  const CkptLayout L(eng);
+  if (dst_bytes < L.total)
+    return fail("%s: the checkpoint has %llu bytes, the buffer %llu", fn, (unsigned long long)L.total,
+                (unsigned long long)dst_bytes);
+  CUDA_TRY(cudaSetDevice(eng->device));
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (ckpt_staging(eng, L.total)) return 1;
+  unsigned char *h = eng->h_ckpt;
+  memset(h, 0, L.total);  // padding included: two saves of one state are byte-identical
+  CkptHeader hd;
+  memset(&hd, 0, sizeof hd);
+  memcpy(hd.magic, kCkptMagic, sizeof hd.magic);
+  hd.version = kCkptVersion;
+  hd.E = eng->st.E; hd.K = eng->st.K; hd.S = eng->st.S;
+  hd.span_class = eng->max_spans;
+  hd.sampler = eng->d_prog != nullptr;
+  hd.seed = hd.sampler ? eng->seed : 0;
+  hd.env_offset = hd.sampler ? eng->env_offset : 0;
+  hd.config_bytes = sizeof(swb_config);
+  memcpy(h, &hd, sizeof hd);
+  const swb_config sig = signature_of(eng);
+  memcpy(h + kCkptFixed, &sig, sizeof sig);
+  for (const CkptField &f : L.f)
+    if (f.dev) CUDA_TRY(cudaMemcpyAsync(h + f.off, f.dev, f.bytes(), cudaMemcpyDeviceToHost, stream));
+  const CkptField &upto = L.f[CkptLayout::REFILLED_UPTO];
+  if (!upto.dev) memset(h + upto.off, 0xFF, upto.bytes());  // -1: no scene sampled on the device
+  CUDA_TRY(cudaStreamSynchronize(stream));
+  memcpy(host_dst, h, L.total);
+  return 0;
+}
+
+int swb_load_engine(swb_engine *eng, const void *host_src, uint64_t src_bytes, void *stream_) {
+  static const char fn[] = "swb_load_engine";
+  if (!eng || !host_src) return fail("%s: null argument", fn);
+  const CkptLayout L(eng);
+  CUDA_TRY(cudaSetDevice(eng->device));
+  // checked in the staging copy: the caller's buffer may be reused once the call returns, and
+  // every field of the copy is aligned
+  if (ckpt_staging(eng, std::max<size_t>(L.total, kCkptFixed))) return 1;
+  unsigned char *h = eng->h_ckpt;
+  memcpy(h, host_src, std::min<uint64_t>(src_bytes, L.total));
+  bool stars = false;
+  if (check_checkpoint(eng, h, src_bytes, L, &stars)) return 1;
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  CkptHeader hd;
+  memcpy(&hd, h, sizeof hd);
+  // as swb_load_envs raises it; a pool holding a star or spoke needs the concave tables anyway
+  eng->max_spans = std::max({eng->max_spans, (int)hd.span_class, stars ? 4 : 1});
+  for (const CkptField &f : L.f)
+    if (f.dev) CUDA_TRY(cudaMemcpyAsync(f.dev, h + f.off, f.bytes(), cudaMemcpyHostToDevice, stream));
+  CUDA_TRY(cudaEventRecord(eng->ckpt_done, stream));
+  eng->ckpt_in_flight = true;
   return 0;
 }
 

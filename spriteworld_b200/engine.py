@@ -503,6 +503,34 @@ class Engine(object):
       out[name] = torch.as_tensor(_DevicePointer(ptr.value, shape, typestr), device=self.device)
     return out
 
+  # -- checkpoints ------------------------------------------------------------------
+  def state_bytes(self):
+    """Bytes of this engine's checkpoint (swb_engine_state_bytes)."""
+    return int(self._lib.swb_engine_state_bytes(self._h))
+
+  def save_state(self):
+    """The whole engine state -- live positions and counters, every ring's scenes, the device
+    sampler's refill bookkeeping -- as a CPU uint8 tensor in the self-describing layout of
+    include/spriteworld_b200.h (swb_save_engine), after the work enqueued on the current stream.
+    Synchronises that stream; changes nothing."""
+    out = torch.empty(self.state_bytes(), dtype=torch.uint8)
+    _native.check(self._lib.swb_save_engine(self._h, ctypes.c_void_p(out.data_ptr()), out.numel(),
+                                            self._stream()))
+    return out
+
+  def load_state(self, state):
+    """Loads a save_state() of an engine of this configuration (same n_envs, pool_depth and
+    signature, and a device sampler of the same seed and env_offset, or none on both sides).  The
+    library checks every byte before anything is enqueued and raises NativeError naming the first
+    bad field, index and value; the copies go to the current stream."""
+    if (not isinstance(state, torch.Tensor) or state.dtype != torch.uint8 or state.device.type != 'cpu'
+        or state.dim() != 1):
+      raise ValueError('state must be a one-dimensional CPU uint8 tensor (save_state()), got %s'
+                       % _describe(state))
+    state = state.contiguous()
+    _native.check(self._lib.swb_load_engine(self._h, ctypes.c_void_p(state.data_ptr()), state.numel(),
+                                            self._stream()))
+
   # -- env records ------------------------------------------------------------------
   # Ids are lists, ndarrays or tensors; with check='host' (the default) the library checks them on
   # the host, so a CUDA tensor of ids costs a device-to-host copy (env_ids_array).  With

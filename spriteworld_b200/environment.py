@@ -72,6 +72,19 @@ def _require_compilable(task, action_space):
           % (what, type(obj).__name__, '/'.join(missing)))
 
 
+def _rng_state(rng):
+  """The state of a RandomState (or of the np.random module: NumPy's global state) as
+  (str, int64 tensor, int, int, float), which torch.load(weights_only=True) reads back."""
+  name, keys, pos, has_gauss, cached = rng.get_state()
+  return (str(name), torch.from_numpy(np.asarray(keys).astype(np.int64)), int(pos), int(has_gauss),
+          float(cached))
+
+
+def _set_rng_state(rng, state):
+  name, keys, pos, has_gauss, cached = state
+  rng.set_state((str(name), keys.numpy().astype(np.uint32), int(pos), int(has_gauss), float(cached)))
+
+
 class Environment(dm_env.Environment):
   """One Spriteworld environment (drop-in for the reference class)."""
 
@@ -401,6 +414,7 @@ class BatchedEnvironment(object):
   def _init_device_sampler(self, seed, env_offset):
     E, K = self.n_envs, self._K
     self.seed = int(self._rng.randint(0, 2 ** 31 - 1)) if seed is None else int(seed)
+    self._env_offset = int(env_offset)
     self._engine.load_sampler(self._program, self.seed, env_offset)
     # every ring gets scenes 0 .. K-1; env e starts on its scene 0 and is about to reset
     self._engine.refill_device()
@@ -801,6 +815,106 @@ class BatchedEnvironment(object):
       status = torch.zeros(len(states), dtype=torch.uint8, device=eng.device)
     return obs, status
 
+  # -- checkpoints -------------------------------------------------------------------------
+  def state_dict(self):
+    """A checkpoint of the whole run, to resume it exactly (load_state_dict), across episode
+    boundaries: the engine's state (Engine.save_state: live sprites, counters, every scene ring,
+    the device sampler's bookkeeping), the host's refill bookkeeping and underflow guard, the
+    state of `rng` (action noise, the sync refill's scenes) and of every asynchronous refill
+    block's RandomState, and the device sampler's seed and env_offset, with a fingerprint of the
+    environment's configuration.  Only tensors, Python scalars, strings, bytes, tuples, lists and
+    dicts: torch.save writes it and torch.load with weights_only=True reads it back.
+
+    Lands an asynchronous refill in flight first (and so may wait for it), so that the rings match
+    the bookkeeping, and restarts the schedule of scene_serial snapshots (pending snapshots are not
+    state; load_state_dict restarts it the same way).  Synchronises the current stream.
+
+    Not carried over: unreported device sampler failures and refused device-checked id reports --
+    call check_sampler() / engine.check_env_ids() first to have those raised -- and the frame
+    buffers of the last step (render() recomputes them from the state).  With the default `rng`
+    (the np.random module) the state saved is NumPy's global one.  A host-sampler fingerprint
+    cannot cover `init_sprites`, a Python callable: resuming with another generator is not
+    detected."""
+    if self._refill_mode == 'async':
+      self._land(block=True)
+      self._restart_snapshots()
+    host = dict(t=self._t, resets=self._resets, safe_step=self._safe_step, safe_resets=self._safe_resets,
+                stats=dict(self._stats))
+    if self._sampler == 'host':
+      host['refilled_upto'] = torch.from_numpy(self._refilled_upto.copy())
+    return dict(
+        fingerprint=self._fingerprint(), engine=self._engine.save_state(), host=host,
+        rng=_rng_state(self._rng), block_rngs=[_rng_state(r) for r in getattr(self, '_block_rngs', ())],
+        sampler=(self.seed, self._env_offset) if self._sampler == 'device' else None)
+
+  def load_state_dict(self, sd):
+    """Resumes the run a state_dict() was taken of, in an environment constructed with the same
+    arguments (a fresh one, in another process or on another device index too, or this one: a
+    rewind).  Afterwards steps with the same actions give, bit for bit, what the saved run gave
+    after the checkpoint -- with sampler='device' or refill='sync' for as many episodes as are
+    stepped; with refill='async' while every env is on a scene its ring held at the checkpoint,
+    since refill timing decides which env gets which newly drawn scene -- and render(),
+    factor_tensors(), rollout(), expand(), observe() and save_envs() give what they gave at the
+    checkpoint.
+
+    Raises ValueError naming the first difference of configuration before anything changes.  Then
+    lands this environment's own refill in flight, reloads the device sampler if its seed or
+    env_offset differ, loads the engine and restores the host bookkeeping and the RNG states
+    (NumPy's global state with the default `rng`)."""
+    fp, got = self._fingerprint(), sd.get('fingerprint') if isinstance(sd, dict) else None
+    if not isinstance(got, dict):
+      raise ValueError('not a BatchedEnvironment state_dict')
+    for key, mine in fp.items():
+      if got.get(key) != mine:
+        shown = ((got.get(key), mine) if not isinstance(mine, bytes) else ('other bytes', 'its own'))
+        raise ValueError('state_dict was taken of another configuration: %s is %r there, %r here'
+                         % ((key,) + shown))
+    if self._refill_mode == 'async':
+      self._land(block=True)       # no upload of this env's may land on the loaded pool
+    eng = self._engine
+    if self._sampler == 'device' and tuple(sd['sampler']) != (self.seed, self._env_offset):
+      seed, env_offset = (int(v) for v in sd['sampler'])
+      backup = eng.save_state()
+      eng.load_sampler(self._program, seed, env_offset)
+      try:
+        eng.load_state(sd['engine'])
+      except Exception:
+        eng.load_sampler(self._program, self.seed, self._env_offset)
+        eng.load_state(backup)
+        raise
+      self.seed, self._env_offset = seed, env_offset
+    else:
+      eng.load_state(sd['engine'])
+    host = sd['host']
+    self._t, self._resets = int(host['t']), int(host['resets'])
+    self._safe_step, self._safe_resets = int(host['safe_step']), int(host['safe_resets'])
+    self._stats = dict(host['stats'])
+    if self._sampler == 'host':
+      self._refilled_upto[:] = host['refilled_upto'].numpy()
+    _set_rng_state(self._rng, sd['rng'])
+    for r, st in zip(getattr(self, '_block_rngs', ()), sd['block_rngs']):
+      _set_rng_state(r, st)
+    if self._refill_mode == 'async':
+      self._restart_snapshots()
+
+  def _restart_snapshots(self):
+    """Drops the pending scene_serial snapshots; the next step takes a fresh one."""
+    self._snaps.clear()
+    self._last_snap = -(1 << 30)
+
+  def _fingerprint(self):
+    """What load_state_dict compares: everything that decides how the saved state steps."""
+    fp = dict(n_envs=self.n_envs, pool_depth=self._K, n_slots=self._engine.n_slots,
+              signature=bytes(self._engine.signature), sampler=self._sampler, refill=self._refill_mode,
+              refill_blocks=len(getattr(self, '_block_rngs', ())),
+              refill_procs=len(self._pool) if getattr(self, '_pool', None) is not None else 0,
+              renderers=list(self._renderers),
+              rasters=[(name, int(r.width), int(r.height), int(r.anti_aliasing),
+                        tuple(int(c) for c in r.bg_color)) for name, r in self._pil.items()])
+    if self._sampler == 'device':
+      fp['program'] = bytes(self._program.struct)
+    return fp
+
   def observation_spec(self):
     """Per-env specs (the leading n_envs axis of the batched observations is not included)."""
     return {name: (r.batch_observation_spec(self) if hasattr(r, 'batch_observation_spec')
@@ -928,6 +1042,22 @@ class ShardedBatchedEnvironment(object):
     env._resets += 1
     env.engine.request_reset()
     return self.step(engine_lib.zero_actions(env._action_space.compile()['kind'], self.n_local))
+
+  def state_dict(self):
+    """This rank's checkpoint: the local BatchedEnvironment.state_dict() with the sharding it
+    belongs to.  Every rank saves and loads its own (at the same step); loading into another
+    sharding -- another rank, world size or env count -- is refused."""
+    return dict(rank=self.rank, world=self.world, n_envs_total=self.n_envs_total, env_start=self.env_start,
+                t=self._t, local=self.local.state_dict())
+
+  def load_state_dict(self, sd):
+    """Resumes this rank from its own state_dict() (see BatchedEnvironment.load_state_dict)."""
+    for key in ('rank', 'world', 'n_envs_total', 'env_start'):
+      if sd.get(key) != getattr(self, key):
+        raise ValueError('state_dict was taken of another sharding: %s is %r there, %r here'
+                         % (key, sd.get(key), getattr(self, key)))
+    self.local.load_state_dict(sd['local'])
+    self._t = int(sd['t'])
 
   def observation_spec(self):
     return self.local.observation_spec()

@@ -18,7 +18,8 @@ Between those, env records: host-checked saves, loads and copies (disjoint and o
 run the device-checked calls' save and load kernels on int32 ids, and device-checked ones with int32
 and int64 device ids, valid and refused (out of range either way, 2^32 + 1, repeated destinations),
 so that memcheck sees that a refused id never indexes engine memory.  Then rollouts from records
-into leaves, from those leaves, and from the live envs into leaves.
+into leaves, from those leaves, and from the live envs into leaves, renders of records, and an
+engine checkpoint saved, loaded and rendered, with a corrupt one refused.
 """
 import ctypes
 import os
@@ -107,6 +108,21 @@ def device_checked_records(torch):
   torch.cuda.synchronize()
   print('record renders: %d frames, %d overflowed, %d kernel launches'
         % (len(frames), int(status.bool().sum()), eng.launch_count()), flush=True)
+  # an engine checkpoint round trip, and a corrupt one refused before anything is enqueued
+  from spriteworld_b200 import _native
+  state = eng.save_state()
+  eng.load_state(state)
+  eng.render(raster)
+  bad = state.clone()
+  bad[12] ^= 1                                   # E
+  try:
+    eng.load_state(bad)
+    raise AssertionError('a corrupt checkpoint was loaded')
+  except _native.NativeError:
+    pass
+  torch.cuda.synchronize()
+  assert torch.equal(eng.save_state(), state)
+  print('checkpoint: %d bytes saved and loaded, a corrupt one refused' % state.numel(), flush=True)
   raster.close()
   eng.close()
 
