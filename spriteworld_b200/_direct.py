@@ -141,3 +141,10 @@ def render(renderer, sprites):
   frames = eng.render(raster)
   eng.check_render()
   return frames[0].cpu().numpy()
+
+
+def render_masks(renderer, sprites):
+  """(H, W) uint8 instance mask of a Python sprite list: i + 1 where sprites[i] is visible."""
+  eng = _engine(max(1, len(sprites)), _DUMMY_ACTION, _NO_TASK, True)
+  _load(eng, sprites)
+  return eng.render_masks(renderer.width, renderer.height, renderer.anti_aliasing)[0].cpu().numpy()

@@ -127,6 +127,7 @@ def load():
   L.swb_rollout_states.argtypes = [vp, vp, ci, ctypes.c_uint64, vp, ci, ci, ci, ctypes.POINTER(StepOut), vp,
                                    ctypes.c_uint64, ctypes.POINTER(ci), vp]
   L.swb_render_states.argtypes = [vp, vp, vp, ci, ctypes.c_uint64, ci, vp, vp, vp]
+  L.swb_render_masks.argtypes = [vp, ci, ci, ci, vp, ci, ctypes.c_uint64, vp, vp]
   L.swb_save_envs_dev.argtypes = [vp, vp, ci, ci, vp, ctypes.c_uint64, ctypes.POINTER(ci), vp]
   L.swb_load_envs_dev.argtypes = [vp, vp, ci, ci, vp, ctypes.c_uint64, ci, vp]
   L.swb_copy_envs_dev.argtypes = [vp, vp, vp, ci, ci, vp]
@@ -157,7 +158,7 @@ EXPORTS = (
     'swb_step', 'swb_eval_task', 'swb_apply_action', 'swb_rollout', 'swb_raster_create', 'swb_raster_destroy', 'swb_render', 'swb_step_render',
     'swb_step_render_gather', 'swb_ipc_alloc', 'swb_ipc_free', 'swb_ipc_open', 'swb_ipc_close', 'swb_peer_copy',
     'swb_step_host', 'swb_state_pointers', 'swb_scene_serial_pointer', 'swb_render_status_pointer', 'swb_download_state', 'swb_upload_state',
-    'swb_env_record_bytes', 'swb_save_envs', 'swb_load_envs', 'swb_copy_envs', 'swb_rollout_states', 'swb_render_states', 'swb_save_envs_dev',
+    'swb_env_record_bytes', 'swb_save_envs', 'swb_load_envs', 'swb_copy_envs', 'swb_rollout_states', 'swb_render_states', 'swb_render_masks', 'swb_save_envs_dev',
     'swb_load_envs_dev', 'swb_copy_envs_dev', 'swb_env_ids_status_pointer', 'swb_launch_count',
     'swb_sampler_sizeof_program', 'swb_sampler_load', 'swb_sample_scenes', 'swb_refill_device',
     'swb_sampler_pointers', 'swb_pool_pointers', 'swb_engine_state_bytes', 'swb_save_engine',

@@ -9,6 +9,7 @@
 #include <vector>
 
 #include "swb_device.cuh"
+#include "swb_masks.cuh"
 #include "swb_render.cuh"
 #include "swb_rollout.cuh"
 #include "swb_sampler.cuh"
@@ -167,7 +168,7 @@ int upload_axis(swb_raster *r, const AxisHost &h, AxisTables *d) {
 extern "C" {
 
 const char *swb_last_error(void) { return g_error.c_str(); }
-int swb_version(void) { return 9; }
+int swb_version(void) { return 10; }
 int swb_sizeof_config(void) { return (int)sizeof(swb_config); }
 int swb_sizeof_task_node(void) { return (int)sizeof(swb_task_node); }
 
@@ -1163,6 +1164,39 @@ int swb_render_states(swb_engine *eng, swb_raster *r, const void *records, int32
   CUDA_TRY(cudaMemsetAsync(status, 0, (size_t)n, stream));
   return enqueue_render(eng, r, *plan, RenderTargets{{frames}, 1, 0, 0}, status, stream, 0, n, false,
                         RenderRecords{static_cast<const unsigned char *>(records), (size_t)rb});
+}
+
+int swb_render_masks(swb_engine *eng, int32_t width, int32_t height, int32_t anti_aliasing,
+                     const void *records, int32_t n, uint64_t records_bytes, uint8_t *masks, void *stream_) {
+  static const char fn[] = "swb_render_masks";
+  if (width < 1 || height < 1 || anti_aliasing < 1)
+    return fail("%s: width %d, height %d and anti_aliasing %d must be >= 1", fn, width, height, anti_aliasing);
+  if (!eng || !masks) return fail("%s: null engine or masks", fn);
+  if ((int64_t)anti_aliasing * width > 4095 || (int64_t)anti_aliasing * height > 4095)
+    return fail("%s: canvas %lld x %lld exceeds 4095 pixels per side", fn, (long long)anti_aliasing * width,
+                (long long)anti_aliasing * height);
+  if (n < 0) return fail("%s: n = %d", fn, n);
+  if (!records && n != eng->st.E)
+    return fail("%s: n = %d must be E = %d when the masks are the live envs'", fn, n, eng->st.E);
+  const MaskLayout L(eng->st.S, width, height, anti_aliasing);
+  if ((int64_t)n * L.n_bands > INT32_MAX)
+    return fail("%s: n = %d masks of %d bands each exceed 2^31 - 1 CTAs", fn, n, L.n_bands);
+  const uint64_t rb = RecordLayout(eng->st.S).bytes();
+  if (records) {
+    if (check_record_buffer(eng, fn, "records", records, records_bytes, n)) return 1;
+    const uint64_t r0 = reinterpret_cast<uintptr_t>(records), m0 = reinterpret_cast<uintptr_t>(masks);
+    if (m0 < r0 + (uint64_t)n * rb && r0 < m0 + (uint64_t)n * height * width)
+      return fail("%s: the masks overlap the records", fn);
+  }
+  if (n == 0) return 0;
+  CUDA_TRY(cudaSetDevice(eng->device));
+  auto kernel = records ? mask_kernel<true> : mask_kernel<false>;
+  CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, L.total));
+  kernel<<<(unsigned)((int64_t)n * L.n_bands), MK_THREADS, L.total, static_cast<cudaStream_t>(stream_)>>>(
+      eng->st, L, masks, RenderRecords{static_cast<const unsigned char *>(records), (size_t)rb});
+  eng->launches++;
+  CUDA_TRY(cudaGetLastError());
+  return 0;
 }
 
 int swb_env_ids_status_pointer(swb_engine *eng, swb_ids_status **status) {

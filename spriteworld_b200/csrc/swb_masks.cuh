@@ -1,0 +1,287 @@
+// Mask kernel: which sprite is visible at each pixel (renderers.SpriteMasks, swb_render_masks).
+//
+// Mask pixel (i, j) of a W x H mask at anti_aliasing aa is the slot + 1 of the top-most sprite
+// whose Pillow polygon fill covers canvas pixel (aa j + aa/2, aa (H-1-i) + aa/2) of the aa W x aa H
+// canvas PILRenderer draws on, or 0 (what Image.resize(NEAREST) of a label canvas picks, flipped
+// like the frames).  Only Pillow's scan conversion is needed, not its LANCZOS filter, and only one
+// canvas row per mask row.
+//
+// One CTA draws one band of mask rows of one env (or record):
+//   A  a warp per sprite, a lane per vertex: the integer canvas vertices, Pillow's edge records,
+//      horizontal edges and corner-join overrides -- the arithmetic of render_kernel's phase A
+//      (swb_render.cuh), restated here without that kernel's tile and bucket plan.
+//   B  a thread per mask row scan-converts its one canvas row for every sprite, back to front:
+//      the crossings of the edges spanning the row (an edge ending on an interior row counts
+//      twice), sorted and paired with ROUND_UP / ROUND_DOWN, plus the horizontal edges on the
+//      row; each canvas span [xs, xe] paints slot + 1 into the mask columns whose sample
+//      aa j + aa/2 lies in it, in a row staged in shared memory.
+//   C  the staged band goes out with 16-byte stores (bytes at its ends).
+// A sprite row has at most 2 crossings per edge, 2 * SWB_MAX_VERTS in all, and every one is kept:
+// the mask is exact for every shape, and there is no overflow status.
+//
+// Nothing but the masks is written: no env, pool entry, frame or render status changes.
+#pragma once
+#include <climits>
+
+#include "swb_device.cuh"
+#include "swb_render.cuh"
+#include "swb_states.cuh"
+
+namespace swb {
+
+constexpr int MK_THREADS = 128;          // threads per CTA = most mask rows per band
+constexpr int MK_STAGE_BYTES = 16384;    // staged mask bytes per band (fewer rows for wide masks)
+constexpr int MK_XCAP = 2 * EV;          // crossings one sprite row can have
+
+// A mask raster and the shared-memory layout of one CTA.
+struct MaskLayout {
+  int S, W, H, aa, CW, CH, band_rows, n_bands;
+  int off_edge, off_hl, off_meta, off_xx, off_stage, total;
+  __host__ __device__ MaskLayout(int S_, int W_, int H_, int aa_) : S(S_), W(W_), H(H_), aa(aa_) {
+    CW = aa * W;
+    CH = aa * H;
+    band_rows = MK_STAGE_BYTES / W;
+    if (band_rows < 1) band_rows = 1;
+    if (band_rows > MK_THREADS) band_rows = MK_THREADS;
+    if (band_rows > H) band_rows = H;
+    n_bands = (H + band_rows - 1) / band_rows;
+    int o = 0;
+    auto take = [&](int bytes) { int r = o; o += (bytes + 15) & ~15; return r; };
+    off_edge = take(S * EV * 6 * 4);        // x0, y0 (int), dx, ovs, ove (float), yr (u32)
+    off_hl = take(S * EV * 3 * 2);          // horizontal edges: y, xmin, xmax (int16)
+    off_meta = take(S * 5 * 4);             // nv, nh, has-join, p_ymax, ymin | ymax << 16
+    off_xx = take(MK_XCAP * MK_THREADS * 4);  // crossings, [k][thread]
+    off_stage = take(band_rows * W + 16);   // staged band, placed at the output's address mod 16
+    total = o;
+  }
+};
+
+template <bool kRecords>
+__global__ void __launch_bounds__(MK_THREADS)
+mask_kernel(DevState st, const MaskLayout L, uint8_t *__restrict__ masks, const RenderRecords recs) {
+  extern __shared__ __align__(16) unsigned char g_mask_smem[];
+  unsigned char *const smem = g_mask_smem;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  constexpr unsigned FULL = 0xFFFFFFFFu;
+  constexpr int NWARP = MK_THREADS / 32;
+  const int S = L.S;
+  const size_t item = blockIdx.x;
+  const size_t e = item / (unsigned)L.n_bands;
+  const int band = (int)(item - e * (unsigned)L.n_bands);
+
+  int *e_x0 = reinterpret_cast<int *>(smem + L.off_edge);
+  int *e_y0 = e_x0 + S * EV;
+  float *e_dx = reinterpret_cast<float *>(e_y0 + S * EV);
+  float *e_ovs = e_dx + S * EV, *e_ove = e_ovs + S * EV;
+  uint32_t *e_yr = reinterpret_cast<uint32_t *>(e_ove + S * EV);
+  short *s_hl = reinterpret_cast<short *>(smem + L.off_hl);  // [S][EV][3]
+  int *s_nv = reinterpret_cast<int *>(smem + L.off_meta);
+  int *s_nh = s_nv + S, *s_hasov = s_nh + S, *s_pymax = s_hasov + S;
+  uint32_t *s_yext = reinterpret_cast<uint32_t *>(s_pymax + S);
+  float *xx = reinterpret_cast<float *>(smem + L.off_xx) + tid;  // crossing k at xx[k * MK_THREADS]
+
+  // ---- phase A: a warp per sprite, a lane per vertex / edge (render_kernel phase A) ----------
+  const int cur = kRecords ? 0 : st.cursor[e];
+  const unsigned char *const rec = kRecords ? recs.rec + e * recs.record_bytes : nullptr;
+  for (int s = warp; s < S; s += NWARP) {
+    const size_t scene = (e * st.K + cur) * S + s;
+    const RecordLayout rl(S);
+    const double *const f64 = reinterpret_cast<const double *>(rec);  // [10][S], see RecordLayout
+    const int shape = kRecords ? sanitize_shape(st, rec[rl.shape() + s]) : st.p_shape[scene];
+    const double px = kRecords ? f64[8 * S + s] : st.pos_x[e * S + s];
+    const double py = kRecords ? f64[9 * S + s] : st.pos_y[e * S + s];
+    const double m00 = kRecords ? f64[2 * S + s] : st.p_m00[scene];
+    const double m01 = kRecords ? f64[3 * S + s] : st.p_m01[scene];
+    const double m10 = kRecords ? f64[4 * S + s] : st.p_m10[scene];
+    const double m11 = kRecords ? f64[5 * S + s] : st.p_m11[scene];
+    const int nv = shape ? st.shape_n[shape] : 0;
+    const int t = s * EV + lane;
+    int ivx = 0, ivy = 0;
+    if (lane < nv) {
+      const double2 v = reinterpret_cast<const double2 *>(st.shape_verts)[(size_t)shape * EV + lane];
+      // centred path (sprite.py:96-101), world position, canvas_size * vertices, Pillow's (int)
+      const double cx = __dadd_rn(__dadd_rn(__dmul_rn(m00, v.x), __dmul_rn(m01, v.y)), 0.0);
+      const double cy = __dadd_rn(__dadd_rn(__dmul_rn(m10, v.x), __dmul_rn(m11, v.y)), 0.0);
+      const double wx = __dadd_rn(cx, px), wy = __dadd_rn(cy, py);
+      ivx = __double2int_rz(__dmul_rn((double)L.CW, wx));
+      ivy = __double2int_rz(__dmul_rn((double)L.CH, wy));
+    }
+    // edge lane -> lane+1 (Pillow add_edge); the closing edge only if the polygon is not closed
+    const int jn = (lane + 1 >= nv) ? 0 : lane + 1;
+    const int x0 = ivx, y0 = ivy;
+    const int x1 = __shfl_sync(FULL, ivx, jn), y1 = __shfl_sync(FULL, ivy, jn);
+    const bool exists = lane < nv && ((lane + 1 < nv) || (x0 != x1 || y0 != y1));
+    const bool scanned = exists && y0 != y1;
+    const int ymin = min(y0, y1), ymax = max(y0, y1);
+    const float dx = scanned ? __fdiv_rn((float)(x1 - x0), (float)(y1 - y0)) : 0.0f;
+    // horizontal edges are drawn directly as hline(xmin, y, xmax), clipped to the canvas
+    const int hxs = max(min(x0, x1), 0), hxe = min(max(x0, x1), L.CW - 1);
+    const bool hline = exists && y0 == y1 && y0 >= 0 && y0 < L.CH && hxs <= hxe;
+    const unsigned hmask = __ballot_sync(FULL, hline);
+    if (hline) {
+      short *h = s_hl + ((size_t)s * EV + __popc(hmask & ((1u << lane) - 1u))) * 3;
+      h[0] = (short)y0; h[1] = (short)hxs; h[2] = (short)hxe;
+    }
+    // rows the edge crosses, both ends clamped to [-1, CH]: canvas rows are 0 .. CH-1, so the
+    // clamped range holds exactly the canvas rows the true one does, and a clamped end equals a
+    // canvas row only where the true end does (the tests of phase B and the join search below).
+    // Empty (no row) if not scanned
+    const uint32_t yr = scanned ? ((uint32_t)(uint16_t)(short)min(max(ymin, -1), L.CH) |
+                                   ((uint32_t)(uint16_t)(short)min(max(ymax, -1), L.CH) << 16))
+                                : 0x80007FFFu;
+    e_x0[t] = x0;
+    e_y0[t] = y0;
+    e_dx[t] = dx;
+    e_yr[t] = yr;
+    e_ovs[t] = nanf("");
+    e_ove[t] = nanf("");
+    const bool isv = lane < nv;
+    const int ymn = __reduce_min_sync(FULL, isv ? ivy : INT_MAX), ymx = __reduce_max_sync(FULL, isv ? ivy : INT_MIN);
+    // Pillow's last polygon row: max(0, edges), clipped to ysize
+    const int p_ymax = min(max(0, ymx), L.CH);
+    __syncwarp();  // the edge table of this sprite is visible to the join search below
+
+    // corner joins: edge i and the FIRST earlier edge k leaving the same corner in the same x
+    // direction -- both starting on row y, or both ending on the polygon's last row -- move k's
+    // crossing on that row (oracle/sw_raster_oracle.c, render_kernel phase A)
+    const unsigned lt = (1u << lane) - 1u;
+    const unsigned pos = __ballot_sync(FULL, scanned && dx > 0.0f);
+    const unsigned neg = __ballot_sync(FULL, scanned && dx < 0.0f);
+    const unsigned same_dir = dx > 0.0f ? pos : (dx < 0.0f ? neg : 0u);
+    const unsigned start_grp = __match_any_sync(FULL, scanned ? (int)(short)(yr & 0xFFFFu) : (0x40000000 | lane));
+    const unsigned end_grp = __ballot_sync(FULL, scanned && (int)(short)(yr >> 16) == p_ymax);
+    bool any_join = false;
+#pragma unroll
+    for (int pass = 0; pass < 2; ++pass) {
+      const int y = pass == 0 ? ymin : p_ymax;
+      unsigned cand = (pass == 0 ? start_grp : end_grp) & lt & same_dir;
+      if (!scanned || (pass == 1 && ymax != p_ymax) || y < 0 || y >= L.CH) cand = 0;
+      int jk = -1;
+      float jv = 0.0f;
+      if (cand) {
+        const float x = edge_x_at(y, y0, dx, x0);
+        while (cand) {
+          const int k = __ffs(cand) - 1;
+          cand &= cand - 1;
+          const int u = s * EV + k;
+          const float odx = e_dx[u];
+          const int oy0 = e_y0[u], ox0 = e_x0[u];
+          const float ox = edge_x_at(y, oy0, odx, ox0);
+          if (roundf(x) != roundf(ox)) continue;
+          const int off = (y == p_ymax) ? -1 : 1;
+          const float adj = edge_x_at(y + off, y0, dx, x0);
+          const float adjo = edge_x_at(y + off, oy0, odx, ox0);
+          const bool right = (y == ymax) ? (dx < 0.0f) : (dx > 0.0f);
+          float nvx = right ? __fsub_rn(fminf(adj, adjo), 1.0f) : __fadd_rn(fmaxf(adj, adjo), 1.0f);
+          nvx = floorf(__fadd_rn(nvx, 0.5f));
+          jv = right ? fmaxf(nvx, x) : fminf(nvx, x);
+          jk = k;
+          break;
+        }
+      }
+      // several later edges may pick the same k: the last one in table order wins
+      const unsigned grp = __match_any_sync(FULL, jk >= 0 ? jk : (64 + lane));
+      if (jk >= 0 && (grp >> lane) == 1u) (pass == 0 ? e_ovs : e_ove)[s * EV + jk] = jv;
+      any_join |= __any_sync(FULL, jk >= 0);
+    }
+    if (lane == 0) {
+      s_nv[s] = nv;
+      s_nh[s] = __popc(hmask);
+      s_hasov[s] = any_join ? 1 : 0;
+      s_pymax[s] = p_ymax;
+      // the canvas rows any edge or horizontal edge of the sprite is on, clamped to [-1, 32767]
+      // (canvas rows are 0 .. 4094); none without vertices
+      s_yext[s] = nv > 0 ? ((uint32_t)(uint16_t)(short)min(max(ymn, -1), 32767) |
+                            ((uint32_t)(uint16_t)(short)min(max(ymx, -1), 32767) << 16))
+                         : 0x8000FFFFu;
+    }
+  }
+
+  // the band's output rows [i0, i0 + nb) are bytes [g, g + nb * W) of the masks; the band is
+  // staged from s_stage + (g mod 16), so that staged and global addresses agree modulo 16
+  const int i0 = band * L.band_rows;
+  const int nb = min(L.band_rows, L.H - i0);
+  const size_t g = (e * (size_t)L.H + (size_t)i0) * (size_t)L.W;
+  const int nbytes = nb * L.W;
+  uint8_t *const gdst = masks + g;
+  const int mis = (int)(reinterpret_cast<uintptr_t>(gdst) & 15u);
+  uint8_t *const stage = smem + L.off_stage + mis;
+  for (int i = tid; i < nbytes; i += MK_THREADS) stage[i] = 0;
+  __syncthreads();
+
+  // ---- phase B: a thread per mask row, its one canvas row, sprites back to front ------------
+  if (tid < nb) {
+    const int i = i0 + tid;
+    const int y = L.aa * (L.H - 1 - i) + L.aa / 2;  // canvas row of mask row i (always on the canvas)
+    const int half = L.aa / 2;
+    uint8_t *const row = stage + (size_t)tid * L.W;
+    // paints the mask columns j with xs <= aa j + aa/2 <= xe (0 <= xs <= xe < CW)
+    auto paint = [&](int xs, int xe, uint8_t label) {
+      const int jlo = (xs - half + L.aa - 1) / L.aa, jhi = (xe - half + L.aa) / L.aa - 1;
+      for (int j = jlo; j <= jhi; ++j) row[j] = label;
+    };
+#pragma unroll 1
+    for (int s = 0; s < S; ++s) {
+      const uint32_t ext = s_yext[s];
+      if (y < (int)(short)(ext & 0xFFFFu) || y > (int)(short)(ext >> 16)) continue;
+      const uint8_t label = (uint8_t)(s + 1);
+      const int nv = s_nv[s], p_ymax = s_pymax[s];
+      const bool hasov = s_hasov[s] != 0;
+      int j = 0;
+#pragma unroll 1
+      for (int k = 0; k < nv; ++k) {
+        const int u = s * EV + k;
+        const uint32_t yr = e_yr[u];
+        const int ymin = (int)(short)(yr & 0xFFFFu), ymax = (int)(short)(yr >> 16);
+        if (y < ymin || y > ymax) continue;
+        float x = edge_x_at(y, e_y0[u], e_dx[u], e_x0[u]);
+        if (hasov) {
+          if (y == ymin) { const float o = e_ovs[u]; if (!isnan(o)) x = o; }
+          if (y == p_ymax && y == ymax) { const float o = e_ove[u]; if (!isnan(o)) x = o; }
+        }
+        xx[j++ * MK_THREADS] = x;
+        if (y == ymax && y < p_ymax) xx[j++ * MK_THREADS] = x;  // edge ending on an interior row
+      }
+#pragma unroll 1
+      for (int a = 1; a < j; ++a) {  // insertion sort, ascending
+        const float v = xx[a * MK_THREADS];
+        int b = a - 1;
+        while (b >= 0 && xx[b * MK_THREADS] > v) { xx[(b + 1) * MK_THREADS] = xx[b * MK_THREADS]; --b; }
+        xx[(b + 1) * MK_THREADS] = v;
+      }
+      int x_pos = 0;
+#pragma unroll 1
+      for (int a = 1; a < j; a += 2) {
+        const int x_end = round_down_f(xx[a * MK_THREADS]);
+        if (x_end < x_pos) continue;
+        const float xa = xx[(a - 1) * MK_THREADS];
+        if (xa > (float)x_pos) {
+          x_pos = round_up_f(xa);
+          if (x_end < x_pos) continue;
+        }
+        const int xs = max(x_pos, 0), xe = min(x_end, L.CW - 1);
+        if (xs <= xe) paint(xs, xe, label);
+        x_pos = x_end + 1;
+      }
+      const int nh = s_nh[s];
+#pragma unroll 1
+      for (int h = 0; h < nh; ++h) {
+        const short *hl = s_hl + ((size_t)s * EV + h) * 3;
+        if (hl[0] == y) paint(hl[1], hl[2], label);
+      }
+    }
+  }
+  __syncthreads();
+
+  // ---- phase C: the staged band to the masks -------------------------------------------------
+  const int head = min((16 - mis) & 15, nbytes);
+  const int n16 = (nbytes - head) >> 4;
+  const int tail0 = head + (n16 << 4);
+  for (int i = tid; i < head; i += MK_THREADS) gdst[i] = stage[i];
+  const uint4 *src16 = reinterpret_cast<const uint4 *>(stage + head);
+  uint4 *dst16 = reinterpret_cast<uint4 *>(gdst + head);
+  for (int i = tid; i < n16; i += MK_THREADS) dst16[i] = src16[i];
+  for (int i = tail0 + tid; i < nbytes; i += MK_THREADS) gdst[i] = stage[i];
+}
+
+}  // namespace swb

@@ -423,6 +423,40 @@ class Engine(object):
         self._stream()))
     return frames, status
 
+  def render_masks(self, width, height, anti_aliasing=1, states=None, out=None):
+    """Sprite instance masks (swb_render_masks): uint8 (n, height, width), pixel value k + 1 where
+    slot k is the top-most sprite covering the pixel's sample point on PILRenderer's
+    anti_aliasing-times canvas, 0 where none does (renderers.SpriteMasks).  Of the live envs (n =
+    n_envs), or with `states` of EnvStates of any n records, as if loaded.  Into `out` if given
+    (a contiguous uint8 tensor of that shape on this device), else a new tensor.  One launch on the
+    current stream; nothing else changes."""
+    if states is not None and not isinstance(states, EnvStates):
+      raise ValueError('states must be EnvStates, got %s' % type(states).__name__)
+    n = self.n_envs if states is None else len(states)
+    if states is not None:
+      self.check_states(states, n)
+    W, H, aa = int(width), int(height), int(anti_aliasing)
+    shape = (n, H, W)
+    if out is None:
+      out = torch.empty((n, max(H, 0), max(W, 0)), dtype=torch.uint8, device=self.device)
+    elif (not isinstance(out, torch.Tensor) or out.dtype != torch.uint8 or out.device != self.device or
+          tuple(out.shape) != shape or not out.is_contiguous()):
+      raise ValueError('masks must be a contiguous uint8 tensor of shape %s on %s, got %s' % (
+          shape, self.device, _describe(out)))
+    masks_ptr = out.data_ptr()
+    rec = (None, 0) if states is None else (states.data.data_ptr(), states.data.numel())
+    if n == 0:
+      # zero records: the call checks its arguments and draws nothing, but an empty tensor may have no
+      # address; any aligned address stands in for the empty buffers (nothing is read or written)
+      probe = torch.empty(16, dtype=torch.uint8, device=self.device)
+      masks_ptr = masks_ptr or probe.data_ptr()
+      if rec[0] is not None:
+        rec = (rec[0] or probe.data_ptr(), rec[1])
+    _native.check(self._lib.swb_render_masks(
+        self._h, W, H, aa, None if rec[0] is None else ctypes.c_void_p(rec[0]), n, rec[1],
+        ctypes.c_void_p(masks_ptr), self._stream()))
+    return out
+
   def render_status(self):
     """Zero-copy uint8 (E,) view of the per-env status of the last render() (ENV_SPAN_OVERFLOW)."""
     if getattr(self, '_render_status_view', None) is None:

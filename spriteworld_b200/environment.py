@@ -21,7 +21,7 @@ from spriteworld_b200 import _dm_env as dm_env
 from spriteworld_b200 import _native, constants, scene
 from spriteworld_b200 import engine as engine_lib
 from spriteworld_b200 import sprite_generators
-from spriteworld_b200.renderers import pil_renderer
+from spriteworld_b200.renderers import handcrafted, pil_renderer
 
 
 def _split_renderers(renderers):
@@ -357,6 +357,10 @@ class BatchedEnvironment(object):
         (name, engine_lib.Raster(self._engine, r.width, r.height, r.anti_aliasing, r.bg_color))
         for name, r in self._pil.items())
     self._frames = {name: r.new_frames() for name, r in self._rasters.items()}
+    # one mask buffer per SpriteMasks renderer, overwritten every step like the frames
+    self._mask_buffers = {
+        id(r): torch.empty((E, r.height, r.width), dtype=torch.uint8, device=self._engine.device)
+        for r in self._other.values() if isinstance(r, handcrafted.SpriteMasks)}
     if sampler == 'device':
       self._init_device_sampler(seed, env_offset)
       return
@@ -779,12 +783,25 @@ class BatchedEnvironment(object):
     return BatchedRollout(res.step_type, res.reward, discount, res.success, res.status)
 
   def render(self):
-    """Re-renders every PILRenderer observation of the current state (a loaded one, say) into
-    this environment's frame buffers, and returns them: dict name -> uint8 (n_envs, H, W, 3)."""
+    """Re-renders every PILRenderer and SpriteMasks observation of the current state (a loaded one,
+    say) into this environment's buffers, and returns them: dict name -> uint8 (n_envs, H, W, 3)
+    frames, then uint8 (n_envs, H, W) masks."""
     out = collections.OrderedDict()
     for name, r in self._rasters.items():
       out[name] = self._engine.render(r, self._frames[name])
+    for name, r in self._other.items():
+      if isinstance(r, handcrafted.SpriteMasks):
+        out[name] = self.render_masks(r)
     return out
+
+  def render_masks(self, renderer, states=None):
+    """SpriteMasks `renderer`'s masks (Engine.render_masks) on the current stream: of the live envs
+    into this environment's buffer for the renderer (a new tensor for a renderer it does not own),
+    or of EnvStates `states` into a new uint8 (n, H, W) tensor."""
+    dims = (renderer.width, renderer.height, renderer.anti_aliasing)
+    if states is not None:
+      return self._engine.render_masks(*dims, states=states)
+    return self._engine.render_masks(*dims, out=self._mask_buffers.get(id(renderer)))
 
   def observe(self, states):
     """The observations of env records without loading them: (observation, status) for EnvStates

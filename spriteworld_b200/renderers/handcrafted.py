@@ -70,6 +70,63 @@ class SpriteFactors(abstract_renderer.AbstractRenderer):
     return spec
 
 
+class SpriteMasks(abstract_renderer.AbstractRenderer):
+  """Instance masks: which sprite is visible at each pixel of a PILRenderer frame.
+
+  Observes uint8 (H, W) for image_size=(W, H) (width, height as PILRenderer hands them to Pillow):
+  k + 1 where sprite k is the top-most sprite covering the pixel's sample point, 0 where none does.
+  Mask pixel (i, j) samples canvas pixel (aa j + aa//2, aa (H-1-i) + aa//2) of the aa W x aa H
+  canvas PILRenderer draws on, with the same integer vertices and Pillow's fill rules, so at
+  anti_aliasing=1 a frame is bg where the mask is 0 and the colour of sprite mask-1 elsewhere.
+  Drawn by the mask kernel (csrc/swb_masks.cuh).
+
+  Ids: in a BatchedEnvironment, slots of SpriteFactors.render_batch (empty slots, padded at the
+  front, are never visible), so factors[f][e, mask - 1] is the visible sprite's factor; on a sprite
+  list (`render`, the drop-in Environment), indices into the list.  Any anti_aliasing is accepted
+  whose canvas sides stay within 4095 pixels."""
+
+  def __init__(self, image_size=(64, 64), anti_aliasing=1):
+    self._image_size = tuple(int(v) for v in image_size)
+    self._anti_aliasing = int(anti_aliasing)
+    if len(self._image_size) != 2 or min(self._image_size) < 1 or self._anti_aliasing < 1:
+      raise ValueError('image_size must be (width, height) >= 1 and anti_aliasing >= 1, got %r, %r'
+                       % (image_size, anti_aliasing))
+    if self._anti_aliasing * max(self._image_size) > 4095:
+      raise ValueError('the canvas (anti_aliasing * image_size) exceeds 4095 pixels per side')
+    self._observation_spec = specs.Array(shape=(self.height, self.width), dtype=np.uint8)
+
+  @property
+  def width(self):
+    return self._image_size[0]
+
+  @property
+  def height(self):
+    return self._image_size[1]
+
+  @property
+  def anti_aliasing(self):
+    return self._anti_aliasing
+
+  def render(self, sprites=(), global_state=None):
+    from spriteworld_b200 import _direct
+    return _direct.render_masks(self, list(sprites))
+
+  def observation_spec(self):
+    return self._observation_spec
+
+  def render_batch(self, env, res):
+    """Batched form: uint8 (n_envs, H, W) device tensor, a buffer of `env` that every step (and
+    env.render()) overwrites, as it does the frames."""
+    return env.render_masks(self)
+
+  def render_states(self, env, states):
+    """The masks of env records (EnvStates) without loading them: a new uint8 (n, H, W) tensor."""
+    return env.render_masks(self, states)
+
+  def batch_observation_spec(self, env):
+    return self._observation_spec
+
+
 class Success(abstract_renderer.AbstractRenderer):
   """global_state['success'] as an observation."""
 
