@@ -35,6 +35,7 @@ extern "C" {
 #define SWB_MAX_NODES 32
 #define SWB_MAX_SLOTS 32    /* sprites per env */
 #define SWB_MAX_FILTERS 32  /* distinct task filter distributions (bits of `member`) */
+#define SWB_MAX_GOALS 8     /* sampled FindGoalPosition goals per task tree (goal slots) */
 #define SWB_MAX_PEERS 8     /* ranks whose frame buffers one render launch can write */
 #define SWB_IPC_HANDLE_BYTES 64
 
@@ -80,6 +81,13 @@ typedef struct {
   int32_t children[SWB_MAX_CHILDREN]; /* node indices < this node's index */
   int32_t aggregator;
   int32_t criterion;
+  /* FindGoalPosition: -1 = the constant `goal`; g in [0, SWB_MAX_GOALS) = the goal drawn with the
+   * env's scene, goal slot g of the pool entry the env is on.  The engine's G (goals per scene) is
+   * the largest slot + 1; slots 0 .. G-1 must each belong to exactly one node.  Added in version 11
+   * in the struct's tail padding (its size did not change): bindings check swb_version() >= 11, and
+   * a zero-filled FIND_GOAL node is a sampled goal, whose engine then refuses scene uploads without
+   * swb_scene_soa.goal. */
+  int32_t goal_slot;
 } swb_task_node;
 
 typedef struct {
@@ -118,6 +126,8 @@ typedef struct {
   const uint8_t *pos_f32;                /* 1: the reference's position ndarray is float32 */
   const uint8_t *rgb;                    /* [n*S*3] color_to_rgb(sprite.color) (pil_renderer.py:82) */
   const float *factors;                  /* optional [n*S*5]: scale, angle, c0, c1, c2 for factor observations */
+  const double *goal;                    /* [n*G*2]: (x, y) of every goal slot of scene i at (i*G + g)*2;
+                                            required when the engine has G > 0 goal slots, else ignored */
 } swb_scene_soa;
 
 /* Per-step outputs, device pointers, one element per env (swb_rollout: per step, env and candidate). */
@@ -302,7 +312,14 @@ int swb_upload_state(swb_engine *eng, const double *pos_x, const double *pos_y,
  *   108 S + 4   uint8     1       reset_next
  *   108 S + 5   uint8     S       shape
  *   109 S + 5   uint8     S       pos_f32
- *   110 S + 5   zero      ..      padding up to swb_env_record_bytes()
+ *   110 S + 5   zero      ..      padding up to swb_env_record_bytes(), when G = 0
+ *
+ * An engine with G > 0 goal slots appends the goals of the current scene, and swb_env_record_bytes()
+ * grows accordingly (it is unchanged for G = 0):
+ *
+ *   P = 110 S + 5 rounded up to 8
+ *   P           double    2 x G   goal (x, y) of goal slot g at P + 16 g
+ *   P + 16 G    zero      ..      padding up to swb_env_record_bytes()
  *
  * Id arrays are HOST pointers, checked on the host; a call its checks refuse enqueues nothing.
  * (swb_save_envs_dev and its siblings below take device ids, checked on the device.)
@@ -441,7 +458,7 @@ int swb_copy_envs(swb_engine *eng, const int32_t *src_ids, const int32_t *dst_id
  * are ordered on one stream at a time (they share the scratch, the status record and the claim
  * array that checks distinctness).
  */
-enum { SWB_IDS_CALL_SAVE = 0, SWB_IDS_CALL_LOAD = 1, SWB_IDS_CALL_COPY = 2 };
+enum { SWB_IDS_CALL_SAVE = 0, SWB_IDS_CALL_LOAD = 1, SWB_IDS_CALL_COPY = 2, SWB_IDS_CALL_SET_GOALS = 3 };
 enum { SWB_IDS_OUT_OF_RANGE = 1, SWB_IDS_REPEATED = 2 };
 typedef struct {
   uint32_t ok;       /* 1: the last device-checked call passed its id checks; 0: it was refused */
@@ -528,6 +545,10 @@ typedef struct {
   /* every angle value the code can draw, ascending (-0.0 before 0.0), with libm's
    * cos / sin of its radians (scene.transform_matrix) */
   double angle[SWB_PROG_MAX_ANGLES], angle_cos[SWB_PROG_MAX_ANGLES], angle_sin[SWB_PROG_MAX_ANGLES];
+  /* sampled FindGoalPosition goals: goal slot g is drawn by the distribution code at goal_pc[g] (its
+   * x and y), after the scene's sprites, from the same stream.  n_goals must equal the engine's G. */
+  int32_t n_goals;
+  int32_t goal_pc[SWB_MAX_GOALS];
 } swb_scene_program;
 
 /* Output of swb_sample_scenes: device pointers, [n * S] per field (rgb [n * S * 3], factors
@@ -541,6 +562,7 @@ typedef struct {
   float *factors;
   double *factor_value;
   uint8_t *factor_kind;
+  double *goal;   /* [n * G * 2] goals (x, y) per goal slot; may be NULL (then not written) */
 } swb_sample_out;
 
 /* The first rejection loop that ran out of tries, since the caller last zeroed `failed`.  The
@@ -572,6 +594,43 @@ int swb_refill_device(swb_engine *eng, void *stream);
  * f64[0..7] = x, y, m00, m01, m10, m11, vx, vy; rgb packed r | g << 8 | b << 16; factors 5 per slot. */
 int swb_pool_pointers(swb_engine *eng, double **f64, uint32_t **member, uint8_t **shape, uint8_t **pos_f32,
                       uint32_t **rgb, float **factors);
+
+/*
+ * Sampled goals.  A FindGoalPosition node with goal_slot g >= 0 reads its goal from the scene the
+ * env is on: goal slot g of pool entry (env, ring slot), (x, y) at ((env * K + ring) * G + g) * 2.
+ * An env stepped with goal (gx, gy) steps bit for bit as one whose node has goal_slot -1 and
+ * goal = {gx, gy}.  Goals arrive with the scenes (swb_scene_soa.goal) and travel in env records
+ * and checkpoints.  An engine with G = 0 allocates no goal array.
+ *
+ * swb_pool_goal_pointer: *goal <- the device array [E * K * G * 2] f64 (NULL when G = 0),
+ * *n_goals <- G.
+ */
+int swb_pool_goal_pointer(swb_engine *eng, double **goal, int32_t *n_goals);
+
+/*
+ * Overwrites the goals of the scene each listed env is on: env env_ids[i] (ids in [0, E), distinct)
+ * gets goals[i * G * 2 .. (i + 1) * G * 2) (device f64) in pool entry (env, cursor).  The env keeps
+ * them until it starts its next scene, which brings that scene's goals.  Like swb_load_envs it writes
+ * only the entry at the env's cursor.  Host ids are checked on the host; swb_set_goals_dev takes
+ * device ids (SWB_DTYPE_I32 / I64) checked by kernels with the rules and status record of the _dev
+ * record calls (call SWB_IDS_CALL_SET_GOALS, all or nothing).  Refused, enqueuing nothing: G = 0,
+ * n < 0, null or unaligned pointers, bad host ids.  n == 0 enqueues nothing.
+ */
+int swb_set_goals(swb_engine *eng, const int32_t *env_ids, int32_t n, const double *goals, void *stream);
+int swb_set_goals_dev(swb_engine *eng, const void *env_ids, int32_t id_dtype, int32_t n, const double *goals,
+                      void *stream);
+
+/*
+ * The task tree's value on env records, as swb_eval_task gives it for a live env (no action cost):
+ * reward[i], success[i] and status[i] of record i at its live positions, with the record's goals, or
+ * with goals[i * G * 2 .. (i + 1) * G * 2) (device f64) in their place when `goals` is not NULL.
+ * `records`: n records of this engine's layout, records_bytes bytes, 16-byte aligned.  One launch;
+ * read-only: no env, pool entry, counter or record changes.  Refused, enqueuing nothing: null
+ * engine or outputs, n < 0, a record buffer too small or unaligned, goals given with G = 0 or
+ * unaligned, outputs that overlap the records.  n == 0 enqueues nothing.
+ */
+int swb_evaluate_states(swb_engine *eng, const void *records, int32_t n, uint64_t records_bytes,
+                        const double *goals, double *reward, uint8_t *success, uint8_t *status, void *stream);
 
 /* Device pointers: refilled_upto [E] int64, and the engine's swb_sampler_status. */
 int swb_sampler_pointers(swb_engine *eng, int64_t **refilled_upto, swb_sampler_status **status);
@@ -607,6 +666,8 @@ int swb_sampler_pointers(swb_engine *eng, int64_t **refilled_upto, swb_sampler_s
  *   ..       float     E*K*S*5     factors, 5 per entry
  *   ..       uint8     E*K*S x 2   shape, pos_f32
  *   ..       int64     E           refilled_upto (-1 throughout without a device sampler)
+ *   ..       double    E*K*G x 2   goals of every pool entry, as swb_pool_goal_pointer (absent when G = 0;
+ *                                  G is part of the signature through the nodes' goal_slot)
  *
  * That is about 94 bytes per pool entry and 16 S + 21 bytes per env; swb_engine_state_bytes()
  * gives the exact size.

@@ -92,6 +92,7 @@ def task_value(task, sprites):
   """(reward, success) of `task` on a Python sprite list."""
   nodes, filters = task.compile()
   task._filters_static()
+  task._constant_goals('task.reward / task.success')
   sprites = list(sprites)
   eng = _engine(max(1, len(sprites)), _DUMMY_ACTION, nodes, True)
   _load_for_task(eng, sprites, filters)

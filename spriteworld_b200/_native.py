@@ -12,6 +12,7 @@ MAX_CHILDREN = 16
 MAX_NODES = 32
 MAX_SLOTS = 32
 MAX_FILTERS = 32
+MAX_GOALS = 8    # SWB_MAX_GOALS
 
 ACT_SELECT_MOVE, ACT_DRAG_AND_DROP, ACT_EMBODIED = 0, 1, 2
 DTYPE_F32, DTYPE_F64, DTYPE_I32, DTYPE_I64 = 0, 1, 2, 3
@@ -21,7 +22,7 @@ CRIT = {'all': 0, 'any': 1}
 STEP_FIRST, STEP_MID, STEP_LAST = 0, 1, 2
 STEP_NONE = -1   # padding of a rollout: no step
 ENV_OK, ENV_CLUSTER_LABELS, ENV_CLUSTER_ZERODIV, ENV_BAD_ACTION, ENV_SPAN_OVERFLOW = 0, 1, 2, 4, 8
-IDS_CALL_SAVE, IDS_CALL_LOAD, IDS_CALL_COPY = 0, 1, 2
+IDS_CALL_SAVE, IDS_CALL_LOAD, IDS_CALL_COPY, IDS_CALL_SET_GOALS = 0, 1, 2, 3
 IDS_OUT_OF_RANGE, IDS_REPEATED = 1, 2
 
 _c32, _f64, _u8p = ctypes.c_int32, ctypes.c_double, ctypes.POINTER(ctypes.c_uint8)
@@ -36,7 +37,7 @@ class TaskNode(ctypes.Structure):
       ('n_clusters', _c32), ('cluster_slots', _c32 * MAX_CHILDREN),
       ('termination_threshold', _f64), ('reward_range', _f64),
       ('n_children', _c32), ('children', _c32 * MAX_CHILDREN),
-      ('aggregator', _c32), ('criterion', _c32),
+      ('aggregator', _c32), ('criterion', _c32), ('goal_slot', _c32),
   ]
 
 
@@ -54,7 +55,7 @@ class Config(ctypes.Structure):
 class SceneSoA(ctypes.Structure):
   _fields_ = [(n, ctypes.c_void_p) for n in
               ('x', 'y', 'm00', 'm01', 'm10', 'm11', 'vx', 'vy', 'member', 'shape', 'pos_f32',
-               'rgb', 'factors')]
+               'rgb', 'factors', 'goal')]
 
 
 class StepOut(ctypes.Structure):
@@ -143,6 +144,10 @@ def load():
   L.swb_engine_state_bytes.restype = ctypes.c_int64
   L.swb_save_engine.argtypes = [vp, vp, ctypes.c_uint64, vp]
   L.swb_load_engine.argtypes = [vp, vp, ctypes.c_uint64, vp]
+  L.swb_pool_goal_pointer.argtypes = [vp, ctypes.POINTER(vp), ctypes.POINTER(ci)]
+  L.swb_set_goals.argtypes = [vp, vp, ci, vp, vp]
+  L.swb_set_goals_dev.argtypes = [vp, vp, ci, ci, vp, vp]
+  L.swb_evaluate_states.argtypes = [vp, vp, ci, ctypes.c_uint64, vp, vp, vp, vp, vp]
   if L.swb_sizeof_config() != ctypes.sizeof(Config):
     raise NativeError('ABI mismatch: swb_config is %d bytes in the library, %d in the binding'
                       % (L.swb_sizeof_config(), ctypes.sizeof(Config)))
@@ -162,7 +167,7 @@ EXPORTS = (
     'swb_load_envs_dev', 'swb_copy_envs_dev', 'swb_env_ids_status_pointer', 'swb_launch_count',
     'swb_sampler_sizeof_program', 'swb_sampler_load', 'swb_sample_scenes', 'swb_refill_device',
     'swb_sampler_pointers', 'swb_pool_pointers', 'swb_engine_state_bytes', 'swb_save_engine',
-    'swb_load_engine')
+    'swb_load_engine', 'swb_pool_goal_pointer', 'swb_set_goals', 'swb_set_goals_dev', 'swb_evaluate_states')
 
 
 def check(rc):

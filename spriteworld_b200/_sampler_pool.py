@@ -49,7 +49,7 @@ def _worker_main(conn, payload, shm_name, cap):
 
   import cloudpickle
   from spriteworld_b200 import scene, sprite_generators
-  init_sprites, n_slots, filters, color_to_rgb = cloudpickle.loads(payload)
+  init_sprites, n_slots, filters, color_to_rgb, goal_distribs = cloudpickle.loads(payload)
   shm = shared_memory.SharedMemory(name=shm_name)
   try:
     while True:
@@ -63,13 +63,17 @@ def _worker_main(conn, payload, shm_name, cap):
       try:
         t0 = time.perf_counter()
         np.random.seed(seed ^ 0x5BD1E995)    # generators whose callables draw from the global stream
-        layout = sprite_generators.batch_of(init_sprites, n, np.random.RandomState(seed))
+        rng = np.random.RandomState(seed)
+        layout = sprite_generators.batch_of(init_sprites, n, rng)
+        goals = scene.draw_goals(goal_distribs, n, rng)   # right after the scenes, same stream
         batch = scene.arrays_from_layout(layout, n_slots, filters, color_to_rgb)
         if n <= cap:
           for name, view in _views(shm.buf, cap, n_slots, n).items():
             view[...] = batch[name]
-          conn.send(('shm', n, time.perf_counter() - t0))
+          conn.send(('shm', (n, goals), time.perf_counter() - t0))
         else:   # larger than the block: through the pipe
+          if goals is not None:
+            batch['goal'] = goals
           conn.send(('pickle', batch, time.perf_counter() - t0))
       except Exception as ex:   # reported to the caller, the worker lives on
         conn.send(('error', ex, 0.0))
@@ -81,11 +85,13 @@ def _worker_main(conn, payload, shm_name, cap):
 
 class SamplerPool(object):
 
-  def __init__(self, n_procs, init_sprites, n_slots, filters, color_to_rgb, capacity=16384):
+  def __init__(self, n_procs, init_sprites, n_slots, filters, color_to_rgb, capacity=16384,
+               goal_distribs=()):
     """capacity: scenes a worker's shared-memory block holds (larger requests fall back to
-    pickling through the pipe)."""
+    pickling through the pipe).  goal_distribs: the task's goal distributions; a block's goals
+    are drawn right after its scenes (scene.draw_goals) and come back as its 'goal' array."""
     import cloudpickle
-    payload = cloudpickle.dumps((init_sprites, n_slots, list(filters), color_to_rgb))
+    payload = cloudpickle.dumps((init_sprites, n_slots, list(filters), color_to_rgb, list(goal_distribs)))
     ctx = mp.get_context('spawn')
     self._conns, self._procs, self._locks, self._shm = [], [], [], []
     self._n_slots, self._cap = int(n_slots), int(capacity)
@@ -132,7 +138,11 @@ class SamplerPool(object):
     if kind == 'error':
       raise out
     if kind == 'shm':
-      return _views(self._shm[worker].buf, self._cap, self._n_slots, out)
+      n, goals = out
+      views = _views(self._shm[worker].buf, self._cap, self._n_slots, n)
+      if goals is not None:
+        views['goal'] = goals
+      return views
     return out
 
   def sample(self, worker, n, seed):

@@ -123,10 +123,13 @@ __global__ void scatter_scenes_kernel(DevState st, int n, const int32_t *__restr
                                       const uint8_t *__restrict__ shape,
                                       const uint8_t *__restrict__ pos_f32,
                                       const uint32_t *__restrict__ rgb,
-                                      const float *__restrict__ factors) {
+                                      const float *__restrict__ factors,
+                                      const double *__restrict__ goal) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n * st.S) return;
   const int sc = i / st.S, s = i - sc * st.S;
+  if (s == 0)
+    for (int j = 0; j < 2 * st.G; ++j) st.p_goal[(size_t)dst[sc] * st.G * 2 + j] = goal[(size_t)sc * st.G * 2 + j];
   const size_t d = (size_t)dst[sc] * st.S + s;
   st.p_x[d] = f64[0 * f64_stride + i];
   st.p_y[d] = f64[1 * f64_stride + i];
@@ -168,7 +171,7 @@ int upload_axis(swb_raster *r, const AxisHost &h, AxisTables *d) {
 extern "C" {
 
 const char *swb_last_error(void) { return g_error.c_str(); }
-int swb_version(void) { return 10; }
+int swb_version(void) { return 11; }
 int swb_sizeof_config(void) { return (int)sizeof(swb_config); }
 int swb_sizeof_task_node(void) { return (int)sizeof(swb_task_node); }
 
@@ -189,10 +192,25 @@ int swb_engine_create(const swb_config *cfg, swb_engine **out) {
       if (nd.n_clusters < 1 || nd.n_clusters > SWB_MAX_CHILDREN) return fail("bad n_clusters");
     } else if (nd.kind == SWB_TASK_FIND_GOAL) {
       if (nd.filter_slot >= SWB_MAX_FILTERS) return fail("bad filter_slot");
+      if (nd.goal_slot < -1 || nd.goal_slot >= SWB_MAX_GOALS)
+        return fail("node %d: goal_slot %d outside [-1, %d) (SWB_MAX_GOALS)", i, nd.goal_slot, SWB_MAX_GOALS);
     } else if (nd.kind != SWB_TASK_NO_REWARD) {
       return fail("unknown task kind %d", nd.kind);
     }
   }
+  // goal slots 0 .. G-1, one node each
+  int n_goals = 0, goal_nodes[SWB_MAX_GOALS];
+  for (int g = 0; g < SWB_MAX_GOALS; ++g) goal_nodes[g] = -1;
+  for (int i = 0; i < cfg->n_nodes; ++i) {
+    const swb_task_node &nd = cfg->nodes[i];
+    if (nd.kind != SWB_TASK_FIND_GOAL || nd.goal_slot < 0) continue;
+    if (goal_nodes[nd.goal_slot] >= 0)
+      return fail("goal_slot %d belongs to nodes %d and %d", nd.goal_slot, goal_nodes[nd.goal_slot], i);
+    goal_nodes[nd.goal_slot] = i;
+    n_goals = std::max(n_goals, nd.goal_slot + 1);
+  }
+  for (int g = 0; g < n_goals; ++g)
+    if (goal_nodes[g] < 0) return fail("goal slots must be 0 .. %d, slot %d has no node", n_goals - 1, g);
   if (cfg->action_kind < 0 || cfg->action_kind > SWB_ACT_EMBODIED) return fail("bad action_kind");
   int n_dev = 0;
   CUDA_TRY(cudaGetDeviceCount(&n_dev));
@@ -220,6 +238,7 @@ int swb_engine_create(const swb_config *cfg, swb_engine **out) {
   st.E = cfg->n_envs;
   st.S = cfg->n_slots;
   st.K = cfg->pool_depth;
+  st.G = n_goals;
   const size_t ES = (size_t)st.E * st.S, EKS = ES * st.K;
   bool ok = true;
   auto A = [&](auto **p, size_t n) {
@@ -234,6 +253,7 @@ int swb_engine_create(const swb_config *cfg, swb_engine **out) {
   A(&st.p_vx, EKS); A(&st.p_vy, EKS);
   A(&st.p_member, EKS); A(&st.p_shape, EKS); A(&st.p_pos_f32, EKS); A(&st.p_rgb, EKS);
   A(&st.p_factors, EKS * 5);
+  if (st.G) A(&st.p_goal, (size_t)st.E * st.K * st.G * 2);
   double *d_verts = nullptr;
   int32_t *d_nv = nullptr;
   A(&eng->d_step_cfg, 1);
@@ -319,9 +339,9 @@ static int release_slot(StagingSlot *slot, cudaStream_t stream) {
 }
 
 // An upload of n scenes in its staging slot: [8 x f64][member u32][rgb u32][factors 5 x f32]
-// [dst i32][shape u8][pos_f32 u8], each array 256-byte aligned, moved with ONE cudaMemcpyAsync and
-// scattered into the pool by one kernel.
-static size_t upload_layout(size_t n, int S, size_t off[7]) {
+// [dst i32][shape u8][pos_f32 u8][goal G x 2 f64], each array 256-byte aligned, moved with ONE
+// cudaMemcpyAsync and scattered into the pool by one kernel.
+static size_t upload_layout(size_t n, int S, int G, size_t off[8]) {
   const size_t nS = n * S;
   size_t o = 0;
   auto take = [&](size_t bytes) { size_t r = o; o += (bytes + 255) & ~(size_t)255; return r; };
@@ -332,6 +352,7 @@ static size_t upload_layout(size_t n, int S, size_t off[7]) {
   off[4] = take(n * sizeof(int32_t));       // dst
   off[5] = take(nS);                        // shape
   off[6] = take(nS);                        // pos_f32
+  off[7] = take(n * G * 2 * sizeof(double)); // goal
   return o;
 }
 
@@ -347,6 +368,8 @@ int swb_upload_scenes(swb_engine *eng, const swb_scene_soa *sc, const int32_t *e
   for (int a = 0; a < 8; ++a)
     if (!f64_src[a]) return fail("swb_upload_scenes: null f64 array %d", a);
   if (!sc->member || !sc->shape || !sc->pos_f32 || !sc->rgb) return fail("swb_upload_scenes: null array");
+  const int G = eng->st.G;
+  if (G && !sc->goal) return fail("swb_upload_scenes: the task samples %d goals per scene, goal is null", G);
   for (int i = 0; i < n; ++i) {
     if (env_ids[i] < 0 || env_ids[i] >= eng->st.E) return fail("env id %d out of range", env_ids[i]);
     if (ring_slots[i] < 0 || ring_slots[i] >= eng->st.K) return fail("ring slot %d out of range", ring_slots[i]);
@@ -357,9 +380,9 @@ int swb_upload_scenes(swb_engine *eng, const swb_scene_soa *sc, const int32_t *e
     if (sh > 6) eng->max_spans = 4;  // stars / spokes: several spans per canvas row
     if (sh && eng->cfg.shape_n_verts[sh] < 3) return fail("shape %d has no vertex table", sh);
   }
-  size_t off[7];
+  size_t off[8];
   StagingSlot *slot = nullptr;
-  if (take_slot(eng->upload_staging, upload_layout(n, S, off), &slot)) return 1;
+  if (take_slot(eng->upload_staging, upload_layout(n, S, G, off), &slot)) return 1;
   unsigned char *h = slot->host;
   for (int a = 0; a < 8; ++a)
     memcpy(h + off[0] + a * nS * sizeof(double), f64_src[a], nS * sizeof(double));
@@ -373,14 +396,17 @@ int swb_upload_scenes(swb_engine *eng, const swb_scene_soa *sc, const int32_t *e
   for (int i = 0; i < n; ++i) dst[i] = env_ids[i] * eng->st.K + ring_slots[i];
   memcpy(h + off[5], sc->shape, nS);
   memcpy(h + off[6], sc->pos_f32, nS);
+  if (G) memcpy(h + off[7], sc->goal, (size_t)n * G * 2 * sizeof(double));
   // everything up to the end of the last used array, in one copy
-  CUDA_TRY(cudaMemcpyAsync(slot->dev, slot->host, off[6] + nS, cudaMemcpyHostToDevice, stream));
+  const size_t end = G ? off[7] + (size_t)n * G * 2 * sizeof(double) : off[6] + nS;
+  CUDA_TRY(cudaMemcpyAsync(slot->dev, slot->host, end, cudaMemcpyHostToDevice, stream));
   const int threads = 256, blocks = (int)((nS + threads - 1) / threads);
   unsigned char *d = slot->dev;
   scatter_scenes_kernel<<<blocks, threads, 0, stream>>>(
       eng->st, n, reinterpret_cast<const int32_t *>(d + off[4]), reinterpret_cast<const double *>(d + off[0]),
       nS, reinterpret_cast<const uint32_t *>(d + off[1]), d + off[5], d + off[6],
-      reinterpret_cast<const uint32_t *>(d + off[2]), reinterpret_cast<const float *>(d + off[3]));
+      reinterpret_cast<const uint32_t *>(d + off[2]), reinterpret_cast<const float *>(d + off[3]),
+      reinterpret_cast<const double *>(d + off[7]));
   eng->launches++;
   CUDA_TRY(cudaGetLastError());
   return release_slot(slot, stream);
@@ -845,7 +871,7 @@ int swb_upload_state(swb_engine *eng, const double *pos_x, const double *pos_y, 
 static int check_record_buffer(const swb_engine *eng, const char *fn, const char *name, const void *rec,
                                uint64_t rec_bytes, int64_t n) {
   if (reinterpret_cast<uintptr_t>(rec) % 16) return fail("%s: %s is not 16-byte aligned", fn, name);
-  const uint64_t need = (uint64_t)n * RecordLayout(eng->st.S).bytes();
+  const uint64_t need = (uint64_t)n * RecordLayout(eng->st.S, eng->st.G).bytes();
   if (rec_bytes < need)
     return fail("%s: %lld records need %llu bytes, the buffer has %llu", fn, (long long)n,
                 (unsigned long long)need, (unsigned long long)rec_bytes);
@@ -950,7 +976,7 @@ static int enqueue_save(swb_engine *eng, const IdCall &c, void *dst, cudaStream_
     eng->launches++;
   }
   save_envs_kernel<T><<<grid_of((size_t)c.n * eng->st.S), 256, 0, stream>>>(
-      eng->st, c, static_cast<unsigned char *>(dst), RecordLayout(eng->st.S).bytes());
+      eng->st, c, static_cast<unsigned char *>(dst), RecordLayout(eng->st.S, eng->st.G).bytes());
   eng->launches++;
   CUDA_TRY(cudaGetLastError());
   return 0;
@@ -964,7 +990,7 @@ static int enqueue_load(swb_engine *eng, const IdCall &c, const void *src, cudaS
     eng->launches += 2;
   }
   load_envs_kernel<T><<<grid_of((size_t)c.n * eng->st.S), 256, 0, stream>>>(
-      eng->st, c, static_cast<const unsigned char *>(src), RecordLayout(eng->st.S).bytes());
+      eng->st, c, static_cast<const unsigned char *>(src), RecordLayout(eng->st.S, eng->st.G).bytes());
   eng->launches++;
   CUDA_TRY(cudaGetLastError());
   return 0;
@@ -975,7 +1001,7 @@ static int enqueue_load(swb_engine *eng, const IdCall &c, const void *src, cudaS
 // read sees the state from before the call.
 template <typename T>
 static int enqueue_copy(swb_engine *eng, const IdCall &c, bool disjoint, cudaStream_t stream) {
-  const size_t threads = (size_t)c.n * eng->st.S, rb = RecordLayout(eng->st.S).bytes();
+  const size_t threads = (size_t)c.n * eng->st.S, rb = RecordLayout(eng->st.S, eng->st.G).bytes();
   if (disjoint) {
     copy_envs_kernel<<<grid_of(threads), 256, 0, stream>>>(eng->st, c);
     eng->launches++;
@@ -1002,7 +1028,7 @@ int64_t swb_env_record_bytes(const swb_engine *eng) {
     fail("swb_env_record_bytes: null engine");
     return -1;
   }
-  return (int64_t)RecordLayout(eng->st.S).bytes();
+  return (int64_t)RecordLayout(eng->st.S, eng->st.G).bytes();
 }
 
 int swb_save_envs(swb_engine *eng, const int32_t *env_ids, int32_t n, void *dst, uint64_t dst_bytes,
@@ -1108,6 +1134,98 @@ int swb_copy_envs_dev(swb_engine *eng, const void *src_ids, const void *dst_ids,
                                    : enqueue_copy<int32_t>(eng, c, false, stream);
 }
 
+}  // extern "C"
+
+// The checks of swb_set_goals / _dev before the ids: the engine has goal slots, n, the goals pointer.
+static int check_set_goals(const swb_engine *eng, const char *fn, int32_t n, const void *ids, const double *goals) {
+  if (!eng) return fail("%s: null engine", fn);
+  if (!eng->st.G) return fail("%s: the task tree samples no goals (G = 0)", fn);
+  if (n < 0) return fail("%s: n = %d", fn, n);
+  if (n == 0) return 0;
+  if (!ids || !goals) return fail("%s: null argument", fn);
+  if (reinterpret_cast<uintptr_t>(goals) % 8) return fail("%s: goals are not 8-byte aligned", fn);
+  return 0;
+}
+
+template <typename T>
+static int enqueue_set_goals(swb_engine *eng, const IdCall &c, const double *goals, cudaStream_t stream) {
+  if (!c.host_checked) {
+    check_ids_kernel<T><<<grid_of(c.n), 256, 0, stream>>>(c, eng->st.E);
+    repeat_ids_kernel<T><<<grid_of(c.n), 256, 0, stream>>>(c, eng->st.E);
+    eng->launches += 2;
+  }
+  set_goals_kernel<T><<<grid_of((size_t)c.n * 2 * eng->st.G), 256, 0, stream>>>(eng->st, c, goals);
+  eng->launches++;
+  CUDA_TRY(cudaGetLastError());
+  return 0;
+}
+
+extern "C" {
+
+int swb_pool_goal_pointer(swb_engine *eng, double **goal, int32_t *n_goals) {
+  if (!eng || !goal || !n_goals) return fail("swb_pool_goal_pointer: null argument");
+  *goal = eng->st.p_goal;
+  *n_goals = eng->st.G;
+  return 0;
+}
+
+int swb_set_goals(swb_engine *eng, const int32_t *env_ids, int32_t n, const double *goals, void *stream_) {
+  static const char fn[] = "swb_set_goals";
+  if (check_set_goals(eng, fn, n, env_ids, goals)) return 1;
+  if (n == 0) return 0;
+  std::vector<uint8_t> mark(eng->st.E, 0);
+  if (check_env_ids(eng, fn, env_ids, n, &mark)) return 1;
+  CUDA_TRY(cudaSetDevice(eng->device));
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  IdCall c;
+  StagingSlot *slot = nullptr;
+  if (stage_ids(eng, env_ids, nullptr, n, 0, stream, &c, &slot) || enqueue_set_goals<int32_t>(eng, c, goals, stream))
+    return 1;
+  return release_slot(slot, stream);
+}
+
+int swb_set_goals_dev(swb_engine *eng, const void *env_ids, int32_t id_dtype, int32_t n, const double *goals,
+                      void *stream_) {
+  static const char fn[] = "swb_set_goals_dev";
+  if (check_set_goals(eng, fn, n, env_ids, goals)) return 1;
+  if (n == 0) return 0;
+  if (check_dev_ids(eng, fn, env_ids, id_dtype)) return 1;
+  CUDA_TRY(cudaSetDevice(eng->device));
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  IdCall c;
+  if (begin_id_call(eng, SWB_IDS_CALL_SET_GOALS, env_ids, nullptr, 0, n, stream, &c)) return 1;
+  return id_dtype == SWB_DTYPE_I64 ? enqueue_set_goals<int64_t>(eng, c, goals, stream)
+                                   : enqueue_set_goals<int32_t>(eng, c, goals, stream);
+}
+
+int swb_evaluate_states(swb_engine *eng, const void *records, int32_t n, uint64_t records_bytes,
+                        const double *goals, double *reward, uint8_t *success, uint8_t *status, void *stream_) {
+  static const char fn[] = "swb_evaluate_states";
+  if (!eng) return fail("%s: null engine", fn);
+  if (n < 0) return fail("%s: n = %d", fn, n);
+  if (goals && !eng->st.G) return fail("%s: goals given, but the task tree samples no goals (G = 0)", fn);
+  if (n == 0) return 0;
+  if (!records || !reward || !success || !status) return fail("%s: null argument", fn);
+  if (check_record_buffer(eng, fn, "records", records, records_bytes, n)) return 1;
+  if (goals && reinterpret_cast<uintptr_t>(goals) % 8) return fail("%s: goals are not 8-byte aligned", fn);
+  const uint64_t rb = RecordLayout(eng->st.S, eng->st.G).bytes();
+  const uint64_t r0 = reinterpret_cast<uintptr_t>(records), r1 = r0 + (uint64_t)n * rb;
+  const struct { const void *p; uint64_t bytes; } outs[3] = {{reward, 8 * (uint64_t)n}, {success, (uint64_t)n},
+                                                             {status, (uint64_t)n}};
+  for (const auto &o : outs) {
+    const uint64_t o0 = reinterpret_cast<uintptr_t>(o.p);
+    if (o0 < r1 && r0 < o0 + o.bytes) return fail("%s: an output overlaps the records", fn);
+  }
+  CUDA_TRY(cudaSetDevice(eng->device));
+  const unsigned blocks = (unsigned)(((int64_t)n + ROLLOUT_WARPS - 1) / ROLLOUT_WARPS);
+  evaluate_kernel<<<blocks, ROLLOUT_WARPS * 32, 0, static_cast<cudaStream_t>(stream_)>>>(
+      eng->st, eng->d_step_cfg, static_cast<const unsigned char *>(records), (size_t)rb, n, goals, reward,
+      success, status);
+  eng->launches++;
+  CUDA_TRY(cudaGetLastError());
+  return 0;
+}
+
 int swb_rollout_states(swb_engine *eng, const void *roots, int32_t n_roots, uint64_t roots_bytes,
                        const void *actions, int32_t action_dtype, int32_t n_steps, int32_t n_candidates,
                        const swb_step_out *out, void *leaves, uint64_t leaves_bytes, int32_t *span_class,
@@ -1121,7 +1239,7 @@ int swb_rollout_states(swb_engine *eng, const void *roots, int32_t n_roots, uint
   if (check_rollout(eng, fn, roots ? "roots" : "envs", actions, action_dtype, n_steps, n_candidates, n_roots,
                     out))
     return 1;
-  const uint64_t rb = RecordLayout(eng->st.S).bytes();
+  const uint64_t rb = RecordLayout(eng->st.S, eng->st.G).bytes();
   const uint64_t plans = (uint64_t)n_roots * n_candidates;
   if (roots && check_record_buffer(eng, fn, "roots", roots, roots_bytes, n_roots)) return 1;
   if (leaves && check_record_buffer(eng, fn, "leaves", leaves, leaves_bytes, (int64_t)plans)) return 1;
@@ -1148,7 +1266,7 @@ int swb_render_states(swb_engine *eng, swb_raster *r, const void *records, int32
   if (span_class != 1 && span_class != 4) return fail("%s: span_class must be 1 or 4, got %d", fn, span_class);
   if (!frames || !status) return fail("%s: null frames or status", fn);
   const RasterDev &rd = r->rd;
-  const uint64_t rb = RecordLayout(eng->st.S).bytes();
+  const uint64_t rb = RecordLayout(eng->st.S, eng->st.G).bytes();
   const uint64_t r0 = reinterpret_cast<uintptr_t>(records), r1 = r0 + (uint64_t)n * rb;
   const uint64_t f0 = reinterpret_cast<uintptr_t>(frames), s0 = reinterpret_cast<uintptr_t>(status);
   if (f0 < r1 && r0 < f0 + (uint64_t)n * rd.H * rd.W * 3) return fail("%s: the frames overlap the records", fn);
@@ -1181,7 +1299,7 @@ int swb_render_masks(swb_engine *eng, int32_t width, int32_t height, int32_t ant
   const MaskLayout L(eng->st.S, width, height, anti_aliasing);
   if ((int64_t)n * L.n_bands > INT32_MAX)
     return fail("%s: n = %d masks of %d bands each exceed 2^31 - 1 CTAs", fn, n, L.n_bands);
-  const uint64_t rb = RecordLayout(eng->st.S).bytes();
+  const uint64_t rb = RecordLayout(eng->st.S, eng->st.G).bytes();
   if (records) {
     if (check_record_buffer(eng, fn, "records", records, records_bytes, n)) return 1;
     const uint64_t r0 = reinterpret_cast<uintptr_t>(records), m0 = reinterpret_cast<uintptr_t>(masks);
@@ -1227,8 +1345,9 @@ __global__ void sample_scenes_kernel(const swb_scene_program *__restrict__ prog,
   if (i >= n) return;
   const int64_t g = env_ids[i], a = scene_idx[i];
   swb_sampler::Scene sc;
+  double goal[2 * SWB_MAX_GOALS];
   const int bad = swb_sampler::sample_and_pack(
-      *prog, seed, (uint64_t)g, (uint64_t)a, S, sc,
+      *prog, seed, (uint64_t)g, (uint64_t)a, S, sc, goal,
       [&](int slot, const swb_sampler::Packed &o, const swb_sampler::Sprite *s) {
         const size_t d = (size_t)i * S + slot;
         out.x[d] = o.x; out.y[d] = o.y;
@@ -1242,6 +1361,8 @@ __global__ void sample_scenes_kernel(const swb_scene_program *__restrict__ prog,
           out.factor_kind[d * swb_sampler::kFactors + f] = s ? s->kind[f] : (uint8_t)SWB_FT_NONE;
         }
       });
+  if (out.goal)
+    for (int j = 0; j < 2 * prog->n_goals; ++j) out.goal[(size_t)i * 2 * prog->n_goals + j] = goal[j];
   if (bad >= 0) sampler_fail(status, bad, g, a);
 }
 
@@ -1262,8 +1383,9 @@ __global__ void refill_device_kernel(const swb_scene_program *__restrict__ prog,
   for (; a <= want; ++a) {
     const size_t base = ((size_t)e * st.K + (size_t)(a % st.K)) * st.S;
     swb_sampler::Scene sc;
+    double goal[2 * SWB_MAX_GOALS];
     const int bad = swb_sampler::sample_and_pack(
-        *prog, seed, (uint64_t)g, (uint64_t)a, st.S, sc,
+        *prog, seed, (uint64_t)g, (uint64_t)a, st.S, sc, goal,
         [&](int slot, const swb_sampler::Packed &o, const swb_sampler::Sprite *) {
           const size_t d = base + slot;
           st.p_x[d] = o.x; st.p_y[d] = o.y;
@@ -1273,6 +1395,8 @@ __global__ void refill_device_kernel(const swb_scene_program *__restrict__ prog,
           st.p_rgb[d] = (uint32_t)o.rgb[0] | ((uint32_t)o.rgb[1] << 8) | ((uint32_t)o.rgb[2] << 16);
           for (int f = 0; f < 5; ++f) st.p_factors[d * 5 + f] = o.factors[f];
         });
+    const size_t gb = ((size_t)e * st.K + (size_t)(a % st.K)) * st.G * 2;
+    for (int j = 0; j < 2 * st.G; ++j) st.p_goal[gb + j] = goal[j];
     if (bad >= 0) sampler_fail(status, bad, g, a);
   }
   if (want > refilled_upto[e]) refilled_upto[e] = want;
@@ -1290,6 +1414,9 @@ int check_program(const swb_scene_program &p, int S) {
   auto consts_ok = [&](int off, int n) { return n >= 1 && off >= 0 && off + n <= p.n_consts; };
   for (int f = 0; f < p.n_filters; ++f)
     if (!pc_ok(p.filter_pc[f])) return fail("program: filter %d has no code", f);
+  if (p.n_goals < 0 || p.n_goals > SWB_MAX_GOALS) return fail("program: n_goals %d out of range", p.n_goals);
+  for (int i = 0; i < p.n_goals; ++i)
+    if (!pc_ok(p.goal_pc[i])) return fail("program: goal %d has no code", i);
   for (int i = 0; i < p.n_ops; ++i) {
     const swb_prog_op &o = p.ops[i];
     const bool key_ok = o.key >= 0 && o.key < swb_sampler::kFactors;
@@ -1323,6 +1450,9 @@ int swb_sampler_load(swb_engine *eng, const swb_scene_program *prog, uint64_t se
   if (!eng || !prog) return fail("swb_sampler_load: null argument");
   if (env_offset < 0) return fail("swb_sampler_load: env_offset must be >= 0");
   if (check_program(*prog, eng->st.S)) return 1;
+  if (prog->n_goals != eng->st.G)
+    return fail("swb_sampler_load: the program draws %d goals per scene, the task tree has %d goal slots",
+                prog->n_goals, eng->st.G);
   CUDA_TRY(cudaSetDevice(eng->device));
   if (!eng->d_prog) {  // all three or none: the other calls test d_prog alone
     swb_scene_program *prog_d = nullptr;
@@ -1429,7 +1559,7 @@ struct CkptField {
 
 struct CkptLayout {
   enum { POS_X, POS_Y, CURSOR, STEP_COUNT, SCENE_SERIAL, RESET_NEXT, P_X, P_Y, P_M00, P_M01, P_M10, P_M11,
-         P_VX, P_VY, MEMBER, RGB, FACTORS, SHAPE, POS_F32, REFILLED_UPTO, N };
+         P_VX, P_VY, MEMBER, RGB, FACTORS, SHAPE, POS_F32, REFILLED_UPTO, GOAL, N };
   CkptField f[N];
   size_t header = 0, total = 0;
 
@@ -1444,7 +1574,8 @@ struct CkptLayout {
         {"m10", st.p_m10, 8, EKS}, {"m11", st.p_m11, 8, EKS}, {"vx", st.p_vx, 8, EKS}, {"vy", st.p_vy, 8, EKS},
         {"member", st.p_member, 4, EKS}, {"rgb", st.p_rgb, 4, EKS}, {"factors", st.p_factors, 4, EKS * 5},
         {"shape", st.p_shape, 1, EKS}, {"pos_f32", st.p_pos_f32, 1, EKS},
-        {"refilled_upto", eng->d_refilled_upto, 8, E}};
+        {"refilled_upto", eng->d_refilled_upto, 8, E},
+        {"goal", st.p_goal, 8, E * st.K * st.G * 2}};   // no bytes when G == 0
     header = align16(kCkptFixed + sizeof(swb_config));
     size_t o = header;
     for (int i = 0; i < N; ++i) {

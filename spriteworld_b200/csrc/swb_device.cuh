@@ -10,7 +10,8 @@
 //                shape,pos_f32           [E*K*S] u8
 //                rgb                     [E*K*S] u32 (r | g<<8 | b<<16)
 //                factors                 [E*K*S*5] f32 (scale, angle, c0, c1, c2)
-//   index of (env e, ring slot k, sprite slot s) = (e*K + k)*S + s
+//                goal                    [E*K*G*2] f64 (sampled FindGoalPosition goals; only when G > 0)
+//   index of (env e, ring slot k, sprite slot s) = (e*K + k)*S + s; goal slot g: ((e*K + k)*G + g)*2
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -31,6 +32,8 @@ struct DevState {
   uint8_t *p_shape, *p_pos_f32;
   uint32_t *p_rgb;
   float *p_factors;
+  int G;            // goal slots per scene (0: every goal of the task tree is a constant)
+  double *p_goal;   // null when G == 0
   const double *shape_verts;  // [13][32][2]
   const int32_t *shape_n;     // [13]
 };

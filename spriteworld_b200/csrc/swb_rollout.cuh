@@ -13,7 +13,8 @@
 // about to reset) lanes < S write record w: the record swb_save_envs would save of an env that
 // started in the root state and took the plan's live steps -- the root's scene, the final
 // positions, step_count after the counted steps and reset_next = 1 iff the last of them was LAST.
-// Leaves and roots share the record format, so one launch is one level of a search tree.
+// Leaves and roots share the record format, so one launch is one level of a search tree.  A leaf
+// keeps its root's goals.
 //
 // Actions are [T][R][C][A]: at a step the warps of a CTA read consecutive rows, every lane the
 // row of its warp (one broadcast transaction), and the row of step t + 1 is loaded before step t
@@ -37,9 +38,11 @@ struct RolloutRecords {
 };
 
 // Root record `rec` in the warp's WarpSprites, as stage_sprites stages an env's pool entry with
-// its live positions (shape ids sanitised by read_record); *vx, *vy: lane s holds slot s's velocity.
+// its live positions and goals (shape ids sanitised by read_record); *vx, *vy: lane s holds slot s's
+// velocity.
 __device__ __forceinline__ void stage_record(const DevState &st, WarpSprites &ws, int S,
                                              const unsigned char *rec, int lane, double *vx, double *vy) {
+  if (lane < 2 * st.G) ws.goal[lane] = record_goals(st, rec)[lane];
   *vx = 0.; *vy = 0.;
   if (lane < S) {
     const SlotRecord r = read_record(st, rec, lane);
@@ -73,6 +76,10 @@ rollout_kernel(DevState st, const StepCfg *__restrict__ step_cfg, const void *__
   const unsigned char *root = kRecordRoots ? io.roots + (size_t)e * io.record_bytes : nullptr;
   // else the env's next step starts another scene: nothing to plan in
   const bool resetting = kRecordRoots ? root[L.reset_next()] != 0 : st.reset_next[e] != 0;
+  // a leaf keeps its root's goals: stored now, before the plan keeps registers busy
+  if (kLeaves && lane < 2 * st.G)
+    record_goals(st, io.leaves + (size_t)w * io.record_bytes)[lane] =
+        (kRecordRoots ? record_goals(st, root) : state_goals(st, e))[lane];
   int t = 0, count = 0;
   bool ended = false;
   if (!resetting) {
@@ -81,7 +88,7 @@ rollout_kernel(DevState st, const StepCfg *__restrict__ step_cfg, const void *__
       stage_record(st, ws, S, root, lane, &vx, &vy);
       count = *reinterpret_cast<const int32_t *>(root + L.step_count());
     } else {
-      stage_sprites(st, ws, S, e, (e * st.K + st.cursor[e]) * S, false, lane, &vx, &vy);
+      stage_sprites(st, ws, S, e, e * st.K + st.cursor[e], false, lane, &vx, &vy);
       count = st.step_count[e];
     }
     ActionRow next = load_action(actions, action_dtype, (size_t)w);
@@ -126,7 +133,32 @@ rollout_kernel(DevState st, const StepCfg *__restrict__ step_cfg, const void *__
       leaf.step_count = count;   // lane 0 counted the steps; write_record stores slot 0's copy
       leaf.reset_next = ended ? 1 : 0;
     }
-    write_record(io.leaves + (size_t)w * io.record_bytes, S, lane, leaf);
+    write_record(io.leaves + (size_t)w * io.record_bytes, S, st.G, lane, leaf);
+  }
+}
+
+// swb_evaluate_states: the task tree's value on record i (one warp each) at its live positions, with
+// row i of `goals` in place of the record's goals when `goals` is not null.  Read-only.
+__global__ void __launch_bounds__(ROLLOUT_WARPS * 32)
+evaluate_kernel(DevState st, const StepCfg *__restrict__ step_cfg, const unsigned char *__restrict__ recs,
+                size_t record_bytes, int n, const double *__restrict__ goals, double *__restrict__ reward,
+                uint8_t *__restrict__ success, uint8_t *__restrict__ status) {
+  __shared__ WarpSprites s_ws[ROLLOUT_WARPS];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int i = blockIdx.x * ROLLOUT_WARPS + warp;
+  if (i >= n) return;
+  WarpSprites &ws = s_ws[warp];
+  double vx, vy;
+  stage_record(st, ws, st.S, recs + (size_t)i * record_bytes, lane, &vx, &vy);
+  if (goals && lane < 2 * st.G) ws.goal[lane] = goals[(size_t)i * 2 * st.G + lane];
+  __syncwarp();
+  if (lane == 0) {
+    double tr;
+    int succ, stat = 0;
+    task_eval(*step_cfg, ws, st.S, &tr, &succ, &stat);
+    reward[i] = tr;
+    success[i] = (uint8_t)succ;
+    status[i] = (uint8_t)stat;
   }
 }
 

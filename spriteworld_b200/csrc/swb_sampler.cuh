@@ -386,14 +386,34 @@ SWB_HD void empty_slot(Packed &o) {
   for (int f = 0; f < 5; ++f) o.factors[f] = 0.f;
 }
 
+// The scene's goals, drawn after its sprites from the same stream: goal slot i is the (x, y) that
+// the distribution code at goal_pc[i] draws.  Returns -1, or the op of a failed rejection loop
+// (that goal is then (0, 0)).
+SWB_HD int sample_goals(const swb_scene_program &p, Stream &rng, double *goal) {
+  int bad = -1;
+  for (int i = 0; i < p.n_goals; ++i) {
+    Sprite s;
+    set_defaults(s);
+    const int b = sample_sprite(p, p.goal_pc[i], rng, s);
+    if (b >= 0 && bad < 0) bad = b;
+    goal[2 * i] = b >= 0 ? 0.0 : s.val[F_X];
+    goal[2 * i + 1] = b >= 0 ? 0.0 : s.val[F_Y];
+  }
+  return bad;
+}
+
 // Samples scene (g, a) and hands every one of its S slots to `put(slot, packed, sprite or null)`,
-// empty slots first.  Returns -1, or the op of a failed rejection loop (all slots empty then).
+// empty slots first, and its goals to goal[0 .. 2 * n_goals).  Returns -1, or the op of a failed
+// rejection loop (all slots empty then, if it was the sprites').  The goals come after the sprites,
+// so a program's sprites do not depend on its goals.
 template <typename Put>
 SWB_HD int sample_and_pack(const swb_scene_program &p, uint64_t seed, uint64_t g, uint64_t a, int S,
-                           Scene &sc, Put &&put) {
+                           Scene &sc, double *goal, Put &&put) {
   Stream rng;
   rng.init(seed, g, a);
-  const int bad = sample_scene(p, rng, sc);
+  int bad = sample_scene(p, rng, sc);
+  const int bad_goal = sample_goals(p, rng, goal);
+  if (bad < 0) bad = bad_goal;
   const int n = sc.n <= S ? sc.n : 0;
   Packed o;
   for (int j = 0; j < S - n; ++j) {

@@ -20,9 +20,10 @@ int64_t swb_host_sample_scenes(const swb_scene_program *prog, uint64_t seed, int
                                int32_t *fail_op, int64_t *fail_index) {
   int64_t failures = 0;
   swb_sampler::Scene sc;
+  double goal[2 * SWB_MAX_GOALS];
   for (int64_t i = 0; i < n; ++i) {
     const int bad = swb_sampler::sample_and_pack(
-        *prog, seed, (uint64_t)env_ids[i], (uint64_t)scene_idx[i], S, sc,
+        *prog, seed, (uint64_t)env_ids[i], (uint64_t)scene_idx[i], S, sc, goal,
         [&](int slot, const swb_sampler::Packed &o, const swb_sampler::Sprite *s) {
           const size_t d = (size_t)i * S + slot;
           out->x[d] = o.x; out->y[d] = o.y;
@@ -36,6 +37,8 @@ int64_t swb_host_sample_scenes(const swb_scene_program *prog, uint64_t seed, int
             out->factor_kind[d * swb_sampler::kFactors + f] = s ? s->kind[f] : (uint8_t)SWB_FT_NONE;
           }
         });
+    if (out->goal)
+      for (int j = 0; j < 2 * prog->n_goals; ++j) out->goal[(size_t)i * 2 * prog->n_goals + j] = goal[j];
     if (bad >= 0) {
       if (!failures) {
         if (fail_op) *fail_op = bad;

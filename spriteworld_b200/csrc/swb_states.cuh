@@ -29,10 +29,10 @@
 
 namespace swb {
 
-// Byte offsets of the fields of one record of an engine with S slots.
+// Byte offsets of the fields of one record of an engine with S slots and G goal slots.
 struct RecordLayout {
-  int S;
-  __host__ __device__ explicit RecordLayout(int S_) : S(S_) {}
+  int S, G;
+  __host__ __device__ explicit RecordLayout(int S_, int G_ = 0) : S(S_), G(G_) {}
   // x0, y0, m00, m01, m10, m11, vx, vy, pos_x, pos_y: f64 [10][S] from offset 0
   __host__ __device__ size_t member() const { return 80 * (size_t)S; }      // u32 [S]
   __host__ __device__ size_t rgb() const { return 84 * (size_t)S; }         // u32 [S]
@@ -41,7 +41,8 @@ struct RecordLayout {
   __host__ __device__ size_t reset_next() const { return 108 * (size_t)S + 4; }  // u8
   __host__ __device__ size_t shape() const { return 108 * (size_t)S + 5; }  // u8 [S]
   __host__ __device__ size_t pos_f32() const { return 109 * (size_t)S + 5; }  // u8 [S]
-  __host__ __device__ size_t used() const { return 110 * (size_t)S + 5; }
+  __host__ __device__ size_t goals() const { return (110 * (size_t)S + 5 + 7) & ~(size_t)7; }  // f64 [G][2]
+  __host__ __device__ size_t used() const { return G ? goals() + 16 * (size_t)G : 110 * (size_t)S + 5; }
   __host__ __device__ size_t bytes() const { return (used() + 15) & ~(size_t)15; }  // zero padded
 };
 
@@ -115,8 +116,10 @@ __device__ __forceinline__ SlotRecord read_record(const DevState &st, const unsi
   return r;
 }
 
-__device__ __forceinline__ void write_record(unsigned char *rec, int S, int s, const SlotRecord &r) {
-  const RecordLayout L(S);
+// Slot s of a record.  Slot 0 also zeroes the padding after the slot fields, around the goals
+// (which write_goals stores, in any order with this).
+__device__ __forceinline__ void write_record(unsigned char *rec, int S, int G, int s, const SlotRecord &r) {
+  const RecordLayout L(S, G);
   double *f64 = reinterpret_cast<double *>(rec);
 #pragma unroll
   for (int a = 0; a < 10; ++a) f64[a * S + s] = r.f64[a];
@@ -129,11 +132,29 @@ __device__ __forceinline__ void write_record(unsigned char *rec, int S, int s, c
   if (s == 0) {
     *reinterpret_cast<int32_t *>(rec + L.step_count()) = r.step_count;
     rec[L.reset_next()] = r.reset_next;
-    for (size_t b = L.used(); b < L.bytes(); ++b) rec[b] = 0;  // saved bytes are deterministic
+    // saved bytes are deterministic
+    const size_t g0 = G ? L.goals() : L.bytes(), g1 = G ? L.used() : L.bytes();
+    for (size_t b = 110 * (size_t)S + 5; b < g0; ++b) rec[b] = 0;
+    for (size_t b = g1; b < L.bytes(); ++b) rec[b] = 0;
   }
 }
 
-// The id lists of a record call (swb_save_envs / swb_load_envs / swb_copy_envs and their _dev
+// The goals (G x (x, y)) of the scene env e is on, of a record, and a copy of G of them (zeros when
+// src is null).
+__device__ __forceinline__ double *state_goals(const DevState &st, int e) {
+  return st.p_goal + ((size_t)e * st.K + st.cursor[e]) * st.G * 2;
+}
+__device__ __forceinline__ const double *record_goals(const DevState &st, const unsigned char *rec) {
+  return reinterpret_cast<const double *>(rec + RecordLayout(st.S, st.G).goals());
+}
+__device__ __forceinline__ void write_goals(double *dst, const double *src, int G) {
+  for (int i = 0; i < 2 * G; ++i) dst[i] = src ? src[i] : 0.;
+}
+__device__ __forceinline__ double *record_goals(const DevState &st, unsigned char *rec) {
+  return reinterpret_cast<double *>(rec + RecordLayout(st.S, st.G).goals());
+}
+
+// The id lists of a record call (and of swb_set_goals) (swb_save_envs / swb_load_envs / swb_copy_envs and their _dev
 // variants).  Ids checked on the host (host_checked) are int32 and all valid: no check kernel runs
 // before the call's kernels, the call is never refused and reports nothing.
 //
@@ -231,7 +252,10 @@ __global__ void save_envs_kernel(DevState st, IdCall c, unsigned char *__restric
   if (i >= (size_t)c.n * st.S) return;
   const int r = (int)(i / st.S), s = (int)(i - (size_t)r * st.S);
   const int id = (int)ids_of<T>(c, 0)[r];
-  write_record(rec + (size_t)r * record_bytes, st.S, s, call_refused(c) ? SlotRecord{} : read_state(st, id, s));
+  const bool refused = call_refused(c);
+  unsigned char *dst = rec + (size_t)r * record_bytes;
+  write_record(dst, st.S, st.G, s, refused ? SlotRecord{} : read_state(st, id, s));
+  if (s == 0 && st.G) write_goals(record_goals(st, dst), refused ? nullptr : state_goals(st, id), st.G);
 }
 
 // Device-checked copy, first half: the repeat check of the destinations, and record i <- env
@@ -245,7 +269,11 @@ __global__ void stage_copy_dev_kernel(DevState st, IdCall c, unsigned char *__re
   const int r = (int)(i / st.S), s = (int)(i - (size_t)r * st.S);
   if (s == 0) check_repeat<T>(c, st.E, r);
   const T id = ids_of<T>(c, 0)[r];
-  if (id_in_range(id, st.E)) write_record(rec + (size_t)r * record_bytes, st.S, s, read_state(st, (int)id, s));
+  if (id_in_range(id, st.E)) {
+    unsigned char *dst = rec + (size_t)r * record_bytes;
+    write_record(dst, st.S, st.G, s, read_state(st, (int)id, s));
+    if (s == 0 && st.G) write_goals(record_goals(st, dst), state_goals(st, (int)id), st.G);
+  }
 }
 
 // env ids[dst_arg][i] <- record i (ids distinct), unless the call is refused
@@ -257,7 +285,9 @@ __global__ void load_envs_kernel(DevState st, IdCall c, const unsigned char *__r
   if (i >= (size_t)c.n * st.S || call_refused(c)) return;
   const int r = (int)(i / st.S), s = (int)(i - (size_t)r * st.S);
   const int id = (int)ids_of<T>(c, c.dst_arg)[r];
-  write_state(st, id, s, read_record(st, rec + (size_t)r * record_bytes, s));
+  const unsigned char *src = rec + (size_t)r * record_bytes;
+  write_state(st, id, s, read_record(st, src, s));
+  if (s == 0 && st.G) write_goals(state_goals(st, id), record_goals(st, src), st.G);
 }
 
 // Host-checked copy of id sets that do not overlap (no thread reads what another writes):
@@ -266,7 +296,21 @@ __global__ void copy_envs_kernel(DevState st, IdCall c) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= c.n * st.S) return;
   const int r = i / st.S, s = i - r * st.S;
-  write_state(st, ids_of<int32_t>(c, 1)[r], s, read_state(st, ids_of<int32_t>(c, 0)[r], s));
+  const int src = ids_of<int32_t>(c, 0)[r], dst = ids_of<int32_t>(c, 1)[r];
+  write_state(st, dst, s, read_state(st, src, s));
+  if (s == 0 && st.G) write_goals(state_goals(st, dst), state_goals(st, src), st.G);
+}
+
+// swb_set_goals / swb_set_goals_dev: one thread per (id, goal value); env ids[0][i] <- goals of row i,
+// unless the call is refused
+template <typename T>
+__global__ void set_goals_kernel(DevState st, IdCall c, const double *__restrict__ goals) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i == 0) report_ids<T>(c, st.E);
+  const size_t per = 2 * (size_t)st.G;
+  if (i >= (size_t)c.n * per || call_refused(c)) return;
+  const int r = (int)(i / per), j = (int)(i - (size_t)r * per);
+  state_goals(st, (int)ids_of<T>(c, 0)[r])[j] = goals[i];
 }
 
 }  // namespace swb

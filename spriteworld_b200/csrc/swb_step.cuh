@@ -19,6 +19,7 @@ struct WarpSprites {
   double m00[SWB_MAX_SLOTS], m01[SWB_MAX_SLOTS], m10[SWB_MAX_SLOTS], m11[SWB_MAX_SLOTS];
   uint32_t member[SWB_MAX_SLOTS];
   uint8_t shape[SWB_MAX_SLOTS], f32[SWB_MAX_SLOTS];
+  double goal[2 * SWB_MAX_GOALS];  // the scene's sampled goals (x, y) per goal slot; G of them staged
 };
 
 // numpy pairwise_sum: < 8 sequential, <= 128 eight accumulators
@@ -128,7 +129,9 @@ struct TaskVal {
   int success;
 };
 
-// tasks.py:126-158
+// tasks.py:126-158.  The goal is the node's constant, or for goal_slot >= 0 the env's staged goal:
+// the same arithmetic on another operand, so an env whose goal is (gx, gy) gets the value of the
+// constant-goal node with goal = {gx, gy}.
 __device__ TaskVal find_goal(const swb_task_node &nd, const WarpSprites &ws, int S) {
   double rewards[SWB_MAX_SLOTS];
   int n = 0;
@@ -136,7 +139,9 @@ __device__ TaskVal find_goal(const swb_task_node &nd, const WarpSprites &ws, int
   for (int s = 0; s < S; s++) {
     if (!ws.shape[s]) continue;
     if (nd.filter_slot >= 0 && !((ws.member[s] >> nd.filter_slot) & 1u)) continue;
-    const double dx = __dsub_rn(ws.x[s], nd.goal[0]), dy = __dsub_rn(ws.y[s], nd.goal[1]);
+    const int g = nd.goal_slot;
+    const double gx = g >= 0 ? ws.goal[2 * g] : nd.goal[0], gy = g >= 0 ? ws.goal[2 * g + 1] : nd.goal[1];
+    const double dx = __dsub_rn(ws.x[s], gx), dy = __dsub_rn(ws.y[s], gy);
     const double t0 = __dmul_rn(nd.weights[0], __dmul_rn(dx, dx));
     const double t1 = __dmul_rn(nd.weights[1], __dmul_rn(dy, dy));
     const double tot = __dadd_rn(__dadd_rn(0., t0), t1);
@@ -504,10 +509,13 @@ __device__ __forceinline__ int finish_step(const StepCfg &c_step, const WarpSpri
   return (succ || oof || timeout) ? SWB_STEP_LAST : SWB_STEP_MID;
 }
 
-// The env's current scene -- the pool entry at `scene0` -- in the warp's WarpSprites, with the
-// pool's initial positions (`from_pool`) or the live ones; *vx, *vy: lane s holds slot s's velocity.
-__device__ __forceinline__ void stage_sprites(const DevState &st, WarpSprites &ws, int S, int e, int scene0,
+// The env's current scene -- pool entry `entry` = e * K + ring slot -- in the warp's WarpSprites, with
+// the pool's initial positions (`from_pool`) or the live ones, and its goals; *vx, *vy: lane s holds
+// slot s's velocity.
+__device__ __forceinline__ void stage_sprites(const DevState &st, WarpSprites &ws, int S, int e, int entry,
                                               bool from_pool, int lane, double *vx, double *vy) {
+  const int scene0 = entry * S;
+  if (lane < 2 * st.G) ws.goal[lane] = st.p_goal[(size_t)entry * st.G * 2 + lane];
   *vx = 0.; *vy = 0.;
   if (lane < S) {
     const int sc = scene0 + lane;
@@ -547,7 +555,7 @@ step_kernel(DevState st, const StepCfg *__restrict__ step_cfg, const void *__res
   int cursor = st.cursor[e];
   if (resetting) cursor = (cursor + 1) % st.K;  // environment.py:90-91 -> reset() :74-78
   double vx, vy;
-  stage_sprites(st, ws, S, e, (e * st.K + cursor) * S, resetting, lane, &vx, &vy);
+  stage_sprites(st, ws, S, e, e * st.K + cursor, resetting, lane, &vx, &vy);
 
   double cost = 0.;
   int status = 0;

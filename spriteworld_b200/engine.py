@@ -198,6 +198,9 @@ class Engine(object):
     h = ctypes.c_void_p()
     _native.check(self._lib.swb_engine_create(ctypes.byref(cfg), ctypes.byref(h)))
     self._h = h
+    gp, ng = ctypes.c_void_p(), ctypes.c_int32()
+    _native.check(self._lib.swb_pool_goal_pointer(h, ctypes.byref(gp), ctypes.byref(ng)))
+    self.n_goals = ng.value   # G: goal slots per scene (sampled FindGoalPosition goals)
     E = self.n_envs
     # the four per-env outputs of a step are slices of ONE buffer (11 bytes per env: reward f64,
     # step_type i8, success u8, status u8), so that a multi-GPU gather moves them in one piece
@@ -242,6 +245,11 @@ class Engine(object):
     soa.pos_f32 = arr('pos_f32', np.uint8)
     soa.rgb = arr('rgb', np.uint8, (3,))
     soa.factors = arr('factors', np.float32, (5,)) if 'factors' in scenes else None
+    if self.n_goals:
+      goal = np.ascontiguousarray(scenes['goal'], dtype=np.float64)
+      assert goal.shape == (n, self.n_goals, 2), ('goal', goal.shape, (n, self.n_goals, 2))
+      keep.append(goal)
+      soa.goal = goal.ctypes.data
     env_ids = np.ascontiguousarray(env_ids, dtype=np.int32)
     ring_slots = np.ascontiguousarray(ring_slots, dtype=np.int32)
     _native.check(self._lib.swb_upload_scenes(self._h, ctypes.byref(soa), _as_ptr(env_ids),
@@ -356,7 +364,7 @@ class Engine(object):
       self.check_states(states, n)
     if leaves is True:
       leaves = EnvStates(torch.empty((n * C, self.record_bytes), dtype=torch.uint8, device=self.device),
-                         1, self.signature, self.n_slots)
+                         1, self.signature, self.n_slots, self.n_goals)
     elif leaves is not None:
       self.check_states(leaves, n * C)
     out, res = rollout_outputs(out, T, n, C, self.device)
@@ -590,12 +598,12 @@ class Engine(object):
       _native.check(self._lib.swb_save_envs_dev(self._h, ctypes.c_void_p(ids.data_ptr()), dt, ids.numel(),
                                                 ctypes.c_void_p(data.data_ptr()), data.numel(),
                                                 ctypes.byref(span), self._stream()))
-      return EnvStates(data, span.value, self.signature, self.n_slots)
+      return EnvStates(data, span.value, self.signature, self.n_slots, self.n_goals)
     ids = self._all_or(env_ids)
     data = torch.empty((len(ids), rb), dtype=torch.uint8, device=self.device)
     _native.check(self._lib.swb_save_envs(self._h, _as_ptr(ids), len(ids), ctypes.c_void_p(data.data_ptr()),
                                           data.numel(), ctypes.byref(span), self._stream()))
-    return EnvStates(data, span.value, self.signature, self.n_slots)
+    return EnvStates(data, span.value, self.signature, self.n_slots, self.n_goals)
 
   def check_states(self, states, n):
     """ValueError unless `states` holds n records that this engine can load."""
@@ -696,7 +704,8 @@ class Engine(object):
   def sample_scenes(self, env_ids, scene_idx):
     """Scenes (env_ids[i], scene_idx[i]) (global env ids, absolute scene indices) as device
     tensors: the fields of a scene batch shaped (n, S[, ...]) plus 'factor_value' float64 and
-    'factor_kind' uint8 (n, S, 10).  The pool is not touched."""
+    'factor_kind' uint8 (n, S, 10), and with sampled goals 'goal' float64 (n, G, 2).  The pool is
+    not touched."""
     from spriteworld_b200 import scene_program
     ids = torch.as_tensor(env_ids, dtype=torch.int64, device=self.device).contiguous()
     idx = torch.as_tensor(scene_idx, dtype=torch.int64, device=self.device).contiguous()
@@ -712,6 +721,8 @@ class Engine(object):
     out['factors'] = torch.zeros((n, S, 5), dtype=torch.float32, device=self.device)
     out['factor_value'] = torch.zeros((n, S, 10), **f64)
     out['factor_kind'] = torch.zeros((n, S, 10), dtype=torch.uint8, device=self.device)
+    if self.n_goals:
+      out['goal'] = torch.zeros((n, self.n_goals, 2), **f64)
     st = scene_program.sample_out_struct(out, lambda t: t.data_ptr())
     _native.check(self._lib.swb_sample_scenes(self._h, ctypes.c_void_p(ids.data_ptr()),
                                               ctypes.c_void_p(idx.data_ptr()), n, ctypes.byref(st),
@@ -724,7 +735,8 @@ class Engine(object):
 
   def pool_tensors(self):
     """Zero-copy views of the scene pool, shaped (E, K, S[, ...]): x .. vy float64, member int32,
-    shape and pos_f32 uint8, rgb uint8 (E, K, S, 4) (r, g, b, 0), factors float32 (E, K, S, 5)."""
+    shape and pos_f32 uint8, rgb uint8 (E, K, S, 4) (r, g, b, 0), factors float32 (E, K, S, 5), and
+    with sampled goals (n_goals = G > 0) goal float64 (E, K, G, 2)."""
     if getattr(self, '_pool_views', None) is None:
       vp = ctypes.c_void_p
       f64 = (vp * 8)()
@@ -741,6 +753,11 @@ class Engine(object):
       out['pos_f32'] = view(ptrs[2].value, '|u1')
       out['rgb'] = view(ptrs[3].value, '|u1', (4,))
       out['factors'] = view(ptrs[4].value, '<f4', (5,))
+      if self.n_goals:
+        gp, ng = ctypes.c_void_p(), ctypes.c_int32()
+        _native.check(self._lib.swb_pool_goal_pointer(self._h, ctypes.byref(gp), ctypes.byref(ng)))
+        out['goal'] = torch.as_tensor(_DevicePointer(gp.value, (E, K, self.n_goals, 2), '<f8'),
+                                      device=self.device)
       self._pool_views = out
     return self._pool_views
 
@@ -771,6 +788,51 @@ class Engine(object):
     err = self._program.error(op)
     raise ValueError('%s (env %d, scene %d)' % (err.args[0], int(rec[1]), int(rec[2])))
 
+  # -- sampled goals ----------------------------------------------------------------------
+  def _check_goals(self, goals, n, fn):
+    """ValueError unless `goals` is a contiguous float64 (n, G, 2) tensor on this engine's device."""
+    if not self.n_goals:
+      raise ValueError('%s: the task tree samples no goals' % fn)
+    if (not isinstance(goals, torch.Tensor) or goals.dtype != torch.float64 or goals.device != self.device
+        or tuple(goals.shape) != (n, self.n_goals, 2)):
+      raise ValueError('%s takes float64 goals (%d, %d, 2) on %s, got %s'
+                       % (fn, n, self.n_goals, self.device, _describe(goals)))
+    return goals.contiguous()
+
+  def set_goals(self, goals, env_ids=None, check='host'):
+    """The goals of the scene env env_ids[i] is on <- goals[i] (default ids: all envs, in order;
+    distinct), until the env starts its next scene.  `goals`: float64 (n, G, 2) on this engine's
+    device.  Ids as load_envs takes them; with check='device' a refused call changes nothing and
+    check_env_ids() reports it."""
+    if device_checked(check, env_ids):
+      ids, dt = self._dev_ids(env_ids, 'set_goals')
+      goals = self._check_goals(goals, ids.numel(), 'set_goals')
+      _native.check(self._lib.swb_set_goals_dev(self._h, ctypes.c_void_p(ids.data_ptr()), dt, ids.numel(),
+                                                ctypes.c_void_p(goals.data_ptr()), self._stream()))
+      return
+    ids = self._all_or(env_ids)
+    goals = self._check_goals(goals, len(ids), 'set_goals')
+    _native.check(self._lib.swb_set_goals(self._h, _as_ptr(ids), len(ids), ctypes.c_void_p(goals.data_ptr()),
+                                          self._stream()))
+
+  def evaluate(self, states, goals=None):
+    """(reward float64, success uint8, status uint8) device tensors (n,): the task tree's value on
+    each record of `states` at its live positions (no action cost), with goals[i] (float64
+    (n, G, 2) on this engine's device) in place of record i's goals if given.  One launch; reads
+    only."""
+    n = len(states) if isinstance(states, EnvStates) else -1
+    self.check_states(states, n)
+    if goals is not None:
+      goals = self._check_goals(goals, n, 'evaluate')
+    reward = torch.empty(n, dtype=torch.float64, device=self.device)
+    success = torch.empty(n, dtype=torch.uint8, device=self.device)
+    status = torch.empty(n, dtype=torch.uint8, device=self.device)
+    _native.check(self._lib.swb_evaluate_states(
+        self._h, ctypes.c_void_p(states.data.data_ptr()), n, states.data.numel(),
+        None if goals is None else ctypes.c_void_p(goals.data_ptr()), ctypes.c_void_p(reward.data_ptr()),
+        ctypes.c_void_p(success.data_ptr()), ctypes.c_void_p(status.data_ptr()), self._stream()))
+    return reward, success, status
+
   def launch_count(self):
     return int(self._lib.swb_launch_count(self._h))
 
@@ -800,11 +862,12 @@ def config_signature(cfg):
   return bytes(sig)
 
 
-def record_layout(n_slots):
-  """(fields, record bytes) of an env record of an engine with n_slots slots: fields is a list of
-  (name, byte offset, NumPy dtype, shape within one record).  The table of
-  include/spriteworld_b200.h; `factors` is (5, S) there: scale, angle, c0, c1, c2."""
-  S = int(n_slots)
+def record_layout(n_slots, n_goals=0):
+  """(fields, record bytes) of an env record of an engine with n_slots slots and n_goals sampled
+  goals: fields is a list of (name, byte offset, NumPy dtype, shape within one record).  The table
+  of include/spriteworld_b200.h; `factors` is (5, S) there: scale, angle, c0, c1, c2.  With
+  n_goals = G > 0 the record ends in `goal` float64 (G, 2)."""
+  S, G = int(n_slots), int(n_goals)
   fields, off = [], 0
   for name in ('x0', 'y0', 'm00', 'm01', 'm10', 'm11', 'vx', 'vy', 'pos_x', 'pos_y'):
     fields.append((name, off, np.dtype('<f8'), (S,)))
@@ -815,6 +878,10 @@ def record_layout(n_slots):
     dtype = np.dtype(dtype)
     fields.append((name, off, dtype, shape))
     off += dtype.itemsize * int(np.prod(shape, dtype=np.int64))
+  if G:
+    off = (off + 7) // 8 * 8
+    fields.append(('goal', off, np.dtype('<f8'), (G, 2)))
+    off += 16 * G
   return fields, (off + 15) // 16 * 16
 
 
@@ -823,7 +890,7 @@ _ID_DTYPES = {torch.int32: _native.DTYPE_I32, torch.int64: _native.DTYPE_I64}
 _IDS_STATUS = np.dtype([('ok', '<u4'), ('failed', '<u4'), ('call', '<i4'), ('arg', '<i4'), ('reason', '<i4'),
                         ('position', '<i4'), ('value', '<i8')])
 _IDS_CALLS = {_native.IDS_CALL_SAVE: 'save_envs', _native.IDS_CALL_LOAD: 'load_envs',
-              _native.IDS_CALL_COPY: 'copy_envs'}
+              _native.IDS_CALL_COPY: 'copy_envs', _native.IDS_CALL_SET_GOALS: 'set_goals'}
 
 
 def device_checked(check, env_ids):
@@ -862,9 +929,9 @@ class EnvStates(object):
   device index tensor, without host synchronisation), `to(device)`, EnvStates.cat() and
   torch.save / torch.load; to_host() decodes the records into NumPy arrays."""
 
-  def __init__(self, data, span_class, signature, n_slots):
+  def __init__(self, data, span_class, signature, n_slots, n_goals=0):
     self.data, self.span_class = data, int(span_class)
-    self.signature, self.n_slots = bytes(signature), int(n_slots)
+    self.signature, self.n_slots, self.n_goals = bytes(signature), int(n_slots), int(n_goals)
 
   @property
   def record_bytes(self):
@@ -878,7 +945,7 @@ class EnvStates(object):
       idx = slice(idx, idx + 1 if idx != -1 else None)
     elif not isinstance(idx, slice):
       idx = torch.as_tensor(env_ids_array(idx).astype(np.int64), device=self.data.device)
-    return EnvStates(self.data[idx].contiguous(), self.span_class, self.signature, self.n_slots)
+    return EnvStates(self.data[idx].contiguous(), self.span_class, self.signature, self.n_slots, self.n_goals)
 
   def take(self, index):
     """EnvStates whose record i is record index[i]: a gather on the device that never waits for
@@ -897,10 +964,10 @@ class EnvStates(object):
       inside = (index >= 0) & (index < n)
       # clamped, so that no index outside the records reaches the gather
       data = self.data.index_select(0, index.clamp(0, n - 1)).masked_fill_(~inside[:, None], 0)
-    return EnvStates(data, self.span_class, self.signature, self.n_slots)
+    return EnvStates(data, self.span_class, self.signature, self.n_slots, self.n_goals)
 
   def to(self, device):
-    return EnvStates(self.data.to(device), self.span_class, self.signature, self.n_slots)
+    return EnvStates(self.data.to(device), self.span_class, self.signature, self.n_slots, self.n_goals)
 
   @staticmethod
   def cat(states):
@@ -909,11 +976,11 @@ class EnvStates(object):
     if not states or any(s.signature != states[0].signature for s in states):
       raise ValueError('EnvStates.cat needs at least one EnvStates, all of one engine configuration')
     return EnvStates(torch.cat([s.data for s in states]), max(s.span_class for s in states),
-                     states[0].signature, states[0].n_slots)
+                     states[0].signature, states[0].n_slots, states[0].n_goals)
 
   def fields(self):
     """dict name -> device tensor view (n,) + shape of every field (uint32 fields as int32)."""
-    layout, _ = record_layout(self.n_slots)
+    layout, _ = record_layout(self.n_slots, self.n_goals)
     n, out = len(self), {}
     for name, off, dtype, shape in layout:
       nbytes = dtype.itemsize * int(np.prod(shape, dtype=np.int64))
@@ -923,7 +990,7 @@ class EnvStates(object):
   def to_host(self):
     """dict of NumPy arrays, one per field: x0 .. vy, pos_x, pos_y (n, S) float64, member (n, S)
     uint32, rgb (n, S, 3) uint8, factors (n, S, 5) float32, shape and pos_f32 (n, S) uint8,
-    step_count (n,) int32, reset_next (n,) uint8."""
+    step_count (n,) int32, reset_next (n,) uint8, and goal (n, G, 2) float64 with sampled goals."""
     out = {name: t.cpu().numpy().copy() for name, t in self.fields().items()}
     out['member'] = out['member'].view(np.uint32)
     out['rgb'] = out['rgb'].view(np.uint32)[..., None].view(np.uint8)[..., :3].copy()
@@ -957,6 +1024,7 @@ def fill_task_nodes(cfg, nodes):
       n.terminate_bonus = float(nd['terminate_bonus'])
       n.raw_reward_multiplier = float(nd['raw_reward_multiplier'])
       n.sparse_reward = int(bool(nd['sparse_reward']))
+      n.goal_slot = int(nd.get('goal_slot', -1))
     elif kind == 'clustering':
       n.kind = _native.TASK_CLUSTERING
       slots = nd['cluster_slots']

@@ -103,6 +103,7 @@ class Environment(dm_env.Environment):
     self._color_to_rgb = _color_map(self._pil)
     self._nodes, self._filters = task.compile()
     task._filters_static()
+    task._constant_goals('the one-env Environment')
     self._engine = None
     self._rasters = {}
     self._max_sprites = max_sprites
@@ -332,6 +333,7 @@ class BatchedEnvironment(object):
     self._color_to_rgb = _color_map(self._pil)
     self._nodes, self._filters = task.compile()
     task._filters_static()
+    self._goal_distribs = task.goal_distributions()
     self._K = max(3, int(pool_depth))
     E, K = self.n_envs, self._K
     if sampler not in ('host', 'device'):
@@ -339,15 +341,16 @@ class BatchedEnvironment(object):
     self._sampler = sampler
     if sampler == 'device':
       from spriteworld_b200 import scene_program
-      self._program = scene_program.compile_program(init_sprites, self._filters, self._color_to_rgb)
+      self._program = scene_program.compile_program(init_sprites, self._filters, self._color_to_rgb,
+                                                    self._goal_distribs)
       slots = n_slots or self._program.max_sprites
     else:
-      first = self._sample(E * K)
+      first, first_goals = self._sample(E * K)
       slots = n_slots or getattr(init_sprites, 'max_sprites', None)
       if not slots:
         # the count is drawn by a user callable: size the slots from a probe sample, so that a
         # later refill cannot meet a larger scene in the middle of a run
-        probe = self._sample(4096)
+        probe, _ = self._sample(4096)
         slots = max(1, int(first.count.max()), int(probe.count.max()))
     slots = max(1, int(slots))
     self._engine = engine_lib.Engine(
@@ -364,7 +367,7 @@ class BatchedEnvironment(object):
     if sampler == 'device':
       self._init_device_sampler(seed, env_offset)
       return
-    batch0 = self._upload(first, np.repeat(np.arange(E), K), np.tile(np.arange(K), E))
+    batch0 = self._upload(first, np.repeat(np.arange(E), K), np.tile(np.arange(K), E), goals=first_goals)
     # env e starts on its scene 0 (the constructor's sample, environment.py:68) and is about
     # to reset (environment.py:70)
     self._engine.upload_state(pos_x=batch0['x'][::K], pos_y=batch0['y'][::K],
@@ -413,7 +416,8 @@ class BatchedEnvironment(object):
       if refill_procs:
         from spriteworld_b200 import _sampler_pool
         self._pool = _sampler_pool.SamplerPool(min(int(refill_procs), n_thr), init_sprites, slots,
-                                               self._filters, self._color_to_rgb)
+                                               self._filters, self._color_to_rgb,
+                                               goal_distribs=self._goal_distribs)
 
   def _init_device_sampler(self, seed, env_offset):
     E, K = self.n_envs, self._K
@@ -439,13 +443,19 @@ class BatchedEnvironment(object):
     self._engine.check_sampler()
 
   # -- scenes ----------------------------------------------------------------------------
-  def _sample(self, n):
-    return sprite_generators.batch_of(self._init_sprites, n, self._rng)
+  def _sample(self, n, rng=None):
+    """(SceneLayout of n scenes, their goals (n, G, 2) or None), the goals drawn right after the
+    scenes from the same RandomState (default: `rng`)."""
+    rng = self._rng if rng is None else rng
+    layout = sprite_generators.batch_of(self._init_sprites, n, rng)
+    return layout, scene.draw_goals(self._goal_distribs, n, rng)
 
-  def _upload(self, layout, env_ids, ring_slots, batch=None):
+  def _upload(self, layout, env_ids, ring_slots, batch=None, goals=None):
     if batch is None:
       batch = scene.arrays_from_layout(layout, self._engine.n_slots, self._filters,
                                        self._color_to_rgb)
+    if goals is not None:
+      batch['goal'] = goals
     self._engine.upload_scenes(batch, env_ids, ring_slots)
     return batch
 
@@ -481,6 +491,55 @@ class BatchedEnvironment(object):
         out[name] = columns[..., self._FACTOR_COLUMNS[name]]
     out['mask'] = shape > 0
     return out
+
+  @property
+  def n_goals(self):
+    """G: goals drawn per scene (the task's FindGoalPosition nodes with a goal distribution)."""
+    return len(self._goal_distribs)
+
+  def goal_tensor(self, states=None):
+    """float64 (n_envs, G, 2) device tensor: the goals of the scene each env is on (GoalPositions),
+    or with `states` (EnvStates of n records) a new (n, G, 2) tensor of the records' goals."""
+    eng = self._engine
+    if states is not None:
+      eng.check_states(states, len(states))
+      if not self.n_goals:
+        return torch.zeros((len(states), 0, 2), dtype=torch.float64, device=states.data.device)
+      return states.fields()['goal'].clone()
+    if not self.n_goals:
+      return torch.zeros((self.n_envs, 0, 2), dtype=torch.float64, device=eng.device)
+    views = getattr(self, '_goal_views', None)
+    if views is None:   # zero-copy views and the entry base e * K, made once
+      K = eng.pool_depth
+      views = self._goal_views = (torch.arange(0, self.n_envs * K, K, dtype=torch.int32, device=eng.device),
+                                  eng.state_tensors()['cursor'], eng.pool_tensors()['goal'].flatten(0, 1))
+    base, cursor, goal = views
+    return goal.index_select(0, base + cursor)
+
+  def set_goals(self, goals, env_ids=None, check='host'):
+    """The goals of the scene env env_ids[i] is on <- goals[i] (float64 (n, G, 2) on the engine's
+    device; default ids: all envs, in order; distinct), on the step stream.  The env keeps them
+    until it starts its next scene, which brings a drawn goal.  Ids as load_envs takes them; a
+    device-checked call is all or nothing (Engine.check_env_ids reports a refused one).  It writes
+    only the pool entry each env is on, as a load does, and counts against the ring's refill guard
+    like a load.
+
+    An env whose last step was LAST is still on the finished scene: goals set now are replaced by
+    the next scene's drawn goals at the reset that follows.  To choose the goal of an env's next
+    episode, set it after the FIRST step of that episode (the reset step observes no reward)."""
+    if engine_lib.device_checked(check, env_ids):
+      self._engine.set_goals(goals, env_ids, check='device')
+    else:
+      self._engine.set_goals(goals, env_ids)
+    self._resets += 1
+
+  def evaluate(self, states, goals=None):
+    """Relabels env records: (reward float64, success uint8, status uint8) device tensors (n,),
+    the task's value on each record of `states` (EnvStates) at its live positions -- without the
+    step's action cost -- with goals[i] (float64 (n, G, 2) on the engine's device) in place of
+    record i's goals, or the records' own goals if `goals` is None.  One launch on the current
+    stream, no host synchronisation; no env, ring or `rng` changes."""
+    return self._engine.evaluate(states, goals)
 
   def _record_factor_tensors(self, factors, states):
     if not isinstance(states, engine_lib.EnvStates):
@@ -527,9 +586,8 @@ class BatchedEnvironment(object):
     if plan is None:
       return 0
     env_ids, absolute, upto = plan
-    layout = sprite_generators.batch_of(self._init_sprites, len(env_ids),
-                                        self._rng if rng is None else rng)
-    self._upload(layout, env_ids, absolute % self._K)
+    layout, goals = self._sample(len(env_ids), rng)
+    self._upload(layout, env_ids, absolute % self._K, goals=goals)
     self._refilled_upto[:] = upto
     return len(env_ids)
 
@@ -562,8 +620,8 @@ class BatchedEnvironment(object):
       else:
         for i, plan in enumerate(plans):
           if plan is not None:
-            layout = sprite_generators.batch_of(self._init_sprites, len(plan[0]), self._block_rngs[i])
-            self._upload(layout, plan[0], plan[1] % K)
+            layout, goals = self._sample(len(plan[0]), self._block_rngs[i])
+            self._upload(layout, plan[0], plan[1] % K, goals=goals)
       for i, plan in enumerate(plans):
         if plan is not None:
           self._refilled_upto[int(edges[i]):int(edges[i + 1])] = plan[2]
@@ -930,6 +988,8 @@ class BatchedEnvironment(object):
                         tuple(int(c) for c in r.bg_color)) for name, r in self._pil.items()])
     if self._sampler == 'device':
       fp['program'] = bytes(self._program.struct)
+    if self._goal_distribs:
+      fp['goals'] = [str(d) for d in self._goal_distribs]
     return fp
 
   def observation_spec(self):
@@ -984,6 +1044,9 @@ class ShardedBatchedEnvironment(object):
 
   def __init__(self, n_envs_total, group=None, device=None, seed=0, frame_slots=2,
                host_barrier=False, **config):
+    if any(isinstance(r, handcrafted.GoalPositions) for r in dict(config.get('renderers') or {}).values()):
+      raise NotImplementedError('ShardedBatchedEnvironment does not gather GoalPositions across ranks; '
+                                "each rank's goals are self.local.goal_tensor()")
     import torch.distributed as dist
     from spriteworld_b200 import distributed
     self.group = group

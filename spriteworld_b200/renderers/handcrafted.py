@@ -127,6 +127,32 @@ class SpriteMasks(abstract_renderer.AbstractRenderer):
     return self._observation_spec
 
 
+class GoalPositions(abstract_renderer.AbstractRenderer):
+  """The goals of the task's sampled FindGoalPosition nodes: float64 (G, 2), (x, y) per goal slot
+  (tasks.AbstractTask.goal_distributions order).  A task with constant goals only has G = 0."""
+
+  def __init__(self):
+    self._observation_spec = specs.Array(shape=(0, 2), dtype=np.float64)
+
+  def render(self, sprites=(), global_state=None):
+    # the one-env Environment refuses sampled goals, so its tasks have none
+    return np.zeros((0, 2), np.float64)
+
+  def observation_spec(self):
+    return self._observation_spec
+
+  def render_batch(self, env, res):
+    """Batched form: float64 (n_envs, G, 2) device tensor of the goals of the scene each env is on."""
+    return env.goal_tensor()
+
+  def render_states(self, env, states):
+    """The goals of env records (EnvStates): a new float64 (n, G, 2) tensor."""
+    return env.goal_tensor(states)
+
+  def batch_observation_spec(self, env):
+    return specs.Array(shape=(env.n_goals, 2), dtype=np.float64)
+
+
 class Success(abstract_renderer.AbstractRenderer):
   """global_state['success'] as an observation."""
 

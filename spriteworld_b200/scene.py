@@ -195,6 +195,19 @@ def _table_rgb(cols, color_to_rgb, num=None):
   return out
 
 
+def draw_goals(goal_distribs, n, rng):
+  """float64 (n, G, 2): the goals of n scenes, drawn per goal slot in slot order, each slot's n
+  goals with one goal_distrib.sample_batch(n, rng) call.  None without goal distributions."""
+  if not goal_distribs:
+    return None
+  out = np.empty((n, len(goal_distribs), 2), np.float64)
+  for g, d in enumerate(goal_distribs):
+    cols = d.sample_batch(n, rng)
+    out[:, g, 0] = np.asarray(cols['x'], dtype=np.float64)
+    out[:, g, 1] = np.asarray(cols['y'], dtype=np.float64)
+  return out
+
+
 def arrays_from_layout(layout, n_slots, filters=(), color_to_rgb=None):
   """SceneLayout -> scene batch (n, n_slots), sprites right-aligned (empty slots first).
 

@@ -28,6 +28,7 @@ from spriteworld_b200 import scene as scene_lib
 from spriteworld_b200 import sprite_generators as gen
 
 MAX_OPS, MAX_CONSTS, MAX_ANGLES, MAX_STACK, MAX_FILTERS, MAX_SLOTS = 512, 1024, 1024, 16, 32, 32
+MAX_GOALS = 8   # SWB_MAX_GOALS
 DOMAIN = 0x53574253434e4531   # SWB_SAMPLER_DOMAIN: second Philox key word of the scene stream
 
 FT_NONE, FT_F32, FT_F64 = 0, 1, 2
@@ -62,13 +63,13 @@ class Program(ctypes.Structure):
               ('max_sprites', _c32), ('color_mode', _c32), ('filter_pc', _c32 * MAX_FILTERS),
               ('ops', ProgOp * MAX_OPS), ('consts', _f64 * MAX_CONSTS), ('const_kind', _c32 * MAX_CONSTS),
               ('angle', _f64 * MAX_ANGLES), ('angle_cos', _f64 * MAX_ANGLES),
-              ('angle_sin', _f64 * MAX_ANGLES)]
+              ('angle_sin', _f64 * MAX_ANGLES), ('n_goals', _c32), ('goal_pc', _c32 * MAX_GOALS)]
 
 
 class SampleOut(ctypes.Structure):
   _fields_ = [(n, ctypes.c_void_p) for n in
               ('x', 'y', 'm00', 'm01', 'm10', 'm11', 'vx', 'vy', 'member', 'shape', 'pos_f32', 'rgb',
-               'factors', 'factor_value', 'factor_kind')]
+               'factors', 'factor_value', 'factor_kind', 'goal')]
 
 
 class SceneProgram(object):
@@ -376,9 +377,10 @@ def _generator_depth(g):
   return max([_generator_depth(c) for c in spec[1]] + [0])
 
 
-def compile_program(init_sprites, filters=(), color_to_rgb=None):
+def compile_program(init_sprites, filters=(), color_to_rgb=None, goals=()):
   """SceneProgram of a scene generator, the task's filter distributions (bit i of `member` is
-  filters[i]) and the PILRenderers' colour map."""
+  filters[i]), the PILRenderers' colour map and the task's goal distributions (goal slot i is drawn
+  by goals[i], after the scene's sprites; tasks.AbstractTask.goal_distributions)."""
   from spriteworld_b200.renderers import color_maps
   if color_to_rgb is None:
     color_mode = COLOR_RGB
@@ -388,6 +390,13 @@ def compile_program(init_sprites, filters=(), color_to_rgb=None):
     _refuse('the colour map %r: only None (RGB colours) and color_maps.hsv_to_rgb' % (color_to_rgb,))
   if len(filters) > MAX_FILTERS:
     _refuse('more than %d task filters' % MAX_FILTERS)
+  if len(goals) > MAX_GOALS:
+    _refuse('more than %d sampled goals' % MAX_GOALS)
+  for d in goals:
+    if set(d.keys) != {'x', 'y'}:
+      _refuse("a goal distribution over %s (it must be over exactly {'x', 'y'})" % sorted(d.keys))
+    if _rejection_depth(d) > MAX_STACK:
+      _refuse('rejection samplers nested more than %d deep' % MAX_STACK)
   c = _Compiler()
   most = c.gen(init_sprites)
   c.op(G_END)
@@ -414,6 +423,13 @@ def compile_program(init_sprites, filters=(), color_to_rgb=None):
       c.dist(dist)
       c.op(D_RET)
     c.ops[i]['a'] = done[id(dist)]
+  goal_pcs = []
+  for dist in goals:
+    if id(dist) not in done:
+      done[id(dist)] = len(c.ops)
+      c.dist(dist)
+      c.op(D_RET)
+    goal_pcs.append(done[id(dist)])
   pred_pc = {}
 
   def predicate(d):
@@ -436,6 +452,9 @@ def compile_program(init_sprites, filters=(), color_to_rgb=None):
   p.max_sprites, p.color_mode = most, color_mode
   for i, pc in enumerate(filter_pcs):
     p.filter_pc[i] = pc
+  p.n_goals = len(goal_pcs)
+  for i, pc in enumerate(goal_pcs):
+    p.goal_pc[i] = pc
   for i, o in enumerate(c.ops):
     for k, v in o.items():
       setattr(p.ops[i], k, v)
@@ -482,9 +501,12 @@ def philox_host(counter, key):
   return out
 
 
-def empty_sample(n, n_slots):
-  """Host arrays of swb_sample_out for n scenes: a scene batch plus the drawn factor table."""
+def empty_sample(n, n_slots, n_goals=0):
+  """Host arrays of swb_sample_out for n scenes: a scene batch plus the drawn factor table and,
+  for n_goals > 0, the goals (n, n_goals, 2)."""
   b = scene_lib.empty_batch(n, n_slots)
+  if n_goals:
+    b['goal'] = np.zeros((n, n_goals, 2), np.float64)
   b['factor_value'] = np.zeros((n, n_slots, len(FACTORS)), np.float64)
   b['factor_kind'] = np.zeros((n, n_slots, len(FACTORS)), np.uint8)
   return b
@@ -493,7 +515,7 @@ def empty_sample(n, n_slots):
 def sample_out_struct(arrays, ptr=lambda a: a.ctypes.data):
   out = SampleOut()
   for name, _ in SampleOut._fields_:
-    setattr(out, name, ptr(arrays[name]))
+    setattr(out, name, ptr(arrays[name]) if name in arrays else None)   # goal: optional
   return out
 
 
@@ -504,7 +526,7 @@ def sample_on_host(program, seed, env_ids, scene_idx, n_slots):
   env_ids = np.ascontiguousarray(env_ids, np.int64)
   scene_idx = np.ascontiguousarray(scene_idx, np.int64)
   n = len(env_ids)
-  b = empty_sample(n, n_slots)
+  b = empty_sample(n, n_slots, program.struct.n_goals)
   op, idx = ctypes.c_int32(-1), ctypes.c_int64(-1)
   failures = _host_lib().swb_host_sample_scenes(
       ctypes.byref(program.struct), int(seed) & (2 ** 64 - 1), int(n_slots), env_ids.ctypes.data,

@@ -4,7 +4,9 @@ Same classes and constructor signatures as the reference's `spriteworld/tasks.py
 (NoReward :70-81, FindGoalPosition :84-158, Clustering :161-245, MetaAggregated :248-296).
 A task here is a *description*: `compile()` flattens the task tree into the POD nodes of
 `swb_config` (include/spriteworld_b200.h) and the list of filter distributions whose
-membership is precomputed per sprite at reset.  The arithmetic itself runs in the step
+membership is precomputed per sprite at reset.  A FindGoalPosition whose goal is a distribution
+over ('x', 'y') gets a goal slot: its goal is drawn with every scene and stored in the scene pool
+entry (goal_distributions() lists them in slot order).  The arithmetic itself runs in the step
 kernel (csrc/swb_step.cuh).  `reward(sprites)` / `success(sprites)` on a Python sprite
 list are kept for the plugin protocol; they evaluate on the GPU through a one-env engine
 (_direct.py) -- there is no CPU implementation of the task math in this package.
@@ -13,6 +15,7 @@ import abc
 
 import numpy as np
 
+MAX_GOALS = 8   # SWB_MAX_GOALS: sampled goals per task tree
 _AGGREGATORS = ('sum', 'max', 'min', 'mean')
 _CRITERIA = ('all', 'any')
 
@@ -25,10 +28,33 @@ class AbstractTask(abc.ABC):
 
   def compile(self):
     """Returns (nodes, filters): POD node dicts, root last, and the distinct filter
-    distributions in slot order (bit i of a sprite's `member` mask <-> filters[i])."""
+    distributions in slot order (bit i of a sprite's `member` mask <-> filters[i]).  A
+    find_goal node's `goal_slot` is -1 for a constant goal, else the index of its distribution
+    in goal_distributions()."""
     nodes, filters = [], []
     self._emit(nodes, filters)
+    slot = 0
+    for nd in nodes:   # a constant goal's node has neither key: its dict is as it always was
+      if 'goal_distrib' in nd:
+        nd['goal_slot'] = slot
+        slot += 1
+    if slot > MAX_GOALS:
+      raise NotImplementedError('task tree has %d sampled goals; at most %d (SWB_MAX_GOALS) are '
+                                'supported' % (slot, MAX_GOALS))
     return nodes, filters
+
+  def goal_distributions(self):
+    """The goal distributions of the tree's sampled goals, in goal-slot order (node post-order;
+    one distribution object used by two nodes gives two slots)."""
+    nodes, _ = self.compile()
+    return [nd['goal_distrib'] for nd in nodes if 'goal_distrib' in nd]
+
+  def _constant_goals(self, where):
+    """NotImplementedError if the tree samples goals: `where` has no per-scene goal."""
+    if self.goal_distributions():
+      raise NotImplementedError(
+          '%s does not support sampled goals (FindGoalPosition with a goal distribution); use '
+          'BatchedEnvironment' % where)
 
   def _filters_static(self):
     """Task filters must depend only on factors that do not change during an episode."""
@@ -78,13 +104,22 @@ class NoReward(AbstractTask):
 
 
 class FindGoalPosition(AbstractTask):
-  """Bring every sprite selected by `filter_distrib` to `goal_position`."""
+  """Bring every sprite selected by `filter_distrib` to `goal_position`: an (x, y) pair, or a
+  factor distribution over exactly {'x', 'y'} from which each scene draws its own goal
+  (BatchedEnvironment only)."""
 
   def __init__(self, filter_distrib=None, goal_position=(0.5, 0.5), terminate_distance=0.05,
                terminate_bonus=0.0, weights_dimensions=(1, 1), sparse_reward=False,
                raw_reward_multiplier=50):
     self._filter_distrib = filter_distrib
-    self._goal_position = np.asarray(goal_position)
+    if hasattr(goal_position, 'sample_batch'):
+      keys = getattr(goal_position, 'keys', None)
+      if keys is None or set(keys) != {'x', 'y'}:
+        raise ValueError("a goal distribution must have keys exactly {'x', 'y'}, got %r"
+                         % (sorted(keys) if keys is not None else None,))
+      self._goal_distrib, self._goal_position = goal_position, np.full(2, np.nan)
+    else:
+      self._goal_distrib, self._goal_position = None, np.asarray(goal_position)
     self._terminate_bonus = terminate_bonus
     self._terminate_distance = terminate_distance
     self._sparse_reward = sparse_reward
@@ -92,9 +127,10 @@ class FindGoalPosition(AbstractTask):
     self._raw_reward_multiplier = raw_reward_multiplier
 
   def _emit(self, nodes, filters):
+    sampled = {} if self._goal_distrib is None else dict(goal_distrib=self._goal_distrib)
     nodes.append(dict(
         kind='find_goal', filter_slot=_slot(filters, self._filter_distrib),
-        goal=[float(v) for v in self._goal_position],
+        goal=[float(v) for v in self._goal_position], **sampled,
         weights=[float(v) for v in self._weights_dimensions],
         terminate_distance=float(self._terminate_distance),
         terminate_bonus=float(self._terminate_bonus),
