@@ -57,7 +57,9 @@ enum {
   SWB_ENV_CLUSTER_LABELS = 1,  /* sklearn ValueError: needs 2 <= n_labels <= n_samples-1 */
   SWB_ENV_CLUSTER_ZERODIV = 2, /* davies_bouldin_score == 0 -> 1./0. (tasks.py:215) */
   SWB_ENV_BAD_ACTION = 4,      /* Embodied direction not in 0..3 -> KeyError (action_spaces.py:203) */
-  SWB_ENV_SPAN_OVERFLOW = 8    /* renderer: more spans on a canvas row than the engine was sized for */
+  SWB_ENV_SPAN_OVERFLOW = 8,   /* renderer: more spans on a canvas row than the engine was sized for */
+  SWB_ENV_NO_SPRITE = 16,      /* swb_sample_contained: the row has no sprite (np.random.randint(0) raises) */
+  SWB_ENV_SAMPLE_TRIES = 32    /* swb_sample_contained: SWB_CONTAINED_MAX_TRIES draws, none inside (sprite.py) */
 };
 
 /* One node of the flattened task tree, post-order, root last. */
@@ -631,6 +633,39 @@ int swb_set_goals_dev(swb_engine *eng, const void *env_ids, int32_t id_dtype, in
  */
 int swb_evaluate_states(swb_engine *eng, const void *records, int32_t n, uint64_t records_bytes,
                         const double *goals, double *reward, uint8_t *success, uint8_t *status, void *stream);
+
+/*
+ * Positions inside sprites (Environment.sample_contained_position, for random agents and plan
+ * proposals): n_samples draws per row, of the E live envs (records == NULL, n == E) or of n env
+ * records of this engine's layout (records_bytes bytes, 16-byte aligned, shape ids sanitised as
+ * swb_load_envs does).  Sample s of row i:
+ *   - the row's sprites are its slots with a non-zero shape id, in slot order; m of them.  m == 0:
+ *     status SWB_ENV_NO_SPRITE.
+ *   - draws come from Philox4x64-10 with key (seed, SWB_CONTAINED_DOMAIN) and counter
+ *     (block, s, i, 0), words consumed in order as the scene sampler consumes them: word 0 picks
+ *     sprite k = mulhi64(word, m), the k-th occupied slot.
+ *   - lo / hi: the min / max over the shape's vertices of the centred path (m00 ax + m01 ay) + 0.0
+ *     (and likewise y).  Each try draws ux, then uy (53-bit uniforms) and proposes
+ *     c = pos + (lo + (hi - lo) u) in float64; it is accepted if the step kernel's even-odd hit test
+ *     of c - pos finds it inside the sprite.  After SWB_CONTAINED_MAX_TRIES tries: status
+ *     SWB_ENV_SAMPLE_TRIES (a sprite of scale 0, say).
+ * position[(i * n_samples + s) * 2 + 0/1] (f64), slot[i * n_samples + s] (i8) and status (u8) are
+ * device arrays of the caller; a failed sample has position NaN and slot -1.  Live envs sample the
+ * scene they are on (pool entry (e, cursor)) at their live positions, also an env about to reset.
+ * A float64 SelectMove / DragAndDrop action whose click is the returned position grabs the sampled
+ * slot or a sprite above it, as c - pos is what swb_step computes from it (action noise aside).
+ *
+ * Each sample is a pure function of (seed, i, s, the row's state): nothing is kept between calls.
+ * An accepted call with n > 0 is one launch on `stream`; n == 0 enqueues nothing.  Read-only: no
+ * env, pool entry, counter or frame changes.  Refused, enqueuing nothing: a null engine or output,
+ * n < 0, n_samples < 1, n * n_samples above 2^31 - 1, n != E for the live envs, records not
+ * 16-byte aligned or too small.
+ */
+#define SWB_CONTAINED_MAX_TRIES 1000000          /* sprite.py _MAX_TRIES */
+#define SWB_CONTAINED_DOMAIN 0x535742434e544431ULL  /* second key word of the contained-position stream */
+int swb_sample_contained(swb_engine *eng, const void *records, int32_t n, uint64_t records_bytes,
+                         int32_t n_samples, uint64_t seed, double *position, int8_t *slot, uint8_t *status,
+                         void *stream);
 
 /* Device pointers: refilled_upto [E] int64, and the engine's swb_sampler_status. */
 int swb_sampler_pointers(swb_engine *eng, int64_t **refilled_upto, swb_sampler_status **status);

@@ -22,6 +22,9 @@ CRIT = {'all': 0, 'any': 1}
 STEP_FIRST, STEP_MID, STEP_LAST = 0, 1, 2
 STEP_NONE = -1   # padding of a rollout: no step
 ENV_OK, ENV_CLUSTER_LABELS, ENV_CLUSTER_ZERODIV, ENV_BAD_ACTION, ENV_SPAN_OVERFLOW = 0, 1, 2, 4, 8
+ENV_NO_SPRITE, ENV_SAMPLE_TRIES = 16, 32   # swb_sample_contained
+CONTAINED_MAX_TRIES = 1000000              # SWB_CONTAINED_MAX_TRIES
+CONTAINED_DOMAIN = 0x535742434e544431      # SWB_CONTAINED_DOMAIN
 IDS_CALL_SAVE, IDS_CALL_LOAD, IDS_CALL_COPY, IDS_CALL_SET_GOALS = 0, 1, 2, 3
 IDS_OUT_OF_RANGE, IDS_REPEATED = 1, 2
 
@@ -148,6 +151,7 @@ def load():
   L.swb_set_goals.argtypes = [vp, vp, ci, vp, vp]
   L.swb_set_goals_dev.argtypes = [vp, vp, ci, ci, vp, vp]
   L.swb_evaluate_states.argtypes = [vp, vp, ci, ctypes.c_uint64, vp, vp, vp, vp, vp]
+  L.swb_sample_contained.argtypes = [vp, vp, ci, ctypes.c_uint64, ci, ctypes.c_uint64, vp, vp, vp, vp]
   if L.swb_sizeof_config() != ctypes.sizeof(Config):
     raise NativeError('ABI mismatch: swb_config is %d bytes in the library, %d in the binding'
                       % (L.swb_sizeof_config(), ctypes.sizeof(Config)))
@@ -167,7 +171,8 @@ EXPORTS = (
     'swb_load_envs_dev', 'swb_copy_envs_dev', 'swb_env_ids_status_pointer', 'swb_launch_count',
     'swb_sampler_sizeof_program', 'swb_sampler_load', 'swb_sample_scenes', 'swb_refill_device',
     'swb_sampler_pointers', 'swb_pool_pointers', 'swb_engine_state_bytes', 'swb_save_engine',
-    'swb_load_engine', 'swb_pool_goal_pointer', 'swb_set_goals', 'swb_set_goals_dev', 'swb_evaluate_states')
+    'swb_load_engine', 'swb_pool_goal_pointer', 'swb_set_goals', 'swb_set_goals_dev', 'swb_evaluate_states',
+    'swb_sample_contained')
 
 
 def check(rc):

@@ -12,7 +12,7 @@ import sys
 CSRC = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'csrc')
 LIB = os.path.join(CSRC, 'libspriteworld_b200.so')
 SOURCES = ['swb_api.cu']
-HEADERS = ['swb_device.cuh', 'swb_masks.cuh', 'swb_render.cuh', 'swb_rollout.cuh', 'swb_sampler.cuh', 'swb_states.cuh', 'swb_step.cuh', 'swb_tables.h',
+HEADERS = ['swb_contained.cuh', 'swb_device.cuh', 'swb_masks.cuh', 'swb_render.cuh', 'swb_rollout.cuh', 'swb_sampler.cuh', 'swb_states.cuh', 'swb_step.cuh', 'swb_tables.h',
            os.path.join('..', '..', 'include', 'spriteworld_b200.h')]
 
 NVCC_FLAGS = [
@@ -64,15 +64,16 @@ def build_host(force=False):
 
 SAMPLER_HOST_LIB = os.path.join(CSRC, 'libswb_sampler_host.so')
 SAMPLER_HOST_SRC = os.path.join(CSRC, 'swb_sampler_host.cpp')
-SAMPLER_HOST_INPUTS = [SAMPLER_HOST_SRC, os.path.join(CSRC, 'swb_sampler.cuh'),
+SAMPLER_HOST_INPUTS = [SAMPLER_HOST_SRC, os.path.join(CSRC, 'swb_sampler.cuh'), os.path.join(CSRC, 'swb_contained.cuh'),
                        os.path.join(CSRC, '..', '..', 'include', 'spriteworld_b200.h')]
 # the same arithmetic as the kernels built with -fmad=false: no contraction
 SAMPLER_HOST_FLAGS = ['-O2', '-std=c++17', '-ffp-contract=off', '-fPIC', '-shared', '-Wall', '-Wextra']
 
 
 def build_sampler_host(force=False):
-  """libswb_sampler_host.so (g++): the device scene sampler built for the CPU
-  (scene_program.sample_on_host), the restatement the kernels are tested against."""
+  """libswb_sampler_host.so (g++): the device scene sampler and contained-position sampler built for
+  the CPU (scene_program.sample_on_host, scene_program.sample_contained_on_host), the restatement
+  the kernels are tested against."""
   if not force and os.path.exists(SAMPLER_HOST_LIB) and os.path.getmtime(SAMPLER_HOST_LIB) >= max(
       [os.path.getmtime(f) for f in SAMPLER_HOST_INPUTS] + [os.path.getmtime(os.path.abspath(__file__))]):
     return SAMPLER_HOST_LIB

@@ -8,6 +8,7 @@
 #include <string>
 #include <vector>
 
+#include "swb_contained.cuh"
 #include "swb_device.cuh"
 #include "swb_masks.cuh"
 #include "swb_render.cuh"
@@ -171,7 +172,7 @@ int upload_axis(swb_raster *r, const AxisHost &h, AxisTables *d) {
 extern "C" {
 
 const char *swb_last_error(void) { return g_error.c_str(); }
-int swb_version(void) { return 11; }
+int swb_version(void) { return 12; }
 int swb_sizeof_config(void) { return (int)sizeof(swb_config); }
 int swb_sizeof_task_node(void) { return (int)sizeof(swb_task_node); }
 
@@ -1312,6 +1313,33 @@ int swb_render_masks(swb_engine *eng, int32_t width, int32_t height, int32_t ant
   CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, L.total));
   kernel<<<(unsigned)((int64_t)n * L.n_bands), MK_THREADS, L.total, static_cast<cudaStream_t>(stream_)>>>(
       eng->st, L, masks, RenderRecords{static_cast<const unsigned char *>(records), (size_t)rb});
+  eng->launches++;
+  CUDA_TRY(cudaGetLastError());
+  return 0;
+}
+
+int swb_sample_contained(swb_engine *eng, const void *records, int32_t n, uint64_t records_bytes,
+                         int32_t n_samples, uint64_t seed, double *position, int8_t *slot, uint8_t *status,
+                         void *stream_) {
+  static const char fn[] = "swb_sample_contained";
+  if (!eng) return fail("%s: null engine", fn);
+  if (n < 0) return fail("%s: n = %d", fn, n);
+  if (n_samples < 1) return fail("%s: n_samples = %d must be >= 1", fn, n_samples);
+  if (!records && n != eng->st.E)
+    return fail("%s: n = %d must be E = %d when the rows are the live envs", fn, n, eng->st.E);
+  // the kernel's thread index and the output arrays' entries are one per (row, sample)
+  if ((int64_t)n * n_samples > INT32_MAX)
+    return fail("%s: n = %d rows of %d samples exceed 2^31 - 1 samples", fn, n, n_samples);
+  if (n == 0) return 0;
+  if (!position || !slot || !status) return fail("%s: null output", fn);
+  const uint64_t rb = RecordLayout(eng->st.S, eng->st.G).bytes();
+  if (records && check_record_buffer(eng, fn, "records", records, records_bytes, n)) return 1;
+  CUDA_TRY(cudaSetDevice(eng->device));
+  const int64_t total = (int64_t)n * n_samples;
+  auto kernel = records ? contained_kernel<true> : contained_kernel<false>;
+  kernel<<<(unsigned)((total + CT_THREADS - 1) / CT_THREADS), CT_THREADS, 0, static_cast<cudaStream_t>(stream_)>>>(
+      eng->st, static_cast<const unsigned char *>(records), (size_t)rb, n, n_samples, seed, position, slot,
+      status);
   eng->launches++;
   CUDA_TRY(cudaGetLastError());
   return 0;

@@ -58,18 +58,19 @@ SWB_HD void philox4x64_10(uint64_t ctr[4], uint64_t k0, uint64_t k1) {
   }
 }
 
-// The draw stream of one scene.
+// The draw stream of one scene (key word 1 = SWB_SAMPLER_DOMAIN), or of another counter-based
+// stream of the library under its own domain word (swb_contained.cuh).
 struct Stream {
-  uint64_t key, g, a, block;
+  uint64_t key, domain, g, a, block;
   uint64_t buf[4];
   int pos;
-  SWB_HD void init(uint64_t seed, uint64_t g_, uint64_t a_) {
-    key = seed; g = g_; a = a_; block = 0; pos = 4;
+  SWB_HD void init(uint64_t seed, uint64_t g_, uint64_t a_, uint64_t domain_ = SWB_SAMPLER_DOMAIN) {
+    key = seed; domain = domain_; g = g_; a = a_; block = 0; pos = 4;
   }
   SWB_HD uint64_t next() {
     if (pos == 4) {
       buf[0] = block++; buf[1] = a; buf[2] = g; buf[3] = 0;
-      philox4x64_10(buf, key, (uint64_t)SWB_SAMPLER_DOMAIN);
+      philox4x64_10(buf, key, domain);
       pos = 0;
     }
     return buf[pos++];

@@ -1,6 +1,8 @@
-// The device scene sampler (swb_sampler.cuh) built for the CPU: the restatement the tests hold the
-// CUDA kernels to, and a way to draw the device's scenes without a GPU.  Same source, no
+// The device scene sampler (swb_sampler.cuh) and contained-position sampler (swb_contained.cuh)
+// built for the CPU: the restatement the tests hold the CUDA kernels to, and a way to draw the
+// device's scenes without a GPU.  Same source, no
 // contraction (-ffp-contract=off), so it computes what the kernels compute, bit for bit.
+#include "swb_contained.cuh"
 #include "swb_sampler.cuh"
 
 extern "C" {
@@ -48,6 +50,28 @@ int64_t swb_host_sample_scenes(const swb_scene_program *prog, uint64_t seed, int
     }
   }
   return failures;
+}
+
+// swb_sample_contained on the host, over n rows of S packed slots each (row i's slot j at i * S + j:
+// live position x, y, centred-path transform m00 .. m11, shape id) with the engine's shape table
+// verts [SWB_NUM_SHAPES][SWB_MAX_VERTS][2], nverts [SWB_NUM_SHAPES].  Outputs as the device call
+// lays them out: position [n][n_samples][2], slot and status [n][n_samples].
+void swb_host_sample_contained(const double *x, const double *y, const double *m00, const double *m01,
+                               const double *m10, const double *m11, const uint8_t *shape, int32_t n,
+                               int32_t S, const double *verts, const int32_t *nverts, int32_t n_samples,
+                               uint64_t seed, double *position, int8_t *slot, uint8_t *status) {
+  for (int64_t i = 0; i < n; ++i) {
+    const size_t r = (size_t)i * S;
+    auto shape_at = [&](int j) -> int { return shape[r + j]; };
+    auto sprite_at = [&](int j) {
+      return swb_contained::Sprite{x[r + j], y[r + j], m00[r + j], m01[r + j], m10[r + j], m11[r + j]};
+    };
+    for (int64_t s = 0; s < n_samples; ++s) {
+      const int64_t t = i * n_samples + s;
+      status[t] = (uint8_t)swb_contained::sample_contained(seed, (uint64_t)i, (uint64_t)s, S, verts, nverts,
+                                                           shape_at, sprite_at, position + 2 * t, slot + t);
+    }
+  }
 }
 
 }  // extern "C"

@@ -833,6 +833,39 @@ class Engine(object):
         ctypes.c_void_p(success.data_ptr()), ctypes.c_void_p(status.data_ptr()), self._stream()))
     return reward, success, status
 
+  def sample_contained(self, seed, n_samples=1, states=None):
+    """Positions inside sprites (swb_sample_contained): n_samples draws per row of the live envs
+    (n = n_envs), or of the records of EnvStates `states`.  Sample s of row i picks one of the
+    row's sprites uniformly and rejection-samples a point of it, from the Philox stream
+    (seed, SWB_CONTAINED_DOMAIN) at counter (block, s, i, 0): a pure function of (seed, i, s, the
+    row's state).  Returns new tensors on this device: position float64 (n, n_samples, 2), slot int8
+    (n, n_samples) and status uint8 (n, n_samples) (ENV_NO_SPRITE, ENV_SAMPLE_TRIES; a failed
+    sample has position NaN and slot -1).  One launch on the current stream; reads only."""
+    if isinstance(seed, (bool, np.bool_)) or not isinstance(seed, (int, np.integer)) or not 0 <= seed < 2 ** 64:
+      raise ValueError('seed must be an int in [0, 2^64), got %r' % (seed,))
+    n = self.n_envs if states is None else len(states)
+    if states is not None:
+      self.check_states(states, n)
+    if isinstance(n_samples, (bool, np.bool_)) or not isinstance(n_samples, (int, np.integer)) or not (
+        1 <= n_samples < 2 ** 31):
+      raise ValueError('n_samples must be an int in [1, 2^31), got %r' % (n_samples,))
+    n_samples = int(n_samples)
+    position = torch.empty((n, n_samples, 2), dtype=torch.float64, device=self.device)
+    slot = torch.empty((n, n_samples), dtype=torch.int8, device=self.device)
+    status = torch.empty((n, n_samples), dtype=torch.uint8, device=self.device)
+    ptrs = [t.data_ptr() for t in (position, slot, status)]
+    rec = (None, 0) if states is None else (states.data.data_ptr(), states.data.numel())
+    if n == 0:
+      # zero rows: checked as any other call and nothing drawn, but an empty tensor may have no address;
+      # any aligned address stands in (nothing is read or written)
+      probe = torch.empty(16, dtype=torch.uint8, device=self.device).data_ptr()
+      ptrs = [p or probe for p in ptrs]
+      rec = rec if states is None else (rec[0] or probe, rec[1])
+    _native.check(self._lib.swb_sample_contained(
+        self._h, None if rec[0] is None else ctypes.c_void_p(rec[0]), n, rec[1], n_samples, int(seed),
+        *[ctypes.c_void_p(p) for p in ptrs], self._stream()))
+    return position, slot, status
+
   def launch_count(self):
     return int(self._lib.swb_launch_count(self._h))
 

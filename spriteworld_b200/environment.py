@@ -277,6 +277,9 @@ BatchedRollout = collections.namedtuple(
     'BatchedRollout', ['step_type', 'reward', 'discount', 'success', 'status'])
 
 
+ContainedPositions = collections.namedtuple('ContainedPositions', ['position', 'slot', 'status'])
+
+
 class BatchedEnvironment(object):
   """`n_envs` Spriteworld environments advanced in lockstep on one GPU.
 
@@ -540,6 +543,29 @@ class BatchedEnvironment(object):
     record i's goals, or the records' own goals if `goals` is None.  One launch on the current
     stream, no host synchronisation; no env, ring or `rng` changes."""
     return self._engine.evaluate(states, goals)
+
+  def sample_contained_positions(self, seed, n_samples=None, states=None):
+    """Positions inside sprites for random agents and plan proposals, drawn on the device: what
+    Environment.sample_contained_position() draws for one env -- a sprite chosen uniformly (not by
+    area), then a point of it by rejection from its bounding box -- for every env, or for every
+    record of EnvStates `states`.  Returns ContainedPositions(position float64, slot int8, status
+    uint8) of new device tensors: shapes (n, 2), (n,), (n,) with n_samples=None, ready for
+    actions[:, :2], or (n, n_samples, 2), (n, n_samples), (n, n_samples) for an int; sample 0 of
+    those equals the n_samples=None call.  slot indexes the slot axis of SpriteFactors and
+    SpriteMasks.  A row without sprites gives status ENV_NO_SPRITE, a sprite no draw lands in (scale
+    0) ENV_SAMPLE_TRIES, each with position NaN and slot -1.
+
+    Each sample is a pure function of (seed, row, sample index, the row's state), from the
+    device's own Philox stream: nothing is drawn from `rng` and nothing is kept, so there is nothing
+    to checkpoint.  Envs sample the scene they are on, also an env about to reset (whose next step
+    replaces it).  A float64 SelectMove / DragAndDrop action clicking `position` grabs `slot` or a
+    sprite above it; with the action space's noise_scale, step() adds noise to the click first, and
+    the grab is no longer certain.  One launch on the current stream, read-only (no env, ring, frame
+    or refill state changes) and without host synchronisation."""
+    position, slot, status = self._engine.sample_contained(seed, 1 if n_samples is None else n_samples, states)
+    if n_samples is None:
+      return ContainedPositions(position[:, 0], slot[:, 0], status[:, 0])
+    return ContainedPositions(position, slot, status)
 
   def _record_factor_tensors(self, factors, states):
     if not isinstance(states, engine_lib.EnvStates):

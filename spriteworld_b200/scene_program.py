@@ -15,6 +15,7 @@ header's size limits.
 
 `sample_on_host` runs the same sampler source built for the CPU (libswb_sampler_host.so): the
 restatement the device is tested against, and a way to draw the device's scenes without a GPU.
+`sample_contained_on_host` is the same for the contained-position sampler (swb_contained.cuh).
 """
 import ctypes
 import math
@@ -487,6 +488,9 @@ def _host_lib():
     L.swb_host_sample_scenes.argtypes = [vp, ctypes.c_uint64, ctypes.c_int32, vp, vp, ctypes.c_int64,
                                          vp, vp, vp]
     L.swb_host_sample_scenes.restype = ctypes.c_int64
+    L.swb_host_sample_contained.argtypes = [vp] * 7 + [ctypes.c_int32, ctypes.c_int32, vp, vp, ctypes.c_int32,
+                                                        ctypes.c_uint64, vp, vp, vp]
+    L.swb_host_sample_contained.restype = None
     if L.swb_host_sampler_sizeof_program() != ctypes.sizeof(Program):
       raise RuntimeError('ABI mismatch: swb_scene_program')
     _host = L
@@ -532,6 +536,37 @@ def sample_on_host(program, seed, env_ids, scene_idx, n_slots):
       ctypes.byref(program.struct), int(seed) & (2 ** 64 - 1), int(n_slots), env_ids.ctypes.data,
       scene_idx.ctypes.data, n, ctypes.byref(sample_out_struct(b)), ctypes.byref(op), ctypes.byref(idx))
   return b, ((int(idx.value), int(op.value)) if failures else None)
+
+
+def shape_table(shapes=None):
+  """(verts float64 (13, 32, 2), n_verts int32 (13,)): the engine's shape table (swb_config) of
+  `shapes` (default constants.SHAPES), indexed by ShapeType id."""
+  shapes = constants.SHAPES if shapes is None else shapes
+  verts = np.zeros((len(constants.SHAPE_NAMES) + 1, 32, 2), np.float64)
+  n_verts = np.zeros(len(constants.SHAPE_NAMES) + 1, np.int32)
+  for sid, name in enumerate(constants.SHAPE_NAMES, 1):
+    v = np.asarray(shapes[name], np.float64)
+    verts[sid, :len(v)], n_verts[sid] = v, len(v)
+  return verts, n_verts
+
+
+def sample_contained_on_host(rows, seed, n_samples=1, shapes=None):
+  """swb_sample_contained on the CPU, built from the kernel's own source (swb_contained.cuh):
+  `rows` is a dict of (n, S) arrays x, y (live positions), m00, m01, m10, m11 and shape (raw ids,
+  sanitised as a record load sanitises them).  Returns (position float64 (n, n_samples, 2), slot
+  int8 (n, n_samples), status uint8 (n, n_samples)), what the device returns for those rows."""
+  f64 = {k: np.ascontiguousarray(rows[k], np.float64) for k in ('x', 'y', 'm00', 'm01', 'm10', 'm11')}
+  shape = np.ascontiguousarray(rows['shape'], np.uint8)
+  n, S = shape.shape
+  verts, n_verts = shape_table(shapes)
+  position = np.zeros((n, n_samples, 2), np.float64)
+  slot = np.zeros((n, n_samples), np.int8)
+  status = np.zeros((n, n_samples), np.uint8)
+  _host_lib().swb_host_sample_contained(
+      *[f64[k].ctypes.data for k in ('x', 'y', 'm00', 'm01', 'm10', 'm11')], shape.ctypes.data, n, S,
+      verts.ctypes.data, n_verts.ctypes.data, int(n_samples), int(seed) & (2 ** 64 - 1), position.ctypes.data,
+      slot.ctypes.data, status.ctypes.data)
+  return position, slot, status
 
 
 def layout_from_factor_table(values, kinds):
