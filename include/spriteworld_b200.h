@@ -427,6 +427,27 @@ int swb_render_masks(swb_engine *eng, int32_t width, int32_t height, int32_t ant
                      const void *records, int32_t n, uint64_t records_bytes, uint8_t *masks,
                      void *stream);
 
+/*
+ * Amodal sprite coverage (renderers.SpriteCoverage): every sprite covering each pixel, hidden or
+ * not.  `cover` is [n][height][width] int32; bit k of pixel (r, c) is set if slot k's Pillow polygon
+ * fill covers the sample point swb_render_masks uses for that pixel, whether or not a sprite above
+ * hides it (bit 31 is the sign bit).  So the mask swb_render_masks draws is the highest set bit + 1,
+ * or 0 where cover is 0.  `visible` and `area` are [n][S] int32: for each slot, the number of
+ * pixels where it is the top-most covering sprite, and the number where its bit is set.  Empty
+ * slots and sprites wholly out of frame have no bits and zero counts.
+ *
+ * Records, sizes and n as swb_render_masks takes them (records == NULL: the E live envs, n == E).
+ * An accepted call with n > 0 zeroes visible and area on `stream` and is then one launch there;
+ * the counts are integer sums, exact and independent of scheduling.  n == 0 enqueues nothing.
+ * Read-only as swb_render_masks.  Refused, enqueuing nothing: what swb_render_masks refuses (with
+ * a null cover, visible or area in place of null masks), an output not 4-byte aligned, an output
+ * that overlaps another output or the records, or an n whose bands (of at most 128 mask rows and
+ * 16 KiB of coverage) exceed 2^31 - 1 CTAs.
+ */
+int swb_render_coverage(swb_engine *eng, int32_t width, int32_t height, int32_t anti_aliasing,
+                        const void *records, int32_t n, uint64_t records_bytes, int32_t *cover,
+                        int32_t *visible, int32_t *area, void *stream);
+
 /* Env dst_ids[i] <- env src_ids[i].  Ids in [0, E), destinations distinct.  Every read sees the
  * state from before the call, also where the two sets overlap (then the records go through
  * device scratch of the engine: two kernels instead of one). */

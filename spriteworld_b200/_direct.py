@@ -149,3 +149,15 @@ def render_masks(renderer, sprites):
   eng = _engine(max(1, len(sprites)), _DUMMY_ACTION, _NO_TASK, True)
   _load(eng, sprites)
   return eng.render_masks(renderer.width, renderer.height, renderer.anti_aliasing)[0].cpu().numpy()
+
+
+def render_coverage(renderer, sprites):
+  """Coverage of a Python sprite list: dict 'cover' (H, W) int32, bit i set where sprites[i]'s
+  polygon covers the pixel's sample point, and 'visible', 'area' (len(sprites),) int32."""
+  n = len(sprites)
+  eng = _engine(max(1, n), _DUMMY_ACTION, _NO_TASK, True)
+  _load(eng, sprites)
+  cover, visible, area = eng.render_coverage(renderer.width, renderer.height, renderer.anti_aliasing)
+  S = eng.n_slots   # n slots for n >= 1 sprites, so bit i is slot i; one empty slot for none
+  return collections.OrderedDict([('cover', cover[0].cpu().numpy()), ('visible', visible[0, S - n:].cpu().numpy()),
+                                  ('area', area[0, S - n:].cpu().numpy())])

@@ -172,7 +172,7 @@ int upload_axis(swb_raster *r, const AxisHost &h, AxisTables *d) {
 extern "C" {
 
 const char *swb_last_error(void) { return g_error.c_str(); }
-int swb_version(void) { return 12; }
+int swb_version(void) { return 13; }
 int swb_sizeof_config(void) { return (int)sizeof(swb_config); }
 int swb_sizeof_task_node(void) { return (int)sizeof(swb_task_node); }
 
@@ -1285,34 +1285,84 @@ int swb_render_states(swb_engine *eng, swb_raster *r, const void *records, int32
                         RenderRecords{static_cast<const unsigned char *>(records), (size_t)rb});
 }
 
-int swb_render_masks(swb_engine *eng, int32_t width, int32_t height, int32_t anti_aliasing,
-                     const void *records, int32_t n, uint64_t records_bytes, uint8_t *masks, void *stream_) {
-  static const char fn[] = "swb_render_masks";
+// The checks swb_render_masks and swb_render_coverage share, in this order (`out`: the first
+// output, null-checked with the engine; `outs` names the outputs in messages).
+static int check_mask_call(const swb_engine *eng, const char *fn, const char *outs, const void *out,
+                           int32_t width, int32_t height, int32_t anti_aliasing, const void *records,
+                           int32_t n, uint64_t records_bytes, bool cover) {
   if (width < 1 || height < 1 || anti_aliasing < 1)
     return fail("%s: width %d, height %d and anti_aliasing %d must be >= 1", fn, width, height, anti_aliasing);
-  if (!eng || !masks) return fail("%s: null engine or masks", fn);
+  if (!eng || !out) return fail("%s: null engine or %s", fn, outs);
   if ((int64_t)anti_aliasing * width > 4095 || (int64_t)anti_aliasing * height > 4095)
     return fail("%s: canvas %lld x %lld exceeds 4095 pixels per side", fn, (long long)anti_aliasing * width,
                 (long long)anti_aliasing * height);
   if (n < 0) return fail("%s: n = %d", fn, n);
   if (!records && n != eng->st.E)
-    return fail("%s: n = %d must be E = %d when the masks are the live envs'", fn, n, eng->st.E);
-  const MaskLayout L(eng->st.S, width, height, anti_aliasing);
+    return fail("%s: n = %d must be E = %d when the %s are the live envs'", fn, n, eng->st.E, outs);
+  const MaskLayout L(eng->st.S, width, height, anti_aliasing, cover);
   if ((int64_t)n * L.n_bands > INT32_MAX)
-    return fail("%s: n = %d masks of %d bands each exceed 2^31 - 1 CTAs", fn, n, L.n_bands);
+    return fail("%s: n = %d %s of %d bands each exceed 2^31 - 1 CTAs", fn, n, outs, L.n_bands);
+  if (records && check_record_buffer(eng, fn, "records", records, records_bytes, n)) return 1;
+  return 0;
+}
+
+// [a, a + na) and [b, b + nb) share a byte
+static bool overlap(const void *a, uint64_t na, const void *b, uint64_t nb) {
+  const uint64_t a0 = reinterpret_cast<uintptr_t>(a), b0 = reinterpret_cast<uintptr_t>(b);
+  return a0 < b0 + nb && b0 < a0 + na;
+}
+
+int swb_render_masks(swb_engine *eng, int32_t width, int32_t height, int32_t anti_aliasing,
+                     const void *records, int32_t n, uint64_t records_bytes, uint8_t *masks, void *stream_) {
+  static const char fn[] = "swb_render_masks";
+  if (check_mask_call(eng, fn, "masks", masks, width, height, anti_aliasing, records, n, records_bytes, false))
+    return 1;
+  const MaskLayout L(eng->st.S, width, height, anti_aliasing);
   const uint64_t rb = RecordLayout(eng->st.S, eng->st.G).bytes();
-  if (records) {
-    if (check_record_buffer(eng, fn, "records", records, records_bytes, n)) return 1;
-    const uint64_t r0 = reinterpret_cast<uintptr_t>(records), m0 = reinterpret_cast<uintptr_t>(masks);
-    if (m0 < r0 + (uint64_t)n * rb && r0 < m0 + (uint64_t)n * height * width)
-      return fail("%s: the masks overlap the records", fn);
-  }
+  if (records && overlap(masks, (uint64_t)n * height * width, records, (uint64_t)n * rb))
+    return fail("%s: the masks overlap the records", fn);
   if (n == 0) return 0;
   CUDA_TRY(cudaSetDevice(eng->device));
-  auto kernel = records ? mask_kernel<true> : mask_kernel<false>;
+  auto kernel = records ? mask_kernel<true, false> : mask_kernel<false, false>;
   CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, L.total));
   kernel<<<(unsigned)((int64_t)n * L.n_bands), MK_THREADS, L.total, static_cast<cudaStream_t>(stream_)>>>(
-      eng->st, L, masks, RenderRecords{static_cast<const unsigned char *>(records), (size_t)rb});
+      eng->st, L, masks, RenderRecords{static_cast<const unsigned char *>(records), (size_t)rb}, CoverCounts{});
+  eng->launches++;
+  CUDA_TRY(cudaGetLastError());
+  return 0;
+}
+
+int swb_render_coverage(swb_engine *eng, int32_t width, int32_t height, int32_t anti_aliasing,
+                        const void *records, int32_t n, uint64_t records_bytes, int32_t *cover,
+                        int32_t *visible, int32_t *area, void *stream_) {
+  static const char fn[] = "swb_render_coverage";
+  if (check_mask_call(eng, fn, "outputs", cover, width, height, anti_aliasing, records, n, records_bytes, true))
+    return 1;
+  if (!visible || !area) return fail("%s: null engine or outputs", fn);
+  const struct { const void *p; uint64_t bytes; const char *name; } outs[3] = {
+      {cover, (uint64_t)n * height * width * 4, "cover"},
+      {visible, (uint64_t)n * eng->st.S * 4, "visible"},
+      {area, (uint64_t)n * eng->st.S * 4, "area"}};
+  const uint64_t rb = RecordLayout(eng->st.S, eng->st.G).bytes();
+  for (int i = 0; i < 3; ++i) {
+    if (reinterpret_cast<uintptr_t>(outs[i].p) % 4) return fail("%s: %s is not 4-byte aligned", fn, outs[i].name);
+    for (int j = 0; j < i; ++j)
+      if (overlap(outs[i].p, outs[i].bytes, outs[j].p, outs[j].bytes))
+        return fail("%s: %s overlaps %s", fn, outs[i].name, outs[j].name);
+    if (records && overlap(outs[i].p, outs[i].bytes, records, (uint64_t)n * rb))
+      return fail("%s: %s overlaps the records", fn, outs[i].name);
+  }
+  if (n == 0) return 0;
+  const MaskLayout L(eng->st.S, width, height, anti_aliasing, true);
+  CUDA_TRY(cudaSetDevice(eng->device));
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  auto kernel = records ? mask_kernel<true, true> : mask_kernel<false, true>;
+  CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, L.total));
+  CUDA_TRY(cudaMemsetAsync(visible, 0, (size_t)n * eng->st.S * 4, stream));
+  CUDA_TRY(cudaMemsetAsync(area, 0, (size_t)n * eng->st.S * 4, stream));
+  kernel<<<(unsigned)((int64_t)n * L.n_bands), MK_THREADS, L.total, stream>>>(
+      eng->st, L, reinterpret_cast<uint8_t *>(cover),
+      RenderRecords{static_cast<const unsigned char *>(records), (size_t)rb}, CoverCounts{visible, area});
   eng->launches++;
   CUDA_TRY(cudaGetLastError());
   return 0;

@@ -1,10 +1,14 @@
-// Mask kernel: which sprite is visible at each pixel (renderers.SpriteMasks, swb_render_masks).
+// Mask kernel: which sprite is visible at each pixel (renderers.SpriteMasks, swb_render_masks),
+// and which sprites cover it (renderers.SpriteCoverage, swb_render_coverage).
 //
 // Mask pixel (i, j) of a W x H mask at anti_aliasing aa is the slot + 1 of the top-most sprite
 // whose Pillow polygon fill covers canvas pixel (aa j + aa/2, aa (H-1-i) + aa/2) of the aa W x aa H
 // canvas PILRenderer draws on, or 0 (what Image.resize(NEAREST) of a label canvas picks, flipped
 // like the frames).  Only Pillow's scan conversion is needed, not its LANCZOS filter, and only one
-// canvas row per mask row.
+// canvas row per mask row.  The coverage of the same pixel (kCover) is the int32 whose bit k is set
+// where slot k's fill covers that canvas pixel, whether or not a sprite above hides it, so the mask
+// is its highest set bit + 1; with it come per-slot counts of the pixels where the slot is the
+// top-most covering sprite (visible) and where its bit is set (area).
 //
 // One CTA draws one band of mask rows of one env (or record):
 //   A  a warp per sprite, a lane per vertex: the integer canvas vertices, Pillow's edge records,
@@ -13,15 +17,19 @@
 //   B  a thread per mask row scan-converts its one canvas row for every sprite, back to front:
 //      the crossings of the edges spanning the row (an edge ending on an interior row counts
 //      twice), sorted and paired with ROUND_UP / ROUND_DOWN, plus the horizontal edges on the
-//      row; each canvas span [xs, xe] paints slot + 1 into the mask columns whose sample
-//      aa j + aa/2 lies in it, in a row staged in shared memory.
-//   C  the staged band goes out with 16-byte stores (bytes at its ends).
+//      row; each canvas span [xs, xe] paints slot + 1 (kCover: ORs 1 << slot) into the mask
+//      columns whose sample aa j + aa/2 lies in it, in a row staged in shared memory.
+//   C  the staged band goes out with 16-byte stores (single pixels at its ends).  kCover: each
+//      warp counts its pixels per slot with ballots, the CTA sums the warps in shared memory and
+//      adds its sums to the outputs with one integer atomic per (band, slot).
 // A sprite row has at most 2 crossings per edge, 2 * SWB_MAX_VERTS in all, and every one is kept:
 // the mask is exact for every shape, and there is no overflow status.
 //
-// Nothing but the masks is written: no env, pool entry, frame or render status changes.
+// Nothing but the masks (kCover: the coverage and its counts) is written: no env, pool entry,
+// frame or render status changes.
 #pragma once
 #include <climits>
+#include <type_traits>
 
 #include "swb_device.cuh"
 #include "swb_render.cuh"
@@ -30,17 +38,20 @@
 namespace swb {
 
 constexpr int MK_THREADS = 128;          // threads per CTA = most mask rows per band
-constexpr int MK_STAGE_BYTES = 16384;    // staged mask bytes per band (fewer rows for wide masks)
+constexpr int MK_STAGE_BYTES = 16384;    // staged bytes per band (fewer rows for wide or coverage masks)
 constexpr int MK_XCAP = 2 * EV;          // crossings one sprite row can have
 
-// A mask raster and the shared-memory layout of one CTA.
+// A mask raster and the shared-memory layout of one CTA; `cover`: staged pixels are the 4-byte
+// coverage words, and the CTA keeps per-slot counts.
 struct MaskLayout {
   int S, W, H, aa, CW, CH, band_rows, n_bands;
   int off_edge, off_hl, off_meta, off_xx, off_stage, total;
-  __host__ __device__ MaskLayout(int S_, int W_, int H_, int aa_) : S(S_), W(W_), H(H_), aa(aa_) {
+  __host__ __device__ MaskLayout(int S_, int W_, int H_, int aa_, bool cover = false)
+      : S(S_), W(W_), H(H_), aa(aa_) {
+    const int px = cover ? 4 : 1;         // bytes per staged pixel
     CW = aa * W;
     CH = aa * H;
-    band_rows = MK_STAGE_BYTES / W;
+    band_rows = MK_STAGE_BYTES / (px * W);
     if (band_rows < 1) band_rows = 1;
     if (band_rows > MK_THREADS) band_rows = MK_THREADS;
     if (band_rows > H) band_rows = H;
@@ -51,14 +62,25 @@ struct MaskLayout {
     off_hl = take(S * EV * 3 * 2);          // horizontal edges: y, xmin, xmax (int16)
     off_meta = take(S * 5 * 4);             // nv, nh, has-join, p_ymax, ymin | ymax << 16
     off_xx = take(MK_XCAP * MK_THREADS * 4);  // crossings, [k][thread]
-    off_stage = take(band_rows * W + 16);   // staged band, placed at the output's address mod 16
+    off_stage = take(band_rows * W * px + 16);  // staged band, placed at the output's address mod 16
+    if (cover) take(S * 2 * 4);             // the band's visible [S], area [S] (int), at cnt_offset()
     total = o;
   }
+  // cover: where the band's counts are, right after the staged band
+  __host__ __device__ int cnt_offset() const { return off_stage + ((band_rows * W * 4 + 16 + 15) & ~15); }
 };
 
-template <bool kRecords>
+// The per-slot counts of the coverage, [n][S] int32 each; zeroed before the launch.
+struct CoverCounts {
+  int32_t *visible, *area;
+};
+
+// kCover: `masks` is the [n][H][W] int32 coverage, and `counts` receives its per-slot counts;
+// otherwise `masks` is the [n][H][W] uint8 mask and `counts` is not read.
+template <bool kRecords, bool kCover>
 __global__ void __launch_bounds__(MK_THREADS)
-mask_kernel(DevState st, const MaskLayout L, uint8_t *__restrict__ masks, const RenderRecords recs) {
+mask_kernel(DevState st, const MaskLayout L, uint8_t *__restrict__ masks, const RenderRecords recs,
+            const CoverCounts counts) {
   extern __shared__ __align__(16) unsigned char g_mask_smem[];
   unsigned char *const smem = g_mask_smem;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -79,6 +101,7 @@ mask_kernel(DevState st, const MaskLayout L, uint8_t *__restrict__ masks, const 
   int *s_nh = s_nv + S, *s_hasov = s_nh + S, *s_pymax = s_hasov + S;
   uint32_t *s_yext = reinterpret_cast<uint32_t *>(s_pymax + S);
   float *xx = reinterpret_cast<float *>(smem + L.off_xx) + tid;  // crossing k at xx[k * MK_THREADS]
+  using Px = std::conditional_t<kCover, uint32_t, uint8_t>;      // a staged pixel
 
   // ---- phase A: a warp per sprite, a lane per vertex / edge (render_kernel phase A) ----------
   const int cur = kRecords ? 0 : st.cursor[e];
@@ -197,16 +220,18 @@ mask_kernel(DevState st, const MaskLayout L, uint8_t *__restrict__ masks, const 
     }
   }
 
-  // the band's output rows [i0, i0 + nb) are bytes [g, g + nb * W) of the masks; the band is
-  // staged from s_stage + (g mod 16), so that staged and global addresses agree modulo 16
+  // the band's output rows [i0, i0 + nb) are pixels [g, g + nb * W) of the masks; the band is
+  // staged from s_stage + (its address mod 16), so that staged and global addresses agree modulo 16
   const int i0 = band * L.band_rows;
   const int nb = min(L.band_rows, L.H - i0);
   const size_t g = (e * (size_t)L.H + (size_t)i0) * (size_t)L.W;
-  const int nbytes = nb * L.W;
-  uint8_t *const gdst = masks + g;
+  const int npx = nb * L.W;
+  Px *const gdst = reinterpret_cast<Px *>(masks) + g;
   const int mis = (int)(reinterpret_cast<uintptr_t>(gdst) & 15u);
-  uint8_t *const stage = smem + L.off_stage + mis;
-  for (int i = tid; i < nbytes; i += MK_THREADS) stage[i] = 0;
+  Px *const stage = reinterpret_cast<Px *>(smem + L.off_stage + mis);
+  int *const s_cnt = reinterpret_cast<int *>(smem + L.cnt_offset());  // kCover: visible [S], area [S]
+  for (int i = tid; i < npx; i += MK_THREADS) stage[i] = 0;
+  if (kCover && tid < 2 * S) s_cnt[tid] = 0;
   __syncthreads();
 
   // ---- phase B: a thread per mask row, its one canvas row, sprites back to front ------------
@@ -214,17 +239,20 @@ mask_kernel(DevState st, const MaskLayout L, uint8_t *__restrict__ masks, const 
     const int i = i0 + tid;
     const int y = L.aa * (L.H - 1 - i) + L.aa / 2;  // canvas row of mask row i (always on the canvas)
     const int half = L.aa / 2;
-    uint8_t *const row = stage + (size_t)tid * L.W;
+    Px *const row = stage + (size_t)tid * L.W;
     // paints the mask columns j with xs <= aa j + aa/2 <= xe (0 <= xs <= xe < CW)
-    auto paint = [&](int xs, int xe, uint8_t label) {
+    auto paint = [&](int xs, int xe, Px label) {
       const int jlo = (xs - half + L.aa - 1) / L.aa, jhi = (xe - half + L.aa) / L.aa - 1;
-      for (int j = jlo; j <= jhi; ++j) row[j] = label;
+      for (int j = jlo; j <= jhi; ++j) {
+        if constexpr (kCover) row[j] |= label;
+        else row[j] = label;
+      }
     };
 #pragma unroll 1
     for (int s = 0; s < S; ++s) {
       const uint32_t ext = s_yext[s];
       if (y < (int)(short)(ext & 0xFFFFu) || y > (int)(short)(ext >> 16)) continue;
-      const uint8_t label = (uint8_t)(s + 1);
+      const Px label = kCover ? (Px)(1u << s) : (Px)(s + 1);
       const int nv = s_nv[s], p_ymax = s_pymax[s];
       const bool hasov = s_hasov[s] != 0;
       int j = 0;
@@ -274,14 +302,40 @@ mask_kernel(DevState st, const MaskLayout L, uint8_t *__restrict__ masks, const 
   __syncthreads();
 
   // ---- phase C: the staged band to the masks -------------------------------------------------
-  const int head = min((16 - mis) & 15, nbytes);
-  const int n16 = (nbytes - head) >> 4;
-  const int tail0 = head + (n16 << 4);
+  constexpr int LOG16 = kCover ? 2 : 4;  // log2 of the pixels per 16-byte store
+  const int head = min(((16 - mis) & 15) / (int)sizeof(Px), npx);
+  const int n16 = (npx - head) >> LOG16;
+  const int tail0 = head + (n16 << LOG16);
   for (int i = tid; i < head; i += MK_THREADS) gdst[i] = stage[i];
   const uint4 *src16 = reinterpret_cast<const uint4 *>(stage + head);
   uint4 *dst16 = reinterpret_cast<uint4 *>(gdst + head);
   for (int i = tid; i < n16; i += MK_THREADS) dst16[i] = src16[i];
-  for (int i = tail0 + tid; i < nbytes; i += MK_THREADS) gdst[i] = stage[i];
+  for (int i = tail0 + tid; i < npx; i += MK_THREADS) gdst[i] = stage[i];
+
+  if constexpr (kCover) {
+    // lane s counts slot s over its warp's pixels: a ballot per slot that any of 32 pixels has
+    int vis = 0, area = 0;
+    for (int p0 = warp * 32; p0 < npx; p0 += MK_THREADS) {
+      const uint32_t c = p0 + lane < npx ? stage[p0 + lane] : 0u;
+      const int top = c ? 31 - __clz(c) : -1;  // the top-most covering slot
+      for (unsigned any = __reduce_or_sync(FULL, c); any; any &= any - 1u) {
+        const int s = __ffs(any) - 1;
+        const int a = __popc(__ballot_sync(FULL, (c >> s) & 1u));
+        const int v = __popc(__ballot_sync(FULL, top == s));
+        if (lane == s) { area += a; vis += v; }
+      }
+    }
+    if (area) {  // vis <= area, and only slots < S have bits
+      atomicAdd(&s_cnt[lane], vis);
+      atomicAdd(&s_cnt[S + lane], area);
+    }
+    __syncthreads();
+    if (tid < S) {
+      const int v = s_cnt[tid], a = s_cnt[S + tid];
+      if (v) atomicAdd(&counts.visible[e * S + tid], v);
+      if (a) atomicAdd(&counts.area[e * S + tid], a);
+    }
+  }
 }
 
 }  // namespace swb

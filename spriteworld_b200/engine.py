@@ -465,6 +465,49 @@ class Engine(object):
         ctypes.c_void_p(masks_ptr), self._stream()))
     return out
 
+  def render_coverage(self, width, height, anti_aliasing=1, states=None, out=None):
+    """Amodal sprite coverage (swb_render_coverage): (cover, visible, area), int32 (n, height,
+    width), (n, n_slots) and (n, n_slots).  Bit k of a cover pixel is set where slot k's polygon
+    covers the pixel's sample point (the one render_masks samples), whether or not a sprite above
+    hides it; visible[i, k] counts the pixels where slot k is the top-most covering sprite (the mask
+    render_masks draws is k + 1 there), area[i, k] those where bit k is set (renderers.SpriteCoverage).
+    Of the live envs (n = n_envs), or with `states` of EnvStates of any n records, as if loaded.
+    Into `out` if given (a triple of contiguous int32 tensors of those shapes on this device), else
+    new tensors.  One launch on the current stream (after zeroing the counts); nothing else changes."""
+    if states is not None and not isinstance(states, EnvStates):
+      raise ValueError('states must be EnvStates, got %s' % type(states).__name__)
+    n = self.n_envs if states is None else len(states)
+    if states is not None:
+      self.check_states(states, n)
+    W, H, aa = int(width), int(height), int(anti_aliasing)
+    shapes = ((n, H, W), (n, self.n_slots), (n, self.n_slots))
+    if out is None:
+      out = (torch.empty((n, max(H, 0), max(W, 0)), dtype=torch.int32, device=self.device),
+             torch.empty(shapes[1], dtype=torch.int32, device=self.device),
+             torch.empty(shapes[2], dtype=torch.int32, device=self.device))
+    else:
+      if not isinstance(out, (tuple, list)) or len(out) != 3:
+        raise ValueError('out must be a (cover, visible, area) triple, got %s' % type(out).__name__)
+      for name, t, shape in zip(('cover', 'visible', 'area'), out, shapes):
+        if (not isinstance(t, torch.Tensor) or t.dtype != torch.int32 or t.device != self.device or
+            tuple(t.shape) != shape or not t.is_contiguous()):
+          raise ValueError('%s must be a contiguous int32 tensor of shape %s on %s, got %s' % (
+              name, shape, self.device, _describe(t)))
+      out = tuple(out)
+    ptrs = [t.data_ptr() for t in out]
+    rec = (None, 0) if states is None else (states.data.data_ptr(), states.data.numel())
+    if n == 0:
+      # zero records: checked as any call, nothing drawn; an aligned address stands in for empty
+      # buffers, which cannot overlap (nothing is read or written)
+      probe = torch.empty(16, dtype=torch.uint8, device=self.device)
+      ptrs = [p or probe.data_ptr() for p in ptrs]
+      if rec[0] is not None:
+        rec = (rec[0] or probe.data_ptr(), rec[1])
+    _native.check(self._lib.swb_render_coverage(
+        self._h, W, H, aa, None if rec[0] is None else ctypes.c_void_p(rec[0]), n, rec[1],
+        *[ctypes.c_void_p(p) for p in ptrs], self._stream()))
+    return out
+
   def render_status(self):
     """Zero-copy uint8 (E,) view of the per-env status of the last render() (ENV_SPAN_OVERFLOW)."""
     if getattr(self, '_render_status_view', None) is None:

@@ -367,6 +367,12 @@ class BatchedEnvironment(object):
     self._mask_buffers = {
         id(r): torch.empty((E, r.height, r.width), dtype=torch.uint8, device=self._engine.device)
         for r in self._other.values() if isinstance(r, handcrafted.SpriteMasks)}
+    # and one (cover, visible, area) per SpriteCoverage renderer
+    self._coverage_buffers = {
+        id(r): (torch.empty((E, r.height, r.width), dtype=torch.int32, device=self._engine.device),
+                torch.empty((E, slots), dtype=torch.int32, device=self._engine.device),
+                torch.empty((E, slots), dtype=torch.int32, device=self._engine.device))
+        for r in self._other.values() if isinstance(r, handcrafted.SpriteCoverage)}
     if sampler == 'device':
       self._init_device_sampler(seed, env_offset)
       return
@@ -867,15 +873,18 @@ class BatchedEnvironment(object):
     return BatchedRollout(res.step_type, res.reward, discount, res.success, res.status)
 
   def render(self):
-    """Re-renders every PILRenderer and SpriteMasks observation of the current state (a loaded one,
-    say) into this environment's buffers, and returns them: dict name -> uint8 (n_envs, H, W, 3)
-    frames, then uint8 (n_envs, H, W) masks."""
+    """Re-renders every PILRenderer, SpriteMasks and SpriteCoverage observation of the current
+    state (a loaded one, say) into this environment's buffers, and returns them: dict name -> uint8
+    (n_envs, H, W, 3) frames, then uint8 (n_envs, H, W) masks and coverage dicts, in renderer
+    order."""
     out = collections.OrderedDict()
     for name, r in self._rasters.items():
       out[name] = self._engine.render(r, self._frames[name])
     for name, r in self._other.items():
       if isinstance(r, handcrafted.SpriteMasks):
         out[name] = self.render_masks(r)
+      elif isinstance(r, handcrafted.SpriteCoverage):
+        out[name] = self.render_coverage(r)
     return out
 
   def render_masks(self, renderer, states=None):
@@ -887,12 +896,25 @@ class BatchedEnvironment(object):
       return self._engine.render_masks(*dims, states=states)
     return self._engine.render_masks(*dims, out=self._mask_buffers.get(id(renderer)))
 
+  def render_coverage(self, renderer, states=None):
+    """SpriteCoverage `renderer`'s observation (Engine.render_coverage) on the current stream: dict
+    'cover' int32 (n, H, W), 'visible' and 'area' int32 (n, n_slots).  Of the live envs into this
+    environment's buffers for the renderer (new tensors for a renderer it does not own), or of
+    EnvStates `states` into new tensors."""
+    dims = (renderer.width, renderer.height, renderer.anti_aliasing)
+    if states is not None:
+      out = self._engine.render_coverage(*dims, states=states)
+    else:
+      out = self._engine.render_coverage(*dims, out=self._coverage_buffers.get(id(renderer)))
+    return collections.OrderedDict(zip(('cover', 'visible', 'area'), out))
+
   def observe(self, states):
     """The observations of env records without loading them: (observation, status) for EnvStates
     `states` of n records, observation an OrderedDict in renderer order of what step() would
     observe for envs that load_envs(states) had loaded -- PILRenderer frames as new uint8
     (n, H, W, 3) tensors (one render launch per raster; never this environment's own frame
-    buffers), SpriteFactors dicts of (n, n_slots) tensors -- and status uint8 (n,), the OR over the
+    buffers), SpriteFactors dicts of (n, n_slots) tensors, SpriteMasks and SpriteCoverage
+    observations in new tensors (one launch each) -- and status uint8 (n,), the OR over the
     rasters of their render status (_native.ENV_SPAN_OVERFLOW).
 
     Enqueued on the current stream without a host synchronisation.  Read-only: no env, scene ring,

@@ -144,6 +144,9 @@ class GymWrapper(object):
 
   def _process_obs(self, obs):
     for k, v in obs.items():
+      if isinstance(v, dict):         # SpriteCoverage: a dict of arrays, as its space describes
+        obs[k] = type(v)((kk, np.asarray(vv)) for kk, vv in v.items())
+        continue
       obs[k] = np.asarray(v)
       if obs[k].dtype == bool:       # boolean 'success' becomes float32 (:83-85)
         obs[k] = obs[k].astype(np.float32)

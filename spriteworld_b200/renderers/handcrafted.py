@@ -70,6 +70,17 @@ class SpriteFactors(abstract_renderer.AbstractRenderer):
     return spec
 
 
+def _check_mask_raster(renderer, image_size, anti_aliasing):
+  """SpriteMasks' and SpriteCoverage's arguments: sets _image_size and _anti_aliasing."""
+  renderer._image_size = tuple(int(v) for v in image_size)
+  renderer._anti_aliasing = int(anti_aliasing)
+  if len(renderer._image_size) != 2 or min(renderer._image_size) < 1 or renderer._anti_aliasing < 1:
+    raise ValueError('image_size must be (width, height) >= 1 and anti_aliasing >= 1, got %r, %r'
+                     % (image_size, anti_aliasing))
+  if renderer._anti_aliasing * max(renderer._image_size) > 4095:
+    raise ValueError('the canvas (anti_aliasing * image_size) exceeds 4095 pixels per side')
+
+
 class SpriteMasks(abstract_renderer.AbstractRenderer):
   """Instance masks: which sprite is visible at each pixel of a PILRenderer frame.
 
@@ -86,13 +97,7 @@ class SpriteMasks(abstract_renderer.AbstractRenderer):
   whose canvas sides stay within 4095 pixels."""
 
   def __init__(self, image_size=(64, 64), anti_aliasing=1):
-    self._image_size = tuple(int(v) for v in image_size)
-    self._anti_aliasing = int(anti_aliasing)
-    if len(self._image_size) != 2 or min(self._image_size) < 1 or self._anti_aliasing < 1:
-      raise ValueError('image_size must be (width, height) >= 1 and anti_aliasing >= 1, got %r, %r'
-                       % (image_size, anti_aliasing))
-    if self._anti_aliasing * max(self._image_size) > 4095:
-      raise ValueError('the canvas (anti_aliasing * image_size) exceeds 4095 pixels per side')
+    _check_mask_raster(self, image_size, anti_aliasing)
     self._observation_spec = specs.Array(shape=(self.height, self.width), dtype=np.uint8)
 
   @property
@@ -125,6 +130,75 @@ class SpriteMasks(abstract_renderer.AbstractRenderer):
 
   def batch_observation_spec(self, env):
     return self._observation_spec
+
+
+class SpriteCoverage(abstract_renderer.AbstractRenderer):
+  """Amodal sprite coverage: every sprite covering each pixel of a PILRenderer frame, hidden or not,
+  with per-sprite visible and total pixel counts.
+
+  Observes a dict for image_size=(W, H) and S sprites:
+    'cover'    int32 (H, W): bit k is set where sprite k's Pillow polygon fill covers the pixel's
+               sample point, whether or not a sprite above hides it (bit 31 is the sign bit).  The
+               sample point, integer vertices and fill rules are SpriteMasks': canvas pixel
+               (aa j + aa//2, aa (H-1-i) + aa//2) of the aa W x aa H canvas PILRenderer draws on.
+    'visible'  int32 (S,): per sprite, the pixels where it is the top-most covering sprite, which
+               is (SpriteMasks mask == k + 1).sum().
+    'area'     int32 (S,): per sprite, the pixels whose bit k is set.
+  So the SpriteMasks mask is the highest set bit + 1 (0 where cover is 0), visible <= area, and
+  empty slots and sprites wholly out of frame have no bits and zero counts.  In Pillow, bit k's
+  plane is sprite k drawn alone with fill 1 into a zero 'L' canvas of aa W x aa H, then
+  resize((W, H), NEAREST) and np.flipud.  Drawn by the mask kernel's coverage mode
+  (csrc/swb_masks.cuh), which also counts.
+
+  Bits: in a BatchedEnvironment, S is n_slots and bit k is slot k of SpriteFactors.render_batch;
+  on a sprite list (`render`, the drop-in Environment), bit i is sprites[i].  The same arguments
+  and limits as SpriteMasks."""
+
+  def __init__(self, image_size=(64, 64), anti_aliasing=1):
+    _check_mask_raster(self, image_size, anti_aliasing)
+    self._num_sprites = 0
+
+  @property
+  def width(self):
+    return self._image_size[0]
+
+  @property
+  def height(self):
+    return self._image_size[1]
+
+  @property
+  def anti_aliasing(self):
+    return self._anti_aliasing
+
+  def _spec(self, n):
+    i32, npx = np.iinfo(np.int32), self.height * self.width
+    return collections.OrderedDict([
+        ('cover', specs.BoundedArray(shape=(self.height, self.width), dtype=np.int32, minimum=i32.min,
+                                     maximum=i32.max)),
+        ('visible', specs.BoundedArray(shape=(n,), dtype=np.int32, minimum=0, maximum=npx)),
+        ('area', specs.BoundedArray(shape=(n,), dtype=np.int32, minimum=0, maximum=npx))])
+
+  def render(self, sprites=(), global_state=None):
+    from spriteworld_b200 import _direct
+    self._num_sprites = len(sprites)
+    return _direct.render_coverage(self, list(sprites))
+
+  def observation_spec(self):
+    """The spec of the last render's sprite count (as SpriteFactors')."""
+    return self._spec(self._num_sprites)
+
+  def render_batch(self, env, res):
+    """Batched form: dict 'cover' int32 (n_envs, H, W), 'visible' and 'area' int32 (n_envs,
+    n_slots) device tensors, buffers of `env` that every step (and env.render()) overwrites, as it
+    does the frames."""
+    return env.render_coverage(self)
+
+  def render_states(self, env, states):
+    """The coverage of env records (EnvStates) without loading them, in new tensors."""
+    return env.render_coverage(self, states)
+
+  def batch_observation_spec(self, env):
+    return self._spec(env.engine.n_slots)
 
 
 class GoalPositions(abstract_renderer.AbstractRenderer):

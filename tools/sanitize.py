@@ -18,8 +18,9 @@ Between those, env records: host-checked saves, loads and copies (disjoint and o
 run the device-checked calls' save and load kernels on int32 ids, and device-checked ones with int32
 and int64 device ids, valid and refused (out of range either way, 2^32 + 1, repeated destinations),
 so that memcheck sees that a refused id never indexes engine memory.  Then rollouts from records
-into leaves, from those leaves, and from the live envs into leaves, renders of records, and an
-engine checkpoint saved, loaded and rendered, with a corrupt one refused.
+into leaves, from those leaves, and from the live envs into leaves, renders of records, the sprite
+coverage (swb_render_coverage) of live envs and records into buffers that are not 16-byte aligned,
+and an engine checkpoint saved, loaded and rendered, with a corrupt one refused.
 """
 import ctypes
 import os
@@ -108,6 +109,20 @@ def device_checked_records(torch):
   torch.cuda.synchronize()
   print('record renders: %d frames, %d overflowed, %d kernel launches'
         % (len(frames), int(status.bool().sum()), eng.launch_count()), flush=True)
+  # coverage of the live envs and of the leaves: odd widths at 4-byte offsets that are not
+  # 16-byte aligned (the write-out's head and tail), bands of one and many rows, and zero records
+  S = eng.n_slots
+  for W, H, aa, skew in ((wl.image_size[0], wl.image_size[1], 1, 0), (13, 7, 5, 1), (1023, 3, 4, 3)):
+    for states in (None, res.leaves, res.leaves[:0]):
+      n = E if states is None else len(states)
+      flat = torch.zeros(n * (H * W + 2 * S) + 4, dtype=torch.int32, device='cuda')
+      cover = flat[skew:skew + n * H * W].view(n, H, W)
+      visible = flat[skew + n * H * W:skew + n * (H * W + S)].view(n, S)
+      area = flat[skew + n * (H * W + S):skew + n * (H * W + 2 * S)].view(n, S)
+      eng.render_coverage(W, H, aa, states=states, out=(cover, visible, area))
+  torch.cuda.synchronize()
+  print('coverage: live envs and %d leaves, %d kernel launches' % (len(res.leaves), eng.launch_count()),
+        flush=True)
   # an engine checkpoint round trip, and a corrupt one refused before anything is enqueued
   from spriteworld_b200 import _native
   state = eng.save_state()
