@@ -333,6 +333,15 @@ int swb_upload_state(swb_engine *eng, const double *pos_x, const double *pos_y,
  * empty slot.  Any other byte of a record that swb_save_envs of an engine of the same
  * configuration did not write -- and a span_class lower than its shapes need -- gives undefined
  * steps and frames.
+ *
+ * Read-only record calls (swb_rollout_states, swb_render_states, swb_render_masks,
+ * swb_render_coverage, swb_evaluate_states, swb_sample_contained) read n rows: n records of this
+ * engine's layout in a device record buffer of records_bytes bytes or, where a call takes them,
+ * the E live envs for records == NULL, and then n == E.  Each of them is refused, enqueuing
+ * nothing, for a null engine, n < 0, records == NULL where the call takes no live envs, a record
+ * buffer not 16-byte aligned or smaller than n records, an output that is null or not aligned to
+ * its element type, or an output that overlaps another output or the records it reads.  Each
+ * call's comment lists what it refuses besides.
  */
 int64_t swb_env_record_bytes(const swb_engine *eng);
 
@@ -369,11 +378,12 @@ int swb_load_envs(swb_engine *eng, const int32_t *env_ids, int32_t n, const void
  * sprite row, as swb_save_envs reports it; with record roots it is not written: the leaves need
  * the span class of their roots.
  *
- * The calls' checks run before anything is enqueued, and a refused call enqueues nothing: every
- * check of swb_rollout with n_roots in place of E (so n_steps * n_roots * n_candidates at most
- * SWB_ROLLOUT_MAX_ENTRIES), record buffers 16-byte aligned and large enough for n_roots and
- * n_roots * n_candidates records, and leaves that do not overlap the roots.  An accepted call is
- * one launch, leaves included.  Read-only but for `out` and `leaves`, as swb_rollout.
+ * A read-only record call (above) with the roots as its rows, and the leaves and every array of
+ * `out` as its outputs.  Refused besides: what swb_rollout refuses, with n_roots in place of E (so
+ * n_steps * n_roots * n_candidates at most SWB_ROLLOUT_MAX_ENTRIES), record roots with
+ * n_roots < 1, and leaves not 16-byte aligned or smaller than n_roots * n_candidates records.  An
+ * accepted call is one launch, leaves included.  Read-only but for `out` and `leaves`, as
+ * swb_rollout.
  *
  * Records are not validated beyond their shape ids: a shape id without a vertex table loads as an
  * empty slot.  Any other byte of a record that swb_save_envs of an engine of the same
@@ -394,11 +404,11 @@ int swb_rollout_states(swb_engine *eng, const void *roots, int32_t n_roots, uint
  *
  * Read-only: no env, pool entry, counter, render status or span class of the engine changes.
  * Records of stars or spokes rendered by an engine whose shapes are all convex get the concave
- * span tables for this call only.  A call is refused, enqueuing nothing, for a null engine or
- * raster, n < 0, a record buffer that is not 16-byte aligned or too small, a span_class other
- * than 1 or 4, null frames or status, frames or status that overlap the records, n * (the
- * raster's bands of 64 rows) above 2^31 - 1, or a render launch that would not fit (as
- * swb_render is refused).  Records are not validated beyond their shape ids, as in swb_load_envs.
+ * span tables for this call only.  A read-only record call (above) without live envs, whose
+ * outputs are frames and status; with n == 0 it checks nothing but the engine and raster.  Refused
+ * besides: a null raster, a span_class other than 1 or 4, n * (the raster's bands of 64 rows) above
+ * 2^31 - 1, or a render launch that would not fit (as swb_render is refused).  Records are not
+ * validated beyond their shape ids, as in swb_load_envs.
  */
 int swb_render_states(swb_engine *eng, swb_raster *r, const void *records, int32_t n,
                       uint64_t records_bytes, int32_t span_class, uint8_t *frames,
@@ -418,10 +428,10 @@ int swb_render_states(swb_engine *eng, swb_raster *r, const void *records, int32
  * no status.  Any anti_aliasing whose canvas sides stay within 4095 pixels is accepted.
  *
  * An accepted call with n > 0 is one launch on `stream`; n == 0 enqueues nothing.  Read-only: no
- * env, pool entry, counter, frame buffer, render status or span class changes.  Refused, enqueuing
- * nothing: a null engine or masks, width, height or anti_aliasing < 1, a canvas side above 4095,
- * n < 0, n != E for the live envs, records not 16-byte aligned or too small, masks that overlap the
- * records, or an n whose bands (of at most 128 mask rows) exceed 2^31 - 1 CTAs.
+ * env, pool entry, counter, frame buffer, render status or span class changes.  A read-only record
+ * call (above) whose output is masks.  Refused besides, width, height and canvas first: width,
+ * height or anti_aliasing < 1, a canvas side above 4095, or an n whose bands (of at most 128 mask
+ * rows) exceed 2^31 - 1 CTAs.
  */
 int swb_render_masks(swb_engine *eng, int32_t width, int32_t height, int32_t anti_aliasing,
                      const void *records, int32_t n, uint64_t records_bytes, uint8_t *masks,
@@ -439,10 +449,8 @@ int swb_render_masks(swb_engine *eng, int32_t width, int32_t height, int32_t ant
  * Records, sizes and n as swb_render_masks takes them (records == NULL: the E live envs, n == E).
  * An accepted call with n > 0 zeroes visible and area on `stream` and is then one launch there;
  * the counts are integer sums, exact and independent of scheduling.  n == 0 enqueues nothing.
- * Read-only as swb_render_masks.  Refused, enqueuing nothing: what swb_render_masks refuses (with
- * a null cover, visible or area in place of null masks), an output not 4-byte aligned, an output
- * that overlaps another output or the records, or an n whose bands (of at most 128 mask rows and
- * 16 KiB of coverage) exceed 2^31 - 1 CTAs.
+ * Read-only as swb_render_masks, with cover, visible and area as outputs.  Refused besides: what
+ * swb_render_masks refuses, with bands of at most 128 mask rows and 16 KiB of coverage.
  */
 int swb_render_coverage(swb_engine *eng, int32_t width, int32_t height, int32_t anti_aliasing,
                         const void *records, int32_t n, uint64_t records_bytes, int32_t *cover,
@@ -647,10 +655,9 @@ int swb_set_goals_dev(swb_engine *eng, const void *env_ids, int32_t id_dtype, in
  * The task tree's value on env records, as swb_eval_task gives it for a live env (no action cost):
  * reward[i], success[i] and status[i] of record i at its live positions, with the record's goals, or
  * with goals[i * G * 2 .. (i + 1) * G * 2) (device f64) in their place when `goals` is not NULL.
- * `records`: n records of this engine's layout, records_bytes bytes, 16-byte aligned.  One launch;
- * read-only: no env, pool entry, counter or record changes.  Refused, enqueuing nothing: null
- * engine or outputs, n < 0, a record buffer too small or unaligned, goals given with G = 0 or
- * unaligned, outputs that overlap the records.  n == 0 enqueues nothing.
+ * One launch; read-only: no env, pool entry, counter or record changes.  A read-only record call
+ * (above) without live envs, whose outputs are reward, success and status.  Refused besides: goals
+ * given with G = 0 or not 8-byte aligned.  n == 0 enqueues nothing.
  */
 int swb_evaluate_states(swb_engine *eng, const void *records, int32_t n, uint64_t records_bytes,
                         const double *goals, double *reward, uint8_t *success, uint8_t *status, void *stream);
@@ -678,9 +685,8 @@ int swb_evaluate_states(swb_engine *eng, const void *records, int32_t n, uint64_
  *
  * Each sample is a pure function of (seed, i, s, the row's state): nothing is kept between calls.
  * An accepted call with n > 0 is one launch on `stream`; n == 0 enqueues nothing.  Read-only: no
- * env, pool entry, counter or frame changes.  Refused, enqueuing nothing: a null engine or output,
- * n < 0, n_samples < 1, n * n_samples above 2^31 - 1, n != E for the live envs, records not
- * 16-byte aligned or too small.
+ * env, pool entry, counter or frame changes.  A read-only record call (above) whose outputs are
+ * position, slot and status.  Refused besides: n_samples < 1, n * n_samples above 2^31 - 1.
  */
 #define SWB_CONTAINED_MAX_TRIES 1000000          /* sprite.py _MAX_TRIES */
 #define SWB_CONTAINED_DOMAIN 0x535742434e544431ULL  /* second key word of the contained-position stream */

@@ -865,9 +865,6 @@ int swb_upload_state(swb_engine *eng, const double *pos_x, const double *pos_y, 
 
 }  // extern "C"
 
-// The argument checks every record call makes before it checks its ids: the engine, n, a load's
-// span class and, for n > 0, the id pointers and the record buffer of a save (dst) or a load (src):
-// set, 16-byte aligned and n records long.  `call` is SWB_IDS_CALL_*; `fn` names the entry point.
 // A record buffer `name` of fn that must hold n records: 16-byte aligned and large enough.
 static int check_record_buffer(const swb_engine *eng, const char *fn, const char *name, const void *rec,
                                uint64_t rec_bytes, int64_t n) {
@@ -879,6 +876,9 @@ static int check_record_buffer(const swb_engine *eng, const char *fn, const char
   return 0;
 }
 
+// The argument checks every save, load and copy makes before it checks its ids: the engine, n, a
+// load's span class and, for n > 0, the id pointers and the record buffer of a save (dst) or a load
+// (src): set, 16-byte aligned and n records long.  `call` is SWB_IDS_CALL_*; `fn` names the entry point.
 static int check_record_args(const swb_engine *eng, const char *fn, int call, int32_t n, const void *ids0,
                              const void *ids1, const void *rec, uint64_t rec_bytes, int32_t span_class) {
   if (!eng) return fail("%s: null engine", fn);
@@ -968,14 +968,21 @@ static int begin_id_call(swb_engine *eng, int call, const void *a, const void *b
 
 static unsigned grid_of(size_t threads) { return (unsigned)((threads + 255) / 256); }
 
+// The check kernels of device-checked ids `c`, enqueued before the kernels that use them: every id
+// in range and, with kDistinct (ids that are destinations), none repeated.  Host-checked ids need none.
+template <typename T, bool kDistinct>
+static void enqueue_id_checks(swb_engine *eng, const IdCall &c, cudaStream_t stream) {
+  if (c.host_checked) return;
+  check_ids_kernel<T><<<grid_of(c.n), 256, 0, stream>>>(c, eng->st.E);
+  if constexpr (kDistinct) repeat_ids_kernel<T><<<grid_of(c.n), 256, 0, stream>>>(c, eng->st.E);
+  eng->launches += kDistinct ? 2 : 1;
+}
+
 // The kernels of a save, load or copy of the ids `c`, checked on the host or, by the check kernels
 // enqueued first, on the device.
 template <typename T>
 static int enqueue_save(swb_engine *eng, const IdCall &c, void *dst, cudaStream_t stream) {
-  if (!c.host_checked) {
-    check_ids_kernel<T><<<grid_of(c.n), 256, 0, stream>>>(c, eng->st.E);
-    eng->launches++;
-  }
+  enqueue_id_checks<T, false>(eng, c, stream);
   save_envs_kernel<T><<<grid_of((size_t)c.n * eng->st.S), 256, 0, stream>>>(
       eng->st, c, static_cast<unsigned char *>(dst), RecordLayout(eng->st.S, eng->st.G).bytes());
   eng->launches++;
@@ -985,11 +992,7 @@ static int enqueue_save(swb_engine *eng, const IdCall &c, void *dst, cudaStream_
 
 template <typename T>
 static int enqueue_load(swb_engine *eng, const IdCall &c, const void *src, cudaStream_t stream) {
-  if (!c.host_checked) {
-    check_ids_kernel<T><<<grid_of(c.n), 256, 0, stream>>>(c, eng->st.E);
-    repeat_ids_kernel<T><<<grid_of(c.n), 256, 0, stream>>>(c, eng->st.E);
-    eng->launches += 2;
-  }
+  enqueue_id_checks<T, true>(eng, c, stream);
   load_envs_kernel<T><<<grid_of((size_t)c.n * eng->st.S), 256, 0, stream>>>(
       eng->st, c, static_cast<const unsigned char *>(src), RecordLayout(eng->st.S, eng->st.G).bytes());
   eng->launches++;
@@ -1022,6 +1025,155 @@ static int enqueue_copy(swb_engine *eng, const IdCall &c, bool disjoint, cudaStr
   return 0;
 }
 
+template <typename T>
+static int enqueue_set_goals(swb_engine *eng, const IdCall &c, const double *goals, cudaStream_t stream) {
+  enqueue_id_checks<T, true>(eng, c, stream);
+  set_goals_kernel<T><<<grid_of((size_t)c.n * 2 * eng->st.G), 256, 0, stream>>>(eng->st, c, goals);
+  eng->launches++;
+  CUDA_TRY(cudaGetLastError());
+  return 0;
+}
+
+// The ids of a save, load, copy or set_goals: host int32 arrays, or device arrays of `dtype`
+// (SWB_DTYPE_I32 or SWB_DTYPE_I64).  ids[1] holds the destinations of a copy and is null otherwise.
+struct EnvIds {
+  const void *ids[2];
+  bool host;
+  int32_t dtype;
+};
+
+static EnvIds host_ids(const int32_t *a, const int32_t *b = nullptr) { return EnvIds{{a, b}, true, SWB_DTYPE_I32}; }
+static EnvIds dev_ids(const void *a, const void *b, int32_t dtype) { return EnvIds{{a, b}, false, dtype}; }
+
+// Checks the n ids of `call` (SWB_IDS_CALL_*), then calls enqueue(c, T(), disjoint) with their
+// IdCall c and id type T.  Host ids: every id in [0, E) and the destinations distinct, checked before
+// anything is enqueued; then staged, with their slot released after `enqueue`; `disjoint` says that
+// no env is among both the sources and the destinations.  Device ids: check_dev_ids, then the next
+// device-checked call (begin_id_call), whose kernels check them; `disjoint` is false.
+template <typename Enqueue>
+static int run_ids(swb_engine *eng, const char *fn, int call, const EnvIds &ids, int32_t n,
+                   cudaStream_t stream, Enqueue enqueue) {
+  const int n_args = ids.ids[1] ? 2 : 1;
+  const int dst_arg = call == SWB_IDS_CALL_SAVE ? -1 : call == SWB_IDS_CALL_COPY ? 1 : 0;
+  IdCall c;
+  if (ids.host) {
+    const int32_t *src = static_cast<const int32_t *>(ids.ids[0]), *dst = static_cast<const int32_t *>(ids.ids[1]);
+    std::vector<uint8_t> mark(dst_arg >= 0 ? eng->st.E : 0, 0);
+    if (dst_arg >= 0 && check_env_ids(eng, fn, dst_arg ? dst : src, n, &mark)) return 1;
+    if (dst_arg != 0 && check_env_ids(eng, fn, src, n, nullptr)) return 1;  // argument 0 holds sources
+    bool disjoint = true;
+    for (int32_t i = 0; dst && i < n && disjoint; ++i) disjoint = !mark[src[i]];
+    CUDA_TRY(cudaSetDevice(eng->device));
+    StagingSlot *slot = nullptr;
+    if (stage_ids(eng, src, dst, n, dst_arg, stream, &c, &slot) || enqueue(c, int32_t(), disjoint)) return 1;
+    return release_slot(slot, stream);
+  }
+  for (int a = 0; a < n_args; ++a)
+    if (check_dev_ids(eng, fn, ids.ids[a], ids.dtype)) return 1;
+  CUDA_TRY(cudaSetDevice(eng->device));
+  if (begin_id_call(eng, call, ids.ids[0], ids.ids[1], dst_arg, n, stream, &c)) return 1;
+  return ids.dtype == SWB_DTYPE_I64 ? enqueue(c, int64_t(), false) : enqueue(c, int32_t(), false);
+}
+
+static int save_envs(swb_engine *eng, const char *fn, const EnvIds &ids, int32_t n, void *dst, uint64_t dst_bytes,
+                     int32_t *span_class, cudaStream_t stream) {
+  if (!eng || !span_class) return fail("%s: null argument", fn);
+  if (check_record_args(eng, fn, SWB_IDS_CALL_SAVE, n, ids.ids[0], nullptr, dst, dst_bytes, 0)) return 1;
+  *span_class = eng->max_spans;
+  if (n == 0) return 0;
+  return run_ids(eng, fn, SWB_IDS_CALL_SAVE, ids, n, stream, [&](const IdCall &c, auto id, bool) {
+    return enqueue_save<decltype(id)>(eng, c, dst, stream);
+  });
+}
+
+static int load_envs(swb_engine *eng, const char *fn, const EnvIds &ids, int32_t n, const void *src,
+                     uint64_t src_bytes, int32_t span_class, cudaStream_t stream) {
+  if (check_record_args(eng, fn, SWB_IDS_CALL_LOAD, n, ids.ids[0], nullptr, src, src_bytes, span_class)) return 1;
+  if (n == 0) return 0;
+  return run_ids(eng, fn, SWB_IDS_CALL_LOAD, ids, n, stream, [&](const IdCall &c, auto id, bool) {
+    // records of stars or spokes need the concave span tables, as if their scenes were uploaded
+    eng->max_spans = std::max(eng->max_spans, (int)span_class);
+    return enqueue_load<decltype(id)>(eng, c, src, stream);
+  });
+}
+
+static int copy_envs(swb_engine *eng, const char *fn, const EnvIds &ids, int32_t n, cudaStream_t stream) {
+  if (check_record_args(eng, fn, SWB_IDS_CALL_COPY, n, ids.ids[0], ids.ids[1], nullptr, 0, 0)) return 1;
+  if (n == 0) return 0;
+  return run_ids(eng, fn, SWB_IDS_CALL_COPY, ids, n, stream, [&](const IdCall &c, auto id, bool disjoint) {
+    return enqueue_copy<decltype(id)>(eng, c, disjoint, stream);
+  });
+}
+
+static int set_goals(swb_engine *eng, const char *fn, const EnvIds &ids, int32_t n, const double *goals,
+                     cudaStream_t stream) {
+  if (!eng) return fail("%s: null engine", fn);
+  if (!eng->st.G) return fail("%s: the task tree samples no goals (G = 0)", fn);
+  if (n < 0) return fail("%s: n = %d", fn, n);
+  if (n == 0) return 0;
+  if (!ids.ids[0] || !goals) return fail("%s: null argument", fn);
+  if (reinterpret_cast<uintptr_t>(goals) % 8) return fail("%s: goals are not 8-byte aligned", fn);
+  return run_ids(eng, fn, SWB_IDS_CALL_SET_GOALS, ids, n, stream, [&](const IdCall &c, auto id, bool) {
+    return enqueue_set_goals<decltype(id)>(eng, c, goals, stream);
+  });
+}
+
+// The rows a read-only record call reads: n >= 0 records in fn's record buffer `name`, or, where
+// the call takes them (live_ok), the E live envs for records == NULL, and then n == E.
+static int check_rows(const swb_engine *eng, const char *fn, const char *name, const void *records, int32_t n,
+                      uint64_t records_bytes, bool live_ok) {
+  if (!eng) return fail("%s: null engine", fn);
+  if (n < 0) return fail("%s: n = %d", fn, n);
+  if (records) return check_record_buffer(eng, fn, name, records, records_bytes, n);
+  if (!live_ok) return fail("%s: null %s", fn, name);
+  if (n != eng->st.E) return fail("%s: n = %d must be E = %d when the rows are the live envs", fn, n, eng->st.E);
+  return 0;
+}
+
+// `bytes` bytes at `ptr`, which hold elements aligned to `align` bytes.
+struct Span {
+  const char *name;
+  const void *ptr;
+  uint64_t bytes;
+  unsigned align;
+};
+
+static bool overlap(const Span &a, const Span &b) {
+  const uint64_t a0 = reinterpret_cast<uintptr_t>(a.ptr), b0 = reinterpret_cast<uintptr_t>(b.ptr);
+  return a0 < b0 + b.bytes && b0 < a0 + a.bytes;
+}
+
+// The outputs outs[0 .. n_outs) of a read-only record call: each set, aligned to its elements, and
+// disjoint from every other output and from the rows it reads (rows.ptr NULL: the live envs).  An
+// output that overlaps the rows would race with the kernel's reads of them.
+static int check_outputs(const char *fn, const Span *outs, int n_outs, const Span &rows) {
+  for (int i = 0; i < n_outs; ++i) {
+    const Span &o = outs[i];
+    if (!o.ptr) return fail("%s: null output %s", fn, o.name);
+    if (reinterpret_cast<uintptr_t>(o.ptr) % o.align) return fail("%s: %s is not %u-byte aligned", fn, o.name, o.align);
+    for (int j = 0; j < i; ++j)
+      if (overlap(o, outs[j])) return fail("%s: %s overlaps %s", fn, o.name, outs[j].name);
+    if (rows.ptr && overlap(o, rows)) return fail("%s: %s overlaps %s", fn, o.name, rows.name);
+  }
+  return 0;
+}
+
+// The checks swb_render_masks and swb_render_coverage make before their outputs': the image sizes
+// first, then the rows, then the grid of n rows of bands.
+static int check_mask_call(const swb_engine *eng, const char *fn, int32_t width, int32_t height,
+                           int32_t anti_aliasing, const void *records, int32_t n, uint64_t records_bytes, bool cover) {
+  if (width < 1 || height < 1 || anti_aliasing < 1)
+    return fail("%s: width %d, height %d and anti_aliasing %d must be >= 1", fn, width, height, anti_aliasing);
+  if ((int64_t)anti_aliasing * width > 4095 || (int64_t)anti_aliasing * height > 4095)
+    return fail("%s: canvas %lld x %lld exceeds 4095 pixels per side", fn, (long long)anti_aliasing * width,
+                (long long)anti_aliasing * height);
+  if (check_rows(eng, fn, "records", records, n, records_bytes, true)) return 1;
+  const MaskLayout L(eng->st.S, width, height, anti_aliasing, cover);
+  if ((int64_t)n * L.n_bands > INT32_MAX)
+    return fail("%s: n = %d rows of %d bands each exceed 2^31 - 1 CTAs", fn, n, L.n_bands);
+  return 0;
+}
+
 extern "C" {
 
 int64_t swb_env_record_bytes(const swb_engine *eng) {
@@ -1033,135 +1185,38 @@ int64_t swb_env_record_bytes(const swb_engine *eng) {
 }
 
 int swb_save_envs(swb_engine *eng, const int32_t *env_ids, int32_t n, void *dst, uint64_t dst_bytes,
-                  int32_t *span_class, void *stream_) {
-  if (!eng || !span_class) return fail("swb_save_envs: null argument");
-  if (check_record_args(eng, "swb_save_envs", SWB_IDS_CALL_SAVE, n, env_ids, nullptr, dst, dst_bytes, 0))
-    return 1;
-  *span_class = eng->max_spans;
-  if (n == 0) return 0;
-  if (check_env_ids(eng, "swb_save_envs", env_ids, n, nullptr)) return 1;
-  CUDA_TRY(cudaSetDevice(eng->device));
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  IdCall c;
-  StagingSlot *slot = nullptr;
-  if (stage_ids(eng, env_ids, nullptr, n, -1, stream, &c, &slot) || enqueue_save<int32_t>(eng, c, dst, stream))
-    return 1;
-  return release_slot(slot, stream);
+                  int32_t *span_class, void *stream) {
+  return save_envs(eng, "swb_save_envs", host_ids(env_ids), n, dst, dst_bytes, span_class,
+                   static_cast<cudaStream_t>(stream));
 }
 
 int swb_save_envs_dev(swb_engine *eng, const void *env_ids, int32_t id_dtype, int32_t n, void *dst,
-                      uint64_t dst_bytes, int32_t *span_class, void *stream_) {
-  if (!eng || !span_class) return fail("swb_save_envs_dev: null argument");
-  if (check_record_args(eng, "swb_save_envs_dev", SWB_IDS_CALL_SAVE, n, env_ids, nullptr, dst, dst_bytes, 0))
-    return 1;
-  *span_class = eng->max_spans;
-  if (n == 0) return 0;
-  if (check_dev_ids(eng, "swb_save_envs_dev", env_ids, id_dtype)) return 1;
-  CUDA_TRY(cudaSetDevice(eng->device));
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  IdCall c;
-  if (begin_id_call(eng, SWB_IDS_CALL_SAVE, env_ids, nullptr, -1, n, stream, &c)) return 1;
-  return id_dtype == SWB_DTYPE_I64 ? enqueue_save<int64_t>(eng, c, dst, stream)
-                                   : enqueue_save<int32_t>(eng, c, dst, stream);
+                      uint64_t dst_bytes, int32_t *span_class, void *stream) {
+  return save_envs(eng, "swb_save_envs_dev", dev_ids(env_ids, nullptr, id_dtype), n, dst, dst_bytes, span_class,
+                   static_cast<cudaStream_t>(stream));
 }
 
 int swb_load_envs(swb_engine *eng, const int32_t *env_ids, int32_t n, const void *src, uint64_t src_bytes,
-                  int32_t span_class, void *stream_) {
-  if (check_record_args(eng, "swb_load_envs", SWB_IDS_CALL_LOAD, n, env_ids, nullptr, src, src_bytes,
-                        span_class))
-    return 1;
-  if (n == 0) return 0;
-  std::vector<uint8_t> mark(eng->st.E, 0);
-  if (check_env_ids(eng, "swb_load_envs", env_ids, n, &mark)) return 1;
-  CUDA_TRY(cudaSetDevice(eng->device));
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  // records of stars or spokes need the concave span tables, as if their scenes were uploaded
-  eng->max_spans = std::max(eng->max_spans, (int)span_class);
-  IdCall c;
-  StagingSlot *slot = nullptr;
-  if (stage_ids(eng, env_ids, nullptr, n, 0, stream, &c, &slot) || enqueue_load<int32_t>(eng, c, src, stream))
-    return 1;
-  return release_slot(slot, stream);
+                  int32_t span_class, void *stream) {
+  return load_envs(eng, "swb_load_envs", host_ids(env_ids), n, src, src_bytes, span_class,
+                   static_cast<cudaStream_t>(stream));
 }
 
 int swb_load_envs_dev(swb_engine *eng, const void *env_ids, int32_t id_dtype, int32_t n, const void *src,
-                      uint64_t src_bytes, int32_t span_class, void *stream_) {
-  if (check_record_args(eng, "swb_load_envs_dev", SWB_IDS_CALL_LOAD, n, env_ids, nullptr, src, src_bytes,
-                        span_class))
-    return 1;
-  if (n == 0) return 0;
-  if (check_dev_ids(eng, "swb_load_envs_dev", env_ids, id_dtype)) return 1;
-  CUDA_TRY(cudaSetDevice(eng->device));
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  eng->max_spans = std::max(eng->max_spans, (int)span_class);
-  IdCall c;
-  if (begin_id_call(eng, SWB_IDS_CALL_LOAD, env_ids, nullptr, 0, n, stream, &c)) return 1;
-  return id_dtype == SWB_DTYPE_I64 ? enqueue_load<int64_t>(eng, c, src, stream)
-                                   : enqueue_load<int32_t>(eng, c, src, stream);
+                      uint64_t src_bytes, int32_t span_class, void *stream) {
+  return load_envs(eng, "swb_load_envs_dev", dev_ids(env_ids, nullptr, id_dtype), n, src, src_bytes, span_class,
+                   static_cast<cudaStream_t>(stream));
 }
 
-int swb_copy_envs(swb_engine *eng, const int32_t *src_ids, const int32_t *dst_ids, int32_t n, void *stream_) {
-  if (check_record_args(eng, "swb_copy_envs", SWB_IDS_CALL_COPY, n, src_ids, dst_ids, nullptr, 0, 0)) return 1;
-  if (n == 0) return 0;
-  std::vector<uint8_t> mark(eng->st.E, 0);
-  if (check_env_ids(eng, "swb_copy_envs", dst_ids, n, &mark) ||
-      check_env_ids(eng, "swb_copy_envs", src_ids, n, nullptr))
-    return 1;
-  bool disjoint = true;
-  for (int32_t i = 0; i < n && disjoint; ++i) disjoint = !mark[src_ids[i]];
-  CUDA_TRY(cudaSetDevice(eng->device));
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  IdCall c;
-  StagingSlot *slot = nullptr;
-  if (stage_ids(eng, src_ids, dst_ids, n, 1, stream, &c, &slot) ||
-      enqueue_copy<int32_t>(eng, c, disjoint, stream))
-    return 1;
-  return release_slot(slot, stream);
+int swb_copy_envs(swb_engine *eng, const int32_t *src_ids, const int32_t *dst_ids, int32_t n, void *stream) {
+  return copy_envs(eng, "swb_copy_envs", host_ids(src_ids, dst_ids), n, static_cast<cudaStream_t>(stream));
 }
 
 int swb_copy_envs_dev(swb_engine *eng, const void *src_ids, const void *dst_ids, int32_t id_dtype, int32_t n,
-                      void *stream_) {
-  if (check_record_args(eng, "swb_copy_envs_dev", SWB_IDS_CALL_COPY, n, src_ids, dst_ids, nullptr, 0, 0))
-    return 1;
-  if (n == 0) return 0;
-  if (check_dev_ids(eng, "swb_copy_envs_dev", src_ids, id_dtype) ||
-      check_dev_ids(eng, "swb_copy_envs_dev", dst_ids, id_dtype))
-    return 1;
-  CUDA_TRY(cudaSetDevice(eng->device));
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  IdCall c;
-  if (begin_id_call(eng, SWB_IDS_CALL_COPY, src_ids, dst_ids, 1, n, stream, &c)) return 1;
-  return id_dtype == SWB_DTYPE_I64 ? enqueue_copy<int64_t>(eng, c, false, stream)
-                                   : enqueue_copy<int32_t>(eng, c, false, stream);
+                      void *stream) {
+  return copy_envs(eng, "swb_copy_envs_dev", dev_ids(src_ids, dst_ids, id_dtype), n,
+                   static_cast<cudaStream_t>(stream));
 }
-
-}  // extern "C"
-
-// The checks of swb_set_goals / _dev before the ids: the engine has goal slots, n, the goals pointer.
-static int check_set_goals(const swb_engine *eng, const char *fn, int32_t n, const void *ids, const double *goals) {
-  if (!eng) return fail("%s: null engine", fn);
-  if (!eng->st.G) return fail("%s: the task tree samples no goals (G = 0)", fn);
-  if (n < 0) return fail("%s: n = %d", fn, n);
-  if (n == 0) return 0;
-  if (!ids || !goals) return fail("%s: null argument", fn);
-  if (reinterpret_cast<uintptr_t>(goals) % 8) return fail("%s: goals are not 8-byte aligned", fn);
-  return 0;
-}
-
-template <typename T>
-static int enqueue_set_goals(swb_engine *eng, const IdCall &c, const double *goals, cudaStream_t stream) {
-  if (!c.host_checked) {
-    check_ids_kernel<T><<<grid_of(c.n), 256, 0, stream>>>(c, eng->st.E);
-    repeat_ids_kernel<T><<<grid_of(c.n), 256, 0, stream>>>(c, eng->st.E);
-    eng->launches += 2;
-  }
-  set_goals_kernel<T><<<grid_of((size_t)c.n * 2 * eng->st.G), 256, 0, stream>>>(eng->st, c, goals);
-  eng->launches++;
-  CUDA_TRY(cudaGetLastError());
-  return 0;
-}
-
-extern "C" {
 
 int swb_pool_goal_pointer(swb_engine *eng, double **goal, int32_t *n_goals) {
   if (!eng || !goal || !n_goals) return fail("swb_pool_goal_pointer: null argument");
@@ -1170,53 +1225,27 @@ int swb_pool_goal_pointer(swb_engine *eng, double **goal, int32_t *n_goals) {
   return 0;
 }
 
-int swb_set_goals(swb_engine *eng, const int32_t *env_ids, int32_t n, const double *goals, void *stream_) {
-  static const char fn[] = "swb_set_goals";
-  if (check_set_goals(eng, fn, n, env_ids, goals)) return 1;
-  if (n == 0) return 0;
-  std::vector<uint8_t> mark(eng->st.E, 0);
-  if (check_env_ids(eng, fn, env_ids, n, &mark)) return 1;
-  CUDA_TRY(cudaSetDevice(eng->device));
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  IdCall c;
-  StagingSlot *slot = nullptr;
-  if (stage_ids(eng, env_ids, nullptr, n, 0, stream, &c, &slot) || enqueue_set_goals<int32_t>(eng, c, goals, stream))
-    return 1;
-  return release_slot(slot, stream);
+int swb_set_goals(swb_engine *eng, const int32_t *env_ids, int32_t n, const double *goals, void *stream) {
+  return set_goals(eng, "swb_set_goals", host_ids(env_ids), n, goals, static_cast<cudaStream_t>(stream));
 }
 
 int swb_set_goals_dev(swb_engine *eng, const void *env_ids, int32_t id_dtype, int32_t n, const double *goals,
-                      void *stream_) {
-  static const char fn[] = "swb_set_goals_dev";
-  if (check_set_goals(eng, fn, n, env_ids, goals)) return 1;
-  if (n == 0) return 0;
-  if (check_dev_ids(eng, fn, env_ids, id_dtype)) return 1;
-  CUDA_TRY(cudaSetDevice(eng->device));
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  IdCall c;
-  if (begin_id_call(eng, SWB_IDS_CALL_SET_GOALS, env_ids, nullptr, 0, n, stream, &c)) return 1;
-  return id_dtype == SWB_DTYPE_I64 ? enqueue_set_goals<int64_t>(eng, c, goals, stream)
-                                   : enqueue_set_goals<int32_t>(eng, c, goals, stream);
+                      void *stream) {
+  return set_goals(eng, "swb_set_goals_dev", dev_ids(env_ids, nullptr, id_dtype), n, goals,
+                   static_cast<cudaStream_t>(stream));
 }
 
 int swb_evaluate_states(swb_engine *eng, const void *records, int32_t n, uint64_t records_bytes,
                         const double *goals, double *reward, uint8_t *success, uint8_t *status, void *stream_) {
   static const char fn[] = "swb_evaluate_states";
-  if (!eng) return fail("%s: null engine", fn);
-  if (n < 0) return fail("%s: n = %d", fn, n);
+  if (check_rows(eng, fn, "records", records, n, records_bytes, false)) return 1;
   if (goals && !eng->st.G) return fail("%s: goals given, but the task tree samples no goals (G = 0)", fn);
   if (n == 0) return 0;
-  if (!records || !reward || !success || !status) return fail("%s: null argument", fn);
-  if (check_record_buffer(eng, fn, "records", records, records_bytes, n)) return 1;
-  if (goals && reinterpret_cast<uintptr_t>(goals) % 8) return fail("%s: goals are not 8-byte aligned", fn);
+  if (reinterpret_cast<uintptr_t>(goals) % 8) return fail("%s: goals are not 8-byte aligned", fn);
   const uint64_t rb = RecordLayout(eng->st.S, eng->st.G).bytes();
-  const uint64_t r0 = reinterpret_cast<uintptr_t>(records), r1 = r0 + (uint64_t)n * rb;
-  const struct { const void *p; uint64_t bytes; } outs[3] = {{reward, 8 * (uint64_t)n}, {success, (uint64_t)n},
-                                                             {status, (uint64_t)n}};
-  for (const auto &o : outs) {
-    const uint64_t o0 = reinterpret_cast<uintptr_t>(o.p);
-    if (o0 < r1 && r0 < o0 + o.bytes) return fail("%s: an output overlaps the records", fn);
-  }
+  const Span outs[] = {{"reward", reward, 8 * (uint64_t)n, 8}, {"success", success, (uint64_t)n, 1},
+                       {"status", status, (uint64_t)n, 1}};
+  if (check_outputs(fn, outs, 3, Span{"the records", records, n * rb, 16})) return 1;
   CUDA_TRY(cudaSetDevice(eng->device));
   const unsigned blocks = (unsigned)(((int64_t)n + ROLLOUT_WARPS - 1) / ROLLOUT_WARPS);
   evaluate_kernel<<<blocks, ROLLOUT_WARPS * 32, 0, static_cast<cudaStream_t>(stream_)>>>(
@@ -1238,17 +1267,16 @@ int swb_rollout_states(swb_engine *eng, const void *roots, int32_t n_roots, uint
                  : fail("%s: n_roots = %d must be E = %d when the roots are the live envs", fn, n_roots,
                         eng->st.E);
   if (check_rollout(eng, fn, roots ? "roots" : "envs", actions, action_dtype, n_steps, n_candidates, n_roots,
-                    out))
+                    out) ||
+      check_rows(eng, fn, "roots", roots, n_roots, roots_bytes, true))
     return 1;
   const uint64_t rb = RecordLayout(eng->st.S, eng->st.G).bytes();
-  const uint64_t plans = (uint64_t)n_roots * n_candidates;
-  if (roots && check_record_buffer(eng, fn, "roots", roots, roots_bytes, n_roots)) return 1;
+  const uint64_t plans = (uint64_t)n_roots * n_candidates, entries = plans * n_steps;
   if (leaves && check_record_buffer(eng, fn, "leaves", leaves, leaves_bytes, (int64_t)plans)) return 1;
-  if (roots && leaves) {
-    const uintptr_t r0 = reinterpret_cast<uintptr_t>(roots), l0 = reinterpret_cast<uintptr_t>(leaves);
-    if (r0 < l0 + plans * rb && l0 < r0 + (uint64_t)n_roots * rb)
-      return fail("%s: the leaves overlap the roots", fn);
-  }
+  const Span outs[] = {{"reward", out->reward, 8 * entries, 8}, {"step_type", out->step_type, entries, 1},
+                       {"success", out->success, entries, 1}, {"status", out->status, entries, 1},
+                       {"leaves", leaves, plans * rb, 16}};
+  if (check_outputs(fn, outs, leaves ? 5 : 4, Span{"the roots", roots, n_roots * rb, 16})) return 1;
   if (!roots && span_class) *span_class = eng->max_spans;
   return enqueue_rollout(eng, actions, action_dtype, n_steps, n_candidates, *out,
                          RolloutRecords{static_cast<const unsigned char *>(roots),
@@ -1260,21 +1288,16 @@ int swb_render_states(swb_engine *eng, swb_raster *r, const void *records, int32
                       int32_t span_class, uint8_t *frames, uint8_t *status, void *stream_) {
   static const char fn[] = "swb_render_states";
   if (!eng || !r) return fail("%s: null engine or raster", fn);
-  if (n < 0) return fail("%s: n = %d", fn, n);
-  if (n == 0) return 0;
-  if (!records) return fail("%s: null records", fn);
-  if (check_record_buffer(eng, fn, "records", records, records_bytes, n)) return 1;
+  if (n == 0) return 0;  // nothing is read or drawn: the buffers may be null
+  if (check_rows(eng, fn, "records", records, n, records_bytes, false)) return 1;
   if (span_class != 1 && span_class != 4) return fail("%s: span_class must be 1 or 4, got %d", fn, span_class);
-  if (!frames || !status) return fail("%s: null frames or status", fn);
   const RasterDev &rd = r->rd;
-  const uint64_t rb = RecordLayout(eng->st.S, eng->st.G).bytes();
-  const uint64_t r0 = reinterpret_cast<uintptr_t>(records), r1 = r0 + (uint64_t)n * rb;
-  const uint64_t f0 = reinterpret_cast<uintptr_t>(frames), s0 = reinterpret_cast<uintptr_t>(status);
-  if (f0 < r1 && r0 < f0 + (uint64_t)n * rd.H * rd.W * 3) return fail("%s: the frames overlap the records", fn);
-  if (s0 < r1 && r0 < s0 + (uint64_t)n) return fail("%s: the status overlaps the records", fn);
   // n_items and the kernel's item index are int
   if ((int64_t)n * rd.n_bands > INT32_MAX)
     return fail("%s: n = %d records of %d bands each exceed 2^31 - 1 render items", fn, n, rd.n_bands);
+  const uint64_t rb = RecordLayout(eng->st.S, eng->st.G).bytes();
+  const Span outs[] = {{"frames", frames, (uint64_t)n * rd.H * rd.W * 3, 1}, {"status", status, (uint64_t)n, 1}};
+  if (check_outputs(fn, outs, 2, Span{"the records", records, n * rb, 16})) return 1;
   // read-only: records of stars or spokes get the concave span tables for this launch only
   std::optional<RenderLayout> plan;
   if (check_render(eng, r, std::max(eng->max_spans, (int)span_class), &plan)) return 1;
@@ -1285,43 +1308,15 @@ int swb_render_states(swb_engine *eng, swb_raster *r, const void *records, int32
                         RenderRecords{static_cast<const unsigned char *>(records), (size_t)rb});
 }
 
-// The checks swb_render_masks and swb_render_coverage share, in this order (`out`: the first
-// output, null-checked with the engine; `outs` names the outputs in messages).
-static int check_mask_call(const swb_engine *eng, const char *fn, const char *outs, const void *out,
-                           int32_t width, int32_t height, int32_t anti_aliasing, const void *records,
-                           int32_t n, uint64_t records_bytes, bool cover) {
-  if (width < 1 || height < 1 || anti_aliasing < 1)
-    return fail("%s: width %d, height %d and anti_aliasing %d must be >= 1", fn, width, height, anti_aliasing);
-  if (!eng || !out) return fail("%s: null engine or %s", fn, outs);
-  if ((int64_t)anti_aliasing * width > 4095 || (int64_t)anti_aliasing * height > 4095)
-    return fail("%s: canvas %lld x %lld exceeds 4095 pixels per side", fn, (long long)anti_aliasing * width,
-                (long long)anti_aliasing * height);
-  if (n < 0) return fail("%s: n = %d", fn, n);
-  if (!records && n != eng->st.E)
-    return fail("%s: n = %d must be E = %d when the %s are the live envs'", fn, n, eng->st.E, outs);
-  const MaskLayout L(eng->st.S, width, height, anti_aliasing, cover);
-  if ((int64_t)n * L.n_bands > INT32_MAX)
-    return fail("%s: n = %d %s of %d bands each exceed 2^31 - 1 CTAs", fn, n, outs, L.n_bands);
-  if (records && check_record_buffer(eng, fn, "records", records, records_bytes, n)) return 1;
-  return 0;
-}
-
-// [a, a + na) and [b, b + nb) share a byte
-static bool overlap(const void *a, uint64_t na, const void *b, uint64_t nb) {
-  const uint64_t a0 = reinterpret_cast<uintptr_t>(a), b0 = reinterpret_cast<uintptr_t>(b);
-  return a0 < b0 + nb && b0 < a0 + na;
-}
-
 int swb_render_masks(swb_engine *eng, int32_t width, int32_t height, int32_t anti_aliasing,
                      const void *records, int32_t n, uint64_t records_bytes, uint8_t *masks, void *stream_) {
   static const char fn[] = "swb_render_masks";
-  if (check_mask_call(eng, fn, "masks", masks, width, height, anti_aliasing, records, n, records_bytes, false))
-    return 1;
-  const MaskLayout L(eng->st.S, width, height, anti_aliasing);
+  if (check_mask_call(eng, fn, width, height, anti_aliasing, records, n, records_bytes, false)) return 1;
   const uint64_t rb = RecordLayout(eng->st.S, eng->st.G).bytes();
-  if (records && overlap(masks, (uint64_t)n * height * width, records, (uint64_t)n * rb))
-    return fail("%s: the masks overlap the records", fn);
+  const Span outs[] = {{"masks", masks, (uint64_t)n * height * width, 1}};
+  if (check_outputs(fn, outs, 1, Span{"the records", records, n * rb, 16})) return 1;
   if (n == 0) return 0;
+  const MaskLayout L(eng->st.S, width, height, anti_aliasing);
   CUDA_TRY(cudaSetDevice(eng->device));
   auto kernel = records ? mask_kernel<true, false> : mask_kernel<false, false>;
   CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, L.total));
@@ -1336,22 +1331,12 @@ int swb_render_coverage(swb_engine *eng, int32_t width, int32_t height, int32_t 
                         const void *records, int32_t n, uint64_t records_bytes, int32_t *cover,
                         int32_t *visible, int32_t *area, void *stream_) {
   static const char fn[] = "swb_render_coverage";
-  if (check_mask_call(eng, fn, "outputs", cover, width, height, anti_aliasing, records, n, records_bytes, true))
-    return 1;
-  if (!visible || !area) return fail("%s: null engine or outputs", fn);
-  const struct { const void *p; uint64_t bytes; const char *name; } outs[3] = {
-      {cover, (uint64_t)n * height * width * 4, "cover"},
-      {visible, (uint64_t)n * eng->st.S * 4, "visible"},
-      {area, (uint64_t)n * eng->st.S * 4, "area"}};
+  if (check_mask_call(eng, fn, width, height, anti_aliasing, records, n, records_bytes, true)) return 1;
   const uint64_t rb = RecordLayout(eng->st.S, eng->st.G).bytes();
-  for (int i = 0; i < 3; ++i) {
-    if (reinterpret_cast<uintptr_t>(outs[i].p) % 4) return fail("%s: %s is not 4-byte aligned", fn, outs[i].name);
-    for (int j = 0; j < i; ++j)
-      if (overlap(outs[i].p, outs[i].bytes, outs[j].p, outs[j].bytes))
-        return fail("%s: %s overlaps %s", fn, outs[i].name, outs[j].name);
-    if (records && overlap(outs[i].p, outs[i].bytes, records, (uint64_t)n * rb))
-      return fail("%s: %s overlaps the records", fn, outs[i].name);
-  }
+  const Span outs[] = {{"cover", cover, (uint64_t)n * height * width * 4, 4},
+                       {"visible", visible, (uint64_t)n * eng->st.S * 4, 4},
+                       {"area", area, (uint64_t)n * eng->st.S * 4, 4}};
+  if (check_outputs(fn, outs, 3, Span{"the records", records, n * rb, 16})) return 1;
   if (n == 0) return 0;
   const MaskLayout L(eng->st.S, width, height, anti_aliasing, true);
   CUDA_TRY(cudaSetDevice(eng->device));
@@ -1372,20 +1357,17 @@ int swb_sample_contained(swb_engine *eng, const void *records, int32_t n, uint64
                          int32_t n_samples, uint64_t seed, double *position, int8_t *slot, uint8_t *status,
                          void *stream_) {
   static const char fn[] = "swb_sample_contained";
-  if (!eng) return fail("%s: null engine", fn);
-  if (n < 0) return fail("%s: n = %d", fn, n);
+  if (check_rows(eng, fn, "records", records, n, records_bytes, true)) return 1;
   if (n_samples < 1) return fail("%s: n_samples = %d must be >= 1", fn, n_samples);
-  if (!records && n != eng->st.E)
-    return fail("%s: n = %d must be E = %d when the rows are the live envs", fn, n, eng->st.E);
   // the kernel's thread index and the output arrays' entries are one per (row, sample)
   if ((int64_t)n * n_samples > INT32_MAX)
     return fail("%s: n = %d rows of %d samples exceed 2^31 - 1 samples", fn, n, n_samples);
   if (n == 0) return 0;
-  if (!position || !slot || !status) return fail("%s: null output", fn);
-  const uint64_t rb = RecordLayout(eng->st.S, eng->st.G).bytes();
-  if (records && check_record_buffer(eng, fn, "records", records, records_bytes, n)) return 1;
+  const uint64_t rb = RecordLayout(eng->st.S, eng->st.G).bytes(), total = (uint64_t)n * n_samples;
+  const Span outs[] = {{"position", position, 16 * total, 8}, {"slot", slot, total, 1},
+                       {"status", status, total, 1}};
+  if (check_outputs(fn, outs, 3, Span{"the records", records, n * rb, 16})) return 1;
   CUDA_TRY(cudaSetDevice(eng->device));
-  const int64_t total = (int64_t)n * n_samples;
   auto kernel = records ? contained_kernel<true> : contained_kernel<false>;
   kernel<<<(unsigned)((total + CT_THREADS - 1) / CT_THREADS), CT_THREADS, 0, static_cast<cudaStream_t>(stream_)>>>(
       eng->st, static_cast<const unsigned char *>(records), (size_t)rb, n, n_samples, seed, position, slot,

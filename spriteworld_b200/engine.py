@@ -104,11 +104,38 @@ def rollout_outputs(out, n_steps, n_envs, n_candidates, device):
   n = shape[0] * shape[1] * shape[2]
   if out is None:
     out = torch.empty(n * OUT_BYTES_PER_ENV, dtype=torch.uint8, device=device)
-  elif (not isinstance(out, torch.Tensor) or out.dtype != torch.uint8 or out.device != device or
-        tuple(out.shape) != (n * OUT_BYTES_PER_ENV,) or not out.is_contiguous() or out.data_ptr() % 8):
-    raise ValueError('out must be a contiguous, 8-byte aligned uint8 tensor of %d bytes on %s, got %s'
-                     % (n * OUT_BYTES_PER_ENV, device, _describe(out)))
+  _check_output(out, 'out', torch.uint8, (n * OUT_BYTES_PER_ENV,), device, align=8)
   return out, RolloutResult(*[v.view(shape) for v in split_outputs(out, n)])
+
+
+def _check_output(t, name, dtype, shape, device, align=1):
+  """ValueError naming `name` unless `t` is a contiguous tensor of `dtype` and `shape` on `device`,
+  `align`-byte aligned: a kernel writes the whole shape from t.data_ptr(), so anything else would be
+  written out of bounds or scrambled."""
+  shape = tuple(shape)
+  if (not isinstance(t, torch.Tensor) or t.dtype != dtype or t.device != device or tuple(t.shape) != shape
+      or not t.is_contiguous() or t.data_ptr() % align):
+    raise ValueError('%s must be a contiguous%s %s tensor of shape %s on %s, got %s' % (
+        name, ', %d-byte aligned' % align if align > 1 else '', str(dtype).replace('torch.', ''), shape,
+        device, _describe(t)))
+
+
+def _address(t):
+  """ctypes pointer to tensor t's data.  An empty tensor may have no address, and the C-ABI refuses a
+  null buffer even where it reads and writes nothing; any aligned address stands in for it then."""
+  return ctypes.c_void_p(t.data_ptr() or 256)
+
+
+def _rows(engine, states, live=True):
+  """(n, records pointer or None, bytes) of a call on `states`: EnvStates of n records `engine` can
+  read, or where the call takes the live envs (`live`) None for its n_envs envs.  ValueError
+  otherwise."""
+  if states is None and live:
+    return engine.n_envs, None, 0
+  if not isinstance(states, EnvStates):
+    raise ValueError('states must be EnvStates, got %s' % type(states).__name__)
+  engine.check_states(states, len(states))
+  return len(states), _address(states.data), states.data.numel()
 
 
 def host_actions(kind, actions):
@@ -318,15 +345,8 @@ class Engine(object):
 
   # -- stepping ---------------------------------------------------------------------
   def _check_frames(self, frames, raster, n_frames):
-    """The render kernel writes n_frames * H * W * 3 bytes from frames.data_ptr(): anything but
-    a contiguous uint8 tensor of exactly that shape on this device would be written out of
-    bounds or scrambled."""
-    shape = (n_frames, raster.height, raster.width, 3)
-    if (not isinstance(frames, torch.Tensor) or frames.dtype != torch.uint8 or
-        frames.device != self.device or tuple(frames.shape) != shape or
-        not frames.is_contiguous()):
-      raise ValueError('frames must be a contiguous uint8 tensor of shape %s on %s, got %s' % (
-          shape, self.device, _describe(frames)))
+    """ValueError unless `frames` holds n_frames frames of `raster` as the render kernel writes them."""
+    _check_output(frames, 'frames', torch.uint8, (n_frames, raster.height, raster.width, 3), self.device)
 
   def step(self, actions, raster=None, frames=None):
     """One Environment.step for every env.  `actions`: device tensor."""
@@ -355,13 +375,9 @@ class Engine(object):
     records to fill in place; record r * C + c is what save_envs would return after loading root r
     and stepping plan c's live steps.  Leaves carry the roots' span class.  Still one launch
     (swb_rollout_states)."""
-    if states is not None and not isinstance(states, EnvStates):
-      raise ValueError('states must be EnvStates, got %s' % type(states).__name__)
-    n = self.n_envs if states is None else len(states)
+    n, roots, roots_bytes = _rows(self, states)
     dt = action_dtype(self.action_kind, n, actions, self.device, plans=True)
     T, _, C, _ = actions.shape
-    if states is not None:
-      self.check_states(states, n)
     if leaves is True:
       leaves = EnvStates(torch.empty((n * C, self.record_bytes), dtype=torch.uint8, device=self.device),
                          1, self.signature, self.n_slots, self.n_goals)
@@ -375,10 +391,9 @@ class Engine(object):
                                           ctypes.byref(ptrs), self._stream()))
       return res
     span = ctypes.c_int32(1 if states is None else states.span_class)
-    roots = (None, 0) if states is None else (ctypes.c_void_p(states.data.data_ptr()), states.data.numel())
     dst = (None, 0) if leaves is None else (ctypes.c_void_p(leaves.data.data_ptr()), leaves.data.numel())
     _native.check(self._lib.swb_rollout_states(
-        self._h, roots[0], n, roots[1], ctypes.c_void_p(actions.data_ptr()), dt, T, C, ctypes.byref(ptrs),
+        self._h, roots, n, roots_bytes, ctypes.c_void_p(actions.data_ptr()), dt, T, C, ctypes.byref(ptrs),
         dst[0], dst[1], ctypes.byref(span), self._stream()))
     if leaves is not None:
       leaves.span_class = span.value
@@ -412,22 +427,15 @@ class Engine(object):
     (ENV_SPAN_OVERFLOW).  `states`: EnvStates of any n records of this engine's configuration.
     Returns (frames (n, H, W, 3) uint8, status (n,) uint8) on this device, new unless given.  One
     launch on the current stream; no env, frame buffer, render_status() or span class changes."""
-    if not isinstance(states, EnvStates):
-      raise ValueError('states must be EnvStates, got %s' % type(states).__name__)
-    n = len(states)
-    self.check_states(states, n)
+    n, rec, rec_bytes = _rows(self, states, live=False)
     if frames is None:
       frames = torch.empty((n, raster.height, raster.width, 3), dtype=torch.uint8, device=self.device)
     self._check_frames(frames, raster, n)
     if status is None:
       status = torch.empty(n, dtype=torch.uint8, device=self.device)
-    if (not isinstance(status, torch.Tensor) or status.dtype != torch.uint8 or status.device != self.device
-        or tuple(status.shape) != (n,) or not status.is_contiguous()):
-      raise ValueError('status must be a contiguous uint8 tensor of shape (%d,) on %s, got %s' % (
-          n, self.device, _describe(status)))
+    _check_output(status, 'status', torch.uint8, (n,), self.device)
     _native.check(self._lib.swb_render_states(
-        self._h, raster._h, ctypes.c_void_p(states.data.data_ptr()), n, states.data.numel(),
-        states.span_class, ctypes.c_void_p(frames.data_ptr()), ctypes.c_void_p(status.data_ptr()),
+        self._h, raster._h, rec, n, rec_bytes, states.span_class, _address(frames), _address(status),
         self._stream()))
     return frames, status
 
@@ -438,31 +446,14 @@ class Engine(object):
     n_envs), or with `states` of EnvStates of any n records, as if loaded.  Into `out` if given
     (a contiguous uint8 tensor of that shape on this device), else a new tensor.  One launch on the
     current stream; nothing else changes."""
-    if states is not None and not isinstance(states, EnvStates):
-      raise ValueError('states must be EnvStates, got %s' % type(states).__name__)
-    n = self.n_envs if states is None else len(states)
-    if states is not None:
-      self.check_states(states, n)
+    n, rec, rec_bytes = _rows(self, states)
     W, H, aa = int(width), int(height), int(anti_aliasing)
-    shape = (n, H, W)
     if out is None:
       out = torch.empty((n, max(H, 0), max(W, 0)), dtype=torch.uint8, device=self.device)
-    elif (not isinstance(out, torch.Tensor) or out.dtype != torch.uint8 or out.device != self.device or
-          tuple(out.shape) != shape or not out.is_contiguous()):
-      raise ValueError('masks must be a contiguous uint8 tensor of shape %s on %s, got %s' % (
-          shape, self.device, _describe(out)))
-    masks_ptr = out.data_ptr()
-    rec = (None, 0) if states is None else (states.data.data_ptr(), states.data.numel())
-    if n == 0:
-      # zero records: the call checks its arguments and draws nothing, but an empty tensor may have no
-      # address; any aligned address stands in for the empty buffers (nothing is read or written)
-      probe = torch.empty(16, dtype=torch.uint8, device=self.device)
-      masks_ptr = masks_ptr or probe.data_ptr()
-      if rec[0] is not None:
-        rec = (rec[0] or probe.data_ptr(), rec[1])
-    _native.check(self._lib.swb_render_masks(
-        self._h, W, H, aa, None if rec[0] is None else ctypes.c_void_p(rec[0]), n, rec[1],
-        ctypes.c_void_p(masks_ptr), self._stream()))
+    else:
+      _check_output(out, 'masks', torch.uint8, (n, H, W), self.device)
+    _native.check(self._lib.swb_render_masks(self._h, W, H, aa, rec, n, rec_bytes, _address(out),
+                                             self._stream()))
     return out
 
   def render_coverage(self, width, height, anti_aliasing=1, states=None, out=None):
@@ -474,11 +465,7 @@ class Engine(object):
     Of the live envs (n = n_envs), or with `states` of EnvStates of any n records, as if loaded.
     Into `out` if given (a triple of contiguous int32 tensors of those shapes on this device), else
     new tensors.  One launch on the current stream (after zeroing the counts); nothing else changes."""
-    if states is not None and not isinstance(states, EnvStates):
-      raise ValueError('states must be EnvStates, got %s' % type(states).__name__)
-    n = self.n_envs if states is None else len(states)
-    if states is not None:
-      self.check_states(states, n)
+    n, rec, rec_bytes = _rows(self, states)
     W, H, aa = int(width), int(height), int(anti_aliasing)
     shapes = ((n, H, W), (n, self.n_slots), (n, self.n_slots))
     if out is None:
@@ -489,23 +476,10 @@ class Engine(object):
       if not isinstance(out, (tuple, list)) or len(out) != 3:
         raise ValueError('out must be a (cover, visible, area) triple, got %s' % type(out).__name__)
       for name, t, shape in zip(('cover', 'visible', 'area'), out, shapes):
-        if (not isinstance(t, torch.Tensor) or t.dtype != torch.int32 or t.device != self.device or
-            tuple(t.shape) != shape or not t.is_contiguous()):
-          raise ValueError('%s must be a contiguous int32 tensor of shape %s on %s, got %s' % (
-              name, shape, self.device, _describe(t)))
+        _check_output(t, name, torch.int32, shape, self.device)
       out = tuple(out)
-    ptrs = [t.data_ptr() for t in out]
-    rec = (None, 0) if states is None else (states.data.data_ptr(), states.data.numel())
-    if n == 0:
-      # zero records: checked as any call, nothing drawn; an aligned address stands in for empty
-      # buffers, which cannot overlap (nothing is read or written)
-      probe = torch.empty(16, dtype=torch.uint8, device=self.device)
-      ptrs = [p or probe.data_ptr() for p in ptrs]
-      if rec[0] is not None:
-        rec = (rec[0] or probe.data_ptr(), rec[1])
-    _native.check(self._lib.swb_render_coverage(
-        self._h, W, H, aa, None if rec[0] is None else ctypes.c_void_p(rec[0]), n, rec[1],
-        *[ctypes.c_void_p(p) for p in ptrs], self._stream()))
+    _native.check(self._lib.swb_render_coverage(self._h, W, H, aa, rec, n, rec_bytes,
+                                                *[_address(t) for t in out], self._stream()))
     return out
 
   def render_status(self):
@@ -863,17 +837,15 @@ class Engine(object):
     each record of `states` at its live positions (no action cost), with goals[i] (float64
     (n, G, 2) on this engine's device) in place of record i's goals if given.  One launch; reads
     only."""
-    n = len(states) if isinstance(states, EnvStates) else -1
-    self.check_states(states, n)
+    n, rec, rec_bytes = _rows(self, states, live=False)
     if goals is not None:
       goals = self._check_goals(goals, n, 'evaluate')
     reward = torch.empty(n, dtype=torch.float64, device=self.device)
     success = torch.empty(n, dtype=torch.uint8, device=self.device)
     status = torch.empty(n, dtype=torch.uint8, device=self.device)
     _native.check(self._lib.swb_evaluate_states(
-        self._h, ctypes.c_void_p(states.data.data_ptr()), n, states.data.numel(),
-        None if goals is None else ctypes.c_void_p(goals.data_ptr()), ctypes.c_void_p(reward.data_ptr()),
-        ctypes.c_void_p(success.data_ptr()), ctypes.c_void_p(status.data_ptr()), self._stream()))
+        self._h, rec, n, rec_bytes, None if goals is None else ctypes.c_void_p(goals.data_ptr()),
+        *[_address(t) for t in (reward, success, status)], self._stream()))
     return reward, success, status
 
   def sample_contained(self, seed, n_samples=1, states=None):
@@ -886,9 +858,7 @@ class Engine(object):
     sample has position NaN and slot -1).  One launch on the current stream; reads only."""
     if isinstance(seed, (bool, np.bool_)) or not isinstance(seed, (int, np.integer)) or not 0 <= seed < 2 ** 64:
       raise ValueError('seed must be an int in [0, 2^64), got %r' % (seed,))
-    n = self.n_envs if states is None else len(states)
-    if states is not None:
-      self.check_states(states, n)
+    n, rec, rec_bytes = _rows(self, states)
     if isinstance(n_samples, (bool, np.bool_)) or not isinstance(n_samples, (int, np.integer)) or not (
         1 <= n_samples < 2 ** 31):
       raise ValueError('n_samples must be an int in [1, 2^31), got %r' % (n_samples,))
@@ -896,17 +866,9 @@ class Engine(object):
     position = torch.empty((n, n_samples, 2), dtype=torch.float64, device=self.device)
     slot = torch.empty((n, n_samples), dtype=torch.int8, device=self.device)
     status = torch.empty((n, n_samples), dtype=torch.uint8, device=self.device)
-    ptrs = [t.data_ptr() for t in (position, slot, status)]
-    rec = (None, 0) if states is None else (states.data.data_ptr(), states.data.numel())
-    if n == 0:
-      # zero rows: checked as any other call and nothing drawn, but an empty tensor may have no address;
-      # any aligned address stands in (nothing is read or written)
-      probe = torch.empty(16, dtype=torch.uint8, device=self.device).data_ptr()
-      ptrs = [p or probe for p in ptrs]
-      rec = rec if states is None else (rec[0] or probe, rec[1])
     _native.check(self._lib.swb_sample_contained(
-        self._h, None if rec[0] is None else ctypes.c_void_p(rec[0]), n, rec[1], n_samples, int(seed),
-        *[ctypes.c_void_p(p) for p in ptrs], self._stream()))
+        self._h, rec, n, rec_bytes, n_samples, int(seed), *[_address(t) for t in (position, slot, status)],
+        self._stream()))
     return position, slot, status
 
   def launch_count(self):

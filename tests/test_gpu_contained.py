@@ -257,12 +257,20 @@ def test_refused_calls_enqueue_nothing():
       ('n = -1', (eng._h, rp, -1, rb, 4, 1, *outs)),
       ('16-byte aligned', (eng._h, odd, 2, rb, 4, 1, *outs)),
       ('bytes', (eng._h, rp, 8, rb - 16, 4, 1, *outs)),
+      ('position is not 8-byte aligned', (eng._h, None, 8, 0, 4, 1, ctypes.c_void_p(pos.data_ptr() + 4),
+                                          outs[1], outs[2])),
+      ('position overlaps the records', (eng._h, rp, 8, rb, 4, 1, ctypes.c_void_p(states.data.data_ptr() + 16),
+                                         outs[1], outs[2])),
+      ('status overlaps slot', (eng._h, rp, 8, rb, 4, 1, outs[0], outs[1], ctypes.c_void_p(slot.data_ptr() + 31))),
   ]
+  records = states.data.clone()
   launches = eng.launch_count()
   for msg, args in cases:
     assert L.swb_sample_contained(*args, stream) != 0, msg
     assert msg.encode() in L.swb_last_error(), (msg, L.swb_last_error())
     assert eng.launch_count() == launches, msg
+  torch.cuda.synchronize()
+  assert torch.equal(states.data, records)
   # zero records are accepted and draw nothing
   assert L.swb_sample_contained(eng._h, rp, 0, 0, 4, 1, *outs, stream) == 0
   assert eng.launch_count() == launches

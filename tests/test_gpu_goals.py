@@ -174,6 +174,50 @@ def test_set_goals_refusals_change_nothing():
     eng.check_env_ids()
 
 
+def test_evaluate_refusals_change_nothing():
+  env = _env(n_envs=8)
+  eng = env.engine
+  env.reset()
+  states = env.save_envs()
+  n, rb = len(states), states.record_bytes
+  no_goals = engine_lib.Engine(n, eng.n_slots, 1, env._action_space.compile(), [dict(kind='no_reward')],
+                               constants.SHAPES)
+  goals = torch.zeros((n, eng.n_goals, 2), dtype=torch.float64, device=eng.device)
+  out = torch.full((16 * n,), 7, dtype=torch.uint8, device=eng.device)   # reward, success, status
+  records = states.data.clone()
+  R, O, G = states.data.data_ptr(), out.data_ptr(), goals.data_ptr()
+  torch.cuda.synchronize()
+  launches = eng.launch_count(), no_goals.launch_count()
+
+  def call(engine=eng._h, records=R, n=n, records_bytes=n * rb, goals=G, reward=O, success=O + 8 * n,
+           status=O + 9 * n):
+    return eng._lib.swb_evaluate_states(engine, records, n, records_bytes, goals, reward, success, status,
+                                        eng._stream())
+
+  def refused(match, **kw):
+    assert call(**kw) != 0 and match in eng._lib.swb_last_error(), (kw, eng._lib.swb_last_error())
+    assert (eng.launch_count(), no_goals.launch_count()) == launches
+
+  refused(b'null', engine=None)
+  refused(b'null', records=None)
+  for name in ('reward', 'success', 'status'):
+    refused(b'null', **{name: None})
+  refused(b'n = -1', n=-1)
+  refused(b'records is not 16-byte aligned', records=R + 8)
+  refused(b'records need', records_bytes=n * rb - 1)
+  refused(b'G = 0', engine=no_goals._h)
+  refused(b'goals are not 8-byte aligned', goals=G + 4)
+  refused(b'reward overlaps the records', reward=R + 16)
+  refused(b'status overlaps the records', status=R + n * rb - 1)
+  refused(b'reward is not 8-byte aligned', reward=O + 4)
+  refused(b'status overlaps success', status=O + 9 * n - 1)
+  torch.cuda.synchronize()
+  assert bool((out == 7).all()) and torch.equal(states.data, records)
+  assert call(n=0) == 0 and eng.launch_count() == launches[0]
+  assert call() == 0 and eng.launch_count() == launches[0] + 1
+  no_goals.close()
+
+
 def test_evaluate_relabels_records_as_the_constant_goal_tree():
   env = _env(n_envs=32)
   eng = env.engine

@@ -316,6 +316,7 @@ def test_refused_calls_enqueue_nothing():
   refused(b'frames overlap', records=B, frames=B + n * rb - 1)
   refused(b'frames overlap', records=B + 16, frames=B)
   refused(b'status overlaps', records=B, status=B + (n - 1) * rb)
+  refused(b'status overlaps frames', status=F + fb - 1)
   tall = engine.Raster(eng, 4, 65, 1)                               # two bands per frame
   refused(b'exceed', raster=tall._h, n=2 ** 30, records_bytes=2 ** 30 * rb, frames=16, status=32)
   other = engine.Engine(E, 2, 1, dict(kind='select_move', scale=0.05), [dict(kind='no_reward')], constants.SHAPES)

@@ -260,6 +260,14 @@ def test_refused_record_rollouts_enqueue_nothing():
   refused(b'overlap', leaves=R, leaves_bytes=E * C * rb)           # the same buffer
   refused(b'overlap', roots=L + (E * C - 1) * rb)                 # roots from the last leaf on
   refused(b'overlap', roots=L, leaves=L + (E - 1) * rb)           # leaves from the last root on
+
+  def outputs(**kw):   # `out` with some arrays replaced by pointers
+    ptrs = dict(reward=out.reward, step_type=out.step_type, success=out.success, status=out.status)
+    return _native.StepOut(**dict(ptrs, **kw))
+  refused(b'reward is not 8-byte aligned', outputs=outputs(reward=out.reward + 4))
+  refused(b'leaves overlaps status', outputs=outputs(status=L + (E * C - 1) * rb))
+  refused(b'success overlaps the roots', outputs=outputs(success=R + E * rb - 1))
+  refused(b'status overlaps step_type', outputs=outputs(status=out.step_type + T * E * C - 1))
   assert call(roots=L + E * C * rb) == 0 and span.value == -5     # adjacent: accepted
   assert call(roots=None) == 0 and span.value == roots.span_class  # live roots: the engine's
   assert _snapshot(eng)[1] == before[1] + 2
