@@ -335,7 +335,7 @@ int swb_upload_state(swb_engine *eng, const double *pos_x, const double *pos_y,
  * steps and frames.
  *
  * Read-only record calls (swb_rollout_states, swb_render_states, swb_render_masks,
- * swb_render_coverage, swb_evaluate_states, swb_sample_contained) read n rows: n records of this
+ * swb_render_coverage, swb_render_soft_masks, swb_evaluate_states, swb_sample_contained) read n rows: n records of this
  * engine's layout in a device record buffer of records_bytes bytes or, where a call takes them,
  * the E live envs for records == NULL, and then n == E.  Each of them is refused, enqueuing
  * nothing, for a null engine, n < 0, records == NULL where the call takes no live envs, a record
@@ -455,6 +455,27 @@ int swb_render_masks(swb_engine *eng, int32_t width, int32_t height, int32_t ant
 int swb_render_coverage(swb_engine *eng, int32_t width, int32_t height, int32_t anti_aliasing,
                         const void *records, int32_t n, uint64_t records_bytes, int32_t *cover,
                         int32_t *visible, int32_t *area, void *stream);
+
+/*
+ * Soft sprite masks (renderers.SoftSpriteMasks): how much of each pixel each sprite owns.  `soft`
+ * is [n][S][height][width] uint8; soft[i][k][r][c] is the number of canvas pixels
+ * (aa c + u, aa (height-1-r) + v), u and v in [0, aa), of the aa*width x aa*height canvas whose
+ * top-most covering sprite is slot k, with the integer vertices and Pillow fill rules of
+ * swb_render_masks.  So soft / aa^2 is the fraction of the pixel's box the slot owns, aa^2 minus the
+ * sum over the slots is the background's count, the sample swb_render_masks reads (u = v = aa/2) is
+ * one of them, and at anti_aliasing 1 soft[i][k] is (mask == k + 1).  Empty slots and sprites out
+ * of frame or wholly hidden are zero.  A box filter of the label canvas: the frames are LANCZOS
+ * filtered, so they are not the soft masks' composite of sprite colours.
+ *
+ * Records, sizes and n as swb_render_masks takes them (records == NULL: the E live envs, n == E).
+ * An accepted call with n > 0 is one launch on `stream` that writes every byte of `soft`; n == 0
+ * enqueues nothing.  Read-only as swb_render_masks, with soft as its output.  Refused besides: what
+ * swb_render_masks refuses, anti_aliasing above 15 (aa^2 = 225 is the largest count a byte holds),
+ * with bands of at most 128 canvas rows and 32 KiB of staged canvas (or one mask row).
+ */
+int swb_render_soft_masks(swb_engine *eng, int32_t width, int32_t height, int32_t anti_aliasing,
+                          const void *records, int32_t n, uint64_t records_bytes, uint8_t *soft,
+                          void *stream);
 
 /* Env dst_ids[i] <- env src_ids[i].  Ids in [0, E), destinations distinct.  Every read sees the
  * state from before the call, also where the two sets overlap (then the records go through

@@ -161,3 +161,13 @@ def render_coverage(renderer, sprites):
   S = eng.n_slots   # n slots for n >= 1 sprites, so bit i is slot i; one empty slot for none
   return collections.OrderedDict([('cover', cover[0].cpu().numpy()), ('visible', visible[0, S - n:].cpu().numpy()),
                                   ('area', area[0, S - n:].cpu().numpy())])
+
+
+def render_soft_masks(renderer, sprites):
+  """(len(sprites), H, W) uint8 soft masks of a Python sprite list: soft[i] counts the
+  anti-aliasing samples of each pixel where sprites[i] is the top-most sprite."""
+  n = len(sprites)
+  eng = _engine(max(1, n), _DUMMY_ACTION, _NO_TASK, True)
+  _load(eng, sprites)
+  soft = eng.render_soft_masks(renderer.width, renderer.height, renderer.anti_aliasing)
+  return soft[0, eng.n_slots - n:].cpu().numpy()   # slot i is sprites[i] for n >= 1 sprites

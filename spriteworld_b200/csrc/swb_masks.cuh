@@ -1,32 +1,42 @@
 // Mask kernel: which sprite is visible at each pixel (renderers.SpriteMasks, swb_render_masks),
-// and which sprites cover it (renderers.SpriteCoverage, swb_render_coverage).
+// which sprites cover it (renderers.SpriteCoverage, swb_render_coverage), and how many of its
+// anti-aliasing samples each sprite owns (renderers.SoftSpriteMasks, swb_render_soft_masks).
 //
 // Mask pixel (i, j) of a W x H mask at anti_aliasing aa is the slot + 1 of the top-most sprite
 // whose Pillow polygon fill covers canvas pixel (aa j + aa/2, aa (H-1-i) + aa/2) of the aa W x aa H
 // canvas PILRenderer draws on, or 0 (what Image.resize(NEAREST) of a label canvas picks, flipped
 // like the frames).  Only Pillow's scan conversion is needed, not its LANCZOS filter, and only one
-// canvas row per mask row.  The coverage of the same pixel (kCover) is the int32 whose bit k is set
-// where slot k's fill covers that canvas pixel, whether or not a sprite above hides it, so the mask
-// is its highest set bit + 1; with it come per-slot counts of the pixels where the slot is the
-// top-most covering sprite (visible) and where its bit is set (area).
+// canvas row per mask row.  The coverage of the same pixel (MASK_COVER) is the int32 whose bit k is
+// set where slot k's fill covers that canvas pixel, whether or not a sprite above hides it, so the
+// mask is its highest set bit + 1; with it come per-slot counts of the pixels where the slot is the
+// top-most covering sprite (visible) and where its bit is set (area).  The soft mask (MASK_SOFT) is
+// [S][H][W] uint8: soft[k][i][j] counts the canvas pixels (aa j + u, aa (H-1-i) + v), u, v in
+// [0, aa), whose top-most covering sprite is slot k -- all aa^2 samples of the pixel, not only the
+// centre one, so aa <= 15 keeps a count in a byte.
 //
 // One CTA draws one band of mask rows of one env (or record):
 //   A  a warp per sprite, a lane per vertex: the integer canvas vertices, Pillow's edge records,
 //      horizontal edges and corner-join overrides -- the arithmetic of render_kernel's phase A
 //      (swb_render.cuh), restated here without that kernel's tile and bucket plan.
-//   B  a thread per mask row scan-converts its one canvas row for every sprite, back to front:
-//      the crossings of the edges spanning the row (an edge ending on an interior row counts
-//      twice), sorted and paired with ROUND_UP / ROUND_DOWN, plus the horizontal edges on the
-//      row; each canvas span [xs, xe] paints slot + 1 (kCover: ORs 1 << slot) into the mask
-//      columns whose sample aa j + aa/2 lies in it, in a row staged in shared memory.
-//   C  the staged band goes out with 16-byte stores (single pixels at its ends).  kCover: each
-//      warp counts its pixels per slot with ballots, the CTA sums the warps in shared memory and
-//      adds its sums to the outputs with one integer atomic per (band, slot).
+//   B  a thread per canvas row scan-converts it for every sprite, back to front: the crossings of
+//      the edges spanning the row (an edge ending on an interior row counts twice), sorted and
+//      paired with ROUND_UP / ROUND_DOWN, plus the horizontal edges on the row.  Label and cover:
+//      a thread per mask row takes its one canvas row, and each canvas span [xs, xe] paints
+//      slot + 1 (MASK_COVER: ORs 1 << slot) into the mask columns whose sample aa j + aa/2 lies in
+//      it, in a row staged in shared memory.  Soft: a thread per canvas row of the band's aa
+//      canvas rows per mask row paints slot + 1 over the whole span, into a staged label row of
+//      the canvas.  One scan serves all three modes; only the rows and the paint differ.
+//   C  label and cover: the staged band goes out with 16-byte stores (single pixels at its ends).
+//      MASK_COVER: each warp counts its pixels per slot with ballots, the CTA sums the warps in
+//      shared memory and adds its sums to the outputs with one integer atomic per (band, slot).
+//      Soft: a thread per mask pixel collects the labels of its aa x aa block as a 32-bit set,
+//      counts the samples of each label in it, and writes one byte to each of the S slot planes;
+//      consecutive threads take consecutive columns, so each plane's stores coalesce.
 // A sprite row has at most 2 crossings per edge, 2 * SWB_MAX_VERTS in all, and every one is kept:
-// the mask is exact for every shape, and there is no overflow status.
+// the masks are exact for every shape, and there is no overflow status.
 //
-// Nothing but the masks (kCover: the coverage and its counts) is written: no env, pool entry,
-// frame or render status changes.
+// Nothing but the outputs (MASK_COVER: the coverage and its counts) is written, every byte of
+// them: no env, pool entry, frame or render status changes.
 #pragma once
 #include <climits>
 #include <type_traits>
@@ -39,30 +49,51 @@ namespace swb {
 
 constexpr int MK_THREADS = 128;          // threads per CTA = most mask rows per band
 constexpr int MK_STAGE_BYTES = 16384;    // staged bytes per band (fewer rows for wide or coverage masks)
+constexpr int MK_SOFT_STAGE_BYTES = 32768;  // soft: staged canvas labels per band (at least one mask row's)
+constexpr int MK_SOFT_MAX_AA = 15;       // soft: aa^2 samples per pixel fit a uint8 count
 constexpr int MK_XCAP = 2 * EV;          // crossings one sprite row can have
 
-// A mask raster and the shared-memory layout of one CTA; `cover`: staged pixels are the 4-byte
-// coverage words, and the CTA keeps per-slot counts.
+// What the mask kernel draws: the uint8 mask, the int32 coverage and its counts, or the uint8
+// soft mask [S][H][W].
+enum MaskMode { MASK_LABEL, MASK_COVER, MASK_SOFT };
+
+// A mask raster and the shared-memory layout of one CTA.  MASK_COVER: staged pixels are the 4-byte
+// coverage words, and the CTA keeps per-slot counts.  MASK_SOFT: the band's aa canvas rows per mask
+// row are staged as CW label bytes each, and band_rows * aa <= MK_THREADS (a thread per canvas row);
+// one mask row (at most 15 * 4095 bytes) is always staged, whatever MK_SOFT_STAGE_BYTES says.
 struct MaskLayout {
   int S, W, H, aa, CW, CH, band_rows, n_bands;
   int off_edge, off_hl, off_meta, off_xx, off_stage, total;
-  __host__ __device__ MaskLayout(int S_, int W_, int H_, int aa_, bool cover = false)
+  __host__ __device__ MaskLayout(int S_, int W_, int H_, int aa_, MaskMode mode = MASK_LABEL)
       : S(S_), W(W_), H(H_), aa(aa_) {
+    const bool cover = mode == MASK_COVER, soft = mode == MASK_SOFT;
     const int px = cover ? 4 : 1;         // bytes per staged pixel
     CW = aa * W;
     CH = aa * H;
-    band_rows = MK_STAGE_BYTES / (px * W);
-    if (band_rows < 1) band_rows = 1;
-    if (band_rows > MK_THREADS) band_rows = MK_THREADS;
-    if (band_rows > H) band_rows = H;
-    n_bands = (H + band_rows - 1) / band_rows;
+    if (soft) {
+      // the fewest bands of at most the budget's rows, then rows spread evenly over them
+      int most = MK_SOFT_STAGE_BYTES / (aa * CW);
+      if (most > MK_THREADS / aa) most = MK_THREADS / aa;
+      if (most < 1) most = 1;
+      n_bands = (H + most - 1) / most;
+      band_rows = (H + n_bands - 1) / n_bands;
+    } else {
+      band_rows = MK_STAGE_BYTES / (px * W);
+      if (band_rows < 1) band_rows = 1;
+      if (band_rows > MK_THREADS) band_rows = MK_THREADS;
+      if (band_rows > H) band_rows = H;
+      n_bands = (H + band_rows - 1) / band_rows;
+    }
     int o = 0;
     auto take = [&](int bytes) { int r = o; o += (bytes + 15) & ~15; return r; };
     off_edge = take(S * EV * 6 * 4);        // x0, y0 (int), dx, ovs, ove (float), yr (u32)
     off_hl = take(S * EV * 3 * 2);          // horizontal edges: y, xmin, xmax (int16)
     off_meta = take(S * 5 * 4);             // nv, nh, has-join, p_ymax, ymin | ymax << 16
     off_xx = take(MK_XCAP * MK_THREADS * 4);  // crossings, [k][thread]
-    off_stage = take(band_rows * W * px + 16);  // staged band, placed at the output's address mod 16
+    if (soft)
+      off_stage = take(band_rows * aa * CW);  // canvas labels, [band_rows * aa][CW]
+    else
+      off_stage = take(band_rows * W * px + 16);  // staged band, placed at the output's address mod 16
     if (cover) take(S * 2 * 4);             // the band's visible [S], area [S] (int), at cnt_offset()
     total = o;
   }
@@ -75,12 +106,14 @@ struct CoverCounts {
   int32_t *visible, *area;
 };
 
-// kCover: `masks` is the [n][H][W] int32 coverage, and `counts` receives its per-slot counts;
-// otherwise `masks` is the [n][H][W] uint8 mask and `counts` is not read.
-template <bool kRecords, bool kCover>
+// MASK_LABEL: `masks` is the [n][H][W] uint8 mask.  MASK_COVER: `masks` is the [n][H][W] int32
+// coverage, and `counts` receives its per-slot counts.  MASK_SOFT: `masks` is the [n][S][H][W]
+// uint8 soft mask.  `counts` is read in MASK_COVER only.
+template <bool kRecords, MaskMode kMode>
 __global__ void __launch_bounds__(MK_THREADS)
 mask_kernel(DevState st, const MaskLayout L, uint8_t *__restrict__ masks, const RenderRecords recs,
             const CoverCounts counts) {
+  constexpr bool kCover = kMode == MASK_COVER, kSoft = kMode == MASK_SOFT;
   extern __shared__ __align__(16) unsigned char g_mask_smem[];
   unsigned char *const smem = g_mask_smem;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -220,32 +253,46 @@ mask_kernel(DevState st, const MaskLayout L, uint8_t *__restrict__ masks, const 
     }
   }
 
+
   // the band's output rows [i0, i0 + nb) are pixels [g, g + nb * W) of the masks; the band is
-  // staged from s_stage + (its address mod 16), so that staged and global addresses agree modulo 16
+  // staged from s_stage + (its address mod 16), so that staged and global addresses agree modulo 16.
+  // kSoft: the stage holds the band's canvas rows aa (H-1-i) + v, v in [0, aa), of mask rows i in
+  // [i0, i0 + nb) as label rows stage[((i - i0) aa + v) CW + x] (0: no sprite), from s_stage
   const int i0 = band * L.band_rows;
   const int nb = min(L.band_rows, L.H - i0);
   const size_t g = (e * (size_t)L.H + (size_t)i0) * (size_t)L.W;
   const int npx = nb * L.W;
   Px *const gdst = reinterpret_cast<Px *>(masks) + g;
-  const int mis = (int)(reinterpret_cast<uintptr_t>(gdst) & 15u);
+  const int mis = kSoft ? 0 : (int)(reinterpret_cast<uintptr_t>(gdst) & 15u);
   Px *const stage = reinterpret_cast<Px *>(smem + L.off_stage + mis);
   int *const s_cnt = reinterpret_cast<int *>(smem + L.cnt_offset());  // kCover: visible [S], area [S]
-  for (int i = tid; i < npx; i += MK_THREADS) stage[i] = 0;
+  const int nstage = kSoft ? nb * L.aa * L.CW : npx;  // staged pixels
+  if constexpr (kSoft)
+    for (int i = tid; i < (nstage >> 4); i += MK_THREADS) reinterpret_cast<uint4 *>(stage)[i] = make_uint4(0, 0, 0, 0);
+  for (int i = (kSoft ? nstage & ~15 : 0) + tid; i < nstage; i += MK_THREADS) stage[i] = 0;
   if (kCover && tid < 2 * S) s_cnt[tid] = 0;
   __syncthreads();
 
-  // ---- phase B: a thread per mask row, its one canvas row, sprites back to front ------------
-  if (tid < nb) {
-    const int i = i0 + tid;
-    const int y = L.aa * (L.H - 1 - i) + L.aa / 2;  // canvas row of mask row i (always on the canvas)
+  // ---- phase B: a thread per mask row, its one canvas row, sprites back to front (kSoft: a
+  // thread per canvas row of the band, nb * aa <= MK_THREADS by MaskLayout) ---------------------
+  if (tid < (kSoft ? nb * L.aa : nb)) {
+    const int i = i0 + (kSoft ? tid / L.aa : tid);
+    // canvas row of mask row i (always on the canvas): its sample row, kSoft its row tid mod aa
+    const int y = L.aa * (L.H - 1 - i) + (kSoft ? tid - (i - i0) * L.aa : L.aa / 2);
     const int half = L.aa / 2;
-    Px *const row = stage + (size_t)tid * L.W;
-    // paints the mask columns j with xs <= aa j + aa/2 <= xe (0 <= xs <= xe < CW)
+    Px *const row = stage + (size_t)tid * (kSoft ? L.CW : L.W);
+    // paints the mask columns j with xs <= aa j + aa/2 <= xe (0 <= xs <= xe < CW); kSoft: the
+    // canvas pixels xs .. xe
     auto paint = [&](int xs, int xe, Px label) {
-      const int jlo = (xs - half + L.aa - 1) / L.aa, jhi = (xe - half + L.aa) / L.aa - 1;
-      for (int j = jlo; j <= jhi; ++j) {
-        if constexpr (kCover) row[j] |= label;
-        else row[j] = label;
+      if constexpr (kSoft) {
+#pragma unroll 1
+        for (int x = xs; x <= xe; ++x) row[x] = label;
+      } else {
+        const int jlo = (xs - half + L.aa - 1) / L.aa, jhi = (xe - half + L.aa) / L.aa - 1;
+        for (int j = jlo; j <= jhi; ++j) {
+          if constexpr (kCover) row[j] |= label;
+          else row[j] = label;
+        }
       }
     };
 #pragma unroll 1
@@ -300,6 +347,44 @@ mask_kernel(DevState st, const MaskLayout L, uint8_t *__restrict__ masks, const 
     }
   }
   __syncthreads();
+
+  if constexpr (kSoft) {
+    // ---- soft phase C: a thread per mask pixel (i0 + r, j), its aa x aa block of labels ------
+    const int aa = L.aa, CW = L.CW, aa2 = aa * aa;
+    const size_t plane = (size_t)L.H * L.W;
+    for (int p = tid; p < npx; p += MK_THREADS) {
+      const int r = p / L.W, j = p - r * L.W;
+      const uint8_t *const blk = stage + (size_t)r * aa * CW + aa * j;
+      uint32_t present = 0;  // bit s: label s + 1 is in the block
+      bool bg = false;       // a sample no sprite covers
+#pragma unroll 1
+      for (int v = 0; v < aa; ++v)
+#pragma unroll 1
+        for (int u = 0; u < aa; ++u) {
+          const int l = blk[v * CW + u];
+          if (l) present |= 1u << (l - 1);
+          else bg = true;
+        }
+      const bool one = !bg && (present & (present - 1u)) == 0u;  // one label on every sample
+      uint8_t *dst = masks + (e * (size_t)S * L.H + (size_t)(i0 + r)) * L.W + j;
+#pragma unroll 1
+      for (int s = 0; s < S; ++s, dst += plane) {
+        int c = 0;
+        if ((present >> s) & 1u) {
+          if (one) {
+            c = aa2;
+          } else {
+#pragma unroll 1
+            for (int v = 0; v < aa; ++v)
+#pragma unroll 1
+              for (int u = 0; u < aa; ++u) c += blk[v * CW + u] == s + 1;
+          }
+        }
+        *dst = (uint8_t)c;
+      }
+    }
+    return;
+  }
 
   // ---- phase C: the staged band to the masks -------------------------------------------------
   constexpr int LOG16 = kCover ? 2 : 4;  // log2 of the pixels per 16-byte store

@@ -482,6 +482,25 @@ class Engine(object):
                                                 *[_address(t) for t in out], self._stream()))
     return out
 
+  def render_soft_masks(self, width, height, anti_aliasing=1, states=None, out=None):
+    """Soft sprite masks (swb_render_soft_masks): uint8 (n, n_slots, height, width), where
+    soft[i, k, r, c] counts the canvas pixels of mask pixel (r, c)'s anti_aliasing x anti_aliasing
+    block on PILRenderer's canvas whose top-most covering sprite is slot k (the pixel render_masks
+    draws k + 1 at samples the block's centre one); soft / anti_aliasing**2 is the slot's share of
+    the pixel (renderers.SoftSpriteMasks).  anti_aliasing at most 15.  Of the live envs (n =
+    n_envs), or with `states` of EnvStates of any n records, as if loaded.  Into `out` if given (a
+    contiguous uint8 tensor of that shape on this device), else a new tensor.  One launch on the
+    current stream; nothing else changes."""
+    n, rec, rec_bytes = _rows(self, states)
+    W, H, aa = int(width), int(height), int(anti_aliasing)
+    if out is None:
+      out = torch.empty((n, self.n_slots, max(H, 0), max(W, 0)), dtype=torch.uint8, device=self.device)
+    else:
+      _check_output(out, 'soft', torch.uint8, (n, self.n_slots, H, W), self.device)
+    _native.check(self._lib.swb_render_soft_masks(self._h, W, H, aa, rec, n, rec_bytes, _address(out),
+                                                  self._stream()))
+    return out
+
   def render_status(self):
     """Zero-copy uint8 (E,) view of the per-env status of the last render() (ENV_SPAN_OVERFLOW)."""
     if getattr(self, '_render_status_view', None) is None:

@@ -373,6 +373,10 @@ class BatchedEnvironment(object):
                 torch.empty((E, slots), dtype=torch.int32, device=self._engine.device),
                 torch.empty((E, slots), dtype=torch.int32, device=self._engine.device))
         for r in self._other.values() if isinstance(r, handcrafted.SpriteCoverage)}
+    # and one (n_envs, n_slots, H, W) soft mask per SoftSpriteMasks renderer
+    self._soft_buffers = {
+        id(r): torch.empty((E, slots, r.height, r.width), dtype=torch.uint8, device=self._engine.device)
+        for r in self._other.values() if isinstance(r, handcrafted.SoftSpriteMasks)}
     if sampler == 'device':
       self._init_device_sampler(seed, env_offset)
       return
@@ -873,10 +877,10 @@ class BatchedEnvironment(object):
     return BatchedRollout(res.step_type, res.reward, discount, res.success, res.status)
 
   def render(self):
-    """Re-renders every PILRenderer, SpriteMasks and SpriteCoverage observation of the current
-    state (a loaded one, say) into this environment's buffers, and returns them: dict name -> uint8
-    (n_envs, H, W, 3) frames, then uint8 (n_envs, H, W) masks and coverage dicts, in renderer
-    order."""
+    """Re-renders every PILRenderer, SpriteMasks, SpriteCoverage and SoftSpriteMasks observation of
+    the current state (a loaded one, say) into this environment's buffers, and returns them: dict
+    name -> uint8 (n_envs, H, W, 3) frames, then uint8 (n_envs, H, W) masks, coverage dicts and
+    uint8 (n_envs, n_slots, H, W) soft masks, in renderer order."""
     out = collections.OrderedDict()
     for name, r in self._rasters.items():
       out[name] = self._engine.render(r, self._frames[name])
@@ -885,6 +889,8 @@ class BatchedEnvironment(object):
         out[name] = self.render_masks(r)
       elif isinstance(r, handcrafted.SpriteCoverage):
         out[name] = self.render_coverage(r)
+      elif isinstance(r, handcrafted.SoftSpriteMasks):
+        out[name] = self.render_soft_masks(r)
     return out
 
   def render_masks(self, renderer, states=None):
@@ -908,13 +914,22 @@ class BatchedEnvironment(object):
       out = self._engine.render_coverage(*dims, out=self._coverage_buffers.get(id(renderer)))
     return collections.OrderedDict(zip(('cover', 'visible', 'area'), out))
 
+  def render_soft_masks(self, renderer, states=None):
+    """SoftSpriteMasks `renderer`'s soft masks (Engine.render_soft_masks) on the current stream: of
+    the live envs into this environment's buffer for the renderer (a new tensor for a renderer it
+    does not own), or of EnvStates `states` into a new uint8 (n, n_slots, H, W) tensor."""
+    dims = (renderer.width, renderer.height, renderer.anti_aliasing)
+    if states is not None:
+      return self._engine.render_soft_masks(*dims, states=states)
+    return self._engine.render_soft_masks(*dims, out=self._soft_buffers.get(id(renderer)))
+
   def observe(self, states):
     """The observations of env records without loading them: (observation, status) for EnvStates
     `states` of n records, observation an OrderedDict in renderer order of what step() would
     observe for envs that load_envs(states) had loaded -- PILRenderer frames as new uint8
     (n, H, W, 3) tensors (one render launch per raster; never this environment's own frame
-    buffers), SpriteFactors dicts of (n, n_slots) tensors, SpriteMasks and SpriteCoverage
-    observations in new tensors (one launch each) -- and status uint8 (n,), the OR over the
+    buffers), SpriteFactors dicts of (n, n_slots) tensors, SpriteMasks, SpriteCoverage and
+    SoftSpriteMasks observations in new tensors (one launch each) -- and status uint8 (n,), the OR over the
     rasters of their render status (_native.ENV_SPAN_OVERFLOW).
 
     Enqueued on the current stream without a host synchronisation.  Read-only: no env, scene ring,

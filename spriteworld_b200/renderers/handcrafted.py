@@ -71,7 +71,8 @@ class SpriteFactors(abstract_renderer.AbstractRenderer):
 
 
 def _check_mask_raster(renderer, image_size, anti_aliasing):
-  """SpriteMasks' and SpriteCoverage's arguments: sets _image_size and _anti_aliasing."""
+  """SpriteMasks', SpriteCoverage's and SoftSpriteMasks' arguments: sets _image_size and
+  _anti_aliasing."""
   renderer._image_size = tuple(int(v) for v in image_size)
   renderer._anti_aliasing = int(anti_aliasing)
   if len(renderer._image_size) != 2 or min(renderer._image_size) < 1 or renderer._anti_aliasing < 1:
@@ -196,6 +197,74 @@ class SpriteCoverage(abstract_renderer.AbstractRenderer):
   def render_states(self, env, states):
     """The coverage of env records (EnvStates) without loading them, in new tensors."""
     return env.render_coverage(self, states)
+
+  def batch_observation_spec(self, env):
+    return self._spec(env.engine.n_slots)
+
+
+class SoftSpriteMasks(abstract_renderer.AbstractRenderer):
+  """Soft instance masks: how much of each pixel of a PILRenderer frame each sprite owns.
+
+  Observes uint8 (S, H, W) for image_size=(W, H) and S sprites: soft[k, i, j] is the number of
+  canvas pixels (aa j + u, aa (H-1-i) + v), u, v in [0, aa), of the aa W x aa H canvas PILRenderer
+  draws on whose top-most covering sprite is sprite k, with SpriteMasks' integer vertices and
+  Pillow fill rules.  So soft / aa**2 is the fraction of the pixel sprite k owns, aa**2 -
+  soft.sum(0) counts the background's samples, and soft[k].sum() / aa**2 is sprite k's visible
+  area in frame pixels, below pixel precision.  In Pillow: draw the label canvas (every sprite back
+  to front, fill k + 1, into a zero 'L' image of aa W x aa H), L = np.flipud(canvas).reshape(H, aa,
+  W, aa), soft[k] = (L == k + 1).sum((1, 3)).
+
+  At anti_aliasing=1, soft[k] == (SpriteMasks mask == k + 1); at any aa the sample SpriteMasks reads
+  is one of the aa**2, so mask == k + 1 implies soft[k] >= 1.  Empty slots and sprites out of frame
+  or wholly hidden are zero.  This is a box filter of the label canvas: the frame is LANCZOS
+  filtered, so it is not in general the composite sum_k rgb_k soft_k / aa**2.  Drawn by the mask
+  kernel's soft mode (csrc/swb_masks.cuh).
+
+  Slots: in a BatchedEnvironment, S is n_slots and k is slot k of SpriteFactors.render_batch; on a
+  sprite list (`render`, the drop-in Environment), k is the list index.  SpriteMasks' arguments
+  and limits, and anti_aliasing at most 15, so that the aa**2 samples of a pixel fit a byte."""
+
+  def __init__(self, image_size=(64, 64), anti_aliasing=1):
+    _check_mask_raster(self, image_size, anti_aliasing)
+    if self._anti_aliasing > 15:
+      raise ValueError('anti_aliasing %d exceeds 15: a pixel\'s anti_aliasing**2 sample count must '
+                       'fit a uint8' % self._anti_aliasing)
+    self._num_sprites = 0
+
+  @property
+  def width(self):
+    return self._image_size[0]
+
+  @property
+  def height(self):
+    return self._image_size[1]
+
+  @property
+  def anti_aliasing(self):
+    return self._anti_aliasing
+
+  def _spec(self, n):
+    return specs.BoundedArray(shape=(n, self.height, self.width), dtype=np.uint8, minimum=0,
+                              maximum=self._anti_aliasing ** 2)
+
+  def render(self, sprites=(), global_state=None):
+    from spriteworld_b200 import _direct
+    self._num_sprites = len(sprites)
+    return _direct.render_soft_masks(self, list(sprites))
+
+  def observation_spec(self):
+    """The spec of the last render's sprite count (as SpriteFactors')."""
+    return self._spec(self._num_sprites)
+
+  def render_batch(self, env, res):
+    """Batched form: uint8 (n_envs, n_slots, H, W) device tensor, a buffer of `env` that every step
+    (and env.render()) overwrites, as it does the frames."""
+    return env.render_soft_masks(self)
+
+  def render_states(self, env, states):
+    """The soft masks of env records (EnvStates) without loading them: a new uint8 (n, n_slots, H,
+    W) tensor."""
+    return env.render_soft_masks(self, states)
 
   def batch_observation_spec(self, env):
     return self._spec(env.engine.n_slots)

@@ -1,0 +1,125 @@
+"""CPU restatement of the soft sprite masks (renderers.SoftSpriteMasks, the mask kernel's soft mode
+in csrc/swb_masks.cuh): test infrastructure, built on the oracle's Pillow polygon fill
+(oracle.polygon_fill, the restatement tests/test_oracle_raster.py pins against Pillow), as
+tests/mask_oracle.py is.
+
+The definition, in Pillow: the label canvas of mask_oracle.pillow_masks (every sprite back to
+front, fill k + 1, into a zero 'L' canvas of aa*W x aa*H pixels) before its resize;
+L = np.flipud(canvas).reshape(H, aa, W, aa); soft[k] = (L == k + 1).sum((1, 3)).
+"""
+import numpy as np
+
+from oracle import oracle
+from spriteworld_b200 import engine as _engine
+from tests import coverage_oracle, mask_oracle
+
+_ENGINE_RENDER_SOFT_MASKS = _engine.Engine.render_soft_masks   # the real one, whatever a test patches later
+
+
+def block_counts(labels, n_slots, W, H, aa):
+  """(n_slots, H, W) uint8 counts of labels k + 1 in each aa x aa block of an (aa H, aa W) label
+  canvas whose rows are already flipped."""
+  L = np.asarray(labels).reshape(H, aa, W, aa)
+  out = np.zeros((n_slots, H, W), np.uint8)
+  for k in range(n_slots):
+    out[k] = (L == k + 1).sum((1, 3))
+  return out
+
+
+def render_soft_masks(raster_cfg, tab, sprites):
+  """sprites: 1-D oracle.SPRITE_DTYPE array, one per slot (back to front).  Returns the (S, H, W)
+  uint8 soft masks: per slot, the canvas pixels of each pixel's aa x aa block where it is top-most."""
+  aa, W, H = raster_cfg.anti_aliasing, raster_cfg.width, raster_cfg.height
+  sprites = np.asarray(sprites, oracle.SPRITE_DTYPE).reshape(-1)
+  assert aa <= 15 and len(sprites) <= 32
+  canvas = np.zeros((aa * H, aa * W, 3), np.uint8)
+  for s, sp in enumerate(sprites):
+    if sp['shape']:
+      oracle.polygon_fill(canvas, mask_oracle.canvas_vertices(raster_cfg, tab, sp), (s + 1, 0, 0))
+  return block_counts(canvas[::-1, :, 0], len(sprites), W, H, aa)
+
+
+def pillow_soft_masks(sprites, width, height, anti_aliasing):
+  """The definition itself, with Pillow, on Sprite objects (back to front): (len(sprites), H, W)."""
+  from PIL import Image, ImageDraw
+  canvas = Image.new('L', (anti_aliasing * width, anti_aliasing * height), 0)
+  draw = ImageDraw.Draw(canvas)
+  for k, s in enumerate(sprites):
+    draw.polygon([tuple(v) for v in canvas.size * s.vertices], fill=k + 1)
+  return block_counts(np.flipud(np.asarray(canvas)), len(sprites), width, height, anti_aliasing)
+
+
+def check_properties(soft, mask, aa, what=()):
+  """The properties SoftSpriteMasks states against the SpriteMasks mask of the same state: at aa 1
+  soft[k] == (mask == k + 1); at any aa, mask == k + 1 implies soft[k] >= 1, mask == 0 implies a
+  background sample, and the counts of a pixel sum to at most aa**2."""
+  soft, mask = np.asarray(soft), np.asarray(mask)
+  S = soft.shape[0]
+  total = soft.astype(np.int64).sum(0)
+  assert (total <= aa * aa).all(), what
+  assert (total[mask == 0] < aa * aa).all(), what
+  for k in range(S):
+    if aa == 1:
+      assert np.array_equal(soft[k], (mask == k + 1).astype(np.uint8)), (what, k)
+    assert (soft[k][mask == k + 1] >= 1).all(), (what, k)
+
+
+# ---------------------------------------------------------------------------------------------
+# the coverage double (tests/coverage_oracle.py) with swb_render_soft_masks
+# ---------------------------------------------------------------------------------------------
+
+class _SoftLib(object):
+  """The coverage double's library plus swb_render_soft_masks."""
+
+  def __init__(self, inner):
+    self._inner = inner
+
+  def __getattr__(self, name):
+    return getattr(self._inner, name)
+
+  def swb_render_soft_masks(self, eng, width, height, aa, records, n, records_bytes, soft, stream):
+    import ctypes
+    assert min(width, height, aa) >= 1 and aa <= 15 and aa * max(width, height) <= 4095
+    assert n >= 0 and (records is not None or n == eng.n_envs)
+    assert soft.value
+    if n == 0:
+      return 0
+    S = eng.n_slots
+    scenes = coverage_oracle._scenes(eng, records, n, records_bytes)
+    out = np.ctypeslib.as_array((ctypes.c_uint8 * (n * S * height * width)).from_address(soft.value))
+    out = out.reshape(n, S, height, width)
+    rc = oracle.raster_cfg(width, height, aa)
+    for i, sprites in enumerate(scenes):
+      out[i] = render_soft_masks(rc, eng._tab, sprites)
+    eng._launches += 1
+    return 0
+
+
+def _lib_with_soft_masks():
+  CoverageOracleEngine, Raster = coverage_oracle._lib_with_coverage()
+
+  class SoftMaskOracleEngine(CoverageOracleEngine):
+    """The coverage double with swb_render_soft_masks under the real Engine.render_soft_masks."""
+
+    render_soft_masks = _ENGINE_RENDER_SOFT_MASKS
+
+    def __init__(self, *args, **kw):
+      super().__init__(*args, **kw)
+      self._lib = _SoftLib(self._lib)
+
+  return SoftMaskOracleEngine, Raster
+
+
+_DOUBLE = None
+
+
+def install(monkeypatch):
+  """Routes the package's host layer to the oracle double with masks, coverage and soft masks for
+  the duration of a test: what tests/coverage_oracle.install does, plus SoftSpriteMasks."""
+  global _DOUBLE
+  from spriteworld_b200 import engine as engine_lib
+  if _DOUBLE is None:
+    _DOUBLE = _lib_with_soft_masks()
+  coverage_oracle.install(monkeypatch)
+  monkeypatch.setattr(engine_lib, 'Engine', _DOUBLE[0])
+  monkeypatch.setattr(engine_lib, 'Raster', _DOUBLE[1])

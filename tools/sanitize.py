@@ -20,7 +20,8 @@ and int64 device ids, valid and refused (out of range either way, 2^32 + 1, repe
 so that memcheck sees that a refused id never indexes engine memory.  Then rollouts from records
 into leaves, from those leaves, and from the live envs into leaves, renders of records, the sprite
 coverage (swb_render_coverage) of live envs and records into buffers that are not 16-byte aligned,
-and an engine checkpoint saved, loaded and rendered, with a corrupt one refused.
+their soft masks (swb_render_soft_masks) into buffers at odd byte offsets, and an engine
+checkpoint saved, loaded and rendered, with a corrupt one refused.
 """
 import ctypes
 import os
@@ -122,6 +123,17 @@ def device_checked_records(torch):
       eng.render_coverage(W, H, aa, states=states, out=(cover, visible, area))
   torch.cuda.synchronize()
   print('coverage: live envs and %d leaves, %d kernel launches' % (len(res.leaves), eng.launch_count()),
+        flush=True)
+  # soft masks of the live envs and of the leaves at odd byte offsets: bands of one mask row (a
+  # 4095-wide canvas at aa 15) and of many, and zero records
+  for W, H, aa, skew in ((wl.image_size[0], wl.image_size[1], 5, 1), (13, 7, 15, 3), (273, 2, 15, 7),
+                         (1023, 3, 4, 5)):
+    for states in (None, res.leaves, res.leaves[:0]):
+      n = E if states is None else len(states)
+      flat = torch.zeros(n * S * H * W + 16, dtype=torch.uint8, device='cuda')
+      eng.render_soft_masks(W, H, aa, states=states, out=flat[skew:skew + n * S * H * W].view(n, S, H, W))
+  torch.cuda.synchronize()
+  print('soft masks: live envs and %d leaves, %d kernel launches' % (len(res.leaves), eng.launch_count()),
         flush=True)
   # an engine checkpoint round trip, and a corrupt one refused before anything is enqueued
   from spriteworld_b200 import _native
