@@ -144,30 +144,14 @@ def render(renderer, sprites):
   return frames[0].cpu().numpy()
 
 
-def render_masks(renderer, sprites):
-  """(H, W) uint8 instance mask of a Python sprite list: i + 1 where sprites[i] is visible."""
-  eng = _engine(max(1, len(sprites)), _DUMMY_ACTION, _NO_TASK, True)
-  _load(eng, sprites)
-  return eng.render_masks(renderer.width, renderer.height, renderer.anti_aliasing)[0].cpu().numpy()
-
-
-def render_coverage(renderer, sprites):
-  """Coverage of a Python sprite list: dict 'cover' (H, W) int32, bit i set where sprites[i]'s
-  polygon covers the pixel's sample point, and 'visible', 'area' (len(sprites),) int32."""
+def render_sprite_masks(renderer, sprites):
+  """A SpriteMasks, SpriteCoverage or SoftSpriteMasks observation of a Python sprite list, as NumPy
+  arrays: index i of a slot axis (and mask value i + 1) is sprites[i]."""
   n = len(sprites)
   eng = _engine(max(1, n), _DUMMY_ACTION, _NO_TASK, True)
   _load(eng, sprites)
-  cover, visible, area = eng.render_coverage(renderer.width, renderer.height, renderer.anti_aliasing)
-  S = eng.n_slots   # n slots for n >= 1 sprites, so bit i is slot i; one empty slot for none
-  return collections.OrderedDict([('cover', cover[0].cpu().numpy()), ('visible', visible[0, S - n:].cpu().numpy()),
-                                  ('area', area[0, S - n:].cpu().numpy())])
-
-
-def render_soft_masks(renderer, sprites):
-  """(len(sprites), H, W) uint8 soft masks of a Python sprite list: soft[i] counts the
-  anti-aliasing samples of each pixel where sprites[i] is the top-most sprite."""
-  n = len(sprites)
-  eng = _engine(max(1, n), _DUMMY_ACTION, _NO_TASK, True)
-  _load(eng, sprites)
-  soft = eng.render_soft_masks(renderer.width, renderer.height, renderer.anti_aliasing)
-  return soft[0, eng.n_slots - n:].cpu().numpy()   # slot i is sprites[i] for n >= 1 sprites
+  out = engine_lib._render_sprite_masks(eng, renderer._kind, renderer.width, renderer.height,
+                                       renderer.anti_aliasing)
+  rows = [t[0].cpu().numpy() for t in ((out,) if isinstance(out, torch.Tensor) else out)]
+  # n slots for n >= 1 sprites, so slot i is sprites[i]; one empty slot for none
+  return renderer._observation(rows[0] if len(rows) == 1 else rows, slice(eng.n_slots - n, None))

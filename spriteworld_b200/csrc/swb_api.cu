@@ -1158,23 +1158,46 @@ static int check_outputs(const char *fn, const Span *outs, int n_outs, const Spa
   return 0;
 }
 
-// The checks swb_render_masks, swb_render_coverage and swb_render_soft_masks make before their
-// outputs': the image sizes first (soft masks: aa <= 15), then the rows, then the grid of n rows of bands.
-static int check_mask_call(const swb_engine *eng, const char *fn, int32_t width, int32_t height,
-                           int32_t anti_aliasing, const void *records, int32_t n, uint64_t records_bytes,
-                           MaskMode mode) {
+// swb_render_masks, swb_render_coverage and swb_render_soft_masks: the image sizes first (soft masks:
+// aa <= 15), then the rows, then the grid of n rows of bands, then the outputs -- `out`, the per-pixel
+// output of the mode, and for MASK_COVER the counts, zeroed on the stream before the launch.
+template <MaskMode kMode>
+static int render_mask_call(swb_engine *eng, const char *fn, int32_t width, int32_t height, int32_t anti_aliasing,
+                            const void *records, int32_t n, uint64_t records_bytes, void *out, int32_t *visible,
+                            int32_t *area, cudaStream_t stream) {
   if (width < 1 || height < 1 || anti_aliasing < 1)
     return fail("%s: width %d, height %d and anti_aliasing %d must be >= 1", fn, width, height, anti_aliasing);
-  if (mode == MASK_SOFT && anti_aliasing > MK_SOFT_MAX_AA)
+  if (kMode == MASK_SOFT && anti_aliasing > MK_SOFT_MAX_AA)
     return fail("%s: anti_aliasing %d exceeds %d: a pixel's anti_aliasing^2 sample count must fit a uint8", fn,
                 anti_aliasing, MK_SOFT_MAX_AA);
   if ((int64_t)anti_aliasing * width > 4095 || (int64_t)anti_aliasing * height > 4095)
     return fail("%s: canvas %lld x %lld exceeds 4095 pixels per side", fn, (long long)anti_aliasing * width,
                 (long long)anti_aliasing * height);
   if (check_rows(eng, fn, "records", records, n, records_bytes, true)) return 1;
-  const MaskLayout L(eng->st.S, width, height, anti_aliasing, mode);
+  const MaskLayout L(eng->st.S, width, height, anti_aliasing, kMode);
   if ((int64_t)n * L.n_bands > INT32_MAX)
     return fail("%s: n = %d rows of %d bands each exceed 2^31 - 1 CTAs", fn, n, L.n_bands);
+  const uint64_t rb = RecordLayout(eng->st.S, eng->st.G).bytes();
+  // `out` holds a byte per pixel, a 4-byte word per pixel (MASK_COVER) or a byte per pixel and slot (MASK_SOFT)
+  const char *name = kMode == MASK_LABEL ? "masks" : kMode == MASK_COVER ? "cover" : "soft";
+  const unsigned px = kMode == MASK_COVER ? 4 : 1;
+  const uint64_t bytes = (uint64_t)n * height * width * px * (kMode == MASK_SOFT ? eng->st.S : 1);
+  const uint64_t counts = (uint64_t)n * eng->st.S * 4;
+  const Span outs[] = {{name, out, bytes, px}, {"visible", visible, counts, 4}, {"area", area, counts, 4}};
+  if (check_outputs(fn, outs, kMode == MASK_COVER ? 3 : 1, Span{"the records", records, n * rb, 16})) return 1;
+  if (n == 0) return 0;
+  CUDA_TRY(cudaSetDevice(eng->device));
+  auto kernel = records ? mask_kernel<true, kMode> : mask_kernel<false, kMode>;
+  CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, L.total));
+  if (kMode == MASK_COVER) {
+    CUDA_TRY(cudaMemsetAsync(visible, 0, (size_t)counts, stream));
+    CUDA_TRY(cudaMemsetAsync(area, 0, (size_t)counts, stream));
+  }
+  kernel<<<(unsigned)((int64_t)n * L.n_bands), MK_THREADS, L.total, stream>>>(
+      eng->st, L, static_cast<uint8_t *>(out), RenderRecords{static_cast<const unsigned char *>(records), (size_t)rb},
+      CoverCounts{visible, area});
+  eng->launches++;
+  CUDA_TRY(cudaGetLastError());
   return 0;
 }
 
@@ -1313,67 +1336,22 @@ int swb_render_states(swb_engine *eng, swb_raster *r, const void *records, int32
 }
 
 int swb_render_masks(swb_engine *eng, int32_t width, int32_t height, int32_t anti_aliasing,
-                     const void *records, int32_t n, uint64_t records_bytes, uint8_t *masks, void *stream_) {
-  static const char fn[] = "swb_render_masks";
-  if (check_mask_call(eng, fn, width, height, anti_aliasing, records, n, records_bytes, MASK_LABEL)) return 1;
-  const uint64_t rb = RecordLayout(eng->st.S, eng->st.G).bytes();
-  const Span outs[] = {{"masks", masks, (uint64_t)n * height * width, 1}};
-  if (check_outputs(fn, outs, 1, Span{"the records", records, n * rb, 16})) return 1;
-  if (n == 0) return 0;
-  const MaskLayout L(eng->st.S, width, height, anti_aliasing);
-  CUDA_TRY(cudaSetDevice(eng->device));
-  auto kernel = records ? mask_kernel<true, MASK_LABEL> : mask_kernel<false, MASK_LABEL>;
-  CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, L.total));
-  kernel<<<(unsigned)((int64_t)n * L.n_bands), MK_THREADS, L.total, static_cast<cudaStream_t>(stream_)>>>(
-      eng->st, L, masks, RenderRecords{static_cast<const unsigned char *>(records), (size_t)rb}, CoverCounts{});
-  eng->launches++;
-  CUDA_TRY(cudaGetLastError());
-  return 0;
+                     const void *records, int32_t n, uint64_t records_bytes, uint8_t *masks, void *stream) {
+  return render_mask_call<MASK_LABEL>(eng, "swb_render_masks", width, height, anti_aliasing, records, n,
+                                      records_bytes, masks, nullptr, nullptr, static_cast<cudaStream_t>(stream));
 }
 
 int swb_render_coverage(swb_engine *eng, int32_t width, int32_t height, int32_t anti_aliasing,
                         const void *records, int32_t n, uint64_t records_bytes, int32_t *cover,
-                        int32_t *visible, int32_t *area, void *stream_) {
-  static const char fn[] = "swb_render_coverage";
-  if (check_mask_call(eng, fn, width, height, anti_aliasing, records, n, records_bytes, MASK_COVER)) return 1;
-  const uint64_t rb = RecordLayout(eng->st.S, eng->st.G).bytes();
-  const Span outs[] = {{"cover", cover, (uint64_t)n * height * width * 4, 4},
-                       {"visible", visible, (uint64_t)n * eng->st.S * 4, 4},
-                       {"area", area, (uint64_t)n * eng->st.S * 4, 4}};
-  if (check_outputs(fn, outs, 3, Span{"the records", records, n * rb, 16})) return 1;
-  if (n == 0) return 0;
-  const MaskLayout L(eng->st.S, width, height, anti_aliasing, MASK_COVER);
-  CUDA_TRY(cudaSetDevice(eng->device));
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  auto kernel = records ? mask_kernel<true, MASK_COVER> : mask_kernel<false, MASK_COVER>;
-  CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, L.total));
-  CUDA_TRY(cudaMemsetAsync(visible, 0, (size_t)n * eng->st.S * 4, stream));
-  CUDA_TRY(cudaMemsetAsync(area, 0, (size_t)n * eng->st.S * 4, stream));
-  kernel<<<(unsigned)((int64_t)n * L.n_bands), MK_THREADS, L.total, stream>>>(
-      eng->st, L, reinterpret_cast<uint8_t *>(cover),
-      RenderRecords{static_cast<const unsigned char *>(records), (size_t)rb}, CoverCounts{visible, area});
-  eng->launches++;
-  CUDA_TRY(cudaGetLastError());
-  return 0;
+                        int32_t *visible, int32_t *area, void *stream) {
+  return render_mask_call<MASK_COVER>(eng, "swb_render_coverage", width, height, anti_aliasing, records, n,
+                                      records_bytes, cover, visible, area, static_cast<cudaStream_t>(stream));
 }
 
 int swb_render_soft_masks(swb_engine *eng, int32_t width, int32_t height, int32_t anti_aliasing,
-                          const void *records, int32_t n, uint64_t records_bytes, uint8_t *soft, void *stream_) {
-  static const char fn[] = "swb_render_soft_masks";
-  if (check_mask_call(eng, fn, width, height, anti_aliasing, records, n, records_bytes, MASK_SOFT)) return 1;
-  const uint64_t rb = RecordLayout(eng->st.S, eng->st.G).bytes();
-  const Span outs[] = {{"soft", soft, (uint64_t)n * eng->st.S * height * width, 1}};
-  if (check_outputs(fn, outs, 1, Span{"the records", records, n * rb, 16})) return 1;
-  if (n == 0) return 0;
-  const MaskLayout L(eng->st.S, width, height, anti_aliasing, MASK_SOFT);
-  CUDA_TRY(cudaSetDevice(eng->device));
-  auto kernel = records ? mask_kernel<true, MASK_SOFT> : mask_kernel<false, MASK_SOFT>;
-  CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, L.total));
-  kernel<<<(unsigned)((int64_t)n * L.n_bands), MK_THREADS, L.total, static_cast<cudaStream_t>(stream_)>>>(
-      eng->st, L, soft, RenderRecords{static_cast<const unsigned char *>(records), (size_t)rb}, CoverCounts{});
-  eng->launches++;
-  CUDA_TRY(cudaGetLastError());
-  return 0;
+                          const void *records, int32_t n, uint64_t records_bytes, uint8_t *soft, void *stream) {
+  return render_mask_call<MASK_SOFT>(eng, "swb_render_soft_masks", width, height, anti_aliasing, records, n,
+                                     records_bytes, soft, nullptr, nullptr, static_cast<cudaStream_t>(stream));
 }
 
 int swb_sample_contained(swb_engine *eng, const void *records, int32_t n, uint64_t records_bytes,

@@ -138,6 +138,52 @@ def _rows(engine, states, live=True):
   return len(states), _address(states.data), states.data.numel()
 
 
+# What each sprite-mask observation writes: its C-ABI call, then the name, dtype and axes of each
+# output, over n rows, S slots and H x W pixels.  Engine.render_masks, render_coverage and
+# render_soft_masks take and return one output as a tensor, several as a tuple.
+_MASK_KINDS = {
+    'masks': ('swb_render_masks', (('masks', torch.uint8, 'nHW'),)),
+    'coverage': ('swb_render_coverage', (('cover', torch.int32, 'nHW'), ('visible', torch.int32, 'nS'),
+                                         ('area', torch.int32, 'nS'))),
+    'soft': ('swb_render_soft_masks', (('soft', torch.uint8, 'nSHW'),)),
+}
+
+
+def _mask_outputs(kind, n, n_slots, height, width):
+  """[(name, dtype, shape)] of the outputs of sprite-mask observation `kind` for n rows."""
+  size = dict(n=n, S=n_slots, H=height, W=width)
+  return [(name, dtype, tuple(size[a] for a in axes)) for name, dtype, axes in _MASK_KINDS[kind][1]]
+
+
+def _new_mask_outputs(engine, kind, n, width, height):
+  """New tensors on `engine`'s device for what sprite-mask observation `kind` writes for n rows, in
+  the form its call takes as `out`."""
+  t = [torch.empty(shape, dtype=dtype, device=engine.device)
+       for _, dtype, shape in _mask_outputs(kind, n, engine.n_slots, max(int(height), 0), max(int(width), 0))]
+  return t[0] if len(t) == 1 else tuple(t)
+
+
+def _render_sprite_masks(engine, kind, width, height, anti_aliasing=1, states=None, out=None):
+  """The body of Engine.render_masks, render_coverage and render_soft_masks, for observation `kind`."""
+  n, rec, rec_bytes = _rows(engine, states)
+  W, H, aa = int(width), int(height), int(anti_aliasing)
+  spec = _mask_outputs(kind, n, engine.n_slots, H, W)
+  if out is None:
+    out = _new_mask_outputs(engine, kind, n, W, H)
+  elif len(spec) == 1:
+    _check_output(out, *spec[0], engine.device)
+  else:
+    if not isinstance(out, (tuple, list)) or len(out) != len(spec):
+      raise ValueError('out must be a (%s) triple, got %s' % (', '.join(s[0] for s in spec), type(out).__name__))
+    for t, s in zip(out, spec):
+      _check_output(t, *s, engine.device)
+    out = tuple(out)
+  call = getattr(engine._lib, _MASK_KINDS[kind][0])
+  _native.check(call(engine._h, W, H, aa, rec, n, rec_bytes,
+                     *[_address(t) for t in ((out,) if len(spec) == 1 else out)], engine._stream()))
+  return out
+
+
 def host_actions(kind, actions):
   """Host actions (array-like, one row per env) as a contiguous array the engine accepts.
   SelectMove / DragAndDrop: float32 stays float32, anything else becomes float64.  Embodied: int32
@@ -446,15 +492,7 @@ class Engine(object):
     n_envs), or with `states` of EnvStates of any n records, as if loaded.  Into `out` if given
     (a contiguous uint8 tensor of that shape on this device), else a new tensor.  One launch on the
     current stream; nothing else changes."""
-    n, rec, rec_bytes = _rows(self, states)
-    W, H, aa = int(width), int(height), int(anti_aliasing)
-    if out is None:
-      out = torch.empty((n, max(H, 0), max(W, 0)), dtype=torch.uint8, device=self.device)
-    else:
-      _check_output(out, 'masks', torch.uint8, (n, H, W), self.device)
-    _native.check(self._lib.swb_render_masks(self._h, W, H, aa, rec, n, rec_bytes, _address(out),
-                                             self._stream()))
-    return out
+    return _render_sprite_masks(self, 'masks', width, height, anti_aliasing, states, out)
 
   def render_coverage(self, width, height, anti_aliasing=1, states=None, out=None):
     """Amodal sprite coverage (swb_render_coverage): (cover, visible, area), int32 (n, height,
@@ -465,22 +503,7 @@ class Engine(object):
     Of the live envs (n = n_envs), or with `states` of EnvStates of any n records, as if loaded.
     Into `out` if given (a triple of contiguous int32 tensors of those shapes on this device), else
     new tensors.  One launch on the current stream (after zeroing the counts); nothing else changes."""
-    n, rec, rec_bytes = _rows(self, states)
-    W, H, aa = int(width), int(height), int(anti_aliasing)
-    shapes = ((n, H, W), (n, self.n_slots), (n, self.n_slots))
-    if out is None:
-      out = (torch.empty((n, max(H, 0), max(W, 0)), dtype=torch.int32, device=self.device),
-             torch.empty(shapes[1], dtype=torch.int32, device=self.device),
-             torch.empty(shapes[2], dtype=torch.int32, device=self.device))
-    else:
-      if not isinstance(out, (tuple, list)) or len(out) != 3:
-        raise ValueError('out must be a (cover, visible, area) triple, got %s' % type(out).__name__)
-      for name, t, shape in zip(('cover', 'visible', 'area'), out, shapes):
-        _check_output(t, name, torch.int32, shape, self.device)
-      out = tuple(out)
-    _native.check(self._lib.swb_render_coverage(self._h, W, H, aa, rec, n, rec_bytes,
-                                                *[_address(t) for t in out], self._stream()))
-    return out
+    return _render_sprite_masks(self, 'coverage', width, height, anti_aliasing, states, out)
 
   def render_soft_masks(self, width, height, anti_aliasing=1, states=None, out=None):
     """Soft sprite masks (swb_render_soft_masks): uint8 (n, n_slots, height, width), where
@@ -491,15 +514,7 @@ class Engine(object):
     n_envs), or with `states` of EnvStates of any n records, as if loaded.  Into `out` if given (a
     contiguous uint8 tensor of that shape on this device), else a new tensor.  One launch on the
     current stream; nothing else changes."""
-    n, rec, rec_bytes = _rows(self, states)
-    W, H, aa = int(width), int(height), int(anti_aliasing)
-    if out is None:
-      out = torch.empty((n, self.n_slots, max(H, 0), max(W, 0)), dtype=torch.uint8, device=self.device)
-    else:
-      _check_output(out, 'soft', torch.uint8, (n, self.n_slots, H, W), self.device)
-    _native.check(self._lib.swb_render_soft_masks(self._h, W, H, aa, rec, n, rec_bytes, _address(out),
-                                                  self._stream()))
-    return out
+    return _render_sprite_masks(self, 'soft', width, height, anti_aliasing, states, out)
 
   def render_status(self):
     """Zero-copy uint8 (E,) view of the per-env status of the last render() (ENV_SPAN_OVERFLOW)."""

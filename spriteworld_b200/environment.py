@@ -363,20 +363,13 @@ class BatchedEnvironment(object):
         (name, engine_lib.Raster(self._engine, r.width, r.height, r.anti_aliasing, r.bg_color))
         for name, r in self._pil.items())
     self._frames = {name: r.new_frames() for name, r in self._rasters.items()}
-    # one mask buffer per SpriteMasks renderer, overwritten every step like the frames
+    # the outputs of each SpriteMasks, SpriteCoverage and SoftSpriteMasks renderer by id(renderer),
+    # overwritten every step like the frames: one dict, also under the coverage and soft-mask buffer
+    # names the test suite reads them by
     self._mask_buffers = {
-        id(r): torch.empty((E, r.height, r.width), dtype=torch.uint8, device=self._engine.device)
-        for r in self._other.values() if isinstance(r, handcrafted.SpriteMasks)}
-    # and one (cover, visible, area) per SpriteCoverage renderer
-    self._coverage_buffers = {
-        id(r): (torch.empty((E, r.height, r.width), dtype=torch.int32, device=self._engine.device),
-                torch.empty((E, slots), dtype=torch.int32, device=self._engine.device),
-                torch.empty((E, slots), dtype=torch.int32, device=self._engine.device))
-        for r in self._other.values() if isinstance(r, handcrafted.SpriteCoverage)}
-    # and one (n_envs, n_slots, H, W) soft mask per SoftSpriteMasks renderer
-    self._soft_buffers = {
-        id(r): torch.empty((E, slots, r.height, r.width), dtype=torch.uint8, device=self._engine.device)
-        for r in self._other.values() if isinstance(r, handcrafted.SoftSpriteMasks)}
+        id(r): engine_lib._new_mask_outputs(self._engine, r._kind, E, r.width, r.height)
+        for r in self._other.values() if isinstance(r, handcrafted._SpriteMaskRenderer)}
+    self._coverage_buffers = self._soft_buffers = self._mask_buffers
     if sampler == 'device':
       self._init_device_sampler(seed, env_offset)
       return
@@ -885,43 +878,37 @@ class BatchedEnvironment(object):
     for name, r in self._rasters.items():
       out[name] = self._engine.render(r, self._frames[name])
     for name, r in self._other.items():
-      if isinstance(r, handcrafted.SpriteMasks):
-        out[name] = self.render_masks(r)
-      elif isinstance(r, handcrafted.SpriteCoverage):
-        out[name] = self.render_coverage(r)
-      elif isinstance(r, handcrafted.SoftSpriteMasks):
-        out[name] = self.render_soft_masks(r)
+      if isinstance(r, handcrafted._SpriteMaskRenderer):
+        out[name] = self._render_sprite_masks(type(r), r)
     return out
+
+  def _render_sprite_masks(self, cls, renderer, states=None):
+    """`renderer`'s observation as a `cls` (SpriteMasks, SpriteCoverage or SoftSpriteMasks) on the
+    current stream: of the live envs into this environment's buffers for the renderer (new tensors
+    for a renderer it does not own), or of EnvStates `states` into new tensors."""
+    # only a renderer of this kind has buffers of this kind's form
+    out = self._mask_buffers.get(id(renderer)) if states is None and isinstance(renderer, cls) else None
+    return cls._observation(engine_lib._render_sprite_masks(
+        self._engine, cls._kind, renderer.width, renderer.height, renderer.anti_aliasing, states=states, out=out))
 
   def render_masks(self, renderer, states=None):
     """SpriteMasks `renderer`'s masks (Engine.render_masks) on the current stream: of the live envs
     into this environment's buffer for the renderer (a new tensor for a renderer it does not own),
     or of EnvStates `states` into a new uint8 (n, H, W) tensor."""
-    dims = (renderer.width, renderer.height, renderer.anti_aliasing)
-    if states is not None:
-      return self._engine.render_masks(*dims, states=states)
-    return self._engine.render_masks(*dims, out=self._mask_buffers.get(id(renderer)))
+    return self._render_sprite_masks(handcrafted.SpriteMasks, renderer, states)
 
   def render_coverage(self, renderer, states=None):
     """SpriteCoverage `renderer`'s observation (Engine.render_coverage) on the current stream: dict
     'cover' int32 (n, H, W), 'visible' and 'area' int32 (n, n_slots).  Of the live envs into this
     environment's buffers for the renderer (new tensors for a renderer it does not own), or of
     EnvStates `states` into new tensors."""
-    dims = (renderer.width, renderer.height, renderer.anti_aliasing)
-    if states is not None:
-      out = self._engine.render_coverage(*dims, states=states)
-    else:
-      out = self._engine.render_coverage(*dims, out=self._coverage_buffers.get(id(renderer)))
-    return collections.OrderedDict(zip(('cover', 'visible', 'area'), out))
+    return self._render_sprite_masks(handcrafted.SpriteCoverage, renderer, states)
 
   def render_soft_masks(self, renderer, states=None):
     """SoftSpriteMasks `renderer`'s soft masks (Engine.render_soft_masks) on the current stream: of
     the live envs into this environment's buffer for the renderer (a new tensor for a renderer it
     does not own), or of EnvStates `states` into a new uint8 (n, n_slots, H, W) tensor."""
-    dims = (renderer.width, renderer.height, renderer.anti_aliasing)
-    if states is not None:
-      return self._engine.render_soft_masks(*dims, states=states)
-    return self._engine.render_soft_masks(*dims, out=self._soft_buffers.get(id(renderer)))
+    return self._render_sprite_masks(handcrafted.SoftSpriteMasks, renderer, states)
 
   def observe(self, states):
     """The observations of env records without loading them: (observation, status) for EnvStates

@@ -70,19 +70,62 @@ class SpriteFactors(abstract_renderer.AbstractRenderer):
     return spec
 
 
-def _check_mask_raster(renderer, image_size, anti_aliasing):
-  """SpriteMasks', SpriteCoverage's and SoftSpriteMasks' arguments: sets _image_size and
-  _anti_aliasing."""
-  renderer._image_size = tuple(int(v) for v in image_size)
-  renderer._anti_aliasing = int(anti_aliasing)
-  if len(renderer._image_size) != 2 or min(renderer._image_size) < 1 or renderer._anti_aliasing < 1:
-    raise ValueError('image_size must be (width, height) >= 1 and anti_aliasing >= 1, got %r, %r'
-                     % (image_size, anti_aliasing))
-  if renderer._anti_aliasing * max(renderer._image_size) > 4095:
-    raise ValueError('the canvas (anti_aliasing * image_size) exceeds 4095 pixels per side')
+class _SpriteMaskRenderer(abstract_renderer.AbstractRenderer):
+  """What SpriteMasks, SpriteCoverage and SoftSpriteMasks share: image_size=(W, H) and
+  anti_aliasing, whose canvas may not exceed 4095 pixels per side, drawn by the mask kernel as
+  observation `_kind` (engine._render_sprite_masks); `_observation` shapes what it writes
+  and `_spec(n)` describes that for n sprites."""
+
+  def __init__(self, image_size=(64, 64), anti_aliasing=1):
+    self._image_size = tuple(int(v) for v in image_size)
+    self._anti_aliasing = int(anti_aliasing)
+    if len(self._image_size) != 2 or min(self._image_size) < 1 or self._anti_aliasing < 1:
+      raise ValueError('image_size must be (width, height) >= 1 and anti_aliasing >= 1, got %r, %r'
+                       % (image_size, anti_aliasing))
+    if self._anti_aliasing * max(self._image_size) > 4095:
+      raise ValueError('the canvas (anti_aliasing * image_size) exceeds 4095 pixels per side')
+    self._num_sprites = 0
+
+  @property
+  def width(self):
+    return self._image_size[0]
+
+  @property
+  def height(self):
+    return self._image_size[1]
+
+  @property
+  def anti_aliasing(self):
+    return self._anti_aliasing
+
+  @staticmethod
+  def _observation(out, slots=slice(None)):
+    """The observation of the engine's outputs `out`, keeping `slots` of any slot axis."""
+    return out
+
+  def render(self, sprites=(), global_state=None):
+    from spriteworld_b200 import _direct
+    self._num_sprites = len(sprites)
+    return _direct.render_sprite_masks(self, list(sprites))
+
+  def observation_spec(self):
+    """The spec of the last render's sprite count (as SpriteFactors')."""
+    return self._spec(self._num_sprites)
+
+  def render_batch(self, env, res):
+    """Batched form: the observation of every env, in buffers of `env` that every step (and
+    env.render()) overwrites, as it does the frames."""
+    return env._render_sprite_masks(type(self), self)
+
+  def render_states(self, env, states):
+    """The observation of env records (EnvStates) without loading them, in new tensors."""
+    return env._render_sprite_masks(type(self), self, states)
+
+  def batch_observation_spec(self, env):
+    return self._spec(env.engine.n_slots)
 
 
-class SpriteMasks(abstract_renderer.AbstractRenderer):
+class SpriteMasks(_SpriteMaskRenderer):
   """Instance masks: which sprite is visible at each pixel of a PILRenderer frame.
 
   Observes uint8 (H, W) for image_size=(W, H) (width, height as PILRenderer hands them to Pillow):
@@ -97,43 +140,13 @@ class SpriteMasks(abstract_renderer.AbstractRenderer):
   list (`render`, the drop-in Environment), indices into the list.  Any anti_aliasing is accepted
   whose canvas sides stay within 4095 pixels."""
 
-  def __init__(self, image_size=(64, 64), anti_aliasing=1):
-    _check_mask_raster(self, image_size, anti_aliasing)
-    self._observation_spec = specs.Array(shape=(self.height, self.width), dtype=np.uint8)
+  _kind = 'masks'
 
-  @property
-  def width(self):
-    return self._image_size[0]
-
-  @property
-  def height(self):
-    return self._image_size[1]
-
-  @property
-  def anti_aliasing(self):
-    return self._anti_aliasing
-
-  def render(self, sprites=(), global_state=None):
-    from spriteworld_b200 import _direct
-    return _direct.render_masks(self, list(sprites))
-
-  def observation_spec(self):
-    return self._observation_spec
-
-  def render_batch(self, env, res):
-    """Batched form: uint8 (n_envs, H, W) device tensor, a buffer of `env` that every step (and
-    env.render()) overwrites, as it does the frames."""
-    return env.render_masks(self)
-
-  def render_states(self, env, states):
-    """The masks of env records (EnvStates) without loading them: a new uint8 (n, H, W) tensor."""
-    return env.render_masks(self, states)
-
-  def batch_observation_spec(self, env):
-    return self._observation_spec
+  def _spec(self, n):
+    return specs.Array(shape=(self.height, self.width), dtype=np.uint8)
 
 
-class SpriteCoverage(abstract_renderer.AbstractRenderer):
+class SpriteCoverage(_SpriteMaskRenderer):
   """Amodal sprite coverage: every sprite covering each pixel of a PILRenderer frame, hidden or not,
   with per-sprite visible and total pixel counts.
 
@@ -155,21 +168,7 @@ class SpriteCoverage(abstract_renderer.AbstractRenderer):
   on a sprite list (`render`, the drop-in Environment), bit i is sprites[i].  The same arguments
   and limits as SpriteMasks."""
 
-  def __init__(self, image_size=(64, 64), anti_aliasing=1):
-    _check_mask_raster(self, image_size, anti_aliasing)
-    self._num_sprites = 0
-
-  @property
-  def width(self):
-    return self._image_size[0]
-
-  @property
-  def height(self):
-    return self._image_size[1]
-
-  @property
-  def anti_aliasing(self):
-    return self._anti_aliasing
+  _kind = 'coverage'
 
   def _spec(self, n):
     i32, npx = np.iinfo(np.int32), self.height * self.width
@@ -179,30 +178,13 @@ class SpriteCoverage(abstract_renderer.AbstractRenderer):
         ('visible', specs.BoundedArray(shape=(n,), dtype=np.int32, minimum=0, maximum=npx)),
         ('area', specs.BoundedArray(shape=(n,), dtype=np.int32, minimum=0, maximum=npx))])
 
-  def render(self, sprites=(), global_state=None):
-    from spriteworld_b200 import _direct
-    self._num_sprites = len(sprites)
-    return _direct.render_coverage(self, list(sprites))
-
-  def observation_spec(self):
-    """The spec of the last render's sprite count (as SpriteFactors')."""
-    return self._spec(self._num_sprites)
-
-  def render_batch(self, env, res):
-    """Batched form: dict 'cover' int32 (n_envs, H, W), 'visible' and 'area' int32 (n_envs,
-    n_slots) device tensors, buffers of `env` that every step (and env.render()) overwrites, as it
-    does the frames."""
-    return env.render_coverage(self)
-
-  def render_states(self, env, states):
-    """The coverage of env records (EnvStates) without loading them, in new tensors."""
-    return env.render_coverage(self, states)
-
-  def batch_observation_spec(self, env):
-    return self._spec(env.engine.n_slots)
+  @staticmethod
+  def _observation(out, slots=slice(None)):
+    cover, visible, area = out
+    return collections.OrderedDict([('cover', cover), ('visible', visible[..., slots]), ('area', area[..., slots])])
 
 
-class SoftSpriteMasks(abstract_renderer.AbstractRenderer):
+class SoftSpriteMasks(_SpriteMaskRenderer):
   """Soft instance masks: how much of each pixel of a PILRenderer frame each sprite owns.
 
   Observes uint8 (S, H, W) for image_size=(W, H) and S sprites: soft[k, i, j] is the number of
@@ -224,50 +206,21 @@ class SoftSpriteMasks(abstract_renderer.AbstractRenderer):
   sprite list (`render`, the drop-in Environment), k is the list index.  SpriteMasks' arguments
   and limits, and anti_aliasing at most 15, so that the aa**2 samples of a pixel fit a byte."""
 
+  _kind = 'soft'
+
   def __init__(self, image_size=(64, 64), anti_aliasing=1):
-    _check_mask_raster(self, image_size, anti_aliasing)
+    super().__init__(image_size, anti_aliasing)
     if self._anti_aliasing > 15:
       raise ValueError('anti_aliasing %d exceeds 15: a pixel\'s anti_aliasing**2 sample count must '
                        'fit a uint8' % self._anti_aliasing)
-    self._num_sprites = 0
-
-  @property
-  def width(self):
-    return self._image_size[0]
-
-  @property
-  def height(self):
-    return self._image_size[1]
-
-  @property
-  def anti_aliasing(self):
-    return self._anti_aliasing
 
   def _spec(self, n):
     return specs.BoundedArray(shape=(n, self.height, self.width), dtype=np.uint8, minimum=0,
                               maximum=self._anti_aliasing ** 2)
 
-  def render(self, sprites=(), global_state=None):
-    from spriteworld_b200 import _direct
-    self._num_sprites = len(sprites)
-    return _direct.render_soft_masks(self, list(sprites))
-
-  def observation_spec(self):
-    """The spec of the last render's sprite count (as SpriteFactors')."""
-    return self._spec(self._num_sprites)
-
-  def render_batch(self, env, res):
-    """Batched form: uint8 (n_envs, n_slots, H, W) device tensor, a buffer of `env` that every step
-    (and env.render()) overwrites, as it does the frames."""
-    return env.render_soft_masks(self)
-
-  def render_states(self, env, states):
-    """The soft masks of env records (EnvStates) without loading them: a new uint8 (n, n_slots, H,
-    W) tensor."""
-    return env.render_soft_masks(self, states)
-
-  def batch_observation_spec(self, env):
-    return self._spec(env.engine.n_slots)
+  @staticmethod
+  def _observation(out, slots=slice(None)):
+    return out[..., slots, :, :]
 
 
 class GoalPositions(abstract_renderer.AbstractRenderer):

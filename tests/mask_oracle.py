@@ -11,7 +11,7 @@ import numpy as np
 from oracle import oracle
 from spriteworld_b200 import engine as _engine
 
-_ENGINE_RENDER_MASKS = _engine.Engine.render_masks   # the real one, whatever a test patches later
+_Engine = _engine.Engine   # the real one, whatever a test patches later
 
 
 def canvas_vertices(raster_cfg, tab, sprite):
@@ -75,52 +75,68 @@ def huge_scene_arrays(rng, E, S, CH):
 
 
 # ---------------------------------------------------------------------------------------------
-# the oracle-backed engine double (tests/oracle_engine.py) with env records and swb_render_masks
+# the oracle-backed engine double (tests/oracle_engine.py) with env records, swb_render_masks,
+# swb_render_coverage and swb_render_soft_masks
 # ---------------------------------------------------------------------------------------------
 
 def _lib_with_masks():
   import ctypes
 
-  import torch
-
-  from spriteworld_b200 import engine as engine_lib
+  from tests import coverage_oracle, oracle_engine, soft_mask_oracle
   from tests import test_render_states_on_oracle as rs
-  from tests.test_expand_on_oracle import _POOL_FIELDS
 
   class MaskLib(rs._RenderLib):
 
-    def swb_render_masks(self, eng, width, height, aa, records, n, records_bytes, masks, stream):
+    def _draw(self, eng, width, height, aa, records, n, records_bytes, outs, render):
+      """A mask call: outs are (ctypes pointer, ctypes type, shape of one row) of each output, and
+      render(raster_cfg, tab, sprites) gives one row of each (a tuple of several)."""
       assert min(width, height, aa) >= 1 and aa * max(width, height) <= 4095
       assert n >= 0 and (records is not None or n == eng.n_envs)
+      spans = [(p.value, ctypes.sizeof(ct), n * int(np.prod(shape)) * ctypes.sizeof(ct)) for p, ct, shape in outs]
+      for i, (p, align, nb) in enumerate(spans):
+        assert p and p % align == 0
+        for q, _, mb in spans[:i]:
+          assert not (p < q + mb and q < p + nb), 'outputs overlap'
       if n == 0:
         return 0
       if records is None:
         scenes = [eng._bo.cur[e] for e in range(n)]
       else:
         assert records_bytes >= n * eng.record_bytes
-        rec = np.ctypeslib.as_array((ctypes.c_uint8 * (n * eng.record_bytes)).from_address(records.value))
-        h = engine_lib.EnvStates(torch.from_numpy(rec.reshape(n, -1).copy()), 1, eng.signature,
-                                 eng.n_slots).to_host()
-        scenes = []
-        for i in range(n):
-          sprites = np.zeros(eng.n_slots, oracle.SPRITE_DTYPE)
-          for f, g in _POOL_FIELDS:
-            sprites[f] = h[g][i]
-          sprites['x'], sprites['y'] = h['pos_x'][i], h['pos_y'][i]
-          sprites['shape'] = rs._SHAPE_IDS[sprites['shape']]
-          scenes.append(sprites)
-      out = np.ctypeslib.as_array((ctypes.c_uint8 * (n * height * width)).from_address(masks.value))
-      out = out.reshape(n, height, width)
+        scenes = oracle_engine.record_sprites(eng, oracle_engine.states_at(eng, records, n))
+      views = [np.ctypeslib.as_array((ct * (n * int(np.prod(shape)))).from_address(p.value)).reshape((n,) + shape)
+               for p, ct, shape in outs]
       rc = oracle.raster_cfg(width, height, aa)
       for i, sprites in enumerate(scenes):
-        out[i] = render_masks(rc, eng._tab, sprites)
+        rows = render(rc, eng._tab, sprites)
+        for view, row in zip(views, rows if isinstance(rows, tuple) else (rows,)):
+          view[i] = row
       eng._launches += 1
       return 0
 
-  class MaskOracleEngine(rs.RenderStatesOracleEngine):
-    """The records double with swb_render_masks under the real Engine.render_masks."""
+    def swb_render_masks(self, eng, width, height, aa, records, n, records_bytes, masks, stream):
+      return self._draw(eng, width, height, aa, records, n, records_bytes,
+                        [(masks, ctypes.c_uint8, (height, width))], render_masks)
 
-    render_masks = _ENGINE_RENDER_MASKS
+    def swb_render_coverage(self, eng, width, height, aa, records, n, records_bytes, cover, visible, area,
+                            stream):
+      S = eng.n_slots
+      return self._draw(eng, width, height, aa, records, n, records_bytes,
+                        [(cover, ctypes.c_int32, (height, width)), (visible, ctypes.c_int32, (S,)),
+                         (area, ctypes.c_int32, (S,))], coverage_oracle.render_coverage)
+
+    def swb_render_soft_masks(self, eng, width, height, aa, records, n, records_bytes, soft, stream):
+      assert aa <= 15
+      return self._draw(eng, width, height, aa, records, n, records_bytes,
+                        [(soft, ctypes.c_uint8, (eng.n_slots, height, width))], soft_mask_oracle.render_soft_masks)
+
+  class MaskOracleEngine(rs.RenderStatesOracleEngine):
+    """The records double with the mask calls under the real Engine.render_masks, render_coverage
+    and render_soft_masks."""
+
+    render_masks = _Engine.render_masks
+    render_coverage = _Engine.render_coverage
+    render_soft_masks = _Engine.render_soft_masks
 
     def __init__(self, *args, **kw):
       super().__init__(*args, **kw)
@@ -133,9 +149,9 @@ _DOUBLE = None
 
 
 def install(monkeypatch):
-  """Routes the package's host layer to the oracle double with masks (and env records, and
-  swb_render_states) for the duration of a test: what tests/oracle_engine.install does, plus
-  SpriteMasks."""
+  """Routes the package's host layer to the oracle double with SpriteMasks, SpriteCoverage and
+  SoftSpriteMasks (and env records, and swb_render_states) for the duration of a test: what
+  tests/oracle_engine.install does, plus the mask calls."""
   global _DOUBLE
   from spriteworld_b200 import engine as engine_lib
   from tests import oracle_engine

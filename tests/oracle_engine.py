@@ -13,11 +13,35 @@ import numpy as np
 import torch
 
 from oracle import oracle
-from spriteworld_b200 import _native
+from spriteworld_b200 import _native, constants
 from spriteworld_b200 import engine as engine_lib
 from tests import fixtures
 
 _FIELDS = ('x', 'y', 'm00', 'm01', 'm10', 'm11', 'vx', 'vy', 'member', 'shape', 'pos_f32', 'rgb')
+# (oracle sprite field, env record field) of each field of a scene's sprites
+_POOL_FIELDS = (('x', 'x0'), ('y', 'y0'), ('m00', 'm00'), ('m01', 'm01'), ('m10', 'm10'), ('m11', 'm11'),
+                ('vx', 'vx'), ('vy', 'vy'), ('member', 'member'), ('shape', 'shape'), ('pos_f32', 'pos_f32'),
+                ('rgb', 'rgb'))
+# the shape id an env record's shape id loads as (swb_load_envs)
+_SHAPE_IDS = engine_lib.shape_id_table(constants.SHAPES)
+
+
+def record_sprites(eng, states):
+  """oracle.SPRITE_DTYPE (n, n_slots) sprites of the n records of EnvStates `states` of engine `eng`:
+  each record's sprites at their live positions, shape ids as swb_load_envs loads them."""
+  h = states.to_host()
+  sprites = np.zeros((len(states), eng.n_slots), oracle.SPRITE_DTYPE)
+  for f, g in _POOL_FIELDS:
+    sprites[f] = h[g]
+  sprites['x'], sprites['y'] = h['pos_x'], h['pos_y']
+  sprites['shape'] = _SHAPE_IDS[sprites['shape']]
+  return sprites
+
+
+def states_at(eng, records, n):
+  """EnvStates of a copy of the n records at ctypes pointer `records`, as a double's C-ABI call gets them."""
+  rec = np.ctypeslib.as_array((ctypes.c_uint8 * (n * eng.record_bytes)).from_address(records.value))
+  return engine_lib.EnvStates(torch.from_numpy(rec.reshape(n, -1).copy()), 1, eng.signature, eng.n_slots)
 
 
 class _Lib(object):

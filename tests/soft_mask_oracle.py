@@ -10,10 +10,7 @@ L = np.flipud(canvas).reshape(H, aa, W, aa); soft[k] = (L == k + 1).sum((1, 3)).
 import numpy as np
 
 from oracle import oracle
-from spriteworld_b200 import engine as _engine
-from tests import coverage_oracle, mask_oracle
-
-_ENGINE_RENDER_SOFT_MASKS = _engine.Engine.render_soft_masks   # the real one, whatever a test patches later
+from tests import mask_oracle
 
 
 def block_counts(labels, n_slots, W, H, aa):
@@ -62,64 +59,3 @@ def check_properties(soft, mask, aa, what=()):
     if aa == 1:
       assert np.array_equal(soft[k], (mask == k + 1).astype(np.uint8)), (what, k)
     assert (soft[k][mask == k + 1] >= 1).all(), (what, k)
-
-
-# ---------------------------------------------------------------------------------------------
-# the coverage double (tests/coverage_oracle.py) with swb_render_soft_masks
-# ---------------------------------------------------------------------------------------------
-
-class _SoftLib(object):
-  """The coverage double's library plus swb_render_soft_masks."""
-
-  def __init__(self, inner):
-    self._inner = inner
-
-  def __getattr__(self, name):
-    return getattr(self._inner, name)
-
-  def swb_render_soft_masks(self, eng, width, height, aa, records, n, records_bytes, soft, stream):
-    import ctypes
-    assert min(width, height, aa) >= 1 and aa <= 15 and aa * max(width, height) <= 4095
-    assert n >= 0 and (records is not None or n == eng.n_envs)
-    assert soft.value
-    if n == 0:
-      return 0
-    S = eng.n_slots
-    scenes = coverage_oracle._scenes(eng, records, n, records_bytes)
-    out = np.ctypeslib.as_array((ctypes.c_uint8 * (n * S * height * width)).from_address(soft.value))
-    out = out.reshape(n, S, height, width)
-    rc = oracle.raster_cfg(width, height, aa)
-    for i, sprites in enumerate(scenes):
-      out[i] = render_soft_masks(rc, eng._tab, sprites)
-    eng._launches += 1
-    return 0
-
-
-def _lib_with_soft_masks():
-  CoverageOracleEngine, Raster = coverage_oracle._lib_with_coverage()
-
-  class SoftMaskOracleEngine(CoverageOracleEngine):
-    """The coverage double with swb_render_soft_masks under the real Engine.render_soft_masks."""
-
-    render_soft_masks = _ENGINE_RENDER_SOFT_MASKS
-
-    def __init__(self, *args, **kw):
-      super().__init__(*args, **kw)
-      self._lib = _SoftLib(self._lib)
-
-  return SoftMaskOracleEngine, Raster
-
-
-_DOUBLE = None
-
-
-def install(monkeypatch):
-  """Routes the package's host layer to the oracle double with masks, coverage and soft masks for
-  the duration of a test: what tests/coverage_oracle.install does, plus SoftSpriteMasks."""
-  global _DOUBLE
-  from spriteworld_b200 import engine as engine_lib
-  if _DOUBLE is None:
-    _DOUBLE = _lib_with_soft_masks()
-  coverage_oracle.install(monkeypatch)
-  monkeypatch.setattr(engine_lib, 'Engine', _DOUBLE[0])
-  monkeypatch.setattr(engine_lib, 'Raster', _DOUBLE[1])

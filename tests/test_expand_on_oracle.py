@@ -19,9 +19,6 @@ from tests.test_env_states_on_oracle import StatesOracleEngine
 from tests.test_rollout_on_oracle import RolloutOracleEngine
 
 _Engine = engine_lib.Engine   # the device engine, for its host-side checks
-_POOL_FIELDS = (('x', 'x0'), ('y', 'y0'), ('m00', 'm00'), ('m01', 'm01'), ('m10', 'm10'), ('m11', 'm11'),
-                ('vx', 'vx'), ('vy', 'vy'), ('member', 'member'), ('shape', 'shape'), ('pos_f32', 'pos_f32'),
-                ('rgb', 'rgb'))
 
 
 def _set_field(data, n_slots, name, values):
@@ -54,11 +51,8 @@ class ExpandOracleEngine(RolloutOracleEngine, StatesOracleEngine):
       _Engine.check_states(self, leaves, n * C)
     out, res = engine_lib.rollout_outputs(out, T, n, C, self.device)
     h = roots.to_host()
-    pool = np.zeros((n, 1, self.n_slots), oracle.SPRITE_DTYPE)
-    for f, g in _POOL_FIELDS:
-      pool[:, 0][f] = h[g]
+    pool = oracle_engine.record_sprites(self, roots)[:, None]   # each root at its live positions
     sub = oracle.BatchOracle(self._cfg, self._tab, None, np.repeat(pool, C, 0))
-    sub.cur['x'], sub.cur['y'] = np.repeat(h['pos_x'], C, 0), np.repeat(h['pos_y'], C, 0)
     sub.step_count[:] = np.repeat(h['step_count'], C)
     sub.reset_next[:] = 0
     live = np.repeat(h['reset_next'] == 0, C)

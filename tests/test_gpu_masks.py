@@ -20,7 +20,7 @@ import pytest
 from oracle import oracle
 from tests import mask_oracle
 from tests import test_gpu_render_geometry as geo
-from tests.test_expand_on_oracle import _POOL_FIELDS
+from tests.oracle_engine import record_sprites as _sprites_of
 
 gpu = pytest.mark.gpu
 
@@ -33,23 +33,6 @@ EXTRA = [
     ('w273h15a15', 273, 15, 15, 32, 2, True),     # canvas 4095 x 225
     ('w2h273a15', 2, 273, 15, 6, 3, False),       # canvas 30 x 4095
 ]
-
-
-def _sprites_of(eng, states):
-  """Oracle sprite arrays of env records (EnvStates), shape ids mapped to the oracle's."""
-  from spriteworld_b200 import constants
-  from spriteworld_b200 import engine as engine_lib
-  ids = engine_lib.shape_id_table(constants.SHAPES)
-  h = states.to_host()
-  out = []
-  for i in range(len(states)):
-    sp = np.zeros(eng.n_slots, oracle.SPRITE_DTYPE)
-    for f, g in _POOL_FIELDS:
-      sp[f] = h[g][i]
-    sp['x'], sp['y'] = h['pos_x'][i], h['pos_y'][i]
-    sp['shape'] = ids[sp['shape']]
-    out.append(sp)
-  return out
 
 
 def _masks_guarded(eng, W, H, aa, n, skew=0, states=None):

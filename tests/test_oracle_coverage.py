@@ -9,7 +9,7 @@
    area each bit's popcount; visible <= area, and empty or out-of-frame sprites have no bits.
 3. The host layer -- Engine.render_coverage's checks, SpriteCoverage in a BatchedEnvironment (step,
    observe, render, specs), the drop-in Environment and the gym wrappers -- on the oracle-backed
-   engine double with swb_render_coverage (tests/coverage_oracle.install).  The kernel is
+   engine double with swb_render_coverage (tests/mask_oracle.install).  The kernel is
    tests/test_gpu_coverage.py's.
 """
 import collections
@@ -139,7 +139,7 @@ def test_sprites_with_edges_beyond_int16_rows_equal_the_pillow_definition():
 
 @pytest.fixture
 def double(monkeypatch):
-  coverage_oracle.install(monkeypatch)
+  mask_oracle.install(monkeypatch)
 
 
 def _renderers(**cover):

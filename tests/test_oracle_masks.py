@@ -8,7 +8,8 @@
    mask - 1 elsewhere.
 3. The host layer -- Engine.render_masks' checks, SpriteMasks in a BatchedEnvironment (step,
    observe, render, specs) and in the gym wrappers' spaces -- on the oracle-backed engine double,
-   with swb_render_masks (tests/mask_oracle.install).  The kernel is tests/test_gpu_masks.py's.
+   with swb_render_masks, swb_render_coverage and swb_render_soft_masks (tests/mask_oracle.install).
+   The kernel is tests/test_gpu_masks.py's.
 """
 import collections
 

@@ -11,8 +11,8 @@
    are zero; soft[k].sum() is slot k's visible canvas area.
 3. The host layer -- Engine.render_soft_masks' checks, SoftSpriteMasks in a BatchedEnvironment
    (step, observe, render, specs), the drop-in Environment and the gym wrappers -- on the
-   oracle-backed engine double with swb_render_soft_masks (tests/soft_mask_oracle.install).  The
-   kernel is tests/test_gpu_soft_masks.py's.
+   oracle-backed engine double with swb_render_soft_masks (tests/mask_oracle.install).  The kernel
+   is tests/test_gpu_soft_masks.py's.
 """
 import collections
 
@@ -160,7 +160,7 @@ def test_32_nested_slots_and_mixed_pixels():
 
 @pytest.fixture
 def double(monkeypatch):
-  soft_mask_oracle.install(monkeypatch)
+  mask_oracle.install(monkeypatch)
 
 
 def _renderers(**soft):

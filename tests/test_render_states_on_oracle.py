@@ -17,14 +17,13 @@ import pytest
 import torch
 
 from oracle import oracle
-from spriteworld_b200 import _native, constants
+from spriteworld_b200 import _native
 from spriteworld_b200 import engine as engine_lib
 from tests import oracle_engine
 from tests.test_env_states_on_oracle import StatesOracleEngine
-from tests.test_expand_on_oracle import _POOL_FIELDS, _set_field
+from tests.test_expand_on_oracle import _set_field
 
 _Engine = engine_lib.Engine
-_SHAPE_IDS = engine_lib.shape_id_table(constants.SHAPES)
 
 
 def _fake_overflow(n, width):
@@ -39,20 +38,12 @@ class _RenderLib(oracle_engine._Lib):
     assert records_bytes == n * eng.record_bytes and span_class in (1, 4)
     if n == 0:
       return 0
-    rec = np.ctypeslib.as_array((ctypes.c_uint8 * records_bytes).from_address(records.value))
-    states = engine_lib.EnvStates(torch.from_numpy(rec.reshape(n, -1).copy()), span_class, eng.signature,
-                                  eng.n_slots)
-    h = states.to_host()
+    sprites = oracle_engine.record_sprites(eng, oracle_engine.states_at(eng, records, n))
     r = eng._rasters[raster]
     out = np.ctypeslib.as_array((ctypes.c_uint8 * (n * r.height * r.width * 3)).from_address(frames.value))
     out = out.reshape(n, r.height, r.width, 3)
     for i in range(n):
-      sprites = np.zeros(eng.n_slots, oracle.SPRITE_DTYPE)
-      for f, g in _POOL_FIELDS:
-        sprites[f] = h[g][i]
-      sprites['x'], sprites['y'] = h['pos_x'][i], h['pos_y'][i]
-      sprites['shape'] = _SHAPE_IDS[sprites['shape']]
-      out[i] = oracle.render(r.rc, eng._tab, sprites)
+      out[i] = oracle.render(r.rc, eng._tab, sprites[i])
     st = np.ctypeslib.as_array((ctypes.c_uint8 * n).from_address(status.value))
     st[:] = _fake_overflow(n, r.width)
     eng._launches += 1
@@ -78,8 +69,8 @@ class RenderStatesOracleEngine(StatesOracleEngine):
     super().load_envs(states, env_ids)
     ids = self._ids(env_ids, True)
     bo = self._bo
-    bo.pool['shape'][ids, bo.cursor[ids]] = _SHAPE_IDS[bo.pool['shape'][ids, bo.cursor[ids]]]
-    bo.cur['shape'][ids] = _SHAPE_IDS[bo.cur['shape'][ids]]
+    bo.pool['shape'][ids, bo.cursor[ids]] = oracle_engine._SHAPE_IDS[bo.pool['shape'][ids, bo.cursor[ids]]]
+    bo.cur['shape'][ids] = oracle_engine._SHAPE_IDS[bo.cur['shape'][ids]]
 
 
 class RenderStatesOracleRaster(oracle_engine.OracleRaster):
