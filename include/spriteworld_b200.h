@@ -335,7 +335,8 @@ int swb_upload_state(swb_engine *eng, const double *pos_x, const double *pos_y,
  * steps and frames.
  *
  * Read-only record calls (swb_rollout_states, swb_render_states, swb_render_masks,
- * swb_render_coverage, swb_render_soft_masks, swb_evaluate_states, swb_sample_contained) read n rows: n records of this
+ * swb_render_coverage, swb_render_soft_masks, swb_render_boxes, swb_evaluate_states,
+ * swb_sample_contained) read n rows: n records of this
  * engine's layout in a device record buffer of records_bytes bytes or, where a call takes them,
  * the E live envs for records == NULL, and then n == E.  Each of them is refused, enqueuing
  * nothing, for a null engine, n < 0, records == NULL where the call takes no live envs, a record
@@ -476,6 +477,28 @@ int swb_render_coverage(swb_engine *eng, int32_t width, int32_t height, int32_t 
 int swb_render_soft_masks(swb_engine *eng, int32_t width, int32_t height, int32_t anti_aliasing,
                           const void *records, int32_t n, uint64_t records_bytes, uint8_t *soft,
                           void *stream);
+
+/*
+ * Sprite bounding boxes (renderers.SpriteBoxes): the per-slot summaries of swb_render_coverage
+ * without its per-pixel output.  `visible_box` and `amodal_box` are [n][S][4] int32, `visible` and
+ * `area` [n][S] int32.  For slot k of row i, with V the pixels (r, c) where it is the top-most
+ * covering sprite (mask == k + 1 in swb_render_masks) and A those where its bit is set in
+ * swb_render_coverage's cover: visible_box = box(V), amodal_box = box(A), visible = |V| and
+ * area = |A|, where box(P) = (min c, min r, max c + 1, max r + 1) -- half-open (x0, y0, x1, y1) in
+ * pixels of the flipped image -- and (0, 0, 0, 0) for an empty P.  So the visible box lies in the
+ * amodal box, visible <= area, and a count is 0 iff its box is.  The counts equal
+ * swb_render_coverage's.  Bit 31 (slot 31) is a slot like any other.
+ *
+ * Records, sizes and n as swb_render_masks takes them (records == NULL: the E live envs, n == E).
+ * An accepted call with n > 0 zeroes the four outputs on `stream` (four memsets), then is two
+ * launches there: the mask kernel, which sends integer atomics per band and slot, and a kernel that
+ * decodes the boxes' mins.  The outputs are exact and independent of scheduling.  n == 0 enqueues
+ * nothing.  Read-only as swb_render_masks, with visible_box, amodal_box, visible and area as outputs.
+ * Refused besides: what swb_render_coverage refuses.
+ */
+int swb_render_boxes(swb_engine *eng, int32_t width, int32_t height, int32_t anti_aliasing,
+                     const void *records, int32_t n, uint64_t records_bytes, int32_t *visible_box,
+                     int32_t *amodal_box, int32_t *visible, int32_t *area, void *stream);
 
 /* Env dst_ids[i] <- env src_ids[i].  Ids in [0, E), destinations distinct.  Every read sees the
  * state from before the call, also where the two sets overlap (then the records go through

@@ -145,7 +145,7 @@ def render(renderer, sprites):
 
 
 def render_sprite_masks(renderer, sprites):
-  """A SpriteMasks, SpriteCoverage or SoftSpriteMasks observation of a Python sprite list, as NumPy
+  """A SpriteMasks, SpriteCoverage, SoftSpriteMasks or SpriteBoxes observation of a Python sprite list, as NumPy
   arrays: index i of a slot axis (and mask value i + 1) is sprites[i]."""
   n = len(sprites)
   eng = _engine(max(1, n), _DUMMY_ACTION, _NO_TASK, True)

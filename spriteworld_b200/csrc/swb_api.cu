@@ -172,7 +172,7 @@ int upload_axis(swb_raster *r, const AxisHost &h, AxisTables *d) {
 extern "C" {
 
 const char *swb_last_error(void) { return g_error.c_str(); }
-int swb_version(void) { return 14; }
+int swb_version(void) { return 15; }
 int swb_sizeof_config(void) { return (int)sizeof(swb_config); }
 int swb_sizeof_task_node(void) { return (int)sizeof(swb_task_node); }
 
@@ -1158,13 +1158,16 @@ static int check_outputs(const char *fn, const Span *outs, int n_outs, const Spa
   return 0;
 }
 
-// swb_render_masks, swb_render_coverage and swb_render_soft_masks: the image sizes first (soft masks:
-// aa <= 15), then the rows, then the grid of n rows of bands, then the outputs -- `out`, the per-pixel
-// output of the mode, and for MASK_COVER the counts, zeroed on the stream before the launch.
+// swb_render_masks, swb_render_coverage, swb_render_soft_masks and swb_render_boxes: the image sizes
+// first (soft masks: aa <= 15), then the rows, then the grid of n rows of bands, then the outputs --
+// `out`, the per-pixel output of the mode (none for MASK_BOX), MASK_BOX's two boxes, and for
+// MASK_COVER and MASK_BOX the counts.  Counts and boxes are zeroed on the stream before the launch,
+// and MASK_BOX's boxes are decoded by a second launch after it.
 template <MaskMode kMode>
 static int render_mask_call(swb_engine *eng, const char *fn, int32_t width, int32_t height, int32_t anti_aliasing,
                             const void *records, int32_t n, uint64_t records_bytes, void *out, int32_t *visible,
-                            int32_t *area, cudaStream_t stream) {
+                            int32_t *area, int32_t *visible_box, int32_t *amodal_box, cudaStream_t stream) {
+  constexpr bool counted = kMode == MASK_COVER || kMode == MASK_BOX;
   if (width < 1 || height < 1 || anti_aliasing < 1)
     return fail("%s: width %d, height %d and anti_aliasing %d must be >= 1", fn, width, height, anti_aliasing);
   if (kMode == MASK_SOFT && anti_aliasing > MK_SOFT_MAX_AA)
@@ -1182,22 +1185,44 @@ static int render_mask_call(swb_engine *eng, const char *fn, int32_t width, int3
   const char *name = kMode == MASK_LABEL ? "masks" : kMode == MASK_COVER ? "cover" : "soft";
   const unsigned px = kMode == MASK_COVER ? 4 : 1;
   const uint64_t bytes = (uint64_t)n * height * width * px * (kMode == MASK_SOFT ? eng->st.S : 1);
-  const uint64_t counts = (uint64_t)n * eng->st.S * 4;
-  const Span outs[] = {{name, out, bytes, px}, {"visible", visible, counts, 4}, {"area", area, counts, 4}};
-  if (check_outputs(fn, outs, kMode == MASK_COVER ? 3 : 1, Span{"the records", records, n * rb, 16})) return 1;
+  const uint64_t counts = (uint64_t)n * eng->st.S * 4, boxes = 4 * counts;
+  Span outs[4];
+  int n_outs = 0;
+  if (kMode == MASK_BOX) {
+    outs[n_outs++] = {"visible_box", visible_box, boxes, 4};
+    outs[n_outs++] = {"amodal_box", amodal_box, boxes, 4};
+  } else {
+    outs[n_outs++] = {name, out, bytes, px};
+  }
+  if (counted) {
+    outs[n_outs++] = {"visible", visible, counts, 4};
+    outs[n_outs++] = {"area", area, counts, 4};
+  }
+  if (check_outputs(fn, outs, n_outs, Span{"the records", records, n * rb, 16})) return 1;
   if (n == 0) return 0;
   CUDA_TRY(cudaSetDevice(eng->device));
   auto kernel = records ? mask_kernel<true, kMode> : mask_kernel<false, kMode>;
   CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, L.total));
-  if (kMode == MASK_COVER) {
+  if (counted) {
     CUDA_TRY(cudaMemsetAsync(visible, 0, (size_t)counts, stream));
     CUDA_TRY(cudaMemsetAsync(area, 0, (size_t)counts, stream));
   }
+  if (kMode == MASK_BOX) {
+    CUDA_TRY(cudaMemsetAsync(visible_box, 0, (size_t)boxes, stream));
+    CUDA_TRY(cudaMemsetAsync(amodal_box, 0, (size_t)boxes, stream));
+  }
   kernel<<<(unsigned)((int64_t)n * L.n_bands), MK_THREADS, L.total, stream>>>(
       eng->st, L, static_cast<uint8_t *>(out), RenderRecords{static_cast<const unsigned char *>(records), (size_t)rb},
-      CoverCounts{visible, area});
+      CoverCounts{visible, area, visible_box, amodal_box});
   eng->launches++;
   CUDA_TRY(cudaGetLastError());
+  if (kMode == MASK_BOX) {
+    const size_t n_boxes = (size_t)n * eng->st.S;
+    box_finish_kernel<<<(unsigned)((2 * n_boxes + BOX_FINISH_THREADS - 1) / BOX_FINISH_THREADS),
+                        BOX_FINISH_THREADS, 0, stream>>>(visible_box, amodal_box, n_boxes);
+    eng->launches++;
+    CUDA_TRY(cudaGetLastError());
+  }
   return 0;
 }
 
@@ -1338,20 +1363,31 @@ int swb_render_states(swb_engine *eng, swb_raster *r, const void *records, int32
 int swb_render_masks(swb_engine *eng, int32_t width, int32_t height, int32_t anti_aliasing,
                      const void *records, int32_t n, uint64_t records_bytes, uint8_t *masks, void *stream) {
   return render_mask_call<MASK_LABEL>(eng, "swb_render_masks", width, height, anti_aliasing, records, n,
-                                      records_bytes, masks, nullptr, nullptr, static_cast<cudaStream_t>(stream));
+                                      records_bytes, masks, nullptr, nullptr, nullptr, nullptr,
+                                      static_cast<cudaStream_t>(stream));
 }
 
 int swb_render_coverage(swb_engine *eng, int32_t width, int32_t height, int32_t anti_aliasing,
                         const void *records, int32_t n, uint64_t records_bytes, int32_t *cover,
                         int32_t *visible, int32_t *area, void *stream) {
   return render_mask_call<MASK_COVER>(eng, "swb_render_coverage", width, height, anti_aliasing, records, n,
-                                      records_bytes, cover, visible, area, static_cast<cudaStream_t>(stream));
+                                      records_bytes, cover, visible, area, nullptr, nullptr,
+                                      static_cast<cudaStream_t>(stream));
 }
 
 int swb_render_soft_masks(swb_engine *eng, int32_t width, int32_t height, int32_t anti_aliasing,
                           const void *records, int32_t n, uint64_t records_bytes, uint8_t *soft, void *stream) {
   return render_mask_call<MASK_SOFT>(eng, "swb_render_soft_masks", width, height, anti_aliasing, records, n,
-                                     records_bytes, soft, nullptr, nullptr, static_cast<cudaStream_t>(stream));
+                                     records_bytes, soft, nullptr, nullptr, nullptr, nullptr,
+                                     static_cast<cudaStream_t>(stream));
+}
+
+int swb_render_boxes(swb_engine *eng, int32_t width, int32_t height, int32_t anti_aliasing,
+                     const void *records, int32_t n, uint64_t records_bytes, int32_t *visible_box,
+                     int32_t *amodal_box, int32_t *visible, int32_t *area, void *stream) {
+  return render_mask_call<MASK_BOX>(eng, "swb_render_boxes", width, height, anti_aliasing, records, n,
+                                    records_bytes, nullptr, visible, area, visible_box, amodal_box,
+                                    static_cast<cudaStream_t>(stream));
 }
 
 int swb_sample_contained(swb_engine *eng, const void *records, int32_t n, uint64_t records_bytes,

@@ -12,7 +12,10 @@
 // top-most covering sprite (visible) and where its bit is set (area).  The soft mask (MASK_SOFT) is
 // [S][H][W] uint8: soft[k][i][j] counts the canvas pixels (aa j + u, aa (H-1-i) + v), u, v in
 // [0, aa), whose top-most covering sprite is slot k -- all aa^2 samples of the pixel, not only the
-// centre one, so aa <= 15 keeps a count in a byte.
+// centre one, so aa <= 15 keeps a count in a byte.  The boxes (MASK_BOX) are the coverage's
+// per-slot summaries without the coverage: for each slot, the half-open pixel box (x0, y0, x1, y1)
+// of the pixels where it is the top-most covering sprite (visible) and of those where its bit is
+// set (amodal), with the two counts; (0, 0, 0, 0) for no pixel.
 //
 // One CTA draws one band of mask rows of one env (or record):
 //   A  a warp per sprite, a lane per vertex: the integer canvas vertices, Pillow's edge records,
@@ -32,11 +35,18 @@
 //      Soft: a thread per mask pixel collects the labels of its aa x aa block as a 32-bit set,
 //      counts the samples of each label in it, and writes one byte to each of the S slot planes;
 //      consecutive threads take consecutive columns, so each plane's stores coalesce.
+//      Box: the staged band (painted as in MASK_COVER) never leaves the CTA.  Each warp takes
+//      32 consecutive pixels at a time; per slot present, two ballots give the amodal and visible
+//      lanes, whose first and last set lanes give the row extent (pixels are in raster order) and,
+//      where the 32 pixels lie on one row, the column extent; else __reduce_max_sync gives it.
+//      The warps combine in shared memory, and each (band, slot) sends integer atomicMax /
+//      atomicAdd to the outputs, which hold the mins as MK_BOX_KEY - min so that a zeroed output
+//      is the identity; box_finish_kernel turns them back.
 // A sprite row has at most 2 crossings per edge, 2 * SWB_MAX_VERTS in all, and every one is kept:
 // the masks are exact for every shape, and there is no overflow status.
 //
-// Nothing but the outputs (MASK_COVER: the coverage and its counts) is written, every byte of
-// them: no env, pool entry, frame or render status changes.
+// Nothing but the outputs (MASK_COVER: the coverage and its counts; MASK_BOX: the boxes and the
+// counts) is written, every byte of them: no env, pool entry, frame or render status changes.
 #pragma once
 #include <climits>
 #include <type_traits>
@@ -52,13 +62,16 @@ constexpr int MK_STAGE_BYTES = 16384;    // staged bytes per band (fewer rows fo
 constexpr int MK_SOFT_STAGE_BYTES = 32768;  // soft: staged canvas labels per band (at least one mask row's)
 constexpr int MK_SOFT_MAX_AA = 15;       // soft: aa^2 samples per pixel fit a uint8 count
 constexpr int MK_XCAP = 2 * EV;          // crossings one sprite row can have
+constexpr int MK_BOX_KEY = 4096;         // box: a min m is held as MK_BOX_KEY - m >= 2 (m <= 4094)
 
-// What the mask kernel draws: the uint8 mask, the int32 coverage and its counts, or the uint8
-// soft mask [S][H][W].
-enum MaskMode { MASK_LABEL, MASK_COVER, MASK_SOFT };
+// What the mask kernel draws: the uint8 mask, the int32 coverage and its counts, the uint8 soft
+// mask [S][H][W], or the per-slot boxes and counts of the coverage.
+enum MaskMode { MASK_LABEL, MASK_COVER, MASK_SOFT, MASK_BOX };
 
 // A mask raster and the shared-memory layout of one CTA.  MASK_COVER: staged pixels are the 4-byte
-// coverage words, and the CTA keeps per-slot counts.  MASK_SOFT: the band's aa canvas rows per mask
+// coverage words, and the CTA keeps per-slot counts.  MASK_BOX: the staged band and its rows are
+// MASK_COVER's (the staging budget and a thread per mask row), though it is never written out, and
+// the CTA keeps the counts and 8 encoded box fields per slot.  MASK_SOFT: the band's aa canvas rows per mask
 // row are staged as CW label bytes each, and band_rows * aa <= MK_THREADS (a thread per canvas row);
 // one mask row (at most 15 * 4095 bytes) is always staged, whatever MK_SOFT_STAGE_BYTES says.
 struct MaskLayout {
@@ -66,8 +79,8 @@ struct MaskLayout {
   int off_edge, off_hl, off_meta, off_xx, off_stage, total;
   __host__ __device__ MaskLayout(int S_, int W_, int H_, int aa_, MaskMode mode = MASK_LABEL)
       : S(S_), W(W_), H(H_), aa(aa_) {
-    const bool cover = mode == MASK_COVER, soft = mode == MASK_SOFT;
-    const int px = cover ? 4 : 1;         // bytes per staged pixel
+    const bool cover = mode == MASK_COVER, soft = mode == MASK_SOFT, box = mode == MASK_BOX;
+    const int px = cover || box ? 4 : 1;  // bytes per staged pixel
     CW = aa * W;
     CH = aa * H;
     if (soft) {
@@ -95,25 +108,30 @@ struct MaskLayout {
     else
       off_stage = take(band_rows * W * px + 16);  // staged band, placed at the output's address mod 16
     if (cover) take(S * 2 * 4);             // the band's visible [S], area [S] (int), at cnt_offset()
+    if (box) take(S * 10 * 4);              // and box: then the encoded boxes [8][S], see mask_kernel
     total = o;
   }
-  // cover: where the band's counts are, right after the staged band
+  // cover and box: where the band's counts are, right after the staged band
   __host__ __device__ int cnt_offset() const { return off_stage + ((band_rows * W * 4 + 16 + 15) & ~15); }
 };
 
-// The per-slot counts of the coverage, [n][S] int32 each; zeroed before the launch.
+// The per-slot counts of the coverage, [n][S] int32 each, and (MASK_BOX) its per-slot boxes,
+// [n][S][4] int32 each, encoded as box_finish_kernel reads them; all zeroed before the launch.
 struct CoverCounts {
   int32_t *visible, *area;
+  int32_t *visible_box, *amodal_box;
 };
 
 // MASK_LABEL: `masks` is the [n][H][W] uint8 mask.  MASK_COVER: `masks` is the [n][H][W] int32
 // coverage, and `counts` receives its per-slot counts.  MASK_SOFT: `masks` is the [n][S][H][W]
-// uint8 soft mask.  `counts` is read in MASK_COVER only.
+// uint8 soft mask.  MASK_BOX: `masks` is unused, and `counts` receives the counts and the encoded
+// boxes.  `counts` is read in MASK_COVER and MASK_BOX only.
 template <bool kRecords, MaskMode kMode>
 __global__ void __launch_bounds__(MK_THREADS)
 mask_kernel(DevState st, const MaskLayout L, uint8_t *__restrict__ masks, const RenderRecords recs,
             const CoverCounts counts) {
-  constexpr bool kCover = kMode == MASK_COVER, kSoft = kMode == MASK_SOFT;
+  constexpr bool kCover = kMode == MASK_COVER, kSoft = kMode == MASK_SOFT, kBox = kMode == MASK_BOX;
+  constexpr bool kBits = kCover || kBox;  // staged pixels are coverage words
   extern __shared__ __align__(16) unsigned char g_mask_smem[];
   unsigned char *const smem = g_mask_smem;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -134,7 +152,7 @@ mask_kernel(DevState st, const MaskLayout L, uint8_t *__restrict__ masks, const 
   int *s_nh = s_nv + S, *s_hasov = s_nh + S, *s_pymax = s_hasov + S;
   uint32_t *s_yext = reinterpret_cast<uint32_t *>(s_pymax + S);
   float *xx = reinterpret_cast<float *>(smem + L.off_xx) + tid;  // crossing k at xx[k * MK_THREADS]
-  using Px = std::conditional_t<kCover, uint32_t, uint8_t>;      // a staged pixel
+  using Px = std::conditional_t<kBits, uint32_t, uint8_t>;       // a staged pixel
 
   // ---- phase A: a warp per sprite, a lane per vertex / edge (render_kernel phase A) ----------
   const int cur = kRecords ? 0 : st.cursor[e];
@@ -263,14 +281,17 @@ mask_kernel(DevState st, const MaskLayout L, uint8_t *__restrict__ masks, const 
   const size_t g = (e * (size_t)L.H + (size_t)i0) * (size_t)L.W;
   const int npx = nb * L.W;
   Px *const gdst = reinterpret_cast<Px *>(masks) + g;
-  const int mis = kSoft ? 0 : (int)(reinterpret_cast<uintptr_t>(gdst) & 15u);
+  const int mis = kSoft || kBox ? 0 : (int)(reinterpret_cast<uintptr_t>(gdst) & 15u);
   Px *const stage = reinterpret_cast<Px *>(smem + L.off_stage + mis);
-  int *const s_cnt = reinterpret_cast<int *>(smem + L.cnt_offset());  // kCover: visible [S], area [S]
+  // kCover: visible [S], area [S]; kBox: then the boxes [8][S]
+  int *const s_cnt = reinterpret_cast<int *>(smem + L.cnt_offset());
   const int nstage = kSoft ? nb * L.aa * L.CW : npx;  // staged pixels
   if constexpr (kSoft)
     for (int i = tid; i < (nstage >> 4); i += MK_THREADS) reinterpret_cast<uint4 *>(stage)[i] = make_uint4(0, 0, 0, 0);
   for (int i = (kSoft ? nstage & ~15 : 0) + tid; i < nstage; i += MK_THREADS) stage[i] = 0;
   if (kCover && tid < 2 * S) s_cnt[tid] = 0;
+  if constexpr (kBox)
+    for (int i = tid; i < 10 * S; i += MK_THREADS) s_cnt[i] = 0;
   __syncthreads();
 
   // ---- phase B: a thread per mask row, its one canvas row, sprites back to front (kSoft: a
@@ -290,7 +311,7 @@ mask_kernel(DevState st, const MaskLayout L, uint8_t *__restrict__ masks, const 
       } else {
         const int jlo = (xs - half + L.aa - 1) / L.aa, jhi = (xe - half + L.aa) / L.aa - 1;
         for (int j = jlo; j <= jhi; ++j) {
-          if constexpr (kCover) row[j] |= label;
+          if constexpr (kBits) row[j] |= label;
           else row[j] = label;
         }
       }
@@ -299,7 +320,7 @@ mask_kernel(DevState st, const MaskLayout L, uint8_t *__restrict__ masks, const 
     for (int s = 0; s < S; ++s) {
       const uint32_t ext = s_yext[s];
       if (y < (int)(short)(ext & 0xFFFFu) || y > (int)(short)(ext >> 16)) continue;
-      const Px label = kCover ? (Px)(1u << s) : (Px)(s + 1);
+      const Px label = kBits ? (Px)(1u << s) : (Px)(s + 1);
       const int nv = s_nv[s], p_ymax = s_pymax[s];
       const bool hasov = s_hasov[s] != 0;
       int j = 0;
@@ -386,6 +407,79 @@ mask_kernel(DevState st, const MaskLayout L, uint8_t *__restrict__ masks, const 
     return;
   }
 
+  if constexpr (kBox) {
+    // ---- box phase C: lane s keeps slot s's counts and encoded boxes over its warp's pixels --
+    // box fields: K - x0, K - y0, x1, y1 (K = MK_BOX_KEY), all 0 while the slot has no pixel
+    constexpr int K = MK_BOX_KEY;
+    int vis = 0, area = 0, vb[4] = {0, 0, 0, 0}, ab[4] = {0, 0, 0, 0};
+    for (int p0 = warp * 32; p0 < npx; p0 += MK_THREADS) {
+      const int p = p0 + lane;
+      const uint32_t c = p < npx ? stage[p] : 0u;
+      const int top = c ? 31 - __clz(c) : -1;  // the top-most covering slot
+      const int r0 = p0 / L.W, c0 = p0 - r0 * L.W, j = p % L.W;
+      // warp-uniform: all 32 pixels are on band row r0, from column c0, so the first and last set
+      // lanes of a ballot give its columns; else (W < 32, or pixels on two rows) reductions do
+      const bool one_row = c0 + 32 <= L.W;
+      for (unsigned any = __reduce_or_sync(FULL, c); any; any &= any - 1u) {
+        const int s = __ffs(any) - 1;
+        const bool in_a = (c >> s) & 1u, in_v = top == s;
+        const unsigned am = __ballot_sync(FULL, in_a), vm = __ballot_sync(FULL, in_v);
+        int ax0, ax1, vx0 = 0, vx1 = 0;  // K - x0 and x1 of the amodal and visible lanes
+        if (one_row) {
+          ax0 = K - (c0 + __ffs(am) - 1);
+          ax1 = c0 + 32 - __clz(am);
+          if (vm) {
+            vx0 = K - (c0 + __ffs(vm) - 1);
+            vx1 = c0 + 32 - __clz(vm);
+          }
+        } else {
+          ax0 = __reduce_max_sync(FULL, in_a ? K - j : 0);
+          ax1 = __reduce_max_sync(FULL, in_a ? j + 1 : 0);
+          if (vm) {
+            vx0 = __reduce_max_sync(FULL, in_v ? K - j : 0);
+            vx1 = __reduce_max_sync(FULL, in_v ? j + 1 : 0);
+          }
+        }
+        if (lane == s) {
+          // raster order: the first and last set lanes hold the top and bottom rows
+          area += __popc(am);
+          ab[0] = max(ab[0], ax0);
+          ab[1] = max(ab[1], K - (i0 + (one_row ? r0 : (p0 + __ffs(am) - 1) / L.W)));
+          ab[2] = max(ab[2], ax1);
+          ab[3] = max(ab[3], i0 + (one_row ? r0 : (p0 + 31 - __clz(am)) / L.W) + 1);
+          if (vm) {
+            vis += __popc(vm);
+            vb[0] = max(vb[0], vx0);
+            vb[1] = max(vb[1], K - (i0 + (one_row ? r0 : (p0 + __ffs(vm) - 1) / L.W)));
+            vb[2] = max(vb[2], vx1);
+            vb[3] = max(vb[3], i0 + (one_row ? r0 : (p0 + 31 - __clz(vm)) / L.W) + 1);
+          }
+        }
+      }
+    }
+    if (area) {  // vis <= area, and only slots < S have bits
+      atomicAdd(&s_cnt[lane], vis);
+      atomicAdd(&s_cnt[S + lane], area);
+#pragma unroll
+      for (int f = 0; f < 4; ++f) {
+        atomicMax(&s_cnt[(2 + f) * S + lane], vb[f]);
+        atomicMax(&s_cnt[(6 + f) * S + lane], ab[f]);
+      }
+    }
+    __syncthreads();
+    // s_cnt[q * S + s]: q = 0 visible, 1 area, 2..5 the visible box, 6..9 the amodal box
+    for (int i = tid; i < 10 * S; i += MK_THREADS) {
+      const int v = s_cnt[i], q = i / S, s = i - q * S;
+      if (!v) continue;
+      const size_t o = e * S + s;
+      if (q == 0) atomicAdd(&counts.visible[o], v);
+      else if (q == 1) atomicAdd(&counts.area[o], v);
+      else if (q < 6) atomicMax(&counts.visible_box[o * 4 + (q - 2)], v);
+      else atomicMax(&counts.amodal_box[o * 4 + (q - 6)], v);
+    }
+    return;
+  }
+
   // ---- phase C: the staged band to the masks -------------------------------------------------
   constexpr int LOG16 = kCover ? 2 : 4;  // log2 of the pixels per 16-byte store
   const int head = min(((16 - mis) & 15) / (int)sizeof(Px), npx);
@@ -420,6 +514,22 @@ mask_kernel(DevState st, const MaskLayout L, uint8_t *__restrict__ masks, const 
       if (v) atomicAdd(&counts.visible[e * S + tid], v);
       if (a) atomicAdd(&counts.area[e * S + tid], a);
     }
+  }
+}
+
+constexpr int BOX_FINISH_THREADS = 256;
+
+// MASK_BOX, after mask_kernel: box i < n_boxes of visible_box, then box i - n_boxes of amodal_box
+// ([n][S][4] int32 each, n_boxes = n S), from MK_BOX_KEY - x0, MK_BOX_KEY - y0 back to x0, y0.  A
+// box no pixel reached is all 0 and stays so; any other has both fields >= 2.
+__global__ void __launch_bounds__(BOX_FINISH_THREADS)
+box_finish_kernel(int32_t *__restrict__ visible_box, int32_t *__restrict__ amodal_box, size_t n_boxes) {
+  const size_t i = (size_t)blockIdx.x * BOX_FINISH_THREADS + threadIdx.x;
+  if (i >= 2 * n_boxes) return;
+  int32_t *const b = i < n_boxes ? visible_box + 4 * i : amodal_box + 4 * (i - n_boxes);
+  if (b[0]) {
+    b[0] = MK_BOX_KEY - b[0];
+    b[1] = MK_BOX_KEY - b[1];
   }
 }
 

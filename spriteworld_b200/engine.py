@@ -139,20 +139,24 @@ def _rows(engine, states, live=True):
 
 
 # What each sprite-mask observation writes: its C-ABI call, then the name, dtype and axes of each
-# output, over n rows, S slots and H x W pixels.  Engine.render_masks, render_coverage and
-# render_soft_masks take and return one output as a tensor, several as a tuple.
+# output, over n rows, S slots and H x W pixels (a digit: an axis of that constant size).
+# Engine.render_masks, render_coverage, render_soft_masks and render_boxes take and return one
+# output as a tensor, several as a tuple.
 _MASK_KINDS = {
     'masks': ('swb_render_masks', (('masks', torch.uint8, 'nHW'),)),
     'coverage': ('swb_render_coverage', (('cover', torch.int32, 'nHW'), ('visible', torch.int32, 'nS'),
                                          ('area', torch.int32, 'nS'))),
     'soft': ('swb_render_soft_masks', (('soft', torch.uint8, 'nSHW'),)),
+    'boxes': ('swb_render_boxes', (('visible_box', torch.int32, 'nS4'), ('amodal_box', torch.int32, 'nS4'),
+                                   ('visible', torch.int32, 'nS'), ('area', torch.int32, 'nS'))),
 }
 
 
 def _mask_outputs(kind, n, n_slots, height, width):
   """[(name, dtype, shape)] of the outputs of sprite-mask observation `kind` for n rows."""
   size = dict(n=n, S=n_slots, H=height, W=width)
-  return [(name, dtype, tuple(size[a] for a in axes)) for name, dtype, axes in _MASK_KINDS[kind][1]]
+  return [(name, dtype, tuple(int(a) if a.isdigit() else size[a] for a in axes))
+          for name, dtype, axes in _MASK_KINDS[kind][1]]
 
 
 def _new_mask_outputs(engine, kind, n, width, height):
@@ -164,7 +168,8 @@ def _new_mask_outputs(engine, kind, n, width, height):
 
 
 def _render_sprite_masks(engine, kind, width, height, anti_aliasing=1, states=None, out=None):
-  """The body of Engine.render_masks, render_coverage and render_soft_masks, for observation `kind`."""
+  """The body of Engine.render_masks, render_coverage, render_soft_masks and render_boxes, for
+  observation `kind`."""
   n, rec, rec_bytes = _rows(engine, states)
   W, H, aa = int(width), int(height), int(anti_aliasing)
   spec = _mask_outputs(kind, n, engine.n_slots, H, W)
@@ -174,7 +179,8 @@ def _render_sprite_masks(engine, kind, width, height, anti_aliasing=1, states=No
     _check_output(out, *spec[0], engine.device)
   else:
     if not isinstance(out, (tuple, list)) or len(out) != len(spec):
-      raise ValueError('out must be a (%s) triple, got %s' % (', '.join(s[0] for s in spec), type(out).__name__))
+      what = 'triple' if len(spec) == 3 else '%d-tuple' % len(spec)
+      raise ValueError('out must be a (%s) %s, got %s' % (', '.join(s[0] for s in spec), what, type(out).__name__))
     for t, s in zip(out, spec):
       _check_output(t, *s, engine.device)
     out = tuple(out)
@@ -515,6 +521,18 @@ class Engine(object):
     contiguous uint8 tensor of that shape on this device), else a new tensor.  One launch on the
     current stream; nothing else changes."""
     return _render_sprite_masks(self, 'soft', width, height, anti_aliasing, states, out)
+
+  def render_boxes(self, width, height, anti_aliasing=1, states=None, out=None):
+    """Sprite bounding boxes (swb_render_boxes): (visible_box, amodal_box, visible, area), int32
+    (n, n_slots, 4), (n, n_slots, 4), (n, n_slots) and (n, n_slots).  Over the pixels where slot k
+    is the top-most covering sprite (the mask render_masks draws is k + 1) and over those where its
+    bit of render_coverage's cover is set: the half-open pixel box (x0, y0, x1, y1) = (min column,
+    min row, max column + 1, max row + 1), (0, 0, 0, 0) for no pixel, and the pixel counts, which
+    are render_coverage's (renderers.SpriteBoxes).  Of the live envs (n = n_envs), or with `states`
+    of EnvStates of any n records, as if loaded.  Into `out` if given (a 4-tuple of contiguous
+    int32 tensors of those shapes on this device), else new tensors.  Two launches on the current
+    stream (after zeroing the four outputs); nothing else changes."""
+    return _render_sprite_masks(self, 'boxes', width, height, anti_aliasing, states, out)
 
   def render_status(self):
     """Zero-copy uint8 (E,) view of the per-env status of the last render() (ENV_SPAN_OVERFLOW)."""

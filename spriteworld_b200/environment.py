@@ -363,9 +363,9 @@ class BatchedEnvironment(object):
         (name, engine_lib.Raster(self._engine, r.width, r.height, r.anti_aliasing, r.bg_color))
         for name, r in self._pil.items())
     self._frames = {name: r.new_frames() for name, r in self._rasters.items()}
-    # the outputs of each SpriteMasks, SpriteCoverage and SoftSpriteMasks renderer by id(renderer),
-    # overwritten every step like the frames: one dict, also under the coverage and soft-mask buffer
-    # names the test suite reads them by
+    # the outputs of each SpriteMasks, SpriteCoverage, SoftSpriteMasks and SpriteBoxes renderer by
+    # id(renderer), overwritten every step like the frames: one dict, also under the coverage and
+    # soft-mask buffer names the test suite reads them by
     self._mask_buffers = {
         id(r): engine_lib._new_mask_outputs(self._engine, r._kind, E, r.width, r.height)
         for r in self._other.values() if isinstance(r, handcrafted._SpriteMaskRenderer)}
@@ -870,10 +870,10 @@ class BatchedEnvironment(object):
     return BatchedRollout(res.step_type, res.reward, discount, res.success, res.status)
 
   def render(self):
-    """Re-renders every PILRenderer, SpriteMasks, SpriteCoverage and SoftSpriteMasks observation of
-    the current state (a loaded one, say) into this environment's buffers, and returns them: dict
-    name -> uint8 (n_envs, H, W, 3) frames, then uint8 (n_envs, H, W) masks, coverage dicts and
-    uint8 (n_envs, n_slots, H, W) soft masks, in renderer order."""
+    """Re-renders every PILRenderer, SpriteMasks, SpriteCoverage, SoftSpriteMasks and SpriteBoxes
+    observation of the current state (a loaded one, say) into this environment's buffers, and
+    returns them: dict name -> uint8 (n_envs, H, W, 3) frames, then uint8 (n_envs, H, W) masks,
+    coverage dicts, uint8 (n_envs, n_slots, H, W) soft masks and box dicts, in renderer order."""
     out = collections.OrderedDict()
     for name, r in self._rasters.items():
       out[name] = self._engine.render(r, self._frames[name])
@@ -883,9 +883,10 @@ class BatchedEnvironment(object):
     return out
 
   def _render_sprite_masks(self, cls, renderer, states=None):
-    """`renderer`'s observation as a `cls` (SpriteMasks, SpriteCoverage or SoftSpriteMasks) on the
-    current stream: of the live envs into this environment's buffers for the renderer (new tensors
-    for a renderer it does not own), or of EnvStates `states` into new tensors."""
+    """`renderer`'s observation as a `cls` (SpriteMasks, SpriteCoverage, SoftSpriteMasks or
+    SpriteBoxes) on the current stream: of the live envs into this environment's buffers for the
+    renderer (new tensors for a renderer it does not own), or of EnvStates `states` into new
+    tensors."""
     # only a renderer of this kind has buffers of this kind's form
     out = self._mask_buffers.get(id(renderer)) if states is None and isinstance(renderer, cls) else None
     return cls._observation(engine_lib._render_sprite_masks(
@@ -910,13 +911,21 @@ class BatchedEnvironment(object):
     does not own), or of EnvStates `states` into a new uint8 (n, n_slots, H, W) tensor."""
     return self._render_sprite_masks(handcrafted.SoftSpriteMasks, renderer, states)
 
+  def render_boxes(self, renderer, states=None):
+    """SpriteBoxes `renderer`'s observation (Engine.render_boxes) on the current stream: dict
+    'visible_box' and 'amodal_box' int32 (n, n_slots, 4), 'visible' and 'area' int32 (n, n_slots).
+    Of the live envs into this environment's buffers for the renderer (new tensors for a renderer
+    it does not own), or of EnvStates `states` into new tensors."""
+    return self._render_sprite_masks(handcrafted.SpriteBoxes, renderer, states)
+
   def observe(self, states):
     """The observations of env records without loading them: (observation, status) for EnvStates
     `states` of n records, observation an OrderedDict in renderer order of what step() would
     observe for envs that load_envs(states) had loaded -- PILRenderer frames as new uint8
     (n, H, W, 3) tensors (one render launch per raster; never this environment's own frame
     buffers), SpriteFactors dicts of (n, n_slots) tensors, SpriteMasks, SpriteCoverage and
-    SoftSpriteMasks observations in new tensors (one launch each) -- and status uint8 (n,), the OR over the
+    SoftSpriteMasks observations in new tensors (one launch each), SpriteBoxes observations in new
+    tensors (two launches each) -- and status uint8 (n,), the OR over the
     rasters of their render status (_native.ENV_SPAN_OVERFLOW).
 
     Enqueued on the current stream without a host synchronisation.  Read-only: no env, scene ring,

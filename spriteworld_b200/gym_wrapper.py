@@ -95,6 +95,10 @@ def _spec_to_space(spec):
   if hasattr(spec, 'num_values'):
     return spaces.Discrete(spec.num_values)
   if hasattr(spec, 'minimum'):
+    low, high = np.broadcast_to(spec.minimum, spec.shape), np.broadcast_to(spec.maximum, spec.shape)
+    if low.size and (low.min() != low.max() or high.min() != high.max()):
+      # bounds per element (SpriteBoxes: x in [0, W], y in [0, H]) stay per element
+      return spaces.Box(low=low, high=high, shape=spec.shape, dtype=spec.dtype)
     return spaces.Box(low=float(np.min(spec.minimum)), high=float(np.max(spec.maximum)),
                       shape=spec.shape, dtype=spec.dtype)
   if spec.dtype == np.uint8:
@@ -144,7 +148,7 @@ class GymWrapper(object):
 
   def _process_obs(self, obs):
     for k, v in obs.items():
-      if isinstance(v, dict):         # SpriteCoverage: a dict of arrays, as its space describes
+      if isinstance(v, dict):         # SpriteCoverage, SpriteBoxes: a dict of arrays, as its space describes
         obs[k] = type(v)((kk, np.asarray(vv)) for kk, vv in v.items())
         continue
       obs[k] = np.asarray(v)

@@ -3,6 +3,7 @@ from spriteworld_b200.renderers import color_maps  # noqa: F401
 from spriteworld_b200.renderers.abstract_renderer import AbstractRenderer  # noqa: F401
 from spriteworld_b200.renderers.handcrafted import GoalPositions  # noqa: F401
 from spriteworld_b200.renderers.handcrafted import SoftSpriteMasks  # noqa: F401
+from spriteworld_b200.renderers.handcrafted import SpriteBoxes  # noqa: F401
 from spriteworld_b200.renderers.handcrafted import SpriteCoverage  # noqa: F401
 from spriteworld_b200.renderers.handcrafted import SpriteFactors  # noqa: F401
 from spriteworld_b200.renderers.handcrafted import SpriteMasks  # noqa: F401

@@ -71,7 +71,7 @@ class SpriteFactors(abstract_renderer.AbstractRenderer):
 
 
 class _SpriteMaskRenderer(abstract_renderer.AbstractRenderer):
-  """What SpriteMasks, SpriteCoverage and SoftSpriteMasks share: image_size=(W, H) and
+  """What SpriteMasks, SpriteCoverage, SoftSpriteMasks and SpriteBoxes share: image_size=(W, H) and
   anti_aliasing, whose canvas may not exceed 4095 pixels per side, drawn by the mask kernel as
   observation `_kind` (engine._render_sprite_masks); `_observation` shapes what it writes
   and `_spec(n)` describes that for n sprites."""
@@ -221,6 +221,49 @@ class SoftSpriteMasks(_SpriteMaskRenderer):
   @staticmethod
   def _observation(out, slots=slice(None)):
     return out[..., slots, :, :]
+
+
+class SpriteBoxes(_SpriteMaskRenderer):
+  """Sprite bounding boxes: where each sprite is visible and where it lies, hidden or not, in a
+  PILRenderer frame, as pixel boxes with pixel counts.
+
+  Observes a dict for image_size=(W, H) and S sprites:
+    'visible_box'  int32 (S, 4): box(V_k), V_k the pixels (i, j) where sprite k is the top-most
+                   covering sprite (SpriteMasks mask == k + 1).
+    'amodal_box'   int32 (S, 4): box(A_k), A_k the pixels whose bit k of SpriteCoverage's 'cover'
+                   is set, whether or not a sprite above hides them.
+    'visible'      int32 (S,): |V_k|, SpriteCoverage's 'visible'.
+    'area'         int32 (S,): |A_k|, SpriteCoverage's 'area'.
+  box(P) = (min j, min i, max j + 1, max i + 1): half-open (x0, y0, x1, y1) in pixels of the
+  observed (flipped) image, x the column and y the row from the top; (0, 0, 0, 0) for an empty P.
+  For a non-empty plane that is torchvision.ops.masks_to_boxes(plane) + (0, 0, 1, 1).  So the
+  visible box lies in the amodal box, visible <= area, a count is 0 exactly where its box is, and
+  (x1 - x0) * (y1 - y0) >= the count.  Empty slots and sprites wholly out of frame have zero boxes
+  and counts; wholly hidden sprites a zero visible box.  The sample point, integer vertices and
+  fill rules are SpriteMasks'.  Reduced inside the mask kernel's box mode (csrc/swb_masks.cuh):
+  no per-pixel output is written.
+
+  Slots: in a BatchedEnvironment, S is n_slots and k is slot k of SpriteFactors.render_batch; on a
+  sprite list (`render`, the drop-in Environment), k is the list index.  The same arguments and
+  limits as SpriteMasks."""
+
+  _kind = 'boxes'
+
+  def _spec(self, n):
+    W, H, npx = self.width, self.height, self.height * self.width
+    box = specs.BoundedArray(shape=(n, 4), dtype=np.int32, minimum=0,
+                             maximum=np.broadcast_to(np.array([W, H, W, H], np.int32), (n, 4)))
+    return collections.OrderedDict([
+        ('visible_box', box), ('amodal_box', box),
+        ('visible', specs.BoundedArray(shape=(n,), dtype=np.int32, minimum=0, maximum=npx)),
+        ('area', specs.BoundedArray(shape=(n,), dtype=np.int32, minimum=0, maximum=npx))])
+
+  @staticmethod
+  def _observation(out, slots=slice(None)):
+    visible_box, amodal_box, visible, area = out
+    return collections.OrderedDict([('visible_box', visible_box[..., slots, :]),
+                                    ('amodal_box', amodal_box[..., slots, :]),
+                                    ('visible', visible[..., slots]), ('area', area[..., slots])])
 
 
 class GoalPositions(abstract_renderer.AbstractRenderer):

@@ -20,7 +20,8 @@ and int64 device ids, valid and refused (out of range either way, 2^32 + 1, repe
 so that memcheck sees that a refused id never indexes engine memory.  Then rollouts from records
 into leaves, from those leaves, and from the live envs into leaves, renders of records, the sprite
 coverage (swb_render_coverage) of live envs and records into buffers that are not 16-byte aligned,
-their soft masks (swb_render_soft_masks) into buffers at odd byte offsets, and an engine
+their soft masks (swb_render_soft_masks) into buffers at odd byte offsets, their boxes
+(swb_render_boxes) at 4-byte offsets that are not 16-byte aligned, and an engine
 checkpoint saved, loaded and rendered, with a corrupt one refused.
 """
 import ctypes
@@ -134,6 +135,18 @@ def device_checked_records(torch):
       eng.render_soft_masks(W, H, aa, states=states, out=flat[skew:skew + n * S * H * W].view(n, S, H, W))
   torch.cuda.synchronize()
   print('soft masks: live envs and %d leaves, %d kernel launches' % (len(res.leaves), eng.launch_count()),
+        flush=True)
+  # boxes of the live envs and of the leaves at 4-byte offsets that are not 16-byte aligned: bands
+  # of one row (4095 wide) and of many, and zero records
+  for W, H, aa, skew in ((wl.image_size[0], wl.image_size[1], 5, 1), (13, 7, 5, 3), (4095, 2, 1, 2)):
+    for states in (None, res.leaves, res.leaves[:0]):
+      n = E if states is None else len(states)
+      flat = torch.zeros(n * 10 * S + 4, dtype=torch.int32, device='cuda')
+      views = [flat[skew + o * n * S:skew + (o + k) * n * S] for o, k in ((0, 4), (4, 4), (8, 1), (9, 1))]
+      eng.render_boxes(W, H, aa, states=states, out=tuple(v.view(n, S, 4) if i < 2 else v.view(n, S)
+                                                          for i, v in enumerate(views)))
+  torch.cuda.synchronize()
+  print('boxes: live envs and %d leaves, %d kernel launches' % (len(res.leaves), eng.launch_count()),
         flush=True)
   # an engine checkpoint round trip, and a corrupt one refused before anything is enqueued
   from spriteworld_b200 import _native
