@@ -334,7 +334,7 @@ int swb_upload_state(swb_engine *eng, const double *pos_x, const double *pos_y,
  * configuration did not write -- and a span_class lower than its shapes need -- gives undefined
  * steps and frames.
  *
- * Read-only record calls (swb_rollout_states, swb_render_states, swb_render_masks,
+ * Read-only record calls (swb_rollout_states, swb_rollout_trajectory, swb_render_states, swb_render_masks,
  * swb_render_coverage, swb_render_soft_masks, swb_render_boxes, swb_evaluate_states,
  * swb_sample_contained) read n rows: n records of this
  * engine's layout in a device record buffer of records_bytes bytes or, where a call takes them,
@@ -394,6 +394,28 @@ int swb_rollout_states(swb_engine *eng, const void *roots, int32_t n_roots, uint
                        const void *actions, int32_t action_dtype, int32_t n_steps, int32_t n_candidates,
                        const swb_step_out *out, void *leaves, uint64_t leaves_bytes,
                        int32_t *span_class, void *stream);
+
+/*
+ * swb_rollout_states with the state after every step of every plan: trajectories of the candidate
+ * plans in one launch, for the frames, masks, boxes or task values of each imagined step.
+ *
+ * Roots, actions, `out` and *span_class are as swb_rollout_states has them, and `out` is bit for bit
+ * what it writes.  `records` (required) is a device buffer of records_bytes bytes: record
+ * (t * n_roots + r) * n_candidates + c is, byte for byte, leaf r * n_candidates + c of
+ * swb_rollout_states called with the same roots and only the first t + 1 steps of the actions.  So
+ * after a plan's first SWB_STEP_LAST every record repeats its end state (reset_next = 1), a root
+ * about to reset is its own record at every t, every record keeps its root's goals, and the last
+ * n_roots * n_candidates records are the leaves.
+ *
+ * A read-only record call (above) with the roots as its rows, and `records` and every array of
+ * `out` as its outputs.  Refused besides: what swb_rollout_states refuses, records NULL, and
+ * records not 16-byte aligned or smaller than n_steps * n_roots * n_candidates records.  An
+ * accepted call is one launch.  Read-only but for `out` and `records`, as swb_rollout.
+ */
+int swb_rollout_trajectory(swb_engine *eng, const void *roots, int32_t n_roots, uint64_t roots_bytes,
+                           const void *actions, int32_t action_dtype, int32_t n_steps, int32_t n_candidates,
+                           const swb_step_out *out, void *records, uint64_t records_bytes,
+                           int32_t *span_class, void *stream);
 
 /*
  * The frames of env records without loading them into envs: frame i (of [n][height][width][3]

@@ -130,6 +130,7 @@ def load():
   L.swb_copy_envs.argtypes = [vp, vp, vp, ci, vp]
   L.swb_rollout_states.argtypes = [vp, vp, ci, ctypes.c_uint64, vp, ci, ci, ci, ctypes.POINTER(StepOut), vp,
                                    ctypes.c_uint64, ctypes.POINTER(ci), vp]
+  L.swb_rollout_trajectory.argtypes = L.swb_rollout_states.argtypes
   L.swb_render_states.argtypes = [vp, vp, vp, ci, ctypes.c_uint64, ci, vp, vp, vp]
   L.swb_render_masks.argtypes = [vp, ci, ci, ci, vp, ci, ctypes.c_uint64, vp, vp]
   L.swb_render_coverage.argtypes = [vp, ci, ci, ci, vp, ci, ctypes.c_uint64, vp, vp, vp, vp]
@@ -175,7 +176,8 @@ EXPORTS = (
     'swb_sampler_sizeof_program', 'swb_sampler_load', 'swb_sample_scenes', 'swb_refill_device',
     'swb_sampler_pointers', 'swb_pool_pointers', 'swb_engine_state_bytes', 'swb_save_engine',
     'swb_load_engine', 'swb_pool_goal_pointer', 'swb_set_goals', 'swb_set_goals_dev', 'swb_evaluate_states',
-    'swb_sample_contained', 'swb_render_coverage', 'swb_render_soft_masks', 'swb_render_boxes')
+    'swb_sample_contained', 'swb_render_coverage', 'swb_render_soft_masks', 'swb_render_boxes',
+    'swb_rollout_trajectory')
 
 
 def check(rc):

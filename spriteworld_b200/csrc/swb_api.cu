@@ -172,7 +172,7 @@ int upload_axis(swb_raster *r, const AxisHost &h, AxisTables *d) {
 extern "C" {
 
 const char *swb_last_error(void) { return g_error.c_str(); }
-int swb_version(void) { return 15; }
+int swb_version(void) { return 16; }
 int swb_sizeof_config(void) { return (int)sizeof(swb_config); }
 int swb_sizeof_task_node(void) { return (int)sizeof(swb_task_node); }
 
@@ -486,15 +486,16 @@ static int check_rollout(const swb_engine *eng, const char *fn, const char *what
 }
 
 // Enqueues the one rollout_kernel launch of a checked call: roots from io.roots unless it is null
-// (the live envs), leaves into io.leaves unless it is null.
+// (the live envs), leaves into io.leaves unless it is null -- every step's records with `trajectory`.
 static int enqueue_rollout(swb_engine *eng, const void *actions, int32_t action_dtype, int32_t n_steps,
                            int32_t n_candidates, const swb_step_out &out, RolloutRecords io,
-                           cudaStream_t stream) {
+                           cudaStream_t stream, bool trajectory = false) {
   CUDA_TRY(cudaSetDevice(eng->device));
   const int64_t plans = (int64_t)(io.roots ? io.n_roots : eng->st.E) * n_candidates;
   const unsigned blocks = (unsigned)((plans + ROLLOUT_WARPS - 1) / ROLLOUT_WARPS);
-  auto kernel = io.roots ? (io.leaves ? rollout_kernel<true, true> : rollout_kernel<true, false>)
-                         : (io.leaves ? rollout_kernel<false, true> : rollout_kernel<false, false>);
+  auto kernel = trajectory ? (io.roots ? rollout_kernel<true, false, true> : rollout_kernel<false, false, true>)
+                : io.roots ? (io.leaves ? rollout_kernel<true, true> : rollout_kernel<true, false>)
+                           : (io.leaves ? rollout_kernel<false, true> : rollout_kernel<false, false>);
   kernel<<<blocks, ROLLOUT_WARPS * 32, 0, stream>>>(eng->st, eng->d_step_cfg, actions, action_dtype, n_steps,
                                                     n_candidates, out, io);
   eng->launches++;
@@ -1308,11 +1309,17 @@ int swb_evaluate_states(swb_engine *eng, const void *records, int32_t n, uint64_
   return 0;
 }
 
-int swb_rollout_states(swb_engine *eng, const void *roots, int32_t n_roots, uint64_t roots_bytes,
-                       const void *actions, int32_t action_dtype, int32_t n_steps, int32_t n_candidates,
-                       const swb_step_out *out, void *leaves, uint64_t leaves_bytes, int32_t *span_class,
-                       void *stream) {
-  static const char fn[] = "swb_rollout_states";
+}  // extern "C"
+
+// swb_rollout_states and swb_rollout_trajectory: the rollout, roots and output checks, then one
+// launch.  `records` are the leaves (NULL: none), or with `trajectory` the n_steps records of
+// every plan, which the call requires.
+static int rollout_records_call(swb_engine *eng, const char *fn, const void *roots, int32_t n_roots,
+                                uint64_t roots_bytes, const void *actions, int32_t action_dtype, int32_t n_steps,
+                                int32_t n_candidates, const swb_step_out *out, void *records,
+                                uint64_t records_bytes, int32_t *span_class, cudaStream_t stream,
+                                bool trajectory) {
+  const char *name = trajectory ? "records" : "leaves";
   if (!eng) return fail("%s: null engine", fn);
   if (roots ? n_roots < 1 : n_roots != eng->st.E)
     return roots ? fail("%s: n_roots = %d must be >= 1", fn, n_roots)
@@ -1322,18 +1329,40 @@ int swb_rollout_states(swb_engine *eng, const void *roots, int32_t n_roots, uint
                     out) ||
       check_rows(eng, fn, "roots", roots, n_roots, roots_bytes, true))
     return 1;
+  if (trajectory && !records) return fail("%s: null output records", fn);
   const uint64_t rb = RecordLayout(eng->st.S, eng->st.G).bytes();
   const uint64_t plans = (uint64_t)n_roots * n_candidates, entries = plans * n_steps;
-  if (leaves && check_record_buffer(eng, fn, "leaves", leaves, leaves_bytes, (int64_t)plans)) return 1;
+  const uint64_t n_records = trajectory ? entries : plans;
+  if (records && check_record_buffer(eng, fn, name, records, records_bytes, (int64_t)n_records)) return 1;
   const Span outs[] = {{"reward", out->reward, 8 * entries, 8}, {"step_type", out->step_type, entries, 1},
                        {"success", out->success, entries, 1}, {"status", out->status, entries, 1},
-                       {"leaves", leaves, plans * rb, 16}};
-  if (check_outputs(fn, outs, leaves ? 5 : 4, Span{"the roots", roots, n_roots * rb, 16})) return 1;
+                       {name, records, n_records * rb, 16}};
+  if (check_outputs(fn, outs, records ? 5 : 4, Span{"the roots", roots, n_roots * rb, 16})) return 1;
   if (!roots && span_class) *span_class = eng->max_spans;
   return enqueue_rollout(eng, actions, action_dtype, n_steps, n_candidates, *out,
                          RolloutRecords{static_cast<const unsigned char *>(roots),
-                                        static_cast<unsigned char *>(leaves), (size_t)rb, n_roots},
-                         static_cast<cudaStream_t>(stream));
+                                        static_cast<unsigned char *>(records), (size_t)rb, n_roots},
+                         stream, trajectory);
+}
+
+extern "C" {
+
+int swb_rollout_states(swb_engine *eng, const void *roots, int32_t n_roots, uint64_t roots_bytes,
+                       const void *actions, int32_t action_dtype, int32_t n_steps, int32_t n_candidates,
+                       const swb_step_out *out, void *leaves, uint64_t leaves_bytes, int32_t *span_class,
+                       void *stream) {
+  return rollout_records_call(eng, "swb_rollout_states", roots, n_roots, roots_bytes, actions, action_dtype,
+                              n_steps, n_candidates, out, leaves, leaves_bytes, span_class,
+                              static_cast<cudaStream_t>(stream), false);
+}
+
+int swb_rollout_trajectory(swb_engine *eng, const void *roots, int32_t n_roots, uint64_t roots_bytes,
+                           const void *actions, int32_t action_dtype, int32_t n_steps, int32_t n_candidates,
+                           const swb_step_out *out, void *records, uint64_t records_bytes, int32_t *span_class,
+                           void *stream) {
+  return rollout_records_call(eng, "swb_rollout_trajectory", roots, n_roots, roots_bytes, actions, action_dtype,
+                              n_steps, n_candidates, out, records, records_bytes, span_class,
+                              static_cast<cudaStream_t>(stream), true);
 }
 
 int swb_render_states(swb_engine *eng, swb_raster *r, const void *records, int32_t n, uint64_t records_bytes,

@@ -16,6 +16,11 @@
 // Leaves and roots share the record format, so one launch is one level of a search tree.  A leaf
 // keeps its root's goals.
 //
+// Trajectories (swb_rollout_trajectory): record t * R * C + w of io.leaves is the leaf of the same
+// plan cut after step t.  Lanes < S write it after each live step, and the warp's final record
+// fills the entries after the plan's first LAST (all T of them for a root about to reset).  The
+// scene fields come from the root at each write, not from registers held across the step loop.
+//
 // Actions are [T][R][C][A]: at a step the warps of a CTA read consecutive rows, every lane the
 // row of its warp (one broadcast transaction), and the row of step t + 1 is loaded before step t
 // is evaluated, so its latency hides behind lane 0's task evaluation.
@@ -28,8 +33,8 @@ namespace swb {
 constexpr int ROLLOUT_WARPS = 4;
 
 // The record buffers of a rollout: roots (n_roots records) unless the roots are the live envs,
-// leaves (n_roots * C records) if asked for.  Each instantiation of rollout_kernel reads only
-// the members its template arguments use.
+// leaves (n_roots * C records, or T * n_roots * C for a trajectory) if asked for.  Each
+// instantiation of rollout_kernel reads only the members its template arguments use.
 struct RolloutRecords {
   const unsigned char *roots;
   unsigned char *leaves;
@@ -57,8 +62,24 @@ __device__ __forceinline__ void stage_record(const DevState &st, WarpSprites &ws
   __syncwarp();
 }
 
-// kRecordRoots: roots are io.roots (else the E live envs); kLeaves: write io.leaves.
-template <bool kRecordRoots, bool kLeaves>
+// Slot `lane` of the record a plan from root e (record `root`, else live env e) has reached: the
+// root's scene fields read now, the positions in ws, step_count `count` (lane 0's copy is the one
+// write_record stores) and reset_next `last`.
+template <bool kRecordRoots>
+__device__ __forceinline__ void write_plan_record(const DevState &st, const WarpSprites &ws,
+                                                  const unsigned char *root, int e, int lane, int count,
+                                                  bool last, unsigned char *dst) {
+  SlotRecord r = kRecordRoots ? read_record(st, root, lane) : read_state(st, e, lane);
+  r.f64[8] = ws.x[lane];
+  r.f64[9] = ws.y[lane];
+  r.step_count = count;
+  r.reset_next = last ? 1 : 0;
+  write_record(dst, st.S, st.G, lane, r);
+}
+
+// kRecordRoots: roots are io.roots (else the E live envs); kLeaves: write io.leaves; kTrajectory
+// (with kLeaves false): write the T * R * C records of every step into io.leaves.
+template <bool kRecordRoots, bool kLeaves, bool kTrajectory = false>
 __global__ void __launch_bounds__(ROLLOUT_WARPS * 32)
 rollout_kernel(DevState st, const StepCfg *__restrict__ step_cfg, const void *__restrict__ actions,
                int action_dtype, int T, int C, swb_step_out out, RolloutRecords io) {
@@ -80,6 +101,10 @@ rollout_kernel(DevState st, const StepCfg *__restrict__ step_cfg, const void *__
   if (kLeaves && lane < 2 * st.G)
     record_goals(st, io.leaves + (size_t)w * io.record_bytes)[lane] =
         (kRecordRoots ? record_goals(st, root) : state_goals(st, e))[lane];
+  if (kTrajectory && lane < 2 * st.G) {
+    const double g = (kRecordRoots ? record_goals(st, root) : state_goals(st, e))[lane];
+    for (int p = 0; p < T; ++p) record_goals(st, io.leaves + ((size_t)p * EC + w) * io.record_bytes)[lane] = g;
+  }
   int t = 0, count = 0;
   bool ended = false;
   if (!resetting) {
@@ -111,6 +136,9 @@ rollout_kernel(DevState st, const StepCfg *__restrict__ step_cfg, const void *__
         out.status[i] = (uint8_t)status;
       }
       step_type = __shfl_sync(0xFFFFFFFFu, step_type, 0);
+      if (kTrajectory && lane < S)
+        write_plan_record<kRecordRoots>(st, ws, root, e, lane, count, step_type == SWB_STEP_LAST,
+                                        io.leaves + ((size_t)t * EC + w) * io.record_bytes);
       t++;
       if (step_type == SWB_STEP_LAST) {
         ended = true;
@@ -124,6 +152,17 @@ rollout_kernel(DevState st, const StepCfg *__restrict__ step_cfg, const void *__
     out.step_type[i] = (int8_t)SWB_STEP_NONE;
     out.success[i] = 0;
     out.status[i] = 0;
+  }
+  if (kTrajectory && lane < S && t < T) {
+    // the end state repeats: the plan's last record, or the root itself
+    SlotRecord end = kRecordRoots ? read_record(st, root, lane) : read_state(st, e, lane);
+    if (!resetting) {
+      end.f64[8] = ws.x[lane];
+      end.f64[9] = ws.y[lane];
+      end.step_count = count;
+      end.reset_next = ended ? 1 : 0;
+    }
+    for (int p = t; p < T; ++p) write_record(io.leaves + ((size_t)p * EC + w) * io.record_bytes, S, st.G, lane, end);
   }
   if (kLeaves && lane < S) {
     SlotRecord leaf = kRecordRoots ? read_record(st, root, lane) : read_state(st, e, lane);

@@ -40,12 +40,14 @@ class RolloutResult(object):
   """Outputs of a rollout, (T, n_envs, C) each: reward float64, step_type int8 (STEP_MID, STEP_LAST
   or, after a plan's first LAST and for an env about to reset, STEP_NONE with reward 0), success
   and status uint8.  The caller's own tensors: no later call overwrites them.  `leaves`: None, or
-  the EnvStates of the state each plan ends in (record r * C + c: root r's plan c)."""
-  __slots__ = ('reward', 'step_type', 'success', 'status', 'leaves')
+  the EnvStates of the state each plan ends in (record r * C + c: root r's plan c).  `trajectory`:
+  None, or the EnvStates of the state after every step (record (t * n + r) * C + c: root r's plan c
+  after step t, its end state once the plan has ended)."""
+  __slots__ = ('reward', 'step_type', 'success', 'status', 'leaves', 'trajectory')
 
-  def __init__(self, reward, step_type, success, status, leaves=None):
+  def __init__(self, reward, step_type, success, status, leaves=None, trajectory=None):
     self.reward, self.step_type, self.success, self.status = reward, step_type, success, status
-    self.leaves = leaves
+    self.leaves, self.trajectory = leaves, trajectory
 
 
 OUT_BYTES_PER_ENV = 8 + 1 + 1 + 1
@@ -415,7 +417,7 @@ class Engine(object):
           ctypes.c_void_p(frames.data_ptr()), self._stream()))
     return StepResult(self._reward, self._step_type, self._success, self._status, frames)
 
-  def rollout(self, actions, out=None, states=None, leaves=None):
+  def rollout(self, actions, out=None, states=None, leaves=None, trajectory=None):
     """What each of C candidate action sequences of T steps would earn from the state every env is
     in now, in one launch that changes nothing (swb_rollout).  `actions`: device tensor
     (T, n_envs, C, columns) of a dtype step() takes.  Returns a RolloutResult; with `out`, a packed
@@ -426,30 +428,42 @@ class Engine(object):
     EnvStates of the n * C states the plans end in (RolloutResult.leaves), or EnvStates of n * C
     records to fill in place; record r * C + c is what save_envs would return after loading root r
     and stepping plan c's live steps.  Leaves carry the roots' span class.  Still one launch
-    (swb_rollout_states)."""
+    (swb_rollout_states).
+
+    `trajectory`: True for new EnvStates of the T * n * C states after every step
+    (RolloutResult.trajectory), or EnvStates of T * n * C records to fill in place; record
+    (t * n + r) * C + c is leaf r * C + c of the same call with actions[:t + 1], so the last n * C
+    records are the leaves.  Not with `leaves`.  Still one launch (swb_rollout_trajectory)."""
+    if trajectory is not None and leaves is not None:
+      raise ValueError('trajectory and leaves are exclusive: the leaves are the last n * C records of '
+                       'the trajectory')
     n, roots, roots_bytes = _rows(self, states)
     dt = action_dtype(self.action_kind, n, actions, self.device, plans=True)
     T, _, C, _ = actions.shape
-    if leaves is True:
-      leaves = EnvStates(torch.empty((n * C, self.record_bytes), dtype=torch.uint8, device=self.device),
-                         1, self.signature, self.n_slots, self.n_goals)
-    elif leaves is not None:
-      self.check_states(leaves, n * C)
+    records, n_records = (leaves, n * C) if trajectory is None else (trajectory, T * n * C)
+    if records is True:
+      records = EnvStates(torch.empty((n_records, self.record_bytes), dtype=torch.uint8, device=self.device),
+                          1, self.signature, self.n_slots, self.n_goals)
+    elif records is not None:
+      self.check_states(records, n_records)
     out, res = rollout_outputs(out, T, n, C, self.device)
     ptrs = _native.StepOut(res.reward.data_ptr(), res.step_type.data_ptr(), res.success.data_ptr(),
                            res.status.data_ptr())
-    if states is None and leaves is None:
+    if states is None and records is None:
       _native.check(self._lib.swb_rollout(self._h, ctypes.c_void_p(actions.data_ptr()), dt, T, C,
                                           ctypes.byref(ptrs), self._stream()))
       return res
     span = ctypes.c_int32(1 if states is None else states.span_class)
-    dst = (None, 0) if leaves is None else (ctypes.c_void_p(leaves.data.data_ptr()), leaves.data.numel())
-    _native.check(self._lib.swb_rollout_states(
-        self._h, roots, n, roots_bytes, ctypes.c_void_p(actions.data_ptr()), dt, T, C, ctypes.byref(ptrs),
-        dst[0], dst[1], ctypes.byref(span), self._stream()))
-    if leaves is not None:
-      leaves.span_class = span.value
-    res.leaves = leaves
+    dst = (None, 0) if records is None else (ctypes.c_void_p(records.data.data_ptr()), records.data.numel())
+    call = self._lib.swb_rollout_states if trajectory is None else self._lib.swb_rollout_trajectory
+    _native.check(call(self._h, roots, n, roots_bytes, ctypes.c_void_p(actions.data_ptr()), dt, T, C,
+                       ctypes.byref(ptrs), dst[0], dst[1], ctypes.byref(span), self._stream()))
+    if records is not None:
+      records.span_class = span.value
+    if trajectory is None:
+      res.leaves = records
+    else:
+      res.trajectory = records
     return res
 
   def step_gather(self, actions, raster, targets):

@@ -294,6 +294,8 @@ class BatchedEnvironment(object):
   step t of candidate c would report for env e from the state it is in now.  No env changes.
   rollout(actions, states) plans from saved env records instead, and expand(actions, states) also
   returns the state each plan ends in, as records: one level of a search tree.
+  rollout_trajectory(actions, states) returns the state after every step instead, for the
+  observations of each imagined step.
   """
 
   def __init__(self, task, action_space, renderers, init_sprites, keep_in_frame=True,
@@ -855,6 +857,20 @@ class BatchedEnvironment(object):
     (load_envs) counts as a reset, as every load does."""
     res = self._engine.rollout(self._plans(actions), states=states, leaves=True)
     return self._batched_rollout(res), res.leaves
+
+  def rollout_trajectory(self, actions, states=None):
+    """rollout(actions, states) that also returns the state after every step of every plan, as
+    (BatchedRollout, EnvStates) of T * n * C records, in one launch.  Record (t * n + r) * C + c is
+    the leaf expand(actions[:t + 1], states) returns for root r's plan c: after a plan's first LAST
+    every record repeats its end state, a root about to reset is its own record at every t, and the
+    last n * C records are expand's leaves.  observe(trajectory) then gives every step's
+    observations; reshape them to (T, n, C, ...).
+
+    As rollout(): no noise, no `rng` draw, and no env or scene ring changes.  The records take
+    T * n * C * engine.record_bytes bytes: to trace a few plans out of many, roll out first, pick
+    the plans, and trace those from the roots they start in (states.take)."""
+    res = self._engine.rollout(self._plans(actions), states=states, trajectory=True)
+    return self._batched_rollout(res), res.trajectory
 
   def _plans(self, actions):
     """Rollout actions as a contiguous tensor on the engine's device (host actions through
