@@ -764,6 +764,61 @@ int swb_sample_contained(swb_engine *eng, const void *records, int32_t n, uint64
 int swb_sampler_pointers(swb_engine *eng, int64_t **refilled_upto, swb_sampler_status **status);
 
 /*
+ * Env records from factor values: scenes the caller chose, packed on the device.
+ *
+ * swb_packer_load gives the engine the packer of swb_make_states: a swb_scene_program of which only
+ * the filters (bit i of `member` is filter_pc[i]'s predicate), color_mode and angle table are used
+ * (scene_program.compile_packer builds it: its generator code is a lone G_END).  The angle table
+ * must hold every integer in [-360, 360] and -0.0, with libm's cos / sin of their radians.  It is
+ * the engine's own copy, apart from the device sampler's program.  Synchronises.
+ *
+ * swb_make_states writes n records (record i at i * swb_env_record_bytes() of `records`).  Record
+ * i is, byte for byte, what swb_save_envs saves of an env that has just taken the reset (FIRST)
+ * step of an episode whose scene is the sprite list [Sprite(**factors at (i, j)) for the occupied
+ * slots j, in slot order], packed by the host packer (scene.arrays_from_layout) with the packer's
+ * filters and colour map, with step_count[i] in place of 0 and goals[i] as its goals: live
+ * position = initial position, reset_next = 0, every padding byte zero.
+ *
+ * Columns: cols->col[f] is a device array [n][S] of factor f (x, y, shape, angle, scale, c0, c1, c2,
+ * x_vel, y_vel), element (i, j) at i * S + j, of dtype cols->kind[f] (SWB_FT_F32, F64, I8, I16, I32,
+ * I64 or U8), aligned to it; or NULL for Sprite's default as a Python scalar (x = y = 0.5, angle 0,
+ * scale 0.1, c0 = c1 = c2 = 0, x_vel = y_vel = 0.0), kind SWB_FT_PYFLOAT or SWB_FT_PYINT.  The shape
+ * column is required: ShapeType ids, 0 for an empty slot, in any of those dtypes.  Under
+ * SWB_COLOR_HSV the colour columns are all F32, all F64 or all NULL.  goals: device f64
+ * [n][G][2], required when G > 0 and refused when G = 0.  step_count: device int32 [n], or NULL for
+ * zeros.
+ *
+ * status[i] (device uint8 [n]) gets the SWB_MAKE_* bits of record i; a record with any bit set is
+ * written as zeros (it loads as an env with only empty slots).  span_flag (device uint8, may be
+ * NULL) is zeroed on `stream` and then set to 1 if an accepted record holds a star or spoke
+ * (ShapeType 7 .. 12): such records need span class 4 (swb_load_envs, swb_render_states).
+ *
+ * An accepted call with n > 0 is (after the span_flag memset) one launch on `stream`, one warp per
+ * record; n == 0 enqueues nothing.  Read-only for the engine: no env, pool entry, counter, frame
+ * buffer or span class changes.  Refused, enqueuing nothing: a null engine, no packer loaded, n < 0,
+ * null cols or shape column, a column of another kind or not aligned to it, a mixed HSV triple,
+ * goals missing for G > 0 or given for G = 0 or not 8-byte aligned, step_count not 4-byte aligned,
+ * records null, not 16-byte aligned or smaller than n records, a null status, and outputs (records,
+ * status, span_flag) that overlap each other or the inputs.
+ */
+enum {
+  SWB_MAKE_ANGLE = 1,  /* an occupied slot's angle is not an integer in [-360, 360] */
+  SWB_MAKE_SHAPE = 2,  /* a shape value is not an integer in 0 .. 12 */
+  SWB_MAKE_HOLE = 4,   /* an empty slot after an occupied one (a scene fills slots S - n .. S - 1) */
+  SWB_MAKE_INT = 8,    /* an occupied slot's integer factor of magnitude above 2^53 */
+  SWB_MAKE_STEP = 16   /* step_count < 0 */
+};
+typedef struct {
+  const void *col[10];  /* x, y, shape, angle, scale, c0, c1, c2, x_vel, y_vel; NULL: the default */
+  int32_t kind[10];     /* SWB_FT_* of each given column */
+} swb_factor_columns;
+
+int swb_packer_load(swb_engine *eng, const swb_scene_program *prog);
+int swb_make_states(swb_engine *eng, const swb_factor_columns *cols, int32_t n, const double *goals,
+                    const int32_t *step_count, void *records, uint64_t records_bytes, uint8_t *status,
+                    uint8_t *span_flag, void *stream);
+
+/*
  * Engine checkpoints: the whole state of an engine -- live positions and counters, every scene of
  * every ring and the device sampler's refill bookkeeping -- as one self-describing buffer in HOST
  * memory, to write to disk and load into an engine of the same configuration (in another process

@@ -156,6 +156,8 @@ def load():
   L.swb_set_goals_dev.argtypes = [vp, vp, ci, ci, vp, vp]
   L.swb_evaluate_states.argtypes = [vp, vp, ci, ctypes.c_uint64, vp, vp, vp, vp, vp]
   L.swb_sample_contained.argtypes = [vp, vp, ci, ctypes.c_uint64, ci, ctypes.c_uint64, vp, vp, vp, vp]
+  L.swb_packer_load.argtypes = [vp, vp]
+  L.swb_make_states.argtypes = [vp, vp, ci, vp, vp, vp, ctypes.c_uint64, vp, vp, vp]
   if L.swb_sizeof_config() != ctypes.sizeof(Config):
     raise NativeError('ABI mismatch: swb_config is %d bytes in the library, %d in the binding'
                       % (L.swb_sizeof_config(), ctypes.sizeof(Config)))
@@ -177,7 +179,7 @@ EXPORTS = (
     'swb_sampler_pointers', 'swb_pool_pointers', 'swb_engine_state_bytes', 'swb_save_engine',
     'swb_load_engine', 'swb_pool_goal_pointer', 'swb_set_goals', 'swb_set_goals_dev', 'swb_evaluate_states',
     'swb_sample_contained', 'swb_render_coverage', 'swb_render_soft_masks', 'swb_render_boxes',
-    'swb_rollout_trajectory')
+    'swb_rollout_trajectory', 'swb_packer_load', 'swb_make_states')
 
 
 def check(rc):

@@ -12,7 +12,8 @@ import sys
 CSRC = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'csrc')
 LIB = os.path.join(CSRC, 'libspriteworld_b200.so')
 SOURCES = ['swb_api.cu']
-HEADERS = ['swb_contained.cuh', 'swb_device.cuh', 'swb_masks.cuh', 'swb_render.cuh', 'swb_rollout.cuh', 'swb_sampler.cuh', 'swb_states.cuh', 'swb_step.cuh', 'swb_tables.h',
+HEADERS = ['swb_contained.cuh', 'swb_device.cuh', 'swb_make_states.cuh', 'swb_masks.cuh', 'swb_record_layout.h',
+           'swb_render.cuh', 'swb_rollout.cuh', 'swb_sampler.cuh', 'swb_states.cuh', 'swb_step.cuh', 'swb_tables.h',
            os.path.join('..', '..', 'include', 'spriteworld_b200.h')]
 
 NVCC_FLAGS = [
@@ -65,6 +66,7 @@ def build_host(force=False):
 SAMPLER_HOST_LIB = os.path.join(CSRC, 'libswb_sampler_host.so')
 SAMPLER_HOST_SRC = os.path.join(CSRC, 'swb_sampler_host.cpp')
 SAMPLER_HOST_INPUTS = [SAMPLER_HOST_SRC, os.path.join(CSRC, 'swb_sampler.cuh'), os.path.join(CSRC, 'swb_contained.cuh'),
+                       os.path.join(CSRC, 'swb_make_states.cuh'), os.path.join(CSRC, 'swb_record_layout.h'),
                        os.path.join(CSRC, '..', '..', 'include', 'spriteworld_b200.h')]
 # the same arithmetic as the kernels built with -fmad=false: no contraction
 SAMPLER_HOST_FLAGS = ['-O2', '-std=c++17', '-ffp-contract=off', '-fPIC', '-shared', '-Wall', '-Wextra']

@@ -10,6 +10,7 @@
 
 #include "swb_contained.cuh"
 #include "swb_device.cuh"
+#include "swb_make_states.cuh"
 #include "swb_masks.cuh"
 #include "swb_render.cuh"
 #include "swb_rollout.cuh"
@@ -91,6 +92,9 @@ struct swb_engine {
   int64_t env_offset = 0;
   int64_t *d_refilled_upto = nullptr;
   swb_sampler_status *d_sampler_status = nullptr;
+  // the packer of swb_make_states (swb_packer_load): filters, colour mode and angle table
+  swb_scene_program *d_packer = nullptr;
+  bool packer_hsv = false;
   std::vector<void *> owned;
   // buffers of swb_step_host
   void *h_actions = nullptr;
@@ -172,7 +176,7 @@ int upload_axis(swb_raster *r, const AxisHost &h, AxisTables *d) {
 extern "C" {
 
 const char *swb_last_error(void) { return g_error.c_str(); }
-int swb_version(void) { return 16; }
+int swb_version(void) { return 17; }
 int swb_sizeof_config(void) { return (int)sizeof(swb_config); }
 int swb_sizeof_task_node(void) { return (int)sizeof(swb_task_node); }
 
@@ -298,6 +302,7 @@ void swb_engine_destroy(swb_engine *eng) {
     }
   cudaFree(eng->d_records);
   cudaFree(eng->d_prog); cudaFree(eng->d_refilled_upto); cudaFree(eng->d_sampler_status);
+  cudaFree(eng->d_packer);
   cudaFree(eng->h_actions); cudaFree(eng->h_out.reward); cudaFree(eng->h_out.step_type);
   cudaFree(eng->h_out.success); cudaFree(eng->h_out.status); cudaFree(eng->h_frames);
   if (eng->copy_stream) cudaStreamDestroy(eng->copy_stream);
@@ -1649,6 +1654,102 @@ int swb_pool_pointers(swb_engine *eng, double **f64, uint32_t **member, uint8_t 
   for (int i = 0; i < 8; ++i) f64[i] = p[i];
   *member = st.p_member; *shape = st.p_shape; *pos_f32 = st.p_pos_f32; *rgb = st.p_rgb;
   *factors = st.p_factors;
+  return 0;
+}
+
+int swb_packer_load(swb_engine *eng, const swb_scene_program *prog) {
+  static const char fn[] = "swb_packer_load";
+  if (!eng || !prog) return fail("%s: null argument", fn);
+  if (check_program(*prog, eng->st.S)) return 1;
+  if (prog->color_mode != SWB_COLOR_RGB && prog->color_mode != SWB_COLOR_HSV)
+    return fail("%s: color_mode %d is neither SWB_COLOR_RGB nor SWB_COLOR_HSV", fn, prog->color_mode);
+  // make_states_kernel looks up only angles it has checked to be integers in [-360, 360]
+  auto has = [&](double a) {
+    for (int i = 0; i < prog->n_angles; ++i)
+      if (prog->angle[i] == a && std::signbit(prog->angle[i]) == std::signbit(a)) return true;
+    return false;
+  };
+  if (!has(-0.0)) return fail("%s: the angle table lacks -0.0", fn);
+  for (int a = -360; a <= 360; ++a)
+    if (!has((double)a)) return fail("%s: the angle table lacks %d", fn, a);
+  CUDA_TRY(cudaSetDevice(eng->device));
+  if (!eng->d_packer && dev_alloc(&eng->d_packer, 1) != cudaSuccess) {
+    eng->d_packer = nullptr;
+    return fail("%s: device allocation failed", fn);
+  }
+  CUDA_TRY(cudaDeviceSynchronize());  // a make_states call in flight may still read the old packer
+  CUDA_TRY(cudaMemcpy(eng->d_packer, prog, sizeof(swb_scene_program), cudaMemcpyHostToDevice));
+  eng->packer_hsv = prog->color_mode == SWB_COLOR_HSV;
+  return 0;
+}
+
+int swb_make_states(swb_engine *eng, const swb_factor_columns *cols, int32_t n, const double *goals,
+                    const int32_t *step_count, void *records, uint64_t records_bytes, uint8_t *status,
+                    uint8_t *span_flag, void *stream_) {
+  static const char fn[] = "swb_make_states";
+  static const char *const names[swb_sampler::kFactors] = {"x", "y", "shape", "angle", "scale",
+                                                          "c0", "c1", "c2", "x_vel", "y_vel"};
+  if (!eng) return fail("%s: null engine", fn);
+  if (!eng->d_packer) return fail("%s: no packer (swb_packer_load)", fn);
+  if (n < 0) return fail("%s: n = %d", fn, n);
+  if (!cols) return fail("%s: null cols", fn);
+  if (!cols->col[swb_sampler::F_SHAPE]) return fail("%s: the shape column is required", fn);
+  const int S = eng->st.S, G = eng->st.G;
+  const uint64_t cells = (uint64_t)n * S;
+  Span ins[swb_sampler::kFactors + 2];
+  int n_ins = 0;
+  for (int f = 0; f < swb_sampler::kFactors; ++f) {
+    if (!cols->col[f]) continue;
+    unsigned size = 0;
+    switch (cols->kind[f]) {
+      case SWB_FT_F64: case SWB_FT_I64: size = 8; break;
+      case SWB_FT_F32: case SWB_FT_I32: size = 4; break;
+      case SWB_FT_I16: size = 2; break;
+      case SWB_FT_I8: case SWB_FT_U8: size = 1; break;
+      default: return fail("%s: column %s has kind %d: not SWB_FT_F32, F64, I8, I16, I32, I64 or U8", fn,
+                           names[f], cols->kind[f]);
+    }
+    if (reinterpret_cast<uintptr_t>(cols->col[f]) % size)
+      return fail("%s: column %s is not %u-byte aligned", fn, names[f], size);
+    ins[n_ins++] = Span{names[f], cols->col[f], cells * size, size};
+  }
+  // hsv_to_rgb takes the triple in one dtype (the device sampler refuses the same mixes)
+  if (eng->packer_hsv) {
+    auto color_kind = [&](int f) { return cols->col[f] ? cols->kind[f] : (int)SWB_FT_NONE; };
+    const int k0 = color_kind(swb_sampler::F_C0);
+    if (k0 != color_kind(swb_sampler::F_C1) || k0 != color_kind(swb_sampler::F_C2) ||
+        (k0 != SWB_FT_NONE && k0 != SWB_FT_F32 && k0 != SWB_FT_F64))
+      return fail("%s: under hsv_to_rgb the colour columns c0, c1, c2 must be all float32, all float64 or all "
+                  "omitted, got kinds %d, %d, %d", fn, k0, color_kind(swb_sampler::F_C1),
+                  color_kind(swb_sampler::F_C2));
+  }
+  if (G ? !goals : goals != nullptr)
+    return G ? fail("%s: the task tree samples %d goals per scene: goals are required", fn, G)
+             : fail("%s: goals given, but the task tree samples no goals (G = 0)", fn);
+  if (reinterpret_cast<uintptr_t>(goals) % 8) return fail("%s: goals are not 8-byte aligned", fn);
+  if (reinterpret_cast<uintptr_t>(step_count) % 4) return fail("%s: step_count is not 4-byte aligned", fn);
+  if (goals) ins[n_ins++] = Span{"goals", goals, (uint64_t)n * G * 16, 8};
+  if (step_count) ins[n_ins++] = Span{"step_count", step_count, (uint64_t)n * 4, 4};
+  if (!records) return fail("%s: null records", fn);
+  if (check_record_buffer(eng, fn, "records", records, records_bytes, n)) return 1;
+  const uint64_t rb = RecordLayout(S, G).bytes();
+  Span outs[3] = {{"records", records, n * rb, 16}, {"status", status, (uint64_t)n, 1}};
+  const int n_outs = span_flag ? 3 : 2;
+  if (span_flag) outs[2] = Span{"span_flag", span_flag, 1, 1};
+  if (check_outputs(fn, outs, n_outs, Span{nullptr, nullptr, 0, 1})) return 1;
+  for (int i = 0; i < n_outs; ++i)
+    for (int k = 0; k < n_ins; ++k)
+      if (overlap(outs[i], ins[k])) return fail("%s: %s overlaps %s", fn, outs[i].name, ins[k].name);
+  if (n == 0) return 0;
+  CUDA_TRY(cudaSetDevice(eng->device));
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (span_flag) CUDA_TRY(cudaMemsetAsync(span_flag, 0, 1, stream));
+  const unsigned blocks = (unsigned)(((int64_t)n + MAKE_WARPS - 1) / MAKE_WARPS);
+  make_states_kernel<<<blocks, MAKE_WARPS * 32, 0, stream>>>(
+      eng->d_packer, *cols, n, S, G, goals, step_count, static_cast<unsigned char *>(records), (size_t)rb, status,
+      span_flag);
+  eng->launches++;
+  CUDA_TRY(cudaGetLastError());
   return 0;
 }
 

@@ -1,8 +1,9 @@
-// The device scene sampler (swb_sampler.cuh) and contained-position sampler (swb_contained.cuh)
-// built for the CPU: the restatement the tests hold the CUDA kernels to, and a way to draw the
-// device's scenes without a GPU.  Same source, no
+// The device scene sampler (swb_sampler.cuh), contained-position sampler (swb_contained.cuh) and
+// record maker (swb_make_states.cuh) built for the CPU: the restatement the tests hold the CUDA
+// kernels to, and a way to draw the device's scenes without a GPU.  Same source, no
 // contraction (-ffp-contract=off), so it computes what the kernels compute, bit for bit.
 #include "swb_contained.cuh"
+#include "swb_make_states.cuh"
 #include "swb_sampler.cuh"
 
 extern "C" {
@@ -71,6 +72,38 @@ void swb_host_sample_contained(const double *x, const double *y, const double *m
       status[t] = (uint8_t)swb_contained::sample_contained(seed, (uint64_t)i, (uint64_t)s, S, verts, nverts,
                                                            shape_at, sprite_at, position + 2 * t, slot + t);
     }
+  }
+}
+
+// swb_make_states on the host, over host arrays laid out as the device call takes them (columns
+// [n][S], goals [n][G][2] or null for G = 0, step_count [n] or null), into n records of
+// record_bytes bytes each, status [n] and *span_flag (may be null; set to 1 if an accepted record
+// holds a star or spoke, else left as it is).
+void swb_host_make_states(const swb_scene_program *prog, const swb_factor_columns *cols, int32_t n, int32_t S,
+                          int32_t G, const double *goals, const int32_t *step_count, unsigned char *records,
+                          uint64_t record_bytes, uint8_t *status, uint8_t *span_flag) {
+  swb_sampler::Sprite s[SWB_MAX_SLOTS];
+  bool occupied[SWB_MAX_SLOTS];
+  for (int64_t r = 0; r < n; ++r) {
+    uint32_t occ = 0, bits = 0;
+    bool any_concave = false;
+    for (int j = 0; j < S; ++j) {
+      bool concave = false;
+      bits |= swb_make::read_slot(*cols, (size_t)r * S + j, s[j], occupied[j], concave);
+      occ |= (uint32_t)occupied[j] << j;
+      any_concave = any_concave || concave;
+    }
+    const int32_t step = step_count ? step_count[r] : 0;
+    const uint32_t st = swb_make::record_status(bits, occ, S, step);
+    unsigned char *rec = records + (size_t)r * record_bytes;
+    for (int j = 0; j < S; ++j) {
+      swb_sampler::Packed o;
+      swb_make::pack_slot(*prog, s[j], occupied[j], st, o);
+      swb_make::write_slot(rec, S, G, j, o);
+    }
+    swb_make::write_header(rec, S, G, st ? 0 : step, st || !G ? nullptr : goals + (size_t)r * G * 2);
+    status[r] = (uint8_t)st;
+    if (span_flag && any_concave && !st) *span_flag = 1;
   }
 }
 

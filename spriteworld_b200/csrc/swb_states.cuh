@@ -26,25 +26,9 @@
 #include <cstdint>
 
 #include "swb_device.cuh"
+#include "swb_record_layout.h"
 
 namespace swb {
-
-// Byte offsets of the fields of one record of an engine with S slots and G goal slots.
-struct RecordLayout {
-  int S, G;
-  __host__ __device__ explicit RecordLayout(int S_, int G_ = 0) : S(S_), G(G_) {}
-  // x0, y0, m00, m01, m10, m11, vx, vy, pos_x, pos_y: f64 [10][S] from offset 0
-  __host__ __device__ size_t member() const { return 80 * (size_t)S; }      // u32 [S]
-  __host__ __device__ size_t rgb() const { return 84 * (size_t)S; }         // u32 [S]
-  __host__ __device__ size_t factors() const { return 88 * (size_t)S; }     // f32 [5][S]
-  __host__ __device__ size_t step_count() const { return 108 * (size_t)S; } // i32
-  __host__ __device__ size_t reset_next() const { return 108 * (size_t)S + 4; }  // u8
-  __host__ __device__ size_t shape() const { return 108 * (size_t)S + 5; }  // u8 [S]
-  __host__ __device__ size_t pos_f32() const { return 109 * (size_t)S + 5; }  // u8 [S]
-  __host__ __device__ size_t goals() const { return (110 * (size_t)S + 5 + 7) & ~(size_t)7; }  // f64 [G][2]
-  __host__ __device__ size_t used() const { return G ? goals() + 16 * (size_t)G : 110 * (size_t)S + 5; }
-  __host__ __device__ size_t bytes() const { return (used() + 15) & ~(size_t)15; }  // zero padded
-};
 
 // One slot of a record in registers; the per-env fields ride along in every slot's copy.
 struct SlotRecord {

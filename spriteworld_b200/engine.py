@@ -937,6 +937,95 @@ class Engine(object):
         self._stream()))
     return position, slot, status
 
+  # -- env records from factor values ----------------------------------------------------
+  def span_class(self):
+    """The engine's spans per sprite row, as save_envs reports it: 1 while every uploaded or loaded
+    shape is convex, else 4.  Enqueues nothing."""
+    span = ctypes.c_int32()
+    _native.check(self._lib.swb_save_envs(self._h, None, 0, None, 0, ctypes.byref(span), self._stream()))
+    return span.value
+
+  def load_packer(self, program):
+    """Gives the engine the packer of make_states (scene_program.compile_packer: task filters, colour
+    map and angle table).  Synchronises."""
+    from spriteworld_b200 import scene_program
+    if self._lib.swb_sampler_sizeof_program() != ctypes.sizeof(scene_program.Program):
+      raise _native.NativeError('ABI mismatch: swb_scene_program')
+    _native.check(self._lib.swb_packer_load(self._h, ctypes.byref(program.struct)))
+    self._packer = program
+
+  def make_states(self, factors, goals=None, step_count=None, span_class=None, out=None):
+    """Env records of scenes chosen by the caller (swb_make_states): (EnvStates, status uint8 (n,)).
+
+    `factors`: dict keyed by a subset of sprite.FACTOR_NAMES.  'shape' is required, (n, n_slots),
+    ShapeType ids with 0 for an empty slot; every other value broadcasts to (n, n_slots).  All are
+    tensors on this device of dtype float32, float64, int8, int16, int32, int64 or uint8; an omitted
+    factor is Sprite's default.  Record i is what save_envs would save of an env right after the
+    reset step of an episode whose scene is [Sprite(**factors at (i, j)) for its occupied slots j],
+    packed with the loaded packer's filters and colour map, with step_count[i] (int32 (n,), default
+    zeros) and goals[i] (float64 (n, G, 2), required when G > 0).  status[i] holds the
+    scene_program.MAKE_* bits of a refused record, which is written as zeros.
+
+    `span_class`: 1 or 4, the EnvStates' span class.  None reads one device flag back -- the call's
+    only host synchronisation -- and gives 4 if an accepted record holds a star or spoke, else
+    span_class().  `out`: EnvStates of n records to fill instead of new ones.  One launch on the
+    current stream; nothing of the engine changes."""
+    from spriteworld_b200 import scene_program, sprite
+    packer = getattr(self, '_packer', None)
+    if packer is None:
+      raise ValueError('make_states: no packer loaded (load_packer)')
+    if not isinstance(factors, dict) or 'shape' not in factors:
+      raise ValueError("make_states: factors must be a dict with a 'shape' entry")
+    unknown = sorted(set(factors) - set(sprite.FACTOR_NAMES))
+    if unknown:
+      raise ValueError('make_states: unknown factors %s (factors are %s)' % (unknown, ', '.join(sprite.FACTOR_NAMES)))
+    shape = factors['shape']
+    if not isinstance(shape, torch.Tensor) or shape.dim() != 2 or shape.shape[1] != self.n_slots:
+      raise ValueError("make_states: factors['shape'] must be a (n, %d) tensor, got %s"
+                       % (self.n_slots, _describe(shape)))
+    n = int(shape.shape[0])
+    for name, t in factors.items():
+      if (not isinstance(t, torch.Tensor) or t.device != self.device or t.dtype not in _MAKE_DTYPES
+          or not _broadcasts(t.shape, (n, self.n_slots))):
+        raise ValueError('make_states: factors[%r] must be a float32, float64, int8, int16, int32, int64 or '
+                         'uint8 tensor on %s that broadcasts to (%d, %d), got %s'
+                         % (name, self.device, n, self.n_slots, _describe(t)))
+    if packer.struct.color_mode == scene_program.COLOR_HSV:
+      kinds = [factors[c].dtype if c in factors else None for c in ('c0', 'c1', 'c2')]
+      if len(set(kinds)) != 1 or kinds[0] not in (None, torch.float32, torch.float64):
+        raise ValueError('make_states: under hsv_to_rgb the colours c0, c1, c2 must be all float32, all '
+                         'float64 or all omitted, got %s' % [str(k).replace('torch.', '') for k in kinds])
+    if goals is not None or self.n_goals:
+      if goals is None:
+        raise ValueError('make_states: the task samples %d goals per scene: goals (n, %d, 2) are required'
+                         % (self.n_goals, self.n_goals))
+      goals = self._check_goals(goals, n, 'make_states')
+    if step_count is not None:
+      _check_output(step_count, 'step_count', torch.int32, (n,), self.device, align=4)
+    if span_class not in (None, 1, 4):
+      raise ValueError('make_states: span_class must be None, 1 or 4, got %r' % (span_class,))
+    if out is None:
+      out = EnvStates(torch.empty((n, self.record_bytes), dtype=torch.uint8, device=self.device), 1,
+                      self.signature, self.n_slots, self.n_goals)
+    else:
+      self.check_states(out, n)
+    status = torch.empty(n, dtype=torch.uint8, device=self.device)
+    flag = torch.empty(1, dtype=torch.uint8, device=self.device) if span_class is None else None
+    cols, keep = scene_program.FactorColumns(), []
+    for f, name in enumerate(sprite.FACTOR_NAMES):
+      if name in factors:
+        t = factors[name].expand(n, self.n_slots).contiguous()
+        keep.append(t)
+        cols.col[f], cols.kind[f] = _address(t).value, _MAKE_DTYPES[t.dtype]
+    _native.check(self._lib.swb_make_states(
+        self._h, ctypes.byref(cols), n, None if goals is None else _address(goals),
+        None if step_count is None else _address(step_count), _address(out.data), out.data.numel(),
+        _address(status), None if flag is None else _address(flag), self._stream()))
+    if span_class is None:
+      span_class = 4 if n and int(flag.item()) else self.span_class()
+    out.span_class = span_class
+    return out, status
+
   def launch_count(self):
     return int(self._lib.swb_launch_count(self._h))
 
@@ -990,6 +1079,15 @@ def record_layout(n_slots, n_goals=0):
 
 
 _ID_DTYPES = {torch.int32: _native.DTYPE_I32, torch.int64: _native.DTYPE_I64}
+# the dtypes of make_states' factor columns and their SWB_FT_* kinds
+_MAKE_DTYPES = {torch.float32: 1, torch.float64: 2, torch.int8: 3, torch.int16: 4, torch.int32: 5,
+                torch.int64: 6, torch.uint8: 7}
+
+
+def _broadcasts(shape, to):
+  """True if a tensor of `shape` broadcasts to `to` (without growing its rank beyond it)."""
+  shape = tuple(shape)
+  return len(shape) <= len(to) and all(a in (1, b) for a, b in zip(shape[::-1], to[::-1]))
 # swb_ids_status
 _IDS_STATUS = np.dtype([('ok', '<u4'), ('failed', '<u4'), ('call', '<i4'), ('arg', '<i4'), ('reason', '<i4'),
                         ('position', '<i4'), ('value', '<i8')])

@@ -821,6 +821,45 @@ class BatchedEnvironment(object):
       self._engine.copy_envs(src_ids, dst_ids)
     self._resets += 1
 
+  def make_states(self, factors, goals=None, step_count=None, span_class=None):
+    """Env records of scenes the caller chose: (EnvStates, status uint8 (n,)), made on the device
+    from factor tensors, for datasets from factor samples, interventions on one factor of one
+    sprite, fixed evaluation suites (load_envs) and rendering predicted factors.
+
+    `factors`: dict keyed by a subset of sprite.FACTOR_NAMES.  'shape' (n, n_slots) is required:
+    constants.ShapeType ids, 0 for an empty slot, in any of the dtypes below (the float32 'shape' of
+    factor_tensors goes straight back in).  Every other value broadcasts to (n, n_slots).  All are
+    tensors on the engine's device of dtype float32, float64, int8, int16, int32, int64 or uint8; an
+    omitted factor is Sprite's default (x = y = 0.5, angle 0, scale 0.1, colours 0, velocities 0.0).
+    Under color_maps.hsv_to_rgb c0, c1 and c2 are all float32, all float64 or all omitted.  `goals`:
+    float64 (n, G, 2), required when the task samples goals (G > 0) and refused otherwise.
+    `step_count`: int32 (n,), default zeros.
+
+    Record i is, byte for byte, what save_envs saves of an env that has just taken the reset (FIRST)
+    step of an episode -- with step_count[i] in place of 0 -- whose scene is
+    [Sprite(**factors at (i, j)) for the occupied slots j, in slot order], packed with this
+    environment's task filters and colour map, and whose goals are goals[i].  A scene of k sprites
+    fills slots n_slots - k .. n_slots - 1.  status[i] holds the scene_program.MAKE_* bits of a
+    refused record, which is written as zeros (an env with only empty slots): MAKE_ANGLE, an
+    occupied slot's angle is not an integer in [-360, 360]; MAKE_SHAPE, a shape value is not an
+    integer in 0 .. 12; MAKE_HOLE, an empty slot after an occupied one; MAKE_INT, an occupied slot's
+    integer factor of magnitude above 2^53; MAKE_STEP, step_count < 0.
+
+    `span_class` (1 or 4) is the records' span class.  None reads one device flag back -- the call's
+    only host synchronisation -- and gives 4 if a record holds a star or spoke, else the engine's.
+    A caller who passes it avoids the read; stars made under class 1 render with ENV_SPAN_OVERFLOW
+    set, never as a wrong frame.
+
+    One launch on the current stream (the first call also uploads the packer, synchronising once).
+    Read-only: no env, scene ring, frame buffer or `rng` changes, and nothing counts against the
+    ring's refill.  A colour map other than None and hsv_to_rgb raises NotImplementedError."""
+    if getattr(self, '_packer', None) is None:
+      from spriteworld_b200 import scene_program
+      packer = scene_program.compile_packer(self._filters, self._color_to_rgb)
+      self._engine.load_packer(packer)
+      self._packer = packer
+    return self._engine.make_states(factors, goals, step_count, span_class)
+
   def rollout(self, actions, states=None):
     """Scores C candidate action sequences of T steps per env from the state every env is in now,
     in one kernel launch, and leaves every env as it is: no position, counter, scene ring or

@@ -73,6 +73,17 @@ class SampleOut(ctypes.Structure):
                'factors', 'factor_value', 'factor_kind', 'goal')]
 
 
+class FactorColumns(ctypes.Structure):
+  """swb_factor_columns: a pointer and an SWB_FT_* kind per factor (NULL: Sprite's default)."""
+  _fields_ = [('col', ctypes.c_void_p * len(FACTORS)), ('kind', _c32 * len(FACTORS))]
+
+
+# the dtypes a factor column of swb_make_states may have, and their SWB_FT_* kinds
+MAKE_KINDS = {np.dtype(t): _NP_KINDS[np.dtype(t)]
+              for t in (np.float32, np.float64, np.int8, np.int16, np.int32, np.int64, np.uint8)}
+MAKE_ANGLE, MAKE_SHAPE, MAKE_HOLE, MAKE_INT, MAKE_STEP = 1, 2, 4, 8, 16   # SWB_MAKE_*
+
+
 class SceneProgram(object):
   """A compiled scene generator: `struct` (the ctypes swb_scene_program), `max_sprites`, and
   `describe(op)`, the distribution a rejection loop draws from (for the reference's error)."""
@@ -134,6 +145,7 @@ class _Compiler(object):
   def __init__(self):
     self.ops, self.consts, self.kinds = [], [], []
     self.pending_dist, self.pending_pred = [], []
+    self.pred_pc = {}   # op of each distribution's predicate code, by id
     self.angles = {}   # angle values by bit pattern (0.0 and -0.0 are distinct)
     self.angle(0.0)    # the default angle 0
     self.rejections = {}
@@ -286,6 +298,16 @@ class _Compiler(object):
     return kind, [float(v) for v in cands]
 
   # -- predicates (containment) ------------------------------------------------------------
+  def predicate(self, d):
+    """Op index of the predicate code of `d` (containment), emitted once per distribution object."""
+    if id(d) not in self.pred_pc:
+      if _stack_depth(d) > MAX_STACK:
+        _refuse('a containment test nested more than %d deep' % MAX_STACK)
+      self.pred_pc[id(d)] = len(self.ops)
+      self.pred(d)
+      self.op(P_RET)
+    return self.pred_pc[id(d)]
+
   def pred(self, d):
     if isinstance(d, fd.Continuous):
       self.op(P_CONT, key=_key(d.key), a=_const_kind(d.minval, 'bound'), b=_const_kind(d.maxval, 'bound'),
@@ -382,15 +404,7 @@ def compile_program(init_sprites, filters=(), color_to_rgb=None, goals=()):
   """SceneProgram of a scene generator, the task's filter distributions (bit i of `member` is
   filters[i]), the PILRenderers' colour map and the task's goal distributions (goal slot i is drawn
   by goals[i], after the scene's sprites; tasks.AbstractTask.goal_distributions)."""
-  from spriteworld_b200.renderers import color_maps
-  if color_to_rgb is None:
-    color_mode = COLOR_RGB
-  elif color_to_rgb is color_maps.hsv_to_rgb:
-    color_mode = COLOR_HSV
-  else:
-    _refuse('the colour map %r: only None (RGB colours) and color_maps.hsv_to_rgb' % (color_to_rgb,))
-  if len(filters) > MAX_FILTERS:
-    _refuse('more than %d task filters' % MAX_FILTERS)
+  color_mode = _color_mode(color_to_rgb, filters)
   if len(goals) > MAX_GOALS:
     _refuse('more than %d sampled goals' % MAX_GOALS)
   for d in goals:
@@ -431,20 +445,28 @@ def compile_program(init_sprites, filters=(), color_to_rgb=None, goals=()):
       c.dist(dist)
       c.op(D_RET)
     goal_pcs.append(done[id(dist)])
-  pred_pc = {}
-
-  def predicate(d):
-    if id(d) not in pred_pc:
-      if _stack_depth(d) > MAX_STACK:
-        _refuse('a containment test nested more than %d deep' % MAX_STACK)
-      pred_pc[id(d)] = len(c.ops)
-      c.pred(d)
-      c.op(P_RET)
-    return pred_pc[id(d)]
-
   for i, d in c.pending_pred:
-    c.ops[i]['a'] = predicate(d)
-  filter_pcs = [predicate(f) for f in filters]
+    c.ops[i]['a'] = c.predicate(d)
+  filter_pcs = [c.predicate(f) for f in filters]
+  return SceneProgram(_program_struct(c, most, color_mode, filter_pcs, goal_pcs), most, c.rejections)
+
+
+def _color_mode(color_to_rgb, filters):
+  """COLOR_RGB or COLOR_HSV of a PILRenderer colour map; refuses other maps and too many filters."""
+  from spriteworld_b200.renderers import color_maps
+  if color_to_rgb is None:
+    mode = COLOR_RGB
+  elif color_to_rgb is color_maps.hsv_to_rgb:
+    mode = COLOR_HSV
+  else:
+    _refuse('the colour map %r: only None (RGB colours) and color_maps.hsv_to_rgb' % (color_to_rgb,))
+  if len(filters) > MAX_FILTERS:
+    _refuse('more than %d task filters' % MAX_FILTERS)
+  return mode
+
+
+def _program_struct(c, most, color_mode, filter_pcs, goal_pcs):
+  """The swb_scene_program of compiler `c`'s code, constants and angles."""
   if len(c.ops) > MAX_OPS or len(c.consts) > MAX_CONSTS or len(c.angles) > MAX_ANGLES:
     _refuse('a program of %d ops, %d constants and %d angles (limits %d, %d, %d)'
             % (len(c.ops), len(c.consts), len(c.angles), MAX_OPS, MAX_CONSTS, MAX_ANGLES))
@@ -467,7 +489,26 @@ def compile_program(init_sprites, filters=(), color_to_rgb=None, goals=()):
   for i, a in enumerate(angles):
     th = math.radians(a)
     p.angle[i], p.angle_cos[i], p.angle_sin[i] = a, math.cos(th), math.sin(th)
-  return SceneProgram(p, most, c.rejections)
+  return p
+
+
+PACKER_ANGLES = tuple(range(-360, 361))   # the integer angles a packer takes (and -0.0)
+
+
+def compile_packer(filters=(), color_to_rgb=None):
+  """SceneProgram of the packer of Engine.make_states: no generator (its code is a lone G_END), the
+  task's filter distributions (bit i of `member` is filters[i]) as compile_program compiles them,
+  the colour map's mode, and the angle table of every integer angle in [-360, 360] and -0.0 (libm's
+  cos / sin of their radians, as scene.transform_matrix takes them).  NotImplementedError for a
+  colour map other than None and color_maps.hsv_to_rgb, more than MAX_FILTERS filters, or a filter
+  compile_program refuses."""
+  color_mode = _color_mode(color_to_rgb, filters)
+  c = _Compiler()
+  c.op(G_END)
+  for a in PACKER_ANGLES + (-0.0,):
+    c.angle(a)
+  filter_pcs = [c.predicate(f) for f in filters]
+  return SceneProgram(_program_struct(c, 0, color_mode, filter_pcs, []), 0, {})
 
 
 # -- the CPU build of the sampler ----------------------------------------------------------
@@ -491,6 +532,9 @@ def _host_lib():
     L.swb_host_sample_contained.argtypes = [vp] * 7 + [ctypes.c_int32, ctypes.c_int32, vp, vp, ctypes.c_int32,
                                                         ctypes.c_uint64, vp, vp, vp]
     L.swb_host_sample_contained.restype = None
+    L.swb_host_make_states.argtypes = [vp, vp, ctypes.c_int32, ctypes.c_int32, ctypes.c_int32, vp, vp, vp,
+                                       ctypes.c_uint64, vp, vp]
+    L.swb_host_make_states.restype = None
     if L.swb_host_sampler_sizeof_program() != ctypes.sizeof(Program):
       raise RuntimeError('ABI mismatch: swb_scene_program')
     _host = L
@@ -536,6 +580,35 @@ def sample_on_host(program, seed, env_ids, scene_idx, n_slots):
       ctypes.byref(program.struct), int(seed) & (2 ** 64 - 1), int(n_slots), env_ids.ctypes.data,
       scene_idx.ctypes.data, n, ctypes.byref(sample_out_struct(b)), ctypes.byref(op), ctypes.byref(idx))
   return b, ((int(idx.value), int(op.value)) if failures else None)
+
+
+def make_states_on_host(packer, columns, n_slots, n_goals=0, goals=None, step_count=None):
+  """swb_make_states on the CPU, built from the kernel's own source (swb_make_states.cuh): `columns`
+  is a dict factor name -> (n, S) array of a MAKE_KINDS dtype ('shape' required; a missing factor
+  takes Sprite's default), goals float64 (n, n_goals, 2), step_count int32 (n,) or None for zeros.
+  Returns (records uint8 (n, record bytes), status uint8 (n,), span flag: True if an accepted record
+  holds a star or spoke)."""
+  from spriteworld_b200 import engine
+  shape = np.asarray(columns['shape'])
+  n, S = shape.shape
+  assert S == n_slots, (S, n_slots)
+  cols, keep = FactorColumns(), []
+  for f, name in enumerate(FACTORS):
+    if name in columns:
+      a = np.ascontiguousarray(columns[name])
+      assert a.shape == (n, S) and a.dtype in MAKE_KINDS, (name, a.shape, a.dtype)
+      keep.append(a)
+      cols.col[f], cols.kind[f] = a.ctypes.data, MAKE_KINDS[a.dtype]
+  _, rb = engine.record_layout(S, n_goals)
+  records = np.zeros((n, rb), np.uint8)
+  status = np.zeros(n, np.uint8)
+  flag = np.zeros(1, np.uint8)
+  g = None if not n_goals else np.ascontiguousarray(goals, np.float64).reshape(n, n_goals, 2)
+  sc = None if step_count is None else np.ascontiguousarray(step_count, np.int32).reshape(n)
+  _host_lib().swb_host_make_states(
+      ctypes.byref(packer.struct), ctypes.byref(cols), n, S, int(n_goals), None if g is None else g.ctypes.data,
+      None if sc is None else sc.ctypes.data, records.ctypes.data, rb, status.ctypes.data, flag.ctypes.data)
+  return records, status, bool(flag[0])
 
 
 def shape_table(shapes=None):

@@ -22,7 +22,9 @@ into leaves, from those leaves, and from the live envs into leaves, renders of r
 coverage (swb_render_coverage) of live envs and records into buffers that are not 16-byte aligned,
 their soft masks (swb_render_soft_masks) into buffers at odd byte offsets, their boxes
 (swb_render_boxes) at 4-byte offsets that are not 16-byte aligned, and an engine
-checkpoint saved, loaded and rendered, with a corrupt one refused.
+checkpoint saved, loaded and rendered, with a corrupt one refused.  Records are then made from
+factor columns (swb_make_states) of every column dtype, with refused records among them, into a
+record buffer one record past the start of its allocation, and rendered.
 """
 import ctypes
 import os
@@ -60,6 +62,7 @@ def main():
     raster.close()
     eng.close()
   device_checked_records(torch)
+  made_records(torch)
   persistent_mixed(torch)
 
 
@@ -163,6 +166,32 @@ def device_checked_records(torch):
   torch.cuda.synchronize()
   assert torch.equal(eng.save_state(), state)
   print('checkpoint: %d bytes saved and loaded, a corrupt one refused' % state.numel(), flush=True)
+  raster.close()
+  eng.close()
+
+
+def made_records(torch):
+  from spriteworld_b200 import engine, scene_program, workloads
+  from spriteworld_b200 import factor_distributions as distribs
+  from spriteworld_b200.renderers import color_maps
+  wl = workloads.WORKLOADS['c3']()
+  eng, raster, _ = workloads.build_engine(wl, 8, 2, device=0, seed=3)
+  eng.load_packer(scene_program.compile_packer([distribs.Continuous('c0', 0.0, 0.5)], color_maps.hsv_to_rgb))
+  n, S, rb = 37, eng.n_slots, eng.record_bytes
+  rng = np.random.RandomState(5)
+  buf = torch.zeros((n + 1, rb), dtype=torch.uint8, device='cuda')
+  out = engine.EnvStates(buf[1:], 1, eng.signature, S)
+  for dt in (torch.float32, torch.float64, torch.int8, torch.int16, torch.int32, torch.int64, torch.uint8):
+    shape = torch.from_numpy(rng.randint(0, 13, (n, S))).cuda().to(dt)
+    shape[:, -1] = 8
+    factors = {'shape': shape, 'x': torch.rand(n, S, device='cuda').to(dt), 'angle': torch.zeros(n, 1, device='cuda').to(dt),
+               'c0': torch.rand(n, S, device='cuda'), 'c1': torch.rand(1, S, device='cuda'), 'c2': torch.rand(n, 1, device='cuda')}
+    states, status = eng.make_states(factors, out=out)
+    eng.render_states(raster, states)
+    eng.make_states({'shape': shape[:0]}, span_class=1)
+  torch.cuda.synchronize()
+  print('made records: %d per dtype, %d refused in the last, %d kernel launches'
+        % (n, int((status != 0).sum()), eng.launch_count()), flush=True)
   raster.close()
   eng.close()
 
