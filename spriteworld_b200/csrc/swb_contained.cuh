@@ -16,6 +16,7 @@
 // kernel tests a float64 click c against slot k with c - pos in float64, so a click at the returned
 // position grabs slot k or a sprite above it.
 #pragma once
+#include "swb_record_layout.h"
 #include "swb_sampler.cuh"
 
 namespace swb_contained {
@@ -24,11 +25,6 @@ namespace swb_contained {
 struct Sprite {
   double x, y, m00, m01, m10, m11;
 };
-
-// A shape id as swb_load_envs sanitises a record's: one without a vertex table is an empty slot.
-SWB_HD int sanitize(int shape, const int32_t *nverts) {
-  return shape < SWB_NUM_SHAPES && nverts[shape] >= 3 ? shape : 0;
-}
 
 // Vertex j of the centred path, as warp_contains transforms it: (m00 ax + m01 ay) + 0.0.
 SWB_HD void centred(const Sprite &sp, const double *v, int j, double &cx, double &cy) {
@@ -59,7 +55,7 @@ SWB_HD bool contains(const Sprite &sp, const double *v, int n, double tx, double
   return inside;
 }
 
-// Sample s of row i.  `shape_at(j)` gives slot j's raw shape id (0 .. S-1), `sprite_at(j)` slot j's
+// Sample s of row i.  `shape_at(j)` gives slot j's shape id (0 .. S-1), `sprite_at(j)` slot j's
 // Sprite; only the chosen slot's sprite is read.  verts / nverts: the engine's shape table
 // ([SWB_NUM_SHAPES][SWB_MAX_VERTS][2], [SWB_NUM_SHAPES]).  Writes pos[0..1] and *slot, returns the
 // status (SWB_ENV_OK, SWB_ENV_NO_SPRITE or SWB_ENV_SAMPLE_TRIES).
@@ -70,14 +66,14 @@ SWB_HD int sample_contained(uint64_t seed, uint64_t i, uint64_t s, int S, const 
   pos[0] = pos[1] = nan("");
   *slot = -1;
   int m = 0;
-  for (int j = 0; j < S; ++j) m += sanitize(shape_at(j), nverts) != 0;
+  for (int j = 0; j < S; ++j) m += swb::sanitize_shape(shape_at(j), nverts) != 0;
   if (m == 0) return SWB_ENV_NO_SPRITE;
   swb_sampler::Stream rng;
   rng.init(seed, i, s, SWB_CONTAINED_DOMAIN);
   int k = (int)rng.below(m);
   int j = 0, shape = 0;
   for (;; ++j) {
-    shape = sanitize(shape_at(j), nverts);
+    shape = swb::sanitize_shape(shape_at(j), nverts);
     if (shape && k-- == 0) break;
   }
   const Sprite sp = sprite_at(j);
@@ -132,14 +128,15 @@ contained_kernel(DevState st, const unsigned char *__restrict__ records, size_t 
   const int S = st.S;
   const unsigned char *const rec = kRecords ? records + (size_t)i * record_bytes : nullptr;
   const size_t entry = kRecords ? 0 : ((size_t)i * st.K + st.cursor[i]) * S;
-  const RecordLayout L(S);
-  auto shape_at = [&](int j) -> int { return kRecords ? rec[L.shape() + j] : st.p_shape[entry + j]; };
+  auto shape_at = [&](int j) -> int {
+    return kRecords ? read_record(st, rec, j).shape : st.p_shape[entry + j];
+  };
   auto sprite_at = [&](int j) {
     swb_contained::Sprite sp;
     if (kRecords) {
-      const double *f64 = reinterpret_cast<const double *>(rec);  // [10][S], see RecordLayout
-      sp.x = f64[8 * S + j]; sp.y = f64[9 * S + j];
-      sp.m00 = f64[2 * S + j]; sp.m01 = f64[3 * S + j]; sp.m10 = f64[4 * S + j]; sp.m11 = f64[5 * S + j];
+      const SlotRecord r = read_record(st, rec, j);
+      sp.x = r.f64[POS_X]; sp.y = r.f64[POS_Y];
+      sp.m00 = r.f64[M00]; sp.m01 = r.f64[M01]; sp.m10 = r.f64[M10]; sp.m11 = r.f64[M11];
     } else {
       sp.x = st.pos_x[(size_t)i * S + j]; sp.y = st.pos_y[(size_t)i * S + j];
       sp.m00 = st.p_m00[entry + j]; sp.m01 = st.p_m01[entry + j];

@@ -5,7 +5,8 @@
 // per record, one lane per slot (make_states_kernel), and csrc/swb_sampler_host.cpp builds the same
 // functions for the CPU (swb_host_make_states), the restatement the tests hold the kernel to.  A
 // record is made in three steps: read_slot per slot (its factors and its SWB_MAKE_* bits),
-// record_status over the record's slots, then write_slot per slot and write_header once.
+// record_status over the record's slots, then swb::write_record of make_slot per slot and
+// swb::write_goals once.
 #pragma once
 #include "swb_record_layout.h"
 #include "swb_sampler.cuh"
@@ -81,36 +82,26 @@ SWB_HD uint32_t record_status(uint32_t slot_bits, uint32_t occupied, int S, int3
   return bits;
 }
 
-// Slot j of a record (S slots, G goal slots): the packed scene fields, live position = initial.
-SWB_HD void write_slot(unsigned char *rec, int S, int G, int j, const Packed &o) {
-  const swb::RecordLayout L(S, G);
-  double *f64 = reinterpret_cast<double *>(rec);
-  const double v[10] = {o.x, o.y, o.m00, o.m01, o.m10, o.m11, o.vx, o.vy, o.x, o.y};
-  for (int a = 0; a < 10; ++a) f64[a * S + j] = v[a];
-  reinterpret_cast<uint32_t *>(rec + L.member())[j] = o.member;
-  reinterpret_cast<uint32_t *>(rec + L.rgb())[j] =
-      (uint32_t)o.rgb[0] | ((uint32_t)o.rgb[1] << 8) | ((uint32_t)o.rgb[2] << 16);
-  for (int f = 0; f < 5; ++f) reinterpret_cast<float *>(rec + L.factors())[f * S + j] = o.factors[f];
-  rec[L.shape() + j] = o.shape;
-  rec[L.pos_f32() + j] = o.pos_f32;
-}
-
-// The per-record fields: step_count, reset_next = 0, the goals (zeros for null) and every padding byte.
-SWB_HD void write_header(unsigned char *rec, int S, int G, int32_t step, const double *goals) {
-  const swb::RecordLayout L(S, G);
-  *reinterpret_cast<int32_t *>(rec + L.step_count()) = step;
-  rec[L.reset_next()] = 0;
-  const size_t g0 = G ? L.goals() : L.bytes(), g1 = G ? L.used() : L.bytes();
-  for (size_t b = 110 * (size_t)S + 5; b < g0; ++b) rec[b] = 0;
-  double *g = reinterpret_cast<double *>(rec + L.goals());
-  for (int q = 0; q < 2 * G; ++q) g[q] = goals ? goals[q] : 0.0;
-  for (size_t b = g1; b < L.bytes(); ++b) rec[b] = 0;
-}
-
-// Slot j's packed fields: the sprite's, or an empty slot's (also every slot of a refused record).
-SWB_HD void pack_slot(const swb_scene_program &p, const Sprite &s, bool occupied, uint32_t status, Packed &o) {
+// A record's slot: the sprite's packed fields, or an empty slot's (also every slot of a refused
+// record), with live position = initial, step_count `step` and reset_next = 0.
+SWB_HD swb::SlotRecord make_slot(const swb_scene_program &p, const Sprite &s, bool occupied, uint32_t status,
+                                 int32_t step) {
+  Packed o;
   if (occupied && !status) swb_sampler::pack_sprite(p, s, o);
   else swb_sampler::empty_slot(o);
+  swb::SlotRecord r;
+  r.f64[swb::X0] = r.f64[swb::POS_X] = o.x;
+  r.f64[swb::Y0] = r.f64[swb::POS_Y] = o.y;
+  r.f64[swb::M00] = o.m00; r.f64[swb::M01] = o.m01; r.f64[swb::M10] = o.m10; r.f64[swb::M11] = o.m11;
+  r.f64[swb::VX] = o.vx; r.f64[swb::VY] = o.vy;
+  r.member = o.member;
+  r.rgb = (uint32_t)o.rgb[0] | ((uint32_t)o.rgb[1] << 8) | ((uint32_t)o.rgb[2] << 16);
+  for (int f = 0; f < 5; ++f) r.factors[f] = o.factors[f];
+  r.shape = o.shape;
+  r.pos_f32 = o.pos_f32;
+  r.reset_next = 0;
+  r.step_count = step;
+  return r;
 }
 
 }  // namespace swb_make
@@ -137,16 +128,13 @@ __global__ void __launch_bounds__(MAKE_WARPS * 32) make_states_kernel(
   const int32_t step = step_count ? step_count[r] : 0;
   const uint32_t st = swb_make::record_status(any_bits, occ, S, step);
   unsigned char *rec = records + (size_t)r * record_bytes;
-  if (j < S) {
-    swb_sampler::Packed o;
-    swb_make::pack_slot(*prog, s, occupied, st, o);
-    swb_make::write_slot(rec, S, G, j, o);
-  }
+  // lane 0's per-record stores first, so that nothing they need stays live across the packer
   if (j == 0) {
-    swb_make::write_header(rec, S, G, st ? 0 : step, st || !G ? nullptr : goals + (size_t)r * G * 2);
+    write_goals(record_goals(rec, S, G), st || !G ? nullptr : goals + (size_t)r * G * 2, G);
     status[r] = (uint8_t)st;
     if (span_flag && any_concave && !st) *span_flag = 1;
   }
+  if (j < S) write_record(rec, S, G, j, swb_make::make_slot(*prog, s, occupied, st, st ? 0 : step));
 }
 
 }  // namespace swb

@@ -159,15 +159,14 @@ mask_kernel(DevState st, const MaskLayout L, uint8_t *__restrict__ masks, const 
   const unsigned char *const rec = kRecords ? recs.rec + e * recs.record_bytes : nullptr;
   for (int s = warp; s < S; s += NWARP) {
     const size_t scene = (e * st.K + cur) * S + s;
-    const RecordLayout rl(S);
-    const double *const f64 = reinterpret_cast<const double *>(rec);  // [10][S], see RecordLayout
-    const int shape = kRecords ? sanitize_shape(st, rec[rl.shape() + s]) : st.p_shape[scene];
-    const double px = kRecords ? f64[8 * S + s] : st.pos_x[e * S + s];
-    const double py = kRecords ? f64[9 * S + s] : st.pos_y[e * S + s];
-    const double m00 = kRecords ? f64[2 * S + s] : st.p_m00[scene];
-    const double m01 = kRecords ? f64[3 * S + s] : st.p_m01[scene];
-    const double m10 = kRecords ? f64[4 * S + s] : st.p_m10[scene];
-    const double m11 = kRecords ? f64[5 * S + s] : st.p_m11[scene];
+    const SlotRecord r = kRecords ? read_record(st, rec, s) : SlotRecord{};
+    const int shape = kRecords ? r.shape : st.p_shape[scene];
+    const double px = kRecords ? r.f64[POS_X] : st.pos_x[e * S + s];
+    const double py = kRecords ? r.f64[POS_Y] : st.pos_y[e * S + s];
+    const double m00 = kRecords ? r.f64[M00] : st.p_m00[scene];
+    const double m01 = kRecords ? r.f64[M01] : st.p_m01[scene];
+    const double m10 = kRecords ? r.f64[M10] : st.p_m10[scene];
+    const double m11 = kRecords ? r.f64[M11] : st.p_m11[scene];
     const int nv = shape ? st.shape_n[shape] : 0;
     const int t = s * EV + lane;
     int ivx = 0, ivy = 0;

@@ -275,9 +275,9 @@ __constant__ uint32_t c_prmt_insert[4] = {0x3214u, 0x3240u, 0x3410u, 0x4210u};  
 // frames and segment tables leave room for few CTAs per SM anyway, so their register budget is
 // set for R_CTAS_PER_SM_WIDE.
 // kRecords: item e is record e of recs (swb_render_states), not live env e: phase A reads the
-// record's pool-entry fields and live positions (RecordLayout) instead of the pool entry at
-// (e, cursor[e]), with shape ids sanitised as a load sanitises them; frame e and status byte e are
-// the record's.  Nothing indexed by env is read, so n may exceed E.  No peer variant.
+// record's slots (read_record) instead of the pool entry at (e, cursor[e]) and the live positions,
+// with shape ids sanitised as a load sanitises them; frame e and status byte e are the record's.
+// Nothing indexed by env is read, so n may exceed E.  No peer variant.
 template <bool kPeers, bool kWide, bool kRecords>
 __global__ void __launch_bounds__(R_THREADS, kWide ? R_CTAS_PER_SM_WIDE : R_CTAS_PER_SM)
 render_kernel(DevState st, RasterDev rd, const RenderLayout L, const RenderTargets targets,
@@ -386,16 +386,15 @@ render_kernel(DevState st, RasterDev rd, const RenderLayout L, const RenderTarge
   for (int s = warp; s < S; s += NWARP) {
     // sprite record of this env's current scene, or slot s of record e (warp-uniform loads)
     const int scene = (e * st.K + cur) * S + s;
-    const RecordLayout rl(S);
-    const double *const f64 = reinterpret_cast<const double *>(rec);  // [10][S], see RecordLayout
-    const int shape = kRecords ? sanitize_shape(st, rec[rl.shape() + s]) : st.p_shape[scene];
-    const uint32_t col = kRecords ? reinterpret_cast<const uint32_t *>(rec + rl.rgb())[s] : st.p_rgb[scene];
-    const double px = kRecords ? f64[8 * S + s] : st.pos_x[e * S + s];
-    const double py = kRecords ? f64[9 * S + s] : st.pos_y[e * S + s];
-    const double m00 = kRecords ? f64[2 * S + s] : st.p_m00[scene];
-    const double m01 = kRecords ? f64[3 * S + s] : st.p_m01[scene];
-    const double m10 = kRecords ? f64[4 * S + s] : st.p_m10[scene];
-    const double m11 = kRecords ? f64[5 * S + s] : st.p_m11[scene];
+    const SlotRecord r = kRecords ? read_record(st, rec, s) : SlotRecord{};
+    const int shape = kRecords ? r.shape : st.p_shape[scene];
+    const uint32_t col = kRecords ? r.rgb : st.p_rgb[scene];
+    const double px = kRecords ? r.f64[POS_X] : st.pos_x[e * S + s];
+    const double py = kRecords ? r.f64[POS_Y] : st.pos_y[e * S + s];
+    const double m00 = kRecords ? r.f64[M00] : st.p_m00[scene];
+    const double m01 = kRecords ? r.f64[M01] : st.p_m01[scene];
+    const double m10 = kRecords ? r.f64[M10] : st.p_m10[scene];
+    const double m11 = kRecords ? r.f64[M11] : st.p_m11[scene];
     const int nv = shape ? st.shape_n[shape] : 0;
     const int t = s * EV + lane;
     // integer canvas vertex of this lane

@@ -47,34 +47,36 @@ struct RolloutRecords {
 // velocity.
 __device__ __forceinline__ void stage_record(const DevState &st, WarpSprites &ws, int S,
                                              const unsigned char *rec, int lane, double *vx, double *vy) {
-  if (lane < 2 * st.G) ws.goal[lane] = record_goals(st, rec)[lane];
+  if (lane < 2 * st.G) ws.goal[lane] = record_goals(rec, S, st.G)[lane];
   *vx = 0.; *vy = 0.;
   if (lane < S) {
     const SlotRecord r = read_record(st, rec, lane);
     ws.shape[lane] = r.shape;
     ws.f32[lane] = r.pos_f32;
     ws.member[lane] = r.member;
-    ws.m00[lane] = r.f64[2]; ws.m01[lane] = r.f64[3];
-    ws.m10[lane] = r.f64[4]; ws.m11[lane] = r.f64[5];
-    ws.x[lane] = r.f64[8]; ws.y[lane] = r.f64[9];
-    *vx = r.f64[6]; *vy = r.f64[7];
+    ws.m00[lane] = r.f64[M00]; ws.m01[lane] = r.f64[M01];
+    ws.m10[lane] = r.f64[M10]; ws.m11[lane] = r.f64[M11];
+    ws.x[lane] = r.f64[POS_X]; ws.y[lane] = r.f64[POS_Y];
+    *vx = r.f64[VX]; *vy = r.f64[VY];
   }
   __syncwarp();
 }
 
 // Slot `lane` of the record a plan from root e (record `root`, else live env e) has reached: the
-// root's scene fields read now, the positions in ws, step_count `count` (lane 0's copy is the one
-// write_record stores) and reset_next `last`.
+// root's slot read now, with the positions in ws, step_count `count` (lane 0's copy is the one
+// write_record stores) and reset_next `last` -- unless the root was resetting, which takes no step.
 template <bool kRecordRoots>
-__device__ __forceinline__ void write_plan_record(const DevState &st, const WarpSprites &ws,
-                                                  const unsigned char *root, int e, int lane, int count,
-                                                  bool last, unsigned char *dst) {
+__device__ __forceinline__ SlotRecord plan_record(const DevState &st, const WarpSprites &ws,
+                                                  const unsigned char *root, int e, int lane, bool resetting,
+                                                  int count, bool last) {
   SlotRecord r = kRecordRoots ? read_record(st, root, lane) : read_state(st, e, lane);
-  r.f64[8] = ws.x[lane];
-  r.f64[9] = ws.y[lane];
-  r.step_count = count;
-  r.reset_next = last ? 1 : 0;
-  write_record(dst, st.S, st.G, lane, r);
+  if (!resetting) {
+    r.f64[POS_X] = ws.x[lane];
+    r.f64[POS_Y] = ws.y[lane];
+    r.step_count = count;
+    r.reset_next = last ? 1 : 0;
+  }
+  return r;
 }
 
 // kRecordRoots: roots are io.roots (else the E live envs); kLeaves: write io.leaves; kTrajectory
@@ -97,13 +99,12 @@ rollout_kernel(DevState st, const StepCfg *__restrict__ step_cfg, const void *__
   const unsigned char *root = kRecordRoots ? io.roots + (size_t)e * io.record_bytes : nullptr;
   // else the env's next step starts another scene: nothing to plan in
   const bool resetting = kRecordRoots ? root[L.reset_next()] != 0 : st.reset_next[e] != 0;
-  // a leaf keeps its root's goals: stored now, before the plan keeps registers busy
-  if (kLeaves && lane < 2 * st.G)
-    record_goals(st, io.leaves + (size_t)w * io.record_bytes)[lane] =
-        (kRecordRoots ? record_goals(st, root) : state_goals(st, e))[lane];
-  if (kTrajectory && lane < 2 * st.G) {
-    const double g = (kRecordRoots ? record_goals(st, root) : state_goals(st, e))[lane];
-    for (int p = 0; p < T; ++p) record_goals(st, io.leaves + ((size_t)p * EC + w) * io.record_bytes)[lane] = g;
+  // a leaf (every trajectory entry) keeps its root's goals: stored now, before the plan keeps
+  // registers busy
+  if ((kLeaves || kTrajectory) && lane < 2 * st.G) {
+    const double g = (kRecordRoots ? record_goals(root, S, st.G) : state_goals(st, e))[lane];
+    for (int p = 0; p < (kTrajectory ? T : 1); ++p)
+      record_goals(io.leaves + ((size_t)p * EC + w) * io.record_bytes, S, st.G)[lane] = g;
   }
   int t = 0, count = 0;
   bool ended = false;
@@ -137,8 +138,8 @@ rollout_kernel(DevState st, const StepCfg *__restrict__ step_cfg, const void *__
       }
       step_type = __shfl_sync(0xFFFFFFFFu, step_type, 0);
       if (kTrajectory && lane < S)
-        write_plan_record<kRecordRoots>(st, ws, root, e, lane, count, step_type == SWB_STEP_LAST,
-                                        io.leaves + ((size_t)t * EC + w) * io.record_bytes);
+        write_record(io.leaves + ((size_t)t * EC + w) * io.record_bytes, S, st.G, lane,
+                     plan_record<kRecordRoots>(st, ws, root, e, lane, resetting, count, step_type == SWB_STEP_LAST));
       t++;
       if (step_type == SWB_STEP_LAST) {
         ended = true;
@@ -155,25 +156,12 @@ rollout_kernel(DevState st, const StepCfg *__restrict__ step_cfg, const void *__
   }
   if (kTrajectory && lane < S && t < T) {
     // the end state repeats: the plan's last record, or the root itself
-    SlotRecord end = kRecordRoots ? read_record(st, root, lane) : read_state(st, e, lane);
-    if (!resetting) {
-      end.f64[8] = ws.x[lane];
-      end.f64[9] = ws.y[lane];
-      end.step_count = count;
-      end.reset_next = ended ? 1 : 0;
-    }
+    const SlotRecord end = plan_record<kRecordRoots>(st, ws, root, e, lane, resetting, count, ended);
     for (int p = t; p < T; ++p) write_record(io.leaves + ((size_t)p * EC + w) * io.record_bytes, S, st.G, lane, end);
   }
-  if (kLeaves && lane < S) {
-    SlotRecord leaf = kRecordRoots ? read_record(st, root, lane) : read_state(st, e, lane);
-    if (!resetting) {
-      leaf.f64[8] = ws.x[lane];
-      leaf.f64[9] = ws.y[lane];
-      leaf.step_count = count;   // lane 0 counted the steps; write_record stores slot 0's copy
-      leaf.reset_next = ended ? 1 : 0;
-    }
-    write_record(io.leaves + (size_t)w * io.record_bytes, S, st.G, lane, leaf);
-  }
+  if (kLeaves && lane < S)
+    write_record(io.leaves + (size_t)w * io.record_bytes, S, st.G, lane,
+                 plan_record<kRecordRoots>(st, ws, root, e, lane, resetting, count, ended));
 }
 
 // swb_evaluate_states: the task tree's value on record i (one warp each) at its live positions, with

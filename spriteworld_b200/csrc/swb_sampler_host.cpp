@@ -96,12 +96,9 @@ void swb_host_make_states(const swb_scene_program *prog, const swb_factor_column
     const int32_t step = step_count ? step_count[r] : 0;
     const uint32_t st = swb_make::record_status(bits, occ, S, step);
     unsigned char *rec = records + (size_t)r * record_bytes;
-    for (int j = 0; j < S; ++j) {
-      swb_sampler::Packed o;
-      swb_make::pack_slot(*prog, s[j], occupied[j], st, o);
-      swb_make::write_slot(rec, S, G, j, o);
-    }
-    swb_make::write_header(rec, S, G, st ? 0 : step, st || !G ? nullptr : goals + (size_t)r * G * 2);
+    for (int j = 0; j < S; ++j)
+      swb::write_record(rec, S, G, j, swb_make::make_slot(*prog, s[j], occupied[j], st, st ? 0 : step));
+    swb::write_goals(swb::record_goals(rec, S, G), st || !G ? nullptr : goals + (size_t)r * G * 2, G);
     status[r] = (uint8_t)st;
     if (span_flag && any_concave && !st) *span_flag = 1;
   }

@@ -30,22 +30,13 @@
 
 namespace swb {
 
-// One slot of a record in registers; the per-env fields ride along in every slot's copy.
-struct SlotRecord {
-  double f64[10];
-  uint32_t member, rgb;
-  float factors[5];
-  uint8_t shape, pos_f32, reset_next;
-  int32_t step_count;
-};
-
 __device__ __forceinline__ SlotRecord read_state(const DevState &st, int e, int s) {
   SlotRecord r;
   const size_t p = ((size_t)e * st.K + st.cursor[e]) * st.S + s, l = (size_t)e * st.S + s;
-  r.f64[0] = st.p_x[p]; r.f64[1] = st.p_y[p];
-  r.f64[2] = st.p_m00[p]; r.f64[3] = st.p_m01[p]; r.f64[4] = st.p_m10[p]; r.f64[5] = st.p_m11[p];
-  r.f64[6] = st.p_vx[p]; r.f64[7] = st.p_vy[p];
-  r.f64[8] = st.pos_x[l]; r.f64[9] = st.pos_y[l];
+  r.f64[X0] = st.p_x[p]; r.f64[Y0] = st.p_y[p];
+  r.f64[M00] = st.p_m00[p]; r.f64[M01] = st.p_m01[p]; r.f64[M10] = st.p_m10[p]; r.f64[M11] = st.p_m11[p];
+  r.f64[VX] = st.p_vx[p]; r.f64[VY] = st.p_vy[p];
+  r.f64[POS_X] = st.pos_x[l]; r.f64[POS_Y] = st.pos_y[l];
   r.member = st.p_member[p];
   r.rgb = st.p_rgb[p];
 #pragma unroll
@@ -59,10 +50,10 @@ __device__ __forceinline__ SlotRecord read_state(const DevState &st, int e, int 
 
 __device__ __forceinline__ void write_state(const DevState &st, int e, int s, const SlotRecord &r) {
   const size_t p = ((size_t)e * st.K + st.cursor[e]) * st.S + s, l = (size_t)e * st.S + s;
-  st.p_x[p] = r.f64[0]; st.p_y[p] = r.f64[1];
-  st.p_m00[p] = r.f64[2]; st.p_m01[p] = r.f64[3]; st.p_m10[p] = r.f64[4]; st.p_m11[p] = r.f64[5];
-  st.p_vx[p] = r.f64[6]; st.p_vy[p] = r.f64[7];
-  st.pos_x[l] = r.f64[8]; st.pos_y[l] = r.f64[9];
+  st.p_x[p] = r.f64[X0]; st.p_y[p] = r.f64[Y0];
+  st.p_m00[p] = r.f64[M00]; st.p_m01[p] = r.f64[M01]; st.p_m10[p] = r.f64[M10]; st.p_m11[p] = r.f64[M11];
+  st.p_vx[p] = r.f64[VX]; st.p_vy[p] = r.f64[VY];
+  st.pos_x[l] = r.f64[POS_X]; st.pos_y[l] = r.f64[POS_Y];
   st.p_member[p] = r.member;
   st.p_rgb[p] = r.rgb;
 #pragma unroll
@@ -75,67 +66,28 @@ __device__ __forceinline__ void write_state(const DevState &st, int e, int s, co
   }
 }
 
-// A shape id without a vertex table (a record that swb_save_envs did not write) is an empty slot
-// (0), so that no kernel indexes the shape table with it.  read_record and the record render path
-// (render_kernel<., ., true>) both take a record's shape ids through this.
-__device__ __forceinline__ int sanitize_shape(const DevState &st, int shape) {
-  return shape < SWB_NUM_SHAPES && st.shape_n[shape] >= 3 ? shape : 0;
-}
-
+// Slot s of a record, with its shape id sanitised as a load sanitises it.  Every kernel that reads
+// records reads them through this; the loads of fields a kernel does not use are dead code.
 __device__ __forceinline__ SlotRecord read_record(const DevState &st, const unsigned char *rec, int s) {
   const int S = st.S;
   const RecordLayout L(S);
   SlotRecord r;
-  const double *f64 = reinterpret_cast<const double *>(rec);
 #pragma unroll
-  for (int a = 0; a < 10; ++a) r.f64[a] = f64[a * S + s];
+  for (int a = 0; a < N_F64; ++a) r.f64[a] = reinterpret_cast<const double *>(rec)[L.f64_at(a, s)];
   r.member = reinterpret_cast<const uint32_t *>(rec + L.member())[s];
   r.rgb = reinterpret_cast<const uint32_t *>(rec + L.rgb())[s];
 #pragma unroll
   for (int f = 0; f < 5; ++f) r.factors[f] = reinterpret_cast<const float *>(rec + L.factors())[f * S + s];
-  r.shape = sanitize_shape(st, rec[L.shape() + s]);
+  r.shape = sanitize_shape(rec[L.shape() + s], st.shape_n);
   r.pos_f32 = rec[L.pos_f32() + s];
   r.step_count = *reinterpret_cast<const int32_t *>(rec + L.step_count());
   r.reset_next = rec[L.reset_next()];
   return r;
 }
 
-// Slot s of a record.  Slot 0 also zeroes the padding after the slot fields, around the goals
-// (which write_goals stores, in any order with this).
-__device__ __forceinline__ void write_record(unsigned char *rec, int S, int G, int s, const SlotRecord &r) {
-  const RecordLayout L(S, G);
-  double *f64 = reinterpret_cast<double *>(rec);
-#pragma unroll
-  for (int a = 0; a < 10; ++a) f64[a * S + s] = r.f64[a];
-  reinterpret_cast<uint32_t *>(rec + L.member())[s] = r.member;
-  reinterpret_cast<uint32_t *>(rec + L.rgb())[s] = r.rgb;
-#pragma unroll
-  for (int f = 0; f < 5; ++f) reinterpret_cast<float *>(rec + L.factors())[f * S + s] = r.factors[f];
-  rec[L.shape() + s] = r.shape;
-  rec[L.pos_f32() + s] = r.pos_f32;
-  if (s == 0) {
-    *reinterpret_cast<int32_t *>(rec + L.step_count()) = r.step_count;
-    rec[L.reset_next()] = r.reset_next;
-    // saved bytes are deterministic
-    const size_t g0 = G ? L.goals() : L.bytes(), g1 = G ? L.used() : L.bytes();
-    for (size_t b = 110 * (size_t)S + 5; b < g0; ++b) rec[b] = 0;
-    for (size_t b = g1; b < L.bytes(); ++b) rec[b] = 0;
-  }
-}
-
-// The goals (G x (x, y)) of the scene env e is on, of a record, and a copy of G of them (zeros when
-// src is null).
+// The goals (G x (x, y)) of the scene env e is on.
 __device__ __forceinline__ double *state_goals(const DevState &st, int e) {
   return st.p_goal + ((size_t)e * st.K + st.cursor[e]) * st.G * 2;
-}
-__device__ __forceinline__ const double *record_goals(const DevState &st, const unsigned char *rec) {
-  return reinterpret_cast<const double *>(rec + RecordLayout(st.S, st.G).goals());
-}
-__device__ __forceinline__ void write_goals(double *dst, const double *src, int G) {
-  for (int i = 0; i < 2 * G; ++i) dst[i] = src ? src[i] : 0.;
-}
-__device__ __forceinline__ double *record_goals(const DevState &st, unsigned char *rec) {
-  return reinterpret_cast<double *>(rec + RecordLayout(st.S, st.G).goals());
 }
 
 // The id lists of a record call (and of swb_set_goals) (swb_save_envs / swb_load_envs / swb_copy_envs and their _dev
@@ -239,7 +191,7 @@ __global__ void save_envs_kernel(DevState st, IdCall c, unsigned char *__restric
   const bool refused = call_refused(c);
   unsigned char *dst = rec + (size_t)r * record_bytes;
   write_record(dst, st.S, st.G, s, refused ? SlotRecord{} : read_state(st, id, s));
-  if (s == 0 && st.G) write_goals(record_goals(st, dst), refused ? nullptr : state_goals(st, id), st.G);
+  if (s == 0 && st.G) write_goals(record_goals(dst, st.S, st.G), refused ? nullptr : state_goals(st, id), st.G);
 }
 
 // Device-checked copy, first half: the repeat check of the destinations, and record i <- env
@@ -256,7 +208,7 @@ __global__ void stage_copy_dev_kernel(DevState st, IdCall c, unsigned char *__re
   if (id_in_range(id, st.E)) {
     unsigned char *dst = rec + (size_t)r * record_bytes;
     write_record(dst, st.S, st.G, s, read_state(st, (int)id, s));
-    if (s == 0 && st.G) write_goals(record_goals(st, dst), state_goals(st, (int)id), st.G);
+    if (s == 0 && st.G) write_goals(record_goals(dst, st.S, st.G), state_goals(st, (int)id), st.G);
   }
 }
 
@@ -271,7 +223,7 @@ __global__ void load_envs_kernel(DevState st, IdCall c, const unsigned char *__r
   const int id = (int)ids_of<T>(c, c.dst_arg)[r];
   const unsigned char *src = rec + (size_t)r * record_bytes;
   write_state(st, id, s, read_record(st, src, s));
-  if (s == 0 && st.G) write_goals(state_goals(st, id), record_goals(st, src), st.G);
+  if (s == 0 && st.G) write_goals(state_goals(st, id), record_goals(src, st.S, st.G), st.G);
 }
 
 // Host-checked copy of id sets that do not overlap (no thread reads what another writes):
