@@ -4,8 +4,10 @@
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
+#include <memory>
 #include <optional>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "swb_contained.cuh"
@@ -42,22 +44,80 @@ int fail(const char *fmt, ...) {
       return fail("%s failed: %s (%s:%d)", #expr, cudaGetErrorString(_e), __FILE__, __LINE__); \
   } while (0)
 
+}  // namespace
+
+// Owners of CUDA resources: each releases its resource when destroyed; they move but do not copy.
+struct FreeDev { void operator()(void *p) const { cudaFree(p); } };
+struct FreeHost { void operator()(void *p) const { cudaFreeHost(p); } };
+struct DestroyEvent { void operator()(cudaEvent_t e) const { cudaEventDestroy(e); } };
+struct DestroyStream { void operator()(cudaStream_t s) const { cudaStreamDestroy(s); } };
+template <typename T> using DevPtr = std::unique_ptr<T, FreeDev>;
+template <typename T> using HostPtr = std::unique_ptr<T, FreeHost>;
+using Event = std::unique_ptr<std::remove_pointer_t<cudaEvent_t>, DestroyEvent>;
+using Stream = std::unique_ptr<std::remove_pointer_t<cudaStream_t>, DestroyStream>;
+
+// *out <- a device array of n T (at least one), zero-filled unless `zero` is false.  The fill runs
+// on the legacy default stream and may finish after the call has returned.
 template <typename T>
-cudaError_t dev_alloc(T **p, size_t n) {
-  cudaError_t e = cudaMalloc(reinterpret_cast<void **>(p), (n ? n : 1) * sizeof(T));
-  if (e == cudaSuccess) e = cudaMemset(*p, 0, (n ? n : 1) * sizeof(T));
-  return e;
+static cudaError_t dev_alloc(DevPtr<T> *out, size_t n, bool zero = true) {
+  const size_t bytes = (n ? n : 1) * sizeof(T);
+  void *p = nullptr;
+  cudaError_t e = cudaMalloc(&p, bytes);
+  if (e == cudaSuccess) out->reset(static_cast<T *>(p));
+  return e == cudaSuccess && zero ? cudaMemset(p, 0, bytes) : e;
 }
 
-}  // namespace
+static cudaError_t make_event(Event *out) {
+  cudaEvent_t e = nullptr;
+  const cudaError_t err = cudaEventCreateWithFlags(&e, cudaEventDisableTiming);
+  if (err == cudaSuccess) out->reset(e);
+  return err;
+}
+
+// A buffer of at least the bytes last asked for.  grow(need, wait) keeps it if it holds `need`
+// bytes; else it calls wait(), which returns once nothing may still read the old bytes, frees them
+// and allocates `need` bytes.  If that allocation fails, the buffer is empty.
+template <typename Owner, cudaError_t (*Alloc)(void **, size_t)>
+struct Growable {
+  Owner buf;
+  size_t bytes = 0;
+  unsigned char *get() const { return buf.get(); }
+  template <typename Wait>
+  cudaError_t grow(size_t need, Wait wait) {
+    if (need <= bytes) return cudaSuccess;
+    cudaError_t e = buf ? wait() : cudaSuccess;
+    if (e != cudaSuccess) return e;
+    buf.reset();
+    bytes = 0;
+    void *p = nullptr;
+    if ((e = Alloc(&p, need)) != cudaSuccess) return e;
+    buf.reset(static_cast<unsigned char *>(p));
+    bytes = need;
+    return cudaSuccess;
+  }
+};
+using DevBuffer = Growable<DevPtr<unsigned char>, cudaMalloc>;
+using HostBuffer = Growable<HostPtr<unsigned char>, cudaMallocHost>;
+// The wait of a grow whose caller has already waited for every reader of the buffer.
+constexpr auto kWaited = [] { return cudaSuccess; };
+
+// The work that reads a buffer the host writes: an event recorded after the last of it.  wait()
+// returns once that work has finished (at once if none was recorded), with an event ready for the
+// next record().  The destructor waits too, so the buffers declared before an InFlight outlive
+// their readers.
+struct InFlight {
+  Event done;
+  cudaError_t wait() { return done ? cudaEventSynchronize(done.get()) : make_event(&done); }
+  cudaError_t record(cudaStream_t stream) { return cudaEventRecord(done.get(), stream); }
+  ~InFlight() { if (done) cudaEventSynchronize(done.get()); }
+};
 
 // A pinned host block and its device twin, grown on demand.  Two alternate (Staging::slots), so
 // the host fills call i+1 while call i's copy is queued; a slot is reused only after its event.
 struct StagingSlot {
-  size_t bytes = 0;
-  unsigned char *host = nullptr, *dev = nullptr;
-  cudaEvent_t done = nullptr;  // recorded after the kernels that read `dev`
-  bool in_flight = false;
+  HostBuffer host;
+  DevBuffer dev;
+  InFlight readers;  // the kernels that read `dev`
 };
 
 struct Staging {
@@ -65,51 +125,62 @@ struct Staging {
   int next = 0;
 };
 
+// The device scene sampler (swb_sampler_load): program, refill bookkeeping, first failure.
+struct SamplerDev {
+  DevPtr<swb_scene_program> prog;
+  DevPtr<int64_t> refilled_upto;
+  DevPtr<swb_sampler_status> status;
+};
+
+// swb_step_host's device copies of the actions and of the step outputs
+struct StepHostDev {
+  DevPtr<double> actions, reward;
+  DevPtr<int8_t> step_type;
+  DevPtr<uint8_t> success, status;
+  swb_step_out out() const { return {reward.get(), step_type.get(), success.get(), status.get()}; }
+};
+
+// swb_step_host's second stream: the D2H of frame chunks overlaps the render of the next chunk
+struct ChunkCopies {
+  Stream stream;
+  Event chunk_done[8], copies_done;
+};
+
 struct swb_engine {
   swb_config cfg;
   StepCfg step_cfg;
-  StepCfg *d_step_cfg = nullptr;  // device copy the step kernel reads (per engine)
-  unsigned *d_work = nullptr;     // render kernel's work counter (monotonic, see render_kernel)
-  unsigned work_base = 0;         // its value when the next launch starts
+  DevPtr<StepCfg> d_step_cfg;  // device copy the step kernel reads (per engine)
+  DevPtr<unsigned> d_work;     // render kernel's work counter (monotonic, see render_kernel)
+  unsigned work_base = 0;      // its value when the next launch starts
   int n_sms = 1;
   DevState st;
+  // the arrays of st; declared before every owner whose destructor waits for copies into them
+  std::vector<DevPtr<void>> arrays;
   int device = 0;
   int max_spans = 1;  // 1 while every uploaded shape is convex, else 4
   int64_t launches = 0;
   // scene uploads (from the refill thread, on its stream) and the ids of host-checked record
   // calls (on the step stream) stage apart, so that neither waits for or overwrites the other
   Staging upload_staging, id_staging;
-  // the records of a copy through engine scratch (grown on demand)
-  unsigned char *d_records = nullptr;
-  size_t records_bytes = 0;
+  DevBuffer records;  // the records of a copy through engine scratch
   // device-checked id lists (IdCall in swb_states.cuh): claims, the failure word, the status record
-  unsigned long long *d_id_claim = nullptr, *d_id_fail = nullptr;
-  swb_ids_status *d_id_status = nullptr;
+  DevPtr<unsigned long long> d_id_claim, d_id_fail;
+  DevPtr<swb_ids_status> d_id_status;
   uint32_t id_seq = 0;
-  // device scene sampler (swb_sampler_load): program, refill bookkeeping, first failure
-  swb_scene_program *d_prog = nullptr;
+  std::unique_ptr<SamplerDev> sampler;  // null until swb_sampler_load
   uint64_t seed = 0;
   int64_t env_offset = 0;
-  int64_t *d_refilled_upto = nullptr;
-  swb_sampler_status *d_sampler_status = nullptr;
   // the packer of swb_make_states (swb_packer_load): filters, colour mode and angle table
-  swb_scene_program *d_packer = nullptr;
+  DevPtr<swb_scene_program> d_packer;
   bool packer_hsv = false;
-  std::vector<void *> owned;
-  // buffers of swb_step_host
-  void *h_actions = nullptr;
-  swb_step_out h_out = {nullptr, nullptr, nullptr, nullptr};
-  uint8_t *h_frames = nullptr;
-  size_t h_frames_bytes = 0;
-  cudaStream_t copy_stream = nullptr;  // D2H of frame chunks overlaps the render of the next chunk
-  cudaEvent_t chunk_done[8] = {};
-  cudaEvent_t copies_done = nullptr;
-  // pinned staging of swb_save_engine / swb_load_engine (grown on demand); `ckpt_done` is recorded
-  // after the copies of the last load, which read it after the call has returned
-  unsigned char *h_ckpt = nullptr;
-  size_t h_ckpt_bytes = 0;
-  cudaEvent_t ckpt_done = nullptr;
-  bool ckpt_in_flight = false;
+  // buffers of swb_step_host, each group made on first use
+  std::unique_ptr<StepHostDev> step_host;
+  DevBuffer h_frames;
+  std::unique_ptr<ChunkCopies> chunk_copies;
+  // pinned staging of swb_save_engine / swb_load_engine; `ckpt_done` is recorded after the copies
+  // of the last load, which read it after the call has returned
+  HostBuffer h_ckpt;
+  InFlight ckpt_done;
 };
 
 struct swb_raster {
@@ -117,7 +188,7 @@ struct swb_raster {
   RasterDev rd;
   AxisHost ax, ay;
   int smem_rows = 0;
-  std::vector<void *> owned;
+  std::vector<DevPtr<void>> tables;  // the device arrays of rd
 };
 
 namespace {
@@ -153,11 +224,11 @@ __global__ void scatter_scenes_kernel(DevState st, int n, const int32_t *__restr
 
 template <typename T>
 int upload_vec(swb_raster *r, const std::vector<T> &v, const T **out) {
-  T *p = nullptr;
-  CUDA_TRY(cudaMalloc(reinterpret_cast<void **>(&p), std::max<size_t>(v.size(), 1) * sizeof(T)));
-  r->owned.push_back(p);
-  CUDA_TRY(cudaMemcpy(p, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice));
-  *out = p;
+  DevPtr<T> p;
+  CUDA_TRY(dev_alloc(&p, v.size(), false));
+  CUDA_TRY(cudaMemcpy(p.get(), v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice));
+  *out = p.get();
+  r->tables.push_back(std::move(p));
   return 0;
 }
 
@@ -217,12 +288,15 @@ int swb_engine_create(const swb_config *cfg, swb_engine **out) {
   for (int g = 0; g < n_goals; ++g)
     if (goal_nodes[g] < 0) return fail("goal slots must be 0 .. %d, slot %d has no node", n_goals - 1, g);
   if (cfg->action_kind < 0 || cfg->action_kind > SWB_ACT_EMBODIED) return fail("bad action_kind");
+  for (int s = 1; s < SWB_NUM_SHAPES; ++s)
+    if (cfg->shape_n_verts[s] < 0 || cfg->shape_n_verts[s] > SWB_MAX_VERTS)
+      return fail("shape %d has %d vertices (max %d)", s, cfg->shape_n_verts[s], SWB_MAX_VERTS);
   int n_dev = 0;
   CUDA_TRY(cudaGetDeviceCount(&n_dev));
   if (cfg->device < 0 || cfg->device >= n_dev) return fail("no CUDA device %d", cfg->device);
   CUDA_TRY(cudaSetDevice(cfg->device));
 
-  swb_engine *eng = new swb_engine();
+  std::unique_ptr<swb_engine> eng(new swb_engine());
   eng->cfg = *cfg;
   eng->device = cfg->device;
   if (cudaDeviceGetAttribute(&eng->n_sms, cudaDevAttrMultiProcessorCount, cfg->device) != cudaSuccess ||
@@ -246,9 +320,12 @@ int swb_engine_create(const swb_config *cfg, swb_engine **out) {
   st.G = n_goals;
   const size_t ES = (size_t)st.E * st.S, EKS = ES * st.K;
   bool ok = true;
-  auto A = [&](auto **p, size_t n) {
-    if (ok && dev_alloc(p, n) != cudaSuccess) ok = false;
-    if (ok) eng->owned.push_back(*p);
+  auto own = [&](auto *owner, size_t n) { ok = ok && dev_alloc(owner, n) == cudaSuccess; };
+  auto A = [&](auto **p, size_t n) {  // an array of st
+    DevPtr<std::remove_pointer_t<std::remove_pointer_t<decltype(p)>>> a;
+    own(&a, n);
+    *p = a.get();
+    eng->arrays.push_back(std::move(a));
   };
   A(&st.pos_x, ES); A(&st.pos_y, ES);
   A(&st.cursor, st.E); A(&st.step_count, st.E);
@@ -261,86 +338,43 @@ int swb_engine_create(const swb_config *cfg, swb_engine **out) {
   if (st.G) A(&st.p_goal, (size_t)st.E * st.K * st.G * 2);
   double *d_verts = nullptr;
   int32_t *d_nv = nullptr;
-  A(&eng->d_step_cfg, 1);
-  A(&eng->d_work, 1);
+  own(&eng->d_step_cfg, 1);
+  own(&eng->d_work, 1);
   A(&st.scene_serial, st.E);
   A(&d_verts, (size_t)SWB_NUM_SHAPES * SWB_MAX_VERTS * 2);
   A(&d_nv, SWB_NUM_SHAPES);
-  A(&eng->d_id_claim, st.E); A(&eng->d_id_fail, 1); A(&eng->d_id_status, 1);
-  if (!ok) {
-    swb_engine_destroy(eng);
-    return fail("device allocation failed: %s", cudaGetErrorString(cudaGetLastError()));
-  }
-  for (int s = 1; s < SWB_NUM_SHAPES; ++s)
-    if (cfg->shape_n_verts[s] < 0 || cfg->shape_n_verts[s] > SWB_MAX_VERTS) {
-      swb_engine_destroy(eng);
-      return fail("shape %d has %d vertices (max %d)", s, cfg->shape_n_verts[s], SWB_MAX_VERTS);
-    }
-  CUDA_TRY(cudaMemcpy(eng->d_step_cfg, &eng->step_cfg, sizeof(StepCfg), cudaMemcpyHostToDevice));
+  own(&eng->d_id_claim, st.E); own(&eng->d_id_fail, 1); own(&eng->d_id_status, 1);
+  if (!ok) return fail("device allocation failed: %s", cudaGetErrorString(cudaGetLastError()));
+  CUDA_TRY(cudaMemcpy(eng->d_step_cfg.get(), &eng->step_cfg, sizeof(StepCfg), cudaMemcpyHostToDevice));
   CUDA_TRY(cudaMemcpy(d_verts, cfg->shape_verts, sizeof cfg->shape_verts, cudaMemcpyHostToDevice));
   CUDA_TRY(cudaMemcpy(d_nv, cfg->shape_n_verts, sizeof cfg->shape_n_verts, cudaMemcpyHostToDevice));
   st.shape_verts = d_verts;
   st.shape_n = d_nv;
   // every env starts "about to reset" (environment.py:70)
   CUDA_TRY(cudaMemset(st.reset_next, 1, st.E));
-  CUDA_TRY(cudaMemset(eng->d_id_claim, 0xFF, (size_t)st.E * sizeof(unsigned long long)));
-  CUDA_TRY(cudaMemset(eng->d_id_fail, 0xFF, sizeof(unsigned long long)));
-  *out = eng;
+  CUDA_TRY(cudaMemset(eng->d_id_claim.get(), 0xFF, (size_t)st.E * sizeof(unsigned long long)));
+  CUDA_TRY(cudaMemset(eng->d_id_fail.get(), 0xFF, sizeof(unsigned long long)));
+  *out = eng.release();
   return 0;
 }
 
 void swb_engine_destroy(swb_engine *eng) {
   if (!eng) return;
   cudaSetDevice(eng->device);
-  for (void *p : eng->owned) cudaFree(p);
-  for (Staging *staging : {&eng->upload_staging, &eng->id_staging})
-    for (StagingSlot &slot : staging->slots) {
-      if (slot.in_flight) cudaEventSynchronize(slot.done);
-      if (slot.host) cudaFreeHost(slot.host);
-      if (slot.dev) cudaFree(slot.dev);
-      if (slot.done) cudaEventDestroy(slot.done);
-    }
-  cudaFree(eng->d_records);
-  cudaFree(eng->d_prog); cudaFree(eng->d_refilled_upto); cudaFree(eng->d_sampler_status);
-  cudaFree(eng->d_packer);
-  cudaFree(eng->h_actions); cudaFree(eng->h_out.reward); cudaFree(eng->h_out.step_type);
-  cudaFree(eng->h_out.success); cudaFree(eng->h_out.status); cudaFree(eng->h_frames);
-  if (eng->copy_stream) cudaStreamDestroy(eng->copy_stream);
-  for (auto &ev : eng->chunk_done) if (ev) cudaEventDestroy(ev);
-  if (eng->copies_done) cudaEventDestroy(eng->copies_done);
-  if (eng->ckpt_in_flight) cudaEventSynchronize(eng->ckpt_done);
-  if (eng->h_ckpt) cudaFreeHost(eng->h_ckpt);
-  if (eng->ckpt_done) cudaEventDestroy(eng->ckpt_done);
   delete eng;
 }
 
 // The next slot of `staging`, of at least `need` bytes, once the kernels that last read it have
-// finished.  The caller enqueues the copy to `dev` and the kernels that read it, then release_slot.
+// finished.  The caller enqueues the copy to `dev` and the kernels that read it, then records them
+// as the slot's readers.
 static int take_slot(Staging &staging, size_t need, StagingSlot **out) {
   StagingSlot &slot = staging.slots[staging.next];
   staging.next ^= 1;
-  if (slot.in_flight) {
-    CUDA_TRY(cudaEventSynchronize(slot.done));
-    slot.in_flight = false;
-  }
-  if (need > slot.bytes) {
-    if (slot.host) cudaFreeHost(slot.host);
-    if (slot.dev) cudaFree(slot.dev);
-    slot.host = slot.dev = nullptr;
-    slot.bytes = 0;
-    const size_t bytes = std::max<size_t>(need, 4096);
-    CUDA_TRY(cudaMallocHost(reinterpret_cast<void **>(&slot.host), bytes));
-    CUDA_TRY(cudaMalloc(reinterpret_cast<void **>(&slot.dev), bytes));
-    if (!slot.done) CUDA_TRY(cudaEventCreateWithFlags(&slot.done, cudaEventDisableTiming));
-    slot.bytes = bytes;
-  }
+  CUDA_TRY(slot.readers.wait());  // the host rewrites the slot whether or not it grows
+  const size_t bytes = std::max<size_t>(need, 4096);
+  CUDA_TRY(slot.host.grow(bytes, kWaited));
+  CUDA_TRY(slot.dev.grow(bytes, kWaited));
   *out = &slot;
-  return 0;
-}
-
-static int release_slot(StagingSlot *slot, cudaStream_t stream) {
-  CUDA_TRY(cudaEventRecord(slot->done, stream));
-  slot->in_flight = true;
   return 0;
 }
 
@@ -389,7 +423,7 @@ int swb_upload_scenes(swb_engine *eng, const swb_scene_soa *sc, const int32_t *e
   size_t off[8];
   StagingSlot *slot = nullptr;
   if (take_slot(eng->upload_staging, upload_layout(n, S, G, off), &slot)) return 1;
-  unsigned char *h = slot->host;
+  unsigned char *h = slot->host.get();
   for (int a = 0; a < 8; ++a)
     memcpy(h + off[0] + a * nS * sizeof(double), f64_src[a], nS * sizeof(double));
   memcpy(h + off[1], sc->member, nS * sizeof(uint32_t));
@@ -405,9 +439,9 @@ int swb_upload_scenes(swb_engine *eng, const swb_scene_soa *sc, const int32_t *e
   if (G) memcpy(h + off[7], sc->goal, (size_t)n * G * 2 * sizeof(double));
   // everything up to the end of the last used array, in one copy
   const size_t end = G ? off[7] + (size_t)n * G * 2 * sizeof(double) : off[6] + nS;
-  CUDA_TRY(cudaMemcpyAsync(slot->dev, slot->host, end, cudaMemcpyHostToDevice, stream));
+  CUDA_TRY(cudaMemcpyAsync(slot->dev.get(), h, end, cudaMemcpyHostToDevice, stream));
   const int threads = 256, blocks = (int)((nS + threads - 1) / threads);
-  unsigned char *d = slot->dev;
+  unsigned char *d = slot->dev.get();
   scatter_scenes_kernel<<<blocks, threads, 0, stream>>>(
       eng->st, n, reinterpret_cast<const int32_t *>(d + off[4]), reinterpret_cast<const double *>(d + off[0]),
       nS, reinterpret_cast<const uint32_t *>(d + off[1]), d + off[5], d + off[6],
@@ -415,7 +449,8 @@ int swb_upload_scenes(swb_engine *eng, const swb_scene_soa *sc, const int32_t *e
       reinterpret_cast<const double *>(d + off[7]));
   eng->launches++;
   CUDA_TRY(cudaGetLastError());
-  return release_slot(slot, stream);
+  CUDA_TRY(slot->readers.record(stream));
+  return 0;
 }
 
 int swb_request_reset(swb_engine *eng, const uint8_t *mask, void *stream_) {
@@ -450,7 +485,8 @@ static int launch_step(swb_engine *eng, const void *actions, int32_t action_dtyp
                        const swb_step_out &out, cudaStream_t stream, int mode) {
   CUDA_TRY(cudaSetDevice(eng->device));
   const int blocks = (eng->st.E + STEP_WARPS - 1) / STEP_WARPS;
-  step_kernel<<<blocks, STEP_WARPS * 32, 0, stream>>>(eng->st, eng->d_step_cfg, actions, action_dtype, out, mode);
+  step_kernel<<<blocks, STEP_WARPS * 32, 0, stream>>>(eng->st, eng->d_step_cfg.get(), actions, action_dtype, out,
+                                                      mode);
   eng->launches++;
   CUDA_TRY(cudaGetLastError());
   return 0;
@@ -501,8 +537,8 @@ static int enqueue_rollout(swb_engine *eng, const void *actions, int32_t action_
   auto kernel = trajectory ? (io.roots ? rollout_kernel<true, false, true> : rollout_kernel<false, false, true>)
                 : io.roots ? (io.leaves ? rollout_kernel<true, true> : rollout_kernel<true, false>)
                            : (io.leaves ? rollout_kernel<false, true> : rollout_kernel<false, false>);
-  kernel<<<blocks, ROLLOUT_WARPS * 32, 0, stream>>>(eng->st, eng->d_step_cfg, actions, action_dtype, n_steps,
-                                                    n_candidates, out, io);
+  kernel<<<blocks, ROLLOUT_WARPS * 32, 0, stream>>>(eng->st, eng->d_step_cfg.get(), actions, action_dtype,
+                                                    n_steps, n_candidates, out, io);
   eng->launches++;
   CUDA_TRY(cudaGetLastError());
   return 0;
@@ -557,13 +593,11 @@ int swb_raster_create(swb_engine *eng, int32_t width, int32_t height, int32_t aa
                 "Pillow resizes such frames vertically first, which the render kernel does not",
                 width, height);
   CUDA_TRY(cudaSetDevice(eng->device));
-  swb_raster *r = new swb_raster();
+  std::unique_ptr<swb_raster> r(new swb_raster());
   r->eng = eng;
   std::string err;
-  if (!build_axis(width * aa, width, &r->ax, &err) || !build_axis(height * aa, height, &r->ay, &err)) {
-    delete r;
+  if (!build_axis(width * aa, width, &r->ax, &err) || !build_axis(height * aa, height, &r->ay, &err))
     return fail("%s", err.c_str());
-  }
   RasterDev &rd = r->rd;
   rd.W = width; rd.H = height; rd.aa = aa; rd.CW = width * aa; rd.CH = height * aa;
   rd.bg = bg_rgb ? ((uint32_t)bg_rgb[0] | ((uint32_t)bg_rgb[1] << 8) | ((uint32_t)bg_rgb[2] << 16)) : 0u;
@@ -582,45 +616,28 @@ int swb_raster_create(swb_engine *eng, int32_t width, int32_t height, int32_t aa
   r->smem_rows = rows;
   // a tile's canvas rows must fit the H tile's row length: as many blocks per tile as fit
   rd.tile_blocks = choose_tile_blocks(r->ay, rd.band_rows, TILE_BLOCKS, 4 * HT_ROWW);
-  if (rd.tile_blocks == 0) {
-    const int span = tile_span(r->ay, rd.band_rows, 1);
-    delete r;
+  if (rd.tile_blocks == 0)
     return fail("vertical tap windows of 8 output rows span %d canvas rows, more than the %d of the "
                 "render kernel's H tile (anti_aliasing %d is too large for a frame %d rows high)",
-                span, 4 * HT_ROWW, aa, height);
-  }
+                tile_span(r->ay, rd.band_rows, 1), 4 * HT_ROWW, aa, height);
   VFragHost vf;
-  if (!build_vfrag(r->ay, &vf, &err)) {
-    delete r;
-    return fail("%s", err.c_str());
-  }
-  if (vf.nks > V_KS_WIDE) {  // cannot happen: one block's windows fit 4 * HT_ROWW canvas rows
-    delete r;
+  if (!build_vfrag(r->ay, &vf, &err)) return fail("%s", err.c_str());
+  if (vf.nks > V_KS_WIDE)  // cannot happen: one block's windows fit 4 * HT_ROWW canvas rows
     return fail("vertical pass needs %d k-steps (limit %d)", vf.nks, V_KS_WIDE);
-  }
   rd.v_nks = vf.nks;
   // refuse a raster that cannot render even convex shapes (a star or spoke may still fail later)
   std::optional<RenderLayout> plan;
-  if (check_render(eng, r, 1, &plan)) {
-    delete r;
-    return 1;
-  }
+  if (check_render(eng, r.get(), 1, &plan)) return 1;
   const uint32_t *d_frag = nullptr;
-  if (upload_axis(r, r->ax, &rd.ax) || upload_axis(r, r->ay, &rd.ay) ||
-      upload_vec(r, vf.blk_cls, &rd.v_blk_cls) || upload_vec(r, vf.frag, &d_frag)) {
-    swb_raster_destroy(r);
+  if (upload_axis(r.get(), r->ax, &rd.ax) || upload_axis(r.get(), r->ay, &rd.ay) ||
+      upload_vec(r.get(), vf.blk_cls, &rd.v_blk_cls) || upload_vec(r.get(), vf.frag, &d_frag))
     return 1;
-  }
   rd.v_frag = reinterpret_cast<const uint2 *>(d_frag);  // cudaMalloc: 256-byte aligned
-  *out = r;
+  *out = r.release();
   return 0;
 }
 
-void swb_raster_destroy(swb_raster *r) {
-  if (!r) return;
-  for (void *p : r->owned) cudaFree(p);
-  delete r;
-}
+void swb_raster_destroy(swb_raster *r) { delete r; }
 
 // Enqueues render_kernel for envs [env_base, env_base + env_count) with a layout check_render
 // returned.  after_step: the launch follows this step's step_kernel on the stream.  It is then
@@ -657,8 +674,8 @@ static int enqueue_render(swb_engine *eng, const swb_raster *r, const RenderLayo
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   lc.attrs = attr;
   lc.numAttrs = after_step ? 1 : 0;
-  CUDA_TRY(cudaLaunchKernelEx(&lc, kernel, st, rd, L, targets, env_base, n_items, eng->d_work, eng->work_base,
-                              recs));
+  CUDA_TRY(cudaLaunchKernelEx(&lc, kernel, st, rd, L, targets, env_base, n_items, eng->d_work.get(),
+                              eng->work_base, recs));
   eng->work_base += (unsigned)(n_items + grid);  // every CTA's last claim fails
   eng->launches++;
   CUDA_TRY(cudaGetLastError());
@@ -756,62 +773,67 @@ int swb_step_host(swb_engine *eng, swb_raster *r, const void *actions, int32_t a
   CUDA_TRY(cudaSetDevice(eng->device));
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   const int E = eng->st.E;
-  if (!eng->h_actions) {
-    CUDA_TRY(cudaMalloc(&eng->h_actions, (size_t)E * 4 * sizeof(double)));
-    CUDA_TRY(cudaMalloc(&eng->h_out.reward, (size_t)E * sizeof(double)));
-    CUDA_TRY(cudaMalloc(&eng->h_out.step_type, E + 4));
-    CUDA_TRY(cudaMalloc(&eng->h_out.success, E + 4));
-    CUDA_TRY(cudaMalloc(&eng->h_out.status, E + 4));
+  if (!eng->step_host) {
+    auto h = std::make_unique<StepHostDev>();
+    // not zero-filled: nothing would order the fill before the writes that follow on `stream`
+    CUDA_TRY(dev_alloc(&h->actions, (size_t)E * 4, false));
+    CUDA_TRY(dev_alloc(&h->reward, E, false));
+    CUDA_TRY(dev_alloc(&h->step_type, E + 4, false));
+    CUDA_TRY(dev_alloc(&h->success, E + 4, false));
+    CUDA_TRY(dev_alloc(&h->status, E + 4, false));
+    eng->step_host = std::move(h);
   }
+  const swb_step_out h_out = eng->step_host->out();
   std::optional<RenderLayout> plan;
-  if (check_step(eng, actions, action_dtype, &eng->h_out, STEP_WHOLE) ||
+  if (check_step(eng, actions, action_dtype, &h_out, STEP_WHOLE) ||
       (r && check_render(eng, r, eng->max_spans, &plan)))
     return 1;
   // [E][2] int32 or [E][4] float32 / float64, as checked
   const size_t abytes = (size_t)E * (action_dtype == SWB_DTYPE_I32 ? 8 : action_dtype == SWB_DTYPE_F32 ? 16 : 32);
-  CUDA_TRY(cudaMemcpyAsync(eng->h_actions, actions, abytes, cudaMemcpyHostToDevice, stream));
+  CUDA_TRY(cudaMemcpyAsync(eng->step_host->actions.get(), actions, abytes, cudaMemcpyHostToDevice, stream));
   const size_t fbytes = r ? (size_t)E * r->rd.H * r->rd.W * 3 : 0;
-  if (fbytes > eng->h_frames_bytes) {
-    CUDA_TRY(cudaStreamSynchronize(stream));
-    cudaFree(eng->h_frames);
-    eng->h_frames_bytes = 0;
-    CUDA_TRY(cudaMalloc(&eng->h_frames, fbytes));
+  if (fbytes > eng->h_frames.bytes) {
+    CUDA_TRY(eng->h_frames.grow(fbytes, [&] { return cudaStreamSynchronize(stream); }));
     // written only by the render kernel's bulk copies, which initcheck does not track: zero
     // it once so that the tool sees every byte the D2H copies read as initialised
-    CUDA_TRY(cudaMemsetAsync(eng->h_frames, 0, fbytes, stream));
-    eng->h_frames_bytes = fbytes;
+    CUDA_TRY(cudaMemsetAsync(eng->h_frames.get(), 0, fbytes, stream));
   }
-  if (launch_step(eng, eng->h_actions, action_dtype, eng->h_out, stream, STEP_WHOLE)) return 1;
+  if (launch_step(eng, eng->step_host->actions.get(), action_dtype, h_out, stream, STEP_WHOLE)) return 1;
   if (r) {
-    const RenderTargets targets{{eng->h_frames}, 1, 0, 0};
+    const RenderTargets targets{{eng->h_frames.get()}, 1, 0, 0};
     if (!frames) {
-      if (enqueue_render(eng, r, *plan, targets, eng->h_out.status, stream, 0, E, true)) return 1;
+      if (enqueue_render(eng, r, *plan, targets, h_out.status, stream, 0, E, true)) return 1;
     } else {
       // render in env chunks; each chunk's frames go to the host on a second stream while
       // the next chunk renders
-      if (!eng->copy_stream) {
-        CUDA_TRY(cudaStreamCreateWithFlags(&eng->copy_stream, cudaStreamNonBlocking));
-        for (auto &ev : eng->chunk_done) CUDA_TRY(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-        CUDA_TRY(cudaEventCreateWithFlags(&eng->copies_done, cudaEventDisableTiming));
+      if (!eng->chunk_copies) {
+        auto c = std::make_unique<ChunkCopies>();
+        cudaStream_t s = nullptr;
+        CUDA_TRY(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
+        c->stream.reset(s);
+        for (Event &ev : c->chunk_done) CUDA_TRY(make_event(&ev));
+        CUDA_TRY(make_event(&c->copies_done));
+        eng->chunk_copies = std::move(c);
       }
+      const ChunkCopies &cc = *eng->chunk_copies;
       const size_t per_env = (size_t)r->rd.H * r->rd.W * 3;
       const int n_chunks = E >= 1024 ? 8 : (E >= 64 ? 2 : 1);
       for (int c = 0; c < n_chunks; ++c) {
         const int e0 = (int)((int64_t)E * c / n_chunks), e1 = (int)((int64_t)E * (c + 1) / n_chunks);
-        if (enqueue_render(eng, r, *plan, targets, eng->h_out.status, stream, e0, e1 - e0, c == 0)) return 1;
-        CUDA_TRY(cudaEventRecord(eng->chunk_done[c], stream));
-        CUDA_TRY(cudaStreamWaitEvent(eng->copy_stream, eng->chunk_done[c], 0));
-        CUDA_TRY(cudaMemcpyAsync(frames + per_env * e0, eng->h_frames + per_env * e0, per_env * (e1 - e0),
-                                 cudaMemcpyDeviceToHost, eng->copy_stream));
+        if (enqueue_render(eng, r, *plan, targets, h_out.status, stream, e0, e1 - e0, c == 0)) return 1;
+        CUDA_TRY(cudaEventRecord(cc.chunk_done[c].get(), stream));
+        CUDA_TRY(cudaStreamWaitEvent(cc.stream.get(), cc.chunk_done[c].get(), 0));
+        CUDA_TRY(cudaMemcpyAsync(frames + per_env * e0, eng->h_frames.get() + per_env * e0, per_env * (e1 - e0),
+                                 cudaMemcpyDeviceToHost, cc.stream.get()));
       }
-      CUDA_TRY(cudaEventRecord(eng->copies_done, eng->copy_stream));
-      CUDA_TRY(cudaStreamWaitEvent(stream, eng->copies_done, 0));
+      CUDA_TRY(cudaEventRecord(cc.copies_done.get(), cc.stream.get()));
+      CUDA_TRY(cudaStreamWaitEvent(stream, cc.copies_done.get(), 0));
     }
   }
-  if (reward) CUDA_TRY(cudaMemcpyAsync(reward, eng->h_out.reward, (size_t)E * sizeof(double), cudaMemcpyDeviceToHost, stream));
-  if (step_type) CUDA_TRY(cudaMemcpyAsync(step_type, eng->h_out.step_type, E, cudaMemcpyDeviceToHost, stream));
-  if (success) CUDA_TRY(cudaMemcpyAsync(success, eng->h_out.success, E, cudaMemcpyDeviceToHost, stream));
-  if (status) CUDA_TRY(cudaMemcpyAsync(status, eng->h_out.status, E, cudaMemcpyDeviceToHost, stream));
+  if (reward) CUDA_TRY(cudaMemcpyAsync(reward, h_out.reward, (size_t)E * sizeof(double), cudaMemcpyDeviceToHost, stream));
+  if (step_type) CUDA_TRY(cudaMemcpyAsync(step_type, h_out.step_type, E, cudaMemcpyDeviceToHost, stream));
+  if (success) CUDA_TRY(cudaMemcpyAsync(success, h_out.success, E, cudaMemcpyDeviceToHost, stream));
+  if (status) CUDA_TRY(cudaMemcpyAsync(status, h_out.status, E, cudaMemcpyDeviceToHost, stream));
   CUDA_TRY(cudaStreamSynchronize(stream));
   return 0;
 }
@@ -913,32 +935,18 @@ static int check_env_ids(const swb_engine *eng, const char *fn, const int32_t *i
 }
 
 // Copies `n` host ids from `a` (and `n` from `b`, if given) into an id staging slot, enqueues their
-// copy to its device twin, and makes *c the IdCall of them, checked on the host.  After the kernels
-// that read them, release_slot(*slot).
+// copy to its device twin, and makes *c the IdCall of them, checked on the host.  The kernels that
+// read them are then recorded as (*slot)->readers.
 static int stage_ids(swb_engine *eng, const int32_t *a, const int32_t *b, int32_t n, int dst_arg,
                      cudaStream_t stream, IdCall *c, StagingSlot **slot) {
   const size_t bytes = (b ? 2 : 1) * (size_t)n * sizeof(int32_t);
   if (take_slot(eng->id_staging, bytes, slot)) return 1;
-  int32_t *h = reinterpret_cast<int32_t *>((*slot)->host);
+  int32_t *h = reinterpret_cast<int32_t *>((*slot)->host.get());
   memcpy(h, a, n * sizeof(int32_t));
   if (b) memcpy(h + n, b, n * sizeof(int32_t));
-  CUDA_TRY(cudaMemcpyAsync((*slot)->dev, h, bytes, cudaMemcpyHostToDevice, stream));
-  const int32_t *d = reinterpret_cast<const int32_t *>((*slot)->dev);
+  CUDA_TRY(cudaMemcpyAsync((*slot)->dev.get(), h, bytes, cudaMemcpyHostToDevice, stream));
+  const int32_t *d = reinterpret_cast<const int32_t *>((*slot)->dev.get());
   *c = IdCall{{d, b ? d + n : nullptr}, n, dst_arg, true};
-  return 0;
-}
-
-// Engine scratch of at least `need` bytes for the records of a copy.
-static int grow_records(swb_engine *eng, size_t need) {
-  if (need <= eng->records_bytes) return 0;
-  if (eng->d_records) {
-    CUDA_TRY(cudaDeviceSynchronize());  // an earlier copy on any stream may still read it
-    cudaFree(eng->d_records);
-    eng->d_records = nullptr;
-    eng->records_bytes = 0;
-  }
-  CUDA_TRY(cudaMalloc(reinterpret_cast<void **>(&eng->d_records), need));
-  eng->records_bytes = need;
   return 0;
 }
 
@@ -963,12 +971,12 @@ static int check_dev_ids(const swb_engine *eng, const char *fn, const void *ids,
 static int begin_id_call(swb_engine *eng, int call, const void *a, const void *b, int dst_arg, int32_t n,
                          cudaStream_t stream, IdCall *c) {
   if (++eng->id_seq == 0xFFFFFFFFu) {
-    CUDA_TRY(cudaMemsetAsync(eng->d_id_claim, 0xFF, (size_t)eng->st.E * sizeof(unsigned long long), stream));
-    CUDA_TRY(cudaMemsetAsync(eng->d_id_fail, 0xFF, sizeof(unsigned long long), stream));
+    CUDA_TRY(cudaMemsetAsync(eng->d_id_claim.get(), 0xFF, (size_t)eng->st.E * sizeof(unsigned long long), stream));
+    CUDA_TRY(cudaMemsetAsync(eng->d_id_fail.get(), 0xFF, sizeof(unsigned long long), stream));
     eng->id_seq = 1;
   }
-  *c = IdCall{{a, b}, n, dst_arg, false, call, (unsigned long long)(~eng->id_seq) << 32, eng->d_id_claim,
-              eng->d_id_fail, eng->d_id_status};
+  *c = IdCall{{a, b}, n, dst_arg, false, call, (unsigned long long)(~eng->id_seq) << 32, eng->d_id_claim.get(),
+              eng->d_id_fail.get(), eng->d_id_status.get()};
   return 0;
 }
 
@@ -1016,15 +1024,16 @@ static int enqueue_copy(swb_engine *eng, const IdCall &c, bool disjoint, cudaStr
     copy_envs_kernel<<<grid_of(threads), 256, 0, stream>>>(eng->st, c);
     eng->launches++;
   } else {
-    if (grow_records(eng, c.n * rb)) return 1;
+    // an earlier copy on any stream may still read the scratch
+    CUDA_TRY(eng->records.grow(c.n * rb, [] { return cudaDeviceSynchronize(); }));
     if (c.host_checked) {
-      save_envs_kernel<T><<<grid_of(threads), 256, 0, stream>>>(eng->st, c, eng->d_records, rb);
+      save_envs_kernel<T><<<grid_of(threads), 256, 0, stream>>>(eng->st, c, eng->records.get(), rb);
     } else {
       check_ids_kernel<T><<<grid_of(2 * (size_t)c.n), 256, 0, stream>>>(c, eng->st.E);
-      stage_copy_dev_kernel<T><<<grid_of(threads), 256, 0, stream>>>(eng->st, c, eng->d_records, rb);
+      stage_copy_dev_kernel<T><<<grid_of(threads), 256, 0, stream>>>(eng->st, c, eng->records.get(), rb);
       eng->launches++;
     }
-    load_envs_kernel<T><<<grid_of(threads), 256, 0, stream>>>(eng->st, c, eng->d_records, rb);
+    load_envs_kernel<T><<<grid_of(threads), 256, 0, stream>>>(eng->st, c, eng->records.get(), rb);
     eng->launches += 2;
   }
   CUDA_TRY(cudaGetLastError());
@@ -1053,7 +1062,7 @@ static EnvIds dev_ids(const void *a, const void *b, int32_t dtype) { return EnvI
 
 // Checks the n ids of `call` (SWB_IDS_CALL_*), then calls enqueue(c, T(), disjoint) with their
 // IdCall c and id type T.  Host ids: every id in [0, E) and the destinations distinct, checked before
-// anything is enqueued; then staged, with their slot released after `enqueue`; `disjoint` says that
+// anything is enqueued; then staged, their slot's readers recorded after `enqueue`; `disjoint` says that
 // no env is among both the sources and the destinations.  Device ids: check_dev_ids, then the next
 // device-checked call (begin_id_call), whose kernels check them; `disjoint` is false.
 template <typename Enqueue>
@@ -1072,7 +1081,8 @@ static int run_ids(swb_engine *eng, const char *fn, int call, const EnvIds &ids,
     CUDA_TRY(cudaSetDevice(eng->device));
     StagingSlot *slot = nullptr;
     if (stage_ids(eng, src, dst, n, dst_arg, stream, &c, &slot) || enqueue(c, int32_t(), disjoint)) return 1;
-    return release_slot(slot, stream);
+    CUDA_TRY(slot->readers.record(stream));
+    return 0;
   }
   for (int a = 0; a < n_args; ++a)
     if (check_dev_ids(eng, fn, ids.ids[a], ids.dtype)) return 1;
@@ -1307,7 +1317,7 @@ int swb_evaluate_states(swb_engine *eng, const void *records, int32_t n, uint64_
   CUDA_TRY(cudaSetDevice(eng->device));
   const unsigned blocks = (unsigned)(((int64_t)n + ROLLOUT_WARPS - 1) / ROLLOUT_WARPS);
   evaluate_kernel<<<blocks, ROLLOUT_WARPS * 32, 0, static_cast<cudaStream_t>(stream_)>>>(
-      eng->st, eng->d_step_cfg, static_cast<const unsigned char *>(records), (size_t)rb, n, goals, reward,
+      eng->st, eng->d_step_cfg.get(), static_cast<const unsigned char *>(records), (size_t)rb, n, goals, reward,
       success, status);
   eng->launches++;
   CUDA_TRY(cudaGetLastError());
@@ -1450,7 +1460,7 @@ int swb_sample_contained(swb_engine *eng, const void *records, int32_t n, uint64
 
 int swb_env_ids_status_pointer(swb_engine *eng, swb_ids_status **status) {
   if (!eng || !status) return fail("swb_env_ids_status_pointer: null argument");
-  *status = eng->d_id_status;
+  *status = eng->d_id_status.get();
   return 0;
 }
 
@@ -1585,22 +1595,19 @@ int swb_sampler_load(swb_engine *eng, const swb_scene_program *prog, uint64_t se
     return fail("swb_sampler_load: the program draws %d goals per scene, the task tree has %d goal slots",
                 prog->n_goals, eng->st.G);
   CUDA_TRY(cudaSetDevice(eng->device));
-  if (!eng->d_prog) {  // all three or none: the other calls test d_prog alone
-    swb_scene_program *prog_d = nullptr;
-    int64_t *upto_d = nullptr;
-    swb_sampler_status *status_d = nullptr;
-    if (dev_alloc(&prog_d, 1) != cudaSuccess || dev_alloc(&upto_d, eng->st.E) != cudaSuccess ||
-        dev_alloc(&status_d, 1) != cudaSuccess) {
-      cudaFree(prog_d); cudaFree(upto_d); cudaFree(status_d);
+  // a first load publishes the sampler once its program is on the device
+  std::unique_ptr<SamplerDev> fresh;
+  if (!eng->sampler) {
+    fresh = std::make_unique<SamplerDev>();
+    if (dev_alloc(&fresh->prog, 1) != cudaSuccess || dev_alloc(&fresh->refilled_upto, eng->st.E) != cudaSuccess ||
+        dev_alloc(&fresh->status, 1) != cudaSuccess)
       return fail("swb_sampler_load: device allocation failed");
-    }
-    eng->d_prog = prog_d;
-    eng->d_refilled_upto = upto_d;
-    eng->d_sampler_status = status_d;
   }
+  const SamplerDev &s = fresh ? *fresh : *eng->sampler;
   CUDA_TRY(cudaDeviceSynchronize());
-  CUDA_TRY(cudaMemcpy(eng->d_prog, prog, sizeof(swb_scene_program), cudaMemcpyHostToDevice));
-  CUDA_TRY(cudaMemset(eng->d_refilled_upto, 0xFF, (size_t)eng->st.E * sizeof(int64_t)));
+  CUDA_TRY(cudaMemcpy(s.prog.get(), prog, sizeof(swb_scene_program), cudaMemcpyHostToDevice));
+  CUDA_TRY(cudaMemset(s.refilled_upto.get(), 0xFF, (size_t)eng->st.E * sizeof(int64_t)));
+  if (fresh) eng->sampler = std::move(fresh);
   eng->seed = seed;
   eng->env_offset = env_offset;
   return 0;
@@ -1609,7 +1616,7 @@ int swb_sampler_load(swb_engine *eng, const swb_scene_program *prog, uint64_t se
 int swb_sample_scenes(swb_engine *eng, const int64_t *env_ids, const int64_t *scene_idx, int32_t n,
                       const swb_sample_out *out, void *stream_) {
   if (!eng || !out) return fail("swb_sample_scenes: null argument");
-  if (!eng->d_prog) return fail("swb_sample_scenes: no program (swb_sampler_load)");
+  if (!eng->sampler) return fail("swb_sample_scenes: no program (swb_sampler_load)");
   if (n < 0) return fail("swb_sample_scenes: n < 0");
   if (n == 0) return 0;
   if (!env_ids || !scene_idx || !out->x || !out->y || !out->m00 || !out->m01 || !out->m10 || !out->m11 ||
@@ -1619,7 +1626,7 @@ int swb_sample_scenes(swb_engine *eng, const int64_t *env_ids, const int64_t *sc
   CUDA_TRY(cudaSetDevice(eng->device));
   const int threads = 128;
   sample_scenes_kernel<<<(n + threads - 1) / threads, threads, 0, static_cast<cudaStream_t>(stream_)>>>(
-      eng->d_prog, eng->seed, eng->st.S, env_ids, scene_idx, n, *out, eng->d_sampler_status);
+      eng->sampler->prog.get(), eng->seed, eng->st.S, env_ids, scene_idx, n, *out, eng->sampler->status.get());
   eng->launches++;
   CUDA_TRY(cudaGetLastError());
   return 0;
@@ -1627,11 +1634,12 @@ int swb_sample_scenes(swb_engine *eng, const int64_t *env_ids, const int64_t *sc
 
 int swb_refill_device(swb_engine *eng, void *stream_) {
   if (!eng) return fail("swb_refill_device: null engine");
-  if (!eng->d_prog) return fail("swb_refill_device: no program (swb_sampler_load)");
+  if (!eng->sampler) return fail("swb_refill_device: no program (swb_sampler_load)");
   CUDA_TRY(cudaSetDevice(eng->device));
   const int threads = 64;
+  const SamplerDev &s = *eng->sampler;
   refill_device_kernel<<<(eng->st.E + threads - 1) / threads, threads, 0, static_cast<cudaStream_t>(stream_)>>>(
-      eng->d_prog, eng->seed, eng->env_offset, eng->st, eng->d_refilled_upto, eng->d_sampler_status);
+      s.prog.get(), eng->seed, eng->env_offset, eng->st, s.refilled_upto.get(), s.status.get());
   eng->launches++;
   CUDA_TRY(cudaGetLastError());
   return 0;
@@ -1639,9 +1647,9 @@ int swb_refill_device(swb_engine *eng, void *stream_) {
 
 int swb_sampler_pointers(swb_engine *eng, int64_t **refilled_upto, swb_sampler_status **status) {
   if (!eng) return fail("swb_sampler_pointers: null engine");
-  if (!eng->d_prog) return fail("swb_sampler_pointers: no program (swb_sampler_load)");
-  if (refilled_upto) *refilled_upto = eng->d_refilled_upto;
-  if (status) *status = eng->d_sampler_status;
+  if (!eng->sampler) return fail("swb_sampler_pointers: no program (swb_sampler_load)");
+  if (refilled_upto) *refilled_upto = eng->sampler->refilled_upto.get();
+  if (status) *status = eng->sampler->status.get();
   return 0;
 }
 
@@ -1673,12 +1681,13 @@ int swb_packer_load(swb_engine *eng, const swb_scene_program *prog) {
   for (int a = -360; a <= 360; ++a)
     if (!has((double)a)) return fail("%s: the angle table lacks %d", fn, a);
   CUDA_TRY(cudaSetDevice(eng->device));
-  if (!eng->d_packer && dev_alloc(&eng->d_packer, 1) != cudaSuccess) {
-    eng->d_packer = nullptr;
-    return fail("%s: device allocation failed", fn);
-  }
+  // a first load publishes the packer once it is on the device
+  DevPtr<swb_scene_program> fresh;
+  if (!eng->d_packer && dev_alloc(&fresh, 1) != cudaSuccess) return fail("%s: device allocation failed", fn);
   CUDA_TRY(cudaDeviceSynchronize());  // a make_states call in flight may still read the old packer
-  CUDA_TRY(cudaMemcpy(eng->d_packer, prog, sizeof(swb_scene_program), cudaMemcpyHostToDevice));
+  CUDA_TRY(cudaMemcpy(fresh ? fresh.get() : eng->d_packer.get(), prog, sizeof(swb_scene_program),
+                      cudaMemcpyHostToDevice));
+  if (fresh) eng->d_packer = std::move(fresh);
   eng->packer_hsv = prog->color_mode == SWB_COLOR_HSV;
   return 0;
 }
@@ -1746,7 +1755,7 @@ int swb_make_states(swb_engine *eng, const swb_factor_columns *cols, int32_t n, 
   if (span_flag) CUDA_TRY(cudaMemsetAsync(span_flag, 0, 1, stream));
   const unsigned blocks = (unsigned)(((int64_t)n + MAKE_WARPS - 1) / MAKE_WARPS);
   make_states_kernel<<<blocks, MAKE_WARPS * 32, 0, stream>>>(
-      eng->d_packer, *cols, n, S, G, goals, step_count, static_cast<unsigned char *>(records), (size_t)rb, status,
+      eng->d_packer.get(), *cols, n, S, G, goals, step_count, static_cast<unsigned char *>(records), (size_t)rb, status,
       span_flag);
   eng->launches++;
   CUDA_TRY(cudaGetLastError());
@@ -1801,7 +1810,7 @@ struct CkptLayout {
         {"m10", st.p_m10, 8, EKS}, {"m11", st.p_m11, 8, EKS}, {"vx", st.p_vx, 8, EKS}, {"vy", st.p_vy, 8, EKS},
         {"member", st.p_member, 4, EKS}, {"rgb", st.p_rgb, 4, EKS}, {"factors", st.p_factors, 4, EKS * 5},
         {"shape", st.p_shape, 1, EKS}, {"pos_f32", st.p_pos_f32, 1, EKS},
-        {"refilled_upto", eng->d_refilled_upto, 8, E},
+        {"refilled_upto", eng->sampler ? eng->sampler->refilled_upto.get() : nullptr, 8, E},
         {"goal", st.p_goal, 8, E * st.K * st.G * 2}};   // no bytes when G == 0
     header = align16(kCkptFixed + sizeof(swb_config));
     size_t o = header;
@@ -1821,24 +1830,6 @@ swb_config signature_of(const swb_engine *eng) {
   memcpy(&sig, &eng->cfg, sizeof sig);
   sig.n_envs = sig.pool_depth = sig.device = 0;
   return sig;
-}
-
-// The engine's pinned checkpoint staging, at least `need` bytes, once the last load's copies from
-// it have finished.
-int ckpt_staging(swb_engine *eng, size_t need) {
-  if (eng->ckpt_in_flight) {
-    CUDA_TRY(cudaEventSynchronize(eng->ckpt_done));
-    eng->ckpt_in_flight = false;
-  }
-  if (!eng->ckpt_done) CUDA_TRY(cudaEventCreateWithFlags(&eng->ckpt_done, cudaEventDisableTiming));
-  if (need > eng->h_ckpt_bytes) {
-    if (eng->h_ckpt) cudaFreeHost(eng->h_ckpt);
-    eng->h_ckpt = nullptr;
-    eng->h_ckpt_bytes = 0;
-    CUDA_TRY(cudaMallocHost(reinterpret_cast<void **>(&eng->h_ckpt), need));
-    eng->h_ckpt_bytes = need;
-  }
-  return 0;
 }
 
 template <typename T>
@@ -1875,7 +1866,7 @@ int check_checkpoint(const swb_engine *eng, const unsigned char *s, uint64_t n, 
   if (h.span_class != 1 && h.span_class != 4)
     return fail("%s: span_class = %d, expected 1 or 4", fn, h.span_class);
   if (h.sampler != 0 && h.sampler != 1) return fail("%s: sampler = %d, expected 0 or 1", fn, h.sampler);
-  const bool has = eng->d_prog != nullptr;
+  const bool has = eng->sampler != nullptr;
   if (h.sampler != (int)has)
     return fail("%s: sampler: the checkpoint was saved %s a device sampler, the engine has %s", fn,
                 h.sampler ? "with" : "without", has ? "one (swb_sampler_load)" : "none");
@@ -1931,8 +1922,9 @@ int swb_save_engine(swb_engine *eng, void *host_dst, uint64_t dst_bytes, void *s
                 (unsigned long long)dst_bytes);
   CUDA_TRY(cudaSetDevice(eng->device));
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  if (ckpt_staging(eng, L.total)) return 1;
-  unsigned char *h = eng->h_ckpt;
+  CUDA_TRY(eng->ckpt_done.wait());  // the copies of the last load may still read the staging
+  CUDA_TRY(eng->h_ckpt.grow(L.total, kWaited));
+  unsigned char *h = eng->h_ckpt.get();
   memset(h, 0, L.total);  // padding included: two saves of one state are byte-identical
   CkptHeader hd;
   memset(&hd, 0, sizeof hd);
@@ -1940,7 +1932,7 @@ int swb_save_engine(swb_engine *eng, void *host_dst, uint64_t dst_bytes, void *s
   hd.version = kCkptVersion;
   hd.E = eng->st.E; hd.K = eng->st.K; hd.S = eng->st.S;
   hd.span_class = eng->max_spans;
-  hd.sampler = eng->d_prog != nullptr;
+  hd.sampler = eng->sampler != nullptr;
   hd.seed = hd.sampler ? eng->seed : 0;
   hd.env_offset = hd.sampler ? eng->env_offset : 0;
   hd.config_bytes = sizeof(swb_config);
@@ -1963,8 +1955,9 @@ int swb_load_engine(swb_engine *eng, const void *host_src, uint64_t src_bytes, v
   CUDA_TRY(cudaSetDevice(eng->device));
   // checked in the staging copy: the caller's buffer may be reused once the call returns, and
   // every field of the copy is aligned
-  if (ckpt_staging(eng, std::max<size_t>(L.total, kCkptFixed))) return 1;
-  unsigned char *h = eng->h_ckpt;
+  CUDA_TRY(eng->ckpt_done.wait());
+  CUDA_TRY(eng->h_ckpt.grow(std::max<size_t>(L.total, kCkptFixed), kWaited));
+  unsigned char *h = eng->h_ckpt.get();
   memcpy(h, host_src, std::min<uint64_t>(src_bytes, L.total));
   bool stars = false;
   if (check_checkpoint(eng, h, src_bytes, L, &stars)) return 1;
@@ -1975,8 +1968,7 @@ int swb_load_engine(swb_engine *eng, const void *host_src, uint64_t src_bytes, v
   eng->max_spans = std::max({eng->max_spans, (int)hd.span_class, stars ? 4 : 1});
   for (const CkptField &f : L.f)
     if (f.dev) CUDA_TRY(cudaMemcpyAsync(f.dev, h + f.off, f.bytes(), cudaMemcpyHostToDevice, stream));
-  CUDA_TRY(cudaEventRecord(eng->ckpt_done, stream));
-  eng->ckpt_in_flight = true;
+  CUDA_TRY(eng->ckpt_done.record(stream));
   return 0;
 }
 
