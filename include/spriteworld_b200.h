@@ -59,7 +59,8 @@ enum {
   SWB_ENV_BAD_ACTION = 4,      /* Embodied direction not in 0..3 -> KeyError (action_spaces.py:203) */
   SWB_ENV_SPAN_OVERFLOW = 8,   /* renderer: more spans on a canvas row than the engine was sized for */
   SWB_ENV_NO_SPRITE = 16,      /* swb_sample_contained: the row has no sprite (np.random.randint(0) raises) */
-  SWB_ENV_SAMPLE_TRIES = 32    /* swb_sample_contained: SWB_CONTAINED_MAX_TRIES draws, none inside (sprite.py) */
+  SWB_ENV_SAMPLE_TRIES = 32,   /* swb_sample_contained: SWB_CONTAINED_MAX_TRIES draws, none inside (sprite.py) */
+  SWB_ENV_BAD_WINDOW = 64      /* swb_render_windows: empty or non-finite window, or a vertex at 2^30 or beyond */
 };
 
 /* One node of the flattened task tree, post-order, root last. */
@@ -436,6 +437,34 @@ int swb_rollout_trajectory(swb_engine *eng, const void *roots, int32_t n_roots, 
 int swb_render_states(swb_engine *eng, swb_raster *r, const void *records, int32_t n,
                       uint64_t records_bytes, int32_t span_class, uint8_t *frames,
                       uint8_t *status, void *stream);
+
+/*
+ * The scene seen through windows: n_views frames of each row, each the raster's PILRenderer frame of
+ * the window (x0, y0, x1, y1) of scene coordinates instead of the unit square.  Zoomed sprite
+ * glimpses, egocentric views.
+ *
+ * Rows: `records` NULL means the E live envs (then n must be E), else n records as in
+ * swb_render_states, with span_class (1 or 4) as saved; live rows pass 1 and render with the
+ * engine's own spans per sprite row, as swb_render does.
+ * windows[(i * n_views + v) * 4 + 0..3] (device f64, 8-byte aligned) is the window of view v of row
+ * i; frames [n][n_views][height][width][3] u8 and status [n][n_views] u8 (SWB_ENV_* bits) are the
+ * item's.  With CW = aa * width, CH = aa * height, a world vertex (wx, wy) -- the one swb_render
+ * multiplies by CW and CH -- goes to the canvas vertex (trunc(u), trunc(v)) with
+ *   sx = CW / (x1 - x0);  u = (wx - x0) * sx       (each op float64, round to nearest)
+ *   sy = CH / (y1 - y0);  v = (wy - y0) * sy
+ * and everything after that is swb_render's: so the window (0, 0, 1, 1) draws swb_render's (or
+ * swb_render_states') frame byte for byte.  An item whose window is not finite or has x1 <= x0 or
+ * y1 <= y0, or with an occupied slot whose vertex has u or v NaN or |u| or |v| >= 2^30, gets
+ * SWB_ENV_BAD_WINDOW and a frame of zeros; a span overflow sets SWB_ENV_SPAN_OVERFLOW as in
+ * swb_render_states.  One memset of status and one launch; n == 0 enqueues nothing.
+ *
+ * Read-only as swb_render_states.  Refused besides what swb_render_states refuses (for live rows,
+ * what swb_render refuses): live rows with n != E, n_views < 1, n * n_views * (the raster's bands)
+ * above 2^31 - 1, and windows that are null, not 8-byte aligned, or overlap the outputs or the records.
+ */
+int swb_render_windows(swb_engine *eng, swb_raster *r, const void *records, int32_t n,
+                       uint64_t records_bytes, int32_t span_class, const double *windows, int32_t n_views,
+                       uint8_t *frames, uint8_t *status, void *stream);
 
 /*
  * Sprite instance masks (renderers.SpriteMasks): which sprite is visible at each pixel.  `masks`

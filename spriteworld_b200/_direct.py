@@ -133,14 +133,35 @@ def render(renderer, sprites):
   """(H, W, 3) uint8 frame of a Python sprite list."""
   eng = _engine(max(1, len(sprites)), _DUMMY_ACTION, _NO_TASK, True)
   _load(eng, sprites, (), renderer.color_to_rgb)
+  frames = eng.render(_raster(eng, renderer))
+  eng.check_render()
+  return frames[0].cpu().numpy()
+
+
+def _raster(eng, renderer):
   key = (eng, renderer.width, renderer.height, renderer.anti_aliasing, renderer.bg_color)
   raster = _rasters.get(key)
   if raster is None:
     raster = engine_lib.Raster(eng, renderer.width, renderer.height, renderer.anti_aliasing,
                                renderer.bg_color)
     _rasters[key] = raster
-  frames = eng.render(raster)
-  eng.check_render()
+  return raster
+
+
+def render_glimpses(renderer, sprites):
+  """(V, H, W, 3) uint8 SpriteGlimpses views of a Python sprite list: slot i is sprites[i]."""
+  n = len(sprites)
+  V = len(renderer.slot_indices(n))
+  if V == 0:
+    return np.zeros((0, renderer.height, renderer.width, 3), np.uint8)
+  eng = _engine(max(1, n), _DUMMY_ACTION, _NO_TASK, True)
+  _load(eng, sprites, (), renderer.color_to_rgb)
+  pos = eng.state_tensors()
+  # n >= 1 here: the sprites fill slots S - n .. S - 1
+  windows = renderer.windows(pos['pos_x'][:, eng.n_slots - n:], pos['pos_y'][:, eng.n_slots - n:])
+  frames, status = eng.render_windows(_raster(eng, renderer), windows)
+  # a flagged view is zeros, as in a BatchedEnvironment; a span overflow raises, as PILRenderer's does
+  _raise_for_status(int(status.max().item()) & ~_native.ENV_BAD_WINDOW)
   return frames[0].cpu().numpy()
 
 

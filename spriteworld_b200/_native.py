@@ -23,6 +23,7 @@ STEP_FIRST, STEP_MID, STEP_LAST = 0, 1, 2
 STEP_NONE = -1   # padding of a rollout: no step
 ENV_OK, ENV_CLUSTER_LABELS, ENV_CLUSTER_ZERODIV, ENV_BAD_ACTION, ENV_SPAN_OVERFLOW = 0, 1, 2, 4, 8
 ENV_NO_SPRITE, ENV_SAMPLE_TRIES = 16, 32   # swb_sample_contained
+ENV_BAD_WINDOW = 64                        # swb_render_windows
 CONTAINED_MAX_TRIES = 1000000              # SWB_CONTAINED_MAX_TRIES
 CONTAINED_DOMAIN = 0x535742434e544431      # SWB_CONTAINED_DOMAIN
 IDS_CALL_SAVE, IDS_CALL_LOAD, IDS_CALL_COPY, IDS_CALL_SET_GOALS = 0, 1, 2, 3
@@ -132,6 +133,7 @@ def load():
                                    ctypes.c_uint64, ctypes.POINTER(ci), vp]
   L.swb_rollout_trajectory.argtypes = L.swb_rollout_states.argtypes
   L.swb_render_states.argtypes = [vp, vp, vp, ci, ctypes.c_uint64, ci, vp, vp, vp]
+  L.swb_render_windows.argtypes = [vp, vp, vp, ci, ctypes.c_uint64, ci, vp, ci, vp, vp, vp]
   L.swb_render_masks.argtypes = [vp, ci, ci, ci, vp, ci, ctypes.c_uint64, vp, vp]
   L.swb_render_coverage.argtypes = [vp, ci, ci, ci, vp, ci, ctypes.c_uint64, vp, vp, vp, vp]
   L.swb_render_soft_masks.argtypes = [vp, ci, ci, ci, vp, ci, ctypes.c_uint64, vp, vp]
@@ -179,7 +181,7 @@ EXPORTS = (
     'swb_sampler_pointers', 'swb_pool_pointers', 'swb_engine_state_bytes', 'swb_save_engine',
     'swb_load_engine', 'swb_pool_goal_pointer', 'swb_set_goals', 'swb_set_goals_dev', 'swb_evaluate_states',
     'swb_sample_contained', 'swb_render_coverage', 'swb_render_soft_masks', 'swb_render_boxes',
-    'swb_rollout_trajectory', 'swb_packer_load', 'swb_make_states')
+    'swb_rollout_trajectory', 'swb_packer_load', 'swb_make_states', 'swb_render_windows')
 
 
 def check(rc):

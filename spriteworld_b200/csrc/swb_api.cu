@@ -247,7 +247,7 @@ int upload_axis(swb_raster *r, const AxisHost &h, AxisTables *d) {
 extern "C" {
 
 const char *swb_last_error(void) { return g_error.c_str(); }
-int swb_version(void) { return 17; }
+int swb_version(void) { return 18; }
 int swb_sizeof_config(void) { return (int)sizeof(swb_config); }
 int swb_sizeof_task_node(void) { return (int)sizeof(swb_task_node); }
 
@@ -645,16 +645,23 @@ void swb_raster_destroy(swb_raster *r) { delete r; }
 // while the step kernel's last CTAs run (step_kernel signals griddepcontrol.launch_dependents at
 // once), and wait (griddepcontrol.wait, after their set-up) until the step grid has completed and
 // its writes are visible.  With recs.rec set, the items are records [0, env_count) of recs instead
-// of live envs (swb_render_states; one target, env_base 0, status [env_count]).
+// of live envs (swb_render_states; one target, env_base 0, status [env_count]).  With wins.win set,
+// each of the env_count rows is drawn wins.V times (swb_render_windows; one target, env_base 0,
+// status [env_count * V]).
 static int enqueue_render(swb_engine *eng, const swb_raster *r, const RenderLayout &L,
                           const RenderTargets &targets, uint8_t *status, cudaStream_t stream,
                           int env_base, int env_count, bool after_step,
-                          const RenderRecords &recs = RenderRecords{nullptr, 0}) {
+                          const RenderRecords &recs = RenderRecords{nullptr, 0},
+                          const RenderWindows &wins = RenderWindows{nullptr, 1}) {
   RasterDev rd = r->rd;
   rd.max_spans = L.M;
   // the wide instantiation only for rasters whose tables the narrow one was not compiled for
   const bool wide = render_wide(rd);
-  auto kernel = recs.rec ? (wide ? render_kernel<false, true, true> : render_kernel<false, false, true>)
+  auto kernel = wins.win ? (recs.rec ? (wide ? render_kernel<false, true, true, true>
+                                             : render_kernel<false, false, true, true>)
+                                     : (wide ? render_kernel<false, true, false, true>
+                                             : render_kernel<false, false, false, true>))
+                : recs.rec ? (wide ? render_kernel<false, true, true> : render_kernel<false, false, true>)
                 : targets.n > 1 ? (wide ? render_kernel<true, true, false> : render_kernel<true, false, false>)
                                 : (wide ? render_kernel<false, true, false> : render_kernel<false, false, false>);
   CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, L.total));
@@ -662,7 +669,7 @@ static int enqueue_render(swb_engine *eng, const swb_raster *r, const RenderLayo
   st.render_status = status;
   // persistent CTAs: one per resident slot (or per item if there are fewer), claiming
   // (env, band) items from the engine's counter; see render_kernel
-  const int n_items = env_count * rd.n_bands;
+  const int n_items = env_count * wins.V * rd.n_bands;
   const int grid = std::min(n_items, eng->n_sms * (wide ? R_CTAS_PER_SM_WIDE : R_CTAS_PER_SM));
   cudaLaunchConfig_t lc = {};
   lc.gridDim = dim3(grid);
@@ -675,7 +682,7 @@ static int enqueue_render(swb_engine *eng, const swb_raster *r, const RenderLayo
   lc.attrs = attr;
   lc.numAttrs = after_step ? 1 : 0;
   CUDA_TRY(cudaLaunchKernelEx(&lc, kernel, st, rd, L, targets, env_base, n_items, eng->d_work.get(),
-                              eng->work_base, recs));
+                              eng->work_base, recs, wins));
   eng->work_base += (unsigned)(n_items + grid);  // every CTA's last claim fails
   eng->launches++;
   CUDA_TRY(cudaGetLastError());
@@ -1402,6 +1409,36 @@ int swb_render_states(swb_engine *eng, swb_raster *r, const void *records, int32
   CUDA_TRY(cudaMemsetAsync(status, 0, (size_t)n, stream));
   return enqueue_render(eng, r, *plan, RenderTargets{{frames}, 1, 0, 0}, status, stream, 0, n, false,
                         RenderRecords{static_cast<const unsigned char *>(records), (size_t)rb});
+}
+
+int swb_render_windows(swb_engine *eng, swb_raster *r, const void *records, int32_t n, uint64_t records_bytes,
+                       int32_t span_class, const double *windows, int32_t n_views, uint8_t *frames,
+                       uint8_t *status, void *stream_) {
+  static const char fn[] = "swb_render_windows";
+  if (!eng || !r) return fail("%s: null engine or raster", fn);
+  if (check_rows(eng, fn, "records", records, n, records_bytes, true)) return 1;
+  if (span_class != 1 && span_class != 4) return fail("%s: span_class must be 1 or 4, got %d", fn, span_class);
+  if (n_views < 1) return fail("%s: n_views = %d must be >= 1", fn, n_views);
+  const RasterDev &rd = r->rd;
+  // n_items and the kernel's item index are int
+  if ((int64_t)n * n_views * rd.n_bands > INT32_MAX)
+    return fail("%s: n = %d rows of %d views of %d bands each exceed 2^31 - 1 render items", fn, n, n_views,
+                rd.n_bands);
+  if (n == 0) return 0;
+  if (!windows) return fail("%s: null windows", fn);
+  if (reinterpret_cast<uintptr_t>(windows) % 8) return fail("%s: windows are not 8-byte aligned", fn);
+  const uint64_t rb = RecordLayout(eng->st.S, eng->st.G).bytes(), items = (uint64_t)n * n_views;
+  const Span outs[] = {{"frames", frames, items * rd.H * rd.W * 3, 1}, {"status", status, items, 1},
+                       {"windows", windows, items * 32, 8}};
+  if (check_outputs(fn, outs, 3, Span{"the records", records, records ? n * rb : 0, 16})) return 1;
+  std::optional<RenderLayout> plan;
+  if (check_render(eng, r, std::max(eng->max_spans, (int)span_class), &plan)) return 1;
+  CUDA_TRY(cudaSetDevice(eng->device));
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  CUDA_TRY(cudaMemsetAsync(status, 0, (size_t)items, stream));
+  return enqueue_render(eng, r, *plan, RenderTargets{{frames}, 1, 0, 0}, status, stream, 0, n, false,
+                        RenderRecords{static_cast<const unsigned char *>(records), (size_t)rb},
+                        RenderWindows{windows, n_views});
 }
 
 int swb_render_masks(swb_engine *eng, int32_t width, int32_t height, int32_t anti_aliasing,

@@ -83,6 +83,14 @@ struct RenderRecords {
   size_t record_bytes;
 };
 
+// The windows render_kernel<., ., ., true> draws through (swb_render_windows): item i is view
+// i % V of row i / V (live env or record), seen through win[4 i .. 4 i + 3] = (x0, y0, x1, y1) in
+// scene coordinates; frame i and status byte i are the item's.  Other instantiations do not read it.
+struct RenderWindows {
+  const double *win;
+  int V;
+};
+
 // Whether a raster needs render_kernel<., true>: tables beyond those of anti_aliasing <= 5
 inline bool render_wide(const RasterDev &rd) {
   return rd.v_nks > V_KS_NARROW || rd.tile_blocks != TILE_BLOCKS || rd.prefix_stride != kNarrowPrefixStride;
@@ -278,12 +286,18 @@ __constant__ uint32_t c_prmt_insert[4] = {0x3214u, 0x3240u, 0x3410u, 0x4210u};  
 // record's slots (read_record) instead of the pool entry at (e, cursor[e]) and the live positions,
 // with shape ids sanitised as a load sanitises them; frame e and status byte e are the record's.
 // Nothing indexed by env is read, so n may exceed E.  No peer variant.
-template <bool kPeers, bool kWide, bool kRecords>
+// kWindows: each row is drawn V times, through the windows of wins (swb_render_windows): phase A
+// maps a world vertex w to the canvas as trunc((w - x0) * (CW / (x1 - x0))) instead of
+// trunc(CW * w); everything after phase A is the raster's.  An item whose window is not finite or
+// empty, or with an occupied slot's window-space vertex NaN or at 2^30 or beyond (phase A's int32
+// differences are exact below that), gets SWB_ENV_BAD_WINDOW and a frame of zeros.  No peer variant.
+template <bool kPeers, bool kWide, bool kRecords, bool kWindows = false>
 __global__ void __launch_bounds__(R_THREADS, kWide ? R_CTAS_PER_SM_WIDE : R_CTAS_PER_SM)
 render_kernel(DevState st, RasterDev rd, const RenderLayout L, const RenderTargets targets,
               int env_base, int n_items, unsigned *work_counter, unsigned work_base,
-              const RenderRecords recs) {
+              const RenderRecords recs, const RenderWindows wins) {
   static_assert(!(kPeers && kRecords), "records render into one buffer");
+  static_assert(!(kPeers && kWindows), "windows render into one buffer");
   unsigned char *const smem = g_render_smem;
   const int tid = threadIdx.x;
   const int S = st.S;
@@ -353,7 +367,9 @@ render_kernel(DevState st, RasterDev rd, const RenderLayout L, const RenderTarge
   const int item = s_item;
   if (item >= n_items) break;
   const int band = rd.n_bands > 1 ? item % rd.n_bands : 0;
-  const int e = env_base + (rd.n_bands > 1 ? item / rd.n_bands : item);  // frames is indexed by the absolute env id
+  // frames is indexed by the absolute env id (with windows: by row * V + view)
+  const int e_out = env_base + (rd.n_bands > 1 ? item / rd.n_bands : item);
+  const int e = kWindows ? e_out / wins.V : e_out;  // the env or record drawn
 
   const int yo_b0 = band * rd.band_rows;
   const int yo_b1 = min(yo_b0 + rd.band_rows, rd.H);
@@ -383,6 +399,13 @@ render_kernel(DevState st, RasterDev rd, const RenderLayout L, const RenderTarge
                   ((uint32_t)rd.ay.win_cls[yo_b0 + i] << 24);
     band_loaded = band;
   }
+  // kWindows: whether this thread has seen a reason to flag the item
+  bool win_bad = false;
+  if constexpr (kWindows) {
+    const double *w = wins.win + (size_t)e_out * 4;
+    const double x0 = w[0], y0 = w[1], x1 = w[2], y1 = w[3];
+    win_bad = !(isfinite(x0) && isfinite(y0) && isfinite(x1) && isfinite(y1) && x1 > x0 && y1 > y0);
+  }
   for (int s = warp; s < S; s += NWARP) {
     // sprite record of this env's current scene, or slot s of record e (warp-uniform loads)
     const int scene = (e * st.K + cur) * S + s;
@@ -405,9 +428,20 @@ render_kernel(DevState st, RasterDev rd, const RenderLayout L, const RenderTarge
       const double cx = __dadd_rn(__dadd_rn(__dmul_rn(m00, v.x), __dmul_rn(m01, v.y)), 0.0);
       const double cy = __dadd_rn(__dadd_rn(__dmul_rn(m10, v.x), __dmul_rn(m11, v.y)), 0.0);
       const double wx = __dadd_rn(cx, px), wy = __dadd_rn(cy, py);
-      // canvas_size * vertices (pil_renderer.py:81), then Pillow's (int) cast
-      ivx = __double2int_rz(__dmul_rn((double)rd.CW, wx));
-      ivy = __double2int_rz(__dmul_rn((double)rd.CH, wy));
+      if constexpr (kWindows) {
+        // u = (wx - x0) * (CW / (x1 - x0)), each op rounded to nearest; the window is read again
+        // here (an L1 hit) rather than held in registers across the sprite loop
+        const double *w = wins.win + (size_t)e_out * 4;
+        const double u = __dmul_rn(__dsub_rn(wx, w[0]), __ddiv_rn((double)rd.CW, __dsub_rn(w[2], w[0])));
+        const double v = __dmul_rn(__dsub_rn(wy, w[1]), __ddiv_rn((double)rd.CH, __dsub_rn(w[3], w[1])));
+        win_bad |= !(fabs(u) < 0x1p30 && fabs(v) < 0x1p30);  // also NaN
+        ivx = __double2int_rz(u);
+        ivy = __double2int_rz(v);
+      } else {
+        // canvas_size * vertices (pil_renderer.py:81), then Pillow's (int) cast
+        ivx = __double2int_rz(__dmul_rn((double)rd.CW, wx));
+        ivy = __double2int_rz(__dmul_rn((double)rd.CH, wy));
+      }
     }
     // edge lane -> lane+1 (Pillow add_edge); the closing edge exists only if the last vertex
     // differs from the first
@@ -546,7 +580,10 @@ render_kernel(DevState st, RasterDev rd, const RenderLayout L, const RenderTarge
     asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
     copy_pending = false;
   }
-  __syncthreads();
+  // kWindows: a flagged item draws nothing (no phase B or C) and writes a frame of zeros
+  bool skip = false;
+  if constexpr (kWindows) skip = __syncthreads_or(win_bad);
+  else __syncthreads();
   SWB_MARK(3);
 
   // ---- phase B: visible segments per canvas row -----------------------------------------
@@ -555,7 +592,7 @@ render_kernel(DevState st, RasterDev rd, const RenderLayout L, const RenderTarge
   //    ROUND_UP/ROUND_DOWN pairing; horizontal edges) -> <= M merged spans.
   // B2 row-parallel: fold the sprites' spans front to back into the row's visible segments.
   // Sprites are taken front to back in chunks whose scratch (crossing lists + spans) fits.
-  for (int s_hi = S; s_hi > 0;) {
+  for (int s_hi = skip ? 0 : S; s_hi > 0;) {
     int s_lo = s_hi, rows_used = 0;
     if (s_hi == S && S <= 32) {  // common case: every sprite fits in one chunk
       const int rows_all = __reduce_add_sync(FULL, lane < S ? s_rcnt[lane] : 0);
@@ -716,7 +753,8 @@ render_kernel(DevState st, RasterDev rd, const RenderLayout L, const RenderTarge
   }
 
   {  // background fill of the staged frame (the scratch area is free again)
-    const uint32_t r = rd.bg & 255u, g = (rd.bg >> 8) & 255u, b = (rd.bg >> 16) & 255u;
+    const uint32_t bg = skip ? 0u : rd.bg;
+    const uint32_t r = bg & 255u, g = (bg >> 8) & 255u, b = (bg >> 16) & 255u;
     const int n_bytes = n_yo * rd.W * 3;
     if (r == g && g == b) {
       const uint32_t w = r * 0x01010101u;
@@ -810,7 +848,13 @@ render_kernel(DevState st, RasterDev rd, const RenderLayout L, const RenderTarge
       s_tile[slot][1] = make_int4(q0 | (q1 << 8), x4lo, x4hi, (int)c_inv20[(nx + H_NC - 1) / H_NC]);
     }
   };
-  if (warp == NWARP - 1) next_tile(0);
+  if (warp == NWARP - 1) {
+    if (skip) {
+      if (lane == 0) s_tile[0][0] = make_int4(0, 0, 0, 0);
+    } else {
+      next_tile(0);
+    }
+  }
   // the background (and later the tiles) is written through the generic proxy; the bulk copy of
   // phase D reads the staged frame through the async proxy
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
@@ -999,7 +1043,7 @@ render_kernel(DevState st, RasterDev rd, const RenderLayout L, const RenderTarge
   // peer memory: the frame gather of the multi-GPU path is issued by the kernel that produced
   // the frame and costs it one instruction per rank ----------------------------------------
   const int n_bytes = n_yo * row_bytes;
-  const size_t band_off = (size_t)(targets.env_offset + e) * rd.H * row_bytes + (size_t)(rd.H - yo_b1) * row_bytes;
+  const size_t band_off = (size_t)(targets.env_offset + e_out) * rd.H * row_bytes + (size_t)(rd.H - yo_b1) * row_bytes;
   // the bulk copy needs a 16-byte aligned size and destination address in every target; the
   // caller's buffers may start anywhere (a view at an odd offset), so test the address itself
   bool bulk = (n_bytes & 15) == 0;
@@ -1032,7 +1076,8 @@ render_kernel(DevState st, RasterDev rd, const RenderLayout L, const RenderTarge
     }
   }
   // several bands of one env may race here, but they all OR in the same bit
-  if (tid == 0 && s_overflow) st.render_status[e] |= (uint8_t)SWB_ENV_SPAN_OVERFLOW;
+  if (tid == 0 && s_overflow) st.render_status[e_out] |= (uint8_t)SWB_ENV_SPAN_OVERFLOW;
+  if (kWindows && tid == 0 && skip) st.render_status[e_out] |= (uint8_t)SWB_ENV_BAD_WINDOW;
   SWB_MARK(10);
   }  // item loop
   // the CTA's shared memory must stay until the engine has read it

@@ -505,6 +505,32 @@ class Engine(object):
         self._stream()))
     return frames, status
 
+  def render_windows(self, raster, windows, states=None, frames=None, status=None):
+    """The scene seen through windows (swb_render_windows): frame (i, v) is `raster`'s PILRenderer
+    frame of row i with the window windows[i, v] = (x0, y0, x1, y1) of scene coordinates stretched
+    over the whole raster, so (0, 0, 1, 1) draws what render() / render_states() draw.  Rows are the
+    live envs (n = n_envs), or with `states` EnvStates of any n records, as if loaded.  `windows`: a
+    contiguous float64 (n, V, 4) tensor on this device, V >= 1.  Returns (frames (n, V, H, W, 3)
+    uint8, status (n, V) uint8: ENV_BAD_WINDOW for an empty or non-finite window or a vertex 2^30
+    canvas pixels or more away, whose frame is zeros, and ENV_SPAN_OVERFLOW), new unless given.  One
+    launch on the current stream; nothing else changes."""
+    n, rec, rec_bytes = _rows(self, states)
+    if not isinstance(windows, torch.Tensor) or windows.dim() != 3 or windows.shape[-1] != 4 or windows.shape[1] < 1:
+      raise ValueError('windows must be a float64 (n, V, 4) tensor with V >= 1, got %s' % _describe(windows))
+    V = int(windows.shape[1])
+    _check_output(windows, 'windows', torch.float64, (n, V, 4), self.device, align=8)
+    if frames is None:
+      frames = torch.empty((n, V, raster.height, raster.width, 3), dtype=torch.uint8, device=self.device)
+    _check_output(frames, 'frames', torch.uint8, (n, V, raster.height, raster.width, 3), self.device)
+    if status is None:
+      status = torch.empty((n, V), dtype=torch.uint8, device=self.device)
+    _check_output(status, 'status', torch.uint8, (n, V), self.device)
+    span = 1 if states is None else states.span_class
+    _native.check(self._lib.swb_render_windows(
+        self._h, raster._h, rec, n, rec_bytes, span, _address(windows), V, _address(frames), _address(status),
+        self._stream()))
+    return frames, status
+
   def render_masks(self, width, height, anti_aliasing=1, states=None, out=None):
     """Sprite instance masks (swb_render_masks): uint8 (n, height, width), pixel value k + 1 where
     slot k is the top-most sprite covering the pixel's sample point on PILRenderer's

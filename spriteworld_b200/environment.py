@@ -21,7 +21,7 @@ from spriteworld_b200 import _dm_env as dm_env
 from spriteworld_b200 import _native, constants, scene
 from spriteworld_b200 import engine as engine_lib
 from spriteworld_b200 import sprite_generators
-from spriteworld_b200.renderers import handcrafted, pil_renderer
+from spriteworld_b200.renderers import glimpses, handcrafted, pil_renderer
 
 
 def _split_renderers(renderers):
@@ -33,9 +33,11 @@ def _split_renderers(renderers):
 
 
 def _color_map(pil_renderers):
+  """The one colour map of `pil_renderers` (PILRenderers, and in a BatchedEnvironment also
+  SpriteGlimpses: colours are packed into the scenes at upload), or None."""
   maps = {id(r.color_to_rgb): r.color_to_rgb for r in pil_renderers.values()}
   if len(maps) > 1:
-    raise NotImplementedError('all PILRenderers of one Environment must share color_to_rgb')
+    raise NotImplementedError('all PILRenderers and SpriteGlimpses of one Environment must share color_to_rgb')
   return next(iter(maps.values())) if maps else None
 
 
@@ -335,7 +337,9 @@ class BatchedEnvironment(object):
     unsupported = [n for n, r in self._other.items() if not hasattr(r, 'render_batch')]
     if unsupported:
       raise NotImplementedError('renderers %s have no batched form' % unsupported)
-    self._color_to_rgb = _color_map(self._pil)
+    self._glimpses = collections.OrderedDict(
+        (n, r) for n, r in self._other.items() if isinstance(r, glimpses.SpriteGlimpses))
+    self._color_to_rgb = _color_map(collections.OrderedDict(list(self._pil.items()) + list(self._glimpses.items())))
     self._nodes, self._filters = task.compile()
     task._filters_static()
     self._goal_distribs = task.goal_distributions()
@@ -372,6 +376,17 @@ class BatchedEnvironment(object):
         id(r): engine_lib._new_mask_outputs(self._engine, r._kind, E, r.width, r.height)
         for r in self._other.values() if isinstance(r, handcrafted._SpriteMaskRenderer)}
     self._coverage_buffers = self._soft_buffers = self._mask_buffers
+    # rasters of render_windows by (W, H, aa, bg), those of the SpriteGlimpses renderers made here
+    # (a raster the engine refuses fails the constructor, not a step), and each SpriteGlimpses
+    # renderer's views and their status by id(renderer), overwritten every step like the frames
+    self._window_rasters = {}
+    self._glimpse_buffers = {}
+    for r in self._glimpses.values():
+      self._window_raster(r)
+      V = len(r.slot_indices(slots))
+      self._glimpse_buffers[id(r)] = (
+          torch.empty((E, V, r.height, r.width, 3), dtype=torch.uint8, device=self._engine.device),
+          torch.empty((E, V), dtype=torch.uint8, device=self._engine.device))
     if sampler == 'device':
       self._init_device_sampler(seed, env_offset)
       return
@@ -928,14 +943,52 @@ class BatchedEnvironment(object):
     """Re-renders every PILRenderer, SpriteMasks, SpriteCoverage, SoftSpriteMasks and SpriteBoxes
     observation of the current state (a loaded one, say) into this environment's buffers, and
     returns them: dict name -> uint8 (n_envs, H, W, 3) frames, then uint8 (n_envs, H, W) masks,
-    coverage dicts, uint8 (n_envs, n_slots, H, W) soft masks and box dicts, in renderer order."""
+    coverage dicts, uint8 (n_envs, n_slots, H, W) soft masks, box dicts and uint8
+    (n_envs, V, H, W, 3) SpriteGlimpses views, in renderer order."""
     out = collections.OrderedDict()
     for name, r in self._rasters.items():
       out[name] = self._engine.render(r, self._frames[name])
     for name, r in self._other.items():
       if isinstance(r, handcrafted._SpriteMaskRenderer):
         out[name] = self._render_sprite_masks(type(r), r)
+      elif isinstance(r, glimpses.SpriteGlimpses):
+        out[name] = self._render_glimpses(r)
     return out
+
+  def render_windows(self, windows, renderer, states=None):
+    """The scene seen through windows (Engine.render_windows) on the current stream: (frames uint8
+    (n, V, H, W, 3), status uint8 (n, V)) for a float64 (n, V, 4) device tensor of windows
+    (x0, y0, x1, y1), each drawn as `renderer` (a PILRenderer or SpriteGlimpses whose colour map is
+    this environment's) draws its frame, with the window stretched over the whole raster.  Rows are
+    the live envs (n = n_envs), or with `states` EnvStates of any n records, as if loaded.  Status
+    holds ENV_BAD_WINDOW (an empty or non-finite window, or a vertex 2^30 canvas pixels or more
+    away; the frame is zeros) and ENV_SPAN_OVERFLOW.  New tensors; one launch, read-only."""
+    if not isinstance(renderer, (pil_renderer.PILRenderer, glimpses.SpriteGlimpses)):
+      raise ValueError('renderer must be a PILRenderer or SpriteGlimpses, got %s' % type(renderer).__name__)
+    if renderer.color_to_rgb is not self._color_to_rgb:
+      raise ValueError("renderer's color_to_rgb is not this environment's: colours are packed at upload")
+    return self._engine.render_windows(self._window_raster(renderer), windows, states)
+
+  def _window_raster(self, renderer):
+    """The Raster of render_windows for `renderer`'s size, anti_aliasing and background."""
+    key = (renderer.width, renderer.height, renderer.anti_aliasing, tuple(renderer.bg_color))
+    r = self._window_rasters.get(key)
+    if r is None:
+      r = self._window_rasters[key] = engine_lib.Raster(self._engine, *key)
+    return r
+
+  def _render_glimpses(self, renderer, states=None, status=None):
+    """SpriteGlimpses `renderer`'s views on the current stream: of the live envs into this
+    environment's buffers for the renderer (new tensors for one it does not own), or of EnvStates
+    `states` into a new tensor.  `status` (uint8 (n,)), if given, is ORed in place with each row's
+    view status (ENV_BAD_WINDOW, ENV_SPAN_OVERFLOW)."""
+    pos = self._engine.state_tensors() if states is None else states.fields()
+    frames, st = self._glimpse_buffers.get(id(renderer), (None, None)) if states is None else (None, None)
+    windows = renderer.windows(pos['pos_x'], pos['pos_y'])
+    frames, st = self._engine.render_windows(self._window_raster(renderer), windows, states, frames, st)
+    if status is not None:
+      status.bitwise_or_(st.amax(1))
+    return frames
 
   def _render_sprite_masks(self, cls, renderer, states=None):
     """`renderer`'s observation as a `cls` (SpriteMasks, SpriteCoverage, SoftSpriteMasks or
@@ -980,8 +1033,9 @@ class BatchedEnvironment(object):
     (n, H, W, 3) tensors (one render launch per raster; never this environment's own frame
     buffers), SpriteFactors dicts of (n, n_slots) tensors, SpriteMasks, SpriteCoverage and
     SoftSpriteMasks observations in new tensors (one launch each), SpriteBoxes observations in new
-    tensors (two launches each) -- and status uint8 (n,), the OR over the
-    rasters of their render status (_native.ENV_SPAN_OVERFLOW).
+    tensors (two launches each), SpriteGlimpses views as new uint8 (n, V, H, W, 3) tensors -- and
+    status uint8 (n,), the OR over the rasters of their render status (_native.ENV_SPAN_OVERFLOW)
+    and over the SpriteGlimpses views of theirs (also _native.ENV_BAD_WINDOW).
 
     Enqueued on the current stream without a host synchronisation.  Read-only: no env, scene ring,
     frame buffer or `rng` changes, and nothing counts against the ring's refill.  A renderer
@@ -998,6 +1052,10 @@ class BatchedEnvironment(object):
         frames, st = eng.render_states(self._rasters[name], states)
         obs[name] = frames
         status = st if status is None else status.bitwise_or_(st)
+      elif name in self._glimpses:
+        if status is None:
+          status = torch.zeros(len(states), dtype=torch.uint8, device=eng.device)
+        obs[name] = self._render_glimpses(self._glimpses[name], states, status)
       else:
         obs[name] = self._other[name].render_states(self, states)
     if status is None:
@@ -1133,7 +1191,7 @@ class BatchedEnvironment(object):
         self._pool = None
     if self._engine.device.type == 'cuda':
       torch.cuda.synchronize(self._engine.device)
-    for r in self._rasters.values():
+    for r in list(self._rasters.values()) + list(self._window_rasters.values()):
       r.close()
     self._engine.close()
 
@@ -1161,6 +1219,9 @@ class ShardedBatchedEnvironment(object):
     if any(isinstance(r, handcrafted.GoalPositions) for r in dict(config.get('renderers') or {}).values()):
       raise NotImplementedError('ShardedBatchedEnvironment does not gather GoalPositions across ranks; '
                                 "each rank's goals are self.local.goal_tensor()")
+    if any(isinstance(r, glimpses.SpriteGlimpses) for r in dict(config.get('renderers') or {}).values()):
+      raise NotImplementedError('ShardedBatchedEnvironment does not gather SpriteGlimpses across ranks; '
+                                "each rank's are in self.local's observations")
     import torch.distributed as dist
     from spriteworld_b200 import distributed
     self.group = group

@@ -18,7 +18,9 @@ Between those, env records: host-checked saves, loads and copies (disjoint and o
 run the device-checked calls' save and load kernels on int32 ids, and device-checked ones with int32
 and int64 device ids, valid and refused (out of range either way, 2^32 + 1, repeated destinations),
 so that memcheck sees that a refused id never indexes engine memory.  Then rollouts from records
-into leaves, from those leaves, and from the live envs into leaves, renders of records, the sprite
+into leaves, from those leaves, and from the live envs into leaves, renders of records, windows of
+live envs and records (swb_render_windows, flagged windows among them) on a narrow and a wide
+raster, the sprite
 coverage (swb_render_coverage) of live envs and records into buffers that are not 16-byte aligned,
 their soft masks (swb_render_soft_masks) into buffers at odd byte offsets, their boxes
 (swb_render_boxes) at 4-byte offsets that are not 16-byte aligned, and an engine
@@ -67,7 +69,7 @@ def main():
 
 
 def device_checked_records(torch):
-  from spriteworld_b200 import workloads
+  from spriteworld_b200 import engine, workloads
   wl = workloads.WORKLOADS['c2']()
   E = 40
   eng, raster, _ = workloads.build_engine(wl, E, 4, device=0, seed=4, max_episode_length=3)
@@ -114,6 +116,21 @@ def device_checked_records(torch):
   torch.cuda.synchronize()
   print('record renders: %d frames, %d overflowed, %d kernel launches'
         % (len(frames), int(status.bool().sum()), eng.launch_count()), flush=True)
+  # windows of the live envs and of the leaves: zoomed, off-scene and flagged (empty, NaN) windows
+  pos = eng.state_tensors()
+  win = torch.stack([pos['pos_x'] - 0.1, pos['pos_y'] - 0.05, pos['pos_x'] + 0.1, pos['pos_y'] + 0.15], -1)
+  win[0, 0] = torch.tensor([0.5, 0.0, 0.5, 1.0], dtype=torch.float64)
+  win[-1, -1] = torch.tensor([float('nan'), 0.0, 1.0, 1.0], dtype=torch.float64)
+  lwin = torch.tensor([-2.0, -2.0, 3.0, 3.0], dtype=torch.float64, device='cuda').repeat(len(res.leaves), 2, 1)
+  # the workload's raster and a wide one (anti_aliasing 7: render_kernel<false, true, *, true>)
+  wide = engine.Raster(eng, 64, 64, 7, (40, 40, 40))
+  for r in (raster, wide):
+    _, wstatus = eng.render_windows(r, win.contiguous())
+    eng.render_windows(r, lwin, res.leaves)
+  torch.cuda.synchronize()
+  wide.close()
+  print('window renders: %d views on 2 rasters, %d flagged, %d kernel launches'
+        % (2 * (wstatus.numel() + lwin.shape[0] * 2), int(wstatus.bool().sum()), eng.launch_count()), flush=True)
   # coverage of the live envs and of the leaves: odd widths at 4-byte offsets that are not
   # 16-byte aligned (the write-out's head and tail), bands of one and many rows, and zero records
   S = eng.n_slots
