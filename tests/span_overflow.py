@@ -146,12 +146,31 @@ def sprite_maxima(xy, W, H, aa, M):
   return int(crossings(ivx, ivy, CH, rows).max()), int(runs(own[rows, :, 0] != 0).max())
 
 
-def restate(W, H, aa, rec, shapes, M):
+_TABLES = {}
+
+
+def _shape_table(shapes):
+  key = tuple((k, np.asarray(v, np.float64).tobytes()) for k, v in sorted(shapes.items()))
+  if key not in _TABLES:
+    _TABLES[key] = oracle.shape_table(shapes)
+  return _TABLES[key]
+
+
+def restate(W, H, aa, rec, shapes, M, window=None):
   """The quantities phase B compares with its capacities, for one env.  rec: its sprite
   records, back to front; shapes: name -> vertices of the engine's shape table; M: the
   launch's span class.  Returns dict(crossings, spans, pieces): the maxima over every sprite
-  and every canvas row a band of the raster scans (the status is the OR over the bands)."""
+  and every canvas row a band of the raster scans (the status is the OR over the bands).
+
+  window: (x0, y0, x1, y1) of swb_render_windows.  The vertices are then the window-space ones
+  of tests/window_oracle.py; bands, capacities and conditions are the same.  An item flagged
+  ENV_BAD_WINDOW has no phase B: every maximum is 0."""
+  from tests import window_oracle
   CW, CH = W * aa, H * aa
+  if window is not None:
+    rc, tab = oracle.raster_cfg(W, H, aa), _shape_table(shapes)
+    if window_oracle.bad_window(rc, tab, rec, window):
+      return dict(crossings=0, spans=0, pieces=0)
   scanned = np.zeros(CH, bool)
   for b0, b1 in bands(H, aa):
     scanned[b0:b1] = True
@@ -162,7 +181,10 @@ def restate(W, H, aa, rec, shapes, M):
   for s, r in enumerate(rec):
     if not r['shape']:
       continue
-    xy = canvas_xy(r, shapes[names[int(r['shape'])]], CW, CH)
+    if window is None:
+      xy = canvas_xy(r, shapes[names[int(r['shape'])]], CW, CH)
+    else:
+      xy = window_oracle.window_vertices(rc, tab, r, window)
     c, n = sprite_maxima(xy, W, H, aa, M)
     out['crossings'], out['spans'] = max(out['crossings'], c), max(out['spans'], n)
     oracle.polygon_fill(lab, xy, (s + 1, 0, 0))

@@ -78,6 +78,33 @@ def test_every_shape_zoomed_on_itself():
       assert not bad and np.array_equal(got, wo.pillow_window([s], 32, 32, 5, win)), (shape, zoom)
 
 
+def test_far_zoom_windows_match_pillow():
+  """Windows zoomed so far that the sprites reach 2^15 .. 2^29 canvas units from the window's origin,
+  both signs on both axes, crossing the canvas: the restatement is Pillow's frame, and no vertex is
+  flagged (every one stays below 2^30)."""
+  rng = np.random.RandomState(11)
+  W, H, aa = 16, 12, 3
+  rc = oracle.raster_cfg(W, H, aa, (3, 4, 5))
+  reach = []
+  for t in range(8):
+    sprites, recs = _scene(rng, 2)
+    s = sprites[t % 2]
+    v = np.asarray(s.vertices, np.float64)
+    k = rng.randint(len(v))
+    p = v[k] + rng.rand() * (v[(k + 1) % len(v)] - v[k])     # a point of one of its edges
+    allv = np.concatenate([np.asarray(q.vertices, np.float64) for q in sprites])
+    far = 2.0 ** rng.uniform(15, 29)
+    sx = min(far / np.ptp(v, 0).max(), 2.0 ** 29 / np.abs(allv - p).max())
+    w, h = W * aa / sx, H * aa / sx
+    win = (p[0] - w * rng.uniform(0.2, 0.8), p[1] - h * rng.uniform(0.2, 0.8))
+    win = win + (win[0] + w, win[1] + h)
+    got, bad = wo.render_window(rc, TAB, recs, win)
+    assert not bad, (t, win)
+    assert np.array_equal(got, wo.pillow_window(sprites, W, H, aa, win, bg=(3, 4, 5))), (t, win)
+    reach.append(max(np.abs(wo.window_vertices(rc, TAB, r, win)).max() for r in recs))
+  assert max(reach) > 2.0 ** 28 and min(reach) > 2.0 ** 15, reach
+
+
 def test_bad_window_conditions():
   rc = oracle.raster_cfg(16, 16, 2)
   _, recs = _scene(np.random.RandomState(3), 3)

@@ -81,6 +81,28 @@ def test_restatement_counts_the_stripes_pieces():
     assert span_overflow.restate(64, 100, 5, rec, constants.SHAPES, M)['pieces'] == pieces
 
 
+def test_full_window_restates_the_frame_maxima():
+  """restate through the window (0, 0, 1, 1) is restate of the frame, on the scenes of every case
+  of the geometry, wide anti-aliasing and far sweeps (the first envs of each, and the ones whose
+  frame overflows): u = (wx - 0) * (CW / 1) is CW * wx exactly."""
+  from tests import test_gpu_render_far as far
+  from tests import test_gpu_render_geometry as geo
+  from tests import test_gpu_render_wide_aa as wide
+  n_flagged = 0
+  cases = ([(c, geo.case_arrays(c, geo._n_envs(c, geo.H100_SMS))) for c in geo.CASES + wide.CASES]
+           + [(c, far.case_arrays(c)) for c in far.CASES])
+  for case, arrs in cases:
+    cid, W, H, aa, bg, S, _, concave, kind = case
+    recs = fixtures.records_from_arrays(arrs)
+    M = 4 if concave else 1
+    for e in range(min(len(recs), 3)):
+      want = span_overflow.restate(W, H, aa, recs[e], constants.SHAPES, M)
+      got = span_overflow.restate(W, H, aa, recs[e], constants.SHAPES, M, window=(0.0, 0.0, 1.0, 1.0))
+      assert got == want, (cid, e, got, want)
+      n_flagged += bool(span_overflow.conditions(want, M, 16))
+  assert n_flagged > 0
+
+
 def test_bands_and_scratch_match_the_layout():
   # one band of 64 rows at aa 5: canvas rows 0..319; 100 rows: two bands that overlap
   assert span_overflow.bands(64, 5) == [(0, 320)]
