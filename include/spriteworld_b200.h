@@ -467,6 +467,24 @@ int swb_render_windows(swb_engine *eng, swb_raster *r, const void *records, int3
                        uint8_t *frames, uint8_t *status, void *stream);
 
 /*
+ * Views of chosen sprites: swb_render_windows with only some slots drawn.  Sprite layers (one slot
+ * drawn alone), scenes with sprites removed, glimpses of a sprite without its occluders.
+ *
+ * draw[(i * n_views + v) * S + s] (device u8, S the engine's slot count) is nonzero where slot s is
+ * drawn in view v of row i.  The view's frame and status are swb_render_windows' of the row in
+ * which every undrawn slot is an empty slot (shape 0; a record's undrawn slot is not read beyond
+ * its draw byte): the sprites drawn keep their back-to-front order, no slot drawn gives the
+ * background, every slot drawn gives swb_render_windows' frame byte for byte.  SWB_ENV_BAD_WINDOW
+ * and SWB_ENV_SPAN_OVERFLOW count drawn slots only.
+ *
+ * Refused besides what swb_render_windows refuses: a null draw, and a draw that overlaps frames or
+ * status.  A refused call enqueues nothing.
+ */
+int swb_render_views(swb_engine *eng, swb_raster *r, const void *records, int32_t n, uint64_t records_bytes,
+                     int32_t span_class, const double *windows, const uint8_t *draw, int32_t n_views,
+                     uint8_t *frames, uint8_t *status, void *stream);
+
+/*
  * Sprite instance masks (renderers.SpriteMasks): which sprite is visible at each pixel.  `masks`
  * is [n][height][width] uint8; mask i's pixel (r, c) is k + 1 if slot k is the top-most sprite whose
  * Pillow polygon fill -- the integer vertices int(canvas_size * vertex) PILRenderer draws at this

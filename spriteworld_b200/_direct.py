@@ -148,8 +148,9 @@ def _raster(eng, renderer):
   return raster
 
 
-def render_glimpses(renderer, sprites):
-  """(V, H, W, 3) uint8 SpriteGlimpses views of a Python sprite list: slot i is sprites[i]."""
+def render_views(renderer, sprites):
+  """(V, H, W, 3) uint8 SpriteGlimpses or SpriteLayers views of a Python sprite list: slot i is
+  sprites[i]."""
   n = len(sprites)
   V = len(renderer.slot_indices(n))
   if V == 0:
@@ -157,9 +158,9 @@ def render_glimpses(renderer, sprites):
   eng = _engine(max(1, n), _DUMMY_ACTION, _NO_TASK, True)
   _load(eng, sprites, (), renderer.color_to_rgb)
   pos = eng.state_tensors()
-  # n >= 1 here: the sprites fill slots S - n .. S - 1
-  windows = renderer.windows(pos['pos_x'][:, eng.n_slots - n:], pos['pos_y'][:, eng.n_slots - n:])
-  frames, status = eng.render_windows(_raster(eng, renderer), windows)
+  # n >= 1 here, so the n sprites fill the engine's n slots
+  windows, draw = renderer.views(pos['pos_x'], pos['pos_y'])
+  frames, status = eng.render_windows(_raster(eng, renderer), windows, draw=draw)
   # a flagged view is zeros, as in a BatchedEnvironment; a span overflow raises, as PILRenderer's does
   _raise_for_status(int(status.max().item()) & ~_native.ENV_BAD_WINDOW)
   return frames[0].cpu().numpy()

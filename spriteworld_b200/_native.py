@@ -134,6 +134,7 @@ def load():
   L.swb_rollout_trajectory.argtypes = L.swb_rollout_states.argtypes
   L.swb_render_states.argtypes = [vp, vp, vp, ci, ctypes.c_uint64, ci, vp, vp, vp]
   L.swb_render_windows.argtypes = [vp, vp, vp, ci, ctypes.c_uint64, ci, vp, ci, vp, vp, vp]
+  L.swb_render_views.argtypes = [vp, vp, vp, ci, ctypes.c_uint64, ci, vp, vp, ci, vp, vp, vp]
   L.swb_render_masks.argtypes = [vp, ci, ci, ci, vp, ci, ctypes.c_uint64, vp, vp]
   L.swb_render_coverage.argtypes = [vp, ci, ci, ci, vp, ci, ctypes.c_uint64, vp, vp, vp, vp]
   L.swb_render_soft_masks.argtypes = [vp, ci, ci, ci, vp, ci, ctypes.c_uint64, vp, vp]
@@ -181,7 +182,8 @@ EXPORTS = (
     'swb_sampler_pointers', 'swb_pool_pointers', 'swb_engine_state_bytes', 'swb_save_engine',
     'swb_load_engine', 'swb_pool_goal_pointer', 'swb_set_goals', 'swb_set_goals_dev', 'swb_evaluate_states',
     'swb_sample_contained', 'swb_render_coverage', 'swb_render_soft_masks', 'swb_render_boxes',
-    'swb_rollout_trajectory', 'swb_packer_load', 'swb_make_states', 'swb_render_windows')
+    'swb_rollout_trajectory', 'swb_packer_load', 'swb_make_states', 'swb_render_windows',
+    'swb_render_views')
 
 
 def check(rc):

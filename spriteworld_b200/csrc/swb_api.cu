@@ -247,7 +247,7 @@ int upload_axis(swb_raster *r, const AxisHost &h, AxisTables *d) {
 extern "C" {
 
 const char *swb_last_error(void) { return g_error.c_str(); }
-int swb_version(void) { return 18; }
+int swb_version(void) { return 19; }
 int swb_sizeof_config(void) { return (int)sizeof(swb_config); }
 int swb_sizeof_task_node(void) { return (int)sizeof(swb_task_node); }
 
@@ -1411,10 +1411,11 @@ int swb_render_states(swb_engine *eng, swb_raster *r, const void *records, int32
                         RenderRecords{static_cast<const unsigned char *>(records), (size_t)rb});
 }
 
-int swb_render_windows(swb_engine *eng, swb_raster *r, const void *records, int32_t n, uint64_t records_bytes,
-                       int32_t span_class, const double *windows, int32_t n_views, uint8_t *frames,
-                       uint8_t *status, void *stream_) {
-  static const char fn[] = "swb_render_windows";
+// swb_render_windows (draw NULL: every slot drawn) and swb_render_views (draw [n][n_views][S]).
+static int render_views_call(const char *fn, swb_engine *eng, swb_raster *r, const void *records, int32_t n,
+                             uint64_t records_bytes, int32_t span_class, const double *windows,
+                             const uint8_t *draw, int32_t n_views, uint8_t *frames, uint8_t *status,
+                             void *stream_) {
   if (!eng || !r) return fail("%s: null engine or raster", fn);
   if (check_rows(eng, fn, "records", records, n, records_bytes, true)) return 1;
   if (span_class != 1 && span_class != 4) return fail("%s: span_class must be 1 or 4, got %d", fn, span_class);
@@ -1431,6 +1432,11 @@ int swb_render_windows(swb_engine *eng, swb_raster *r, const void *records, int3
   const Span outs[] = {{"frames", frames, items * rd.H * rd.W * 3, 1}, {"status", status, items, 1},
                        {"windows", windows, items * 32, 8}};
   if (check_outputs(fn, outs, 3, Span{"the records", records, records ? n * rb : 0, 16})) return 1;
+  if (draw) {  // read-only like the windows and records: only the outputs may not overlap it
+    const Span d{"draw", draw, items * eng->st.S, 1};
+    for (int i = 0; i < 2; ++i)
+      if (overlap(d, outs[i])) return fail("%s: draw overlaps %s", fn, outs[i].name);
+  }
   std::optional<RenderLayout> plan;
   if (check_render(eng, r, std::max(eng->max_spans, (int)span_class), &plan)) return 1;
   CUDA_TRY(cudaSetDevice(eng->device));
@@ -1438,7 +1444,22 @@ int swb_render_windows(swb_engine *eng, swb_raster *r, const void *records, int3
   CUDA_TRY(cudaMemsetAsync(status, 0, (size_t)items, stream));
   return enqueue_render(eng, r, *plan, RenderTargets{{frames}, 1, 0, 0}, status, stream, 0, n, false,
                         RenderRecords{static_cast<const unsigned char *>(records), (size_t)rb},
-                        RenderWindows{windows, n_views});
+                        RenderWindows{windows, n_views, draw});
+}
+
+int swb_render_windows(swb_engine *eng, swb_raster *r, const void *records, int32_t n, uint64_t records_bytes,
+                       int32_t span_class, const double *windows, int32_t n_views, uint8_t *frames,
+                       uint8_t *status, void *stream) {
+  return render_views_call("swb_render_windows", eng, r, records, n, records_bytes, span_class, windows, nullptr,
+                           n_views, frames, status, stream);
+}
+
+int swb_render_views(swb_engine *eng, swb_raster *r, const void *records, int32_t n, uint64_t records_bytes,
+                     int32_t span_class, const double *windows, const uint8_t *draw, int32_t n_views,
+                     uint8_t *frames, uint8_t *status, void *stream) {
+  if (!draw) return fail("swb_render_views: null draw");
+  return render_views_call("swb_render_views", eng, r, records, n, records_bytes, span_class, windows, draw,
+                           n_views, frames, status, stream);
 }
 
 int swb_render_masks(swb_engine *eng, int32_t width, int32_t height, int32_t anti_aliasing,

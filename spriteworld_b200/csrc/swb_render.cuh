@@ -85,10 +85,13 @@ struct RenderRecords {
 
 // The windows render_kernel<., ., ., true> draws through (swb_render_windows): item i is view
 // i % V of row i / V (live env or record), seen through win[4 i .. 4 i + 3] = (x0, y0, x1, y1) in
-// scene coordinates; frame i and status byte i are the item's.  Other instantiations do not read it.
+// scene coordinates; frame i and status byte i are the item's.  With draw set (swb_render_views),
+// slot s of item i is drawn only where draw[i * S + s] is nonzero; an undrawn slot is an empty slot.
+// Other instantiations do not read it.
 struct RenderWindows {
   const double *win;
   int V;
+  const uint8_t *draw;
 };
 
 // Whether a raster needs render_kernel<., true>: tables beyond those of anti_aliasing <= 5
@@ -290,7 +293,9 @@ __constant__ uint32_t c_prmt_insert[4] = {0x3214u, 0x3240u, 0x3410u, 0x4210u};  
 // maps a world vertex w to the canvas as trunc((w - x0) * (CW / (x1 - x0))) instead of
 // trunc(CW * w); everything after phase A is the raster's.  An item whose window is not finite or
 // empty, or with an occupied slot's window-space vertex NaN or at 2^30 or beyond (phase A's int32
-// differences are exact below that), gets SWB_ENV_BAD_WINDOW and a frame of zeros.  No peer variant.
+// differences are exact below that), gets SWB_ENV_BAD_WINDOW and a frame of zeros.  With wins.draw
+// set, a slot whose draw byte is zero has shape 0 in phase A (a record's slot is not read further),
+// so it draws nothing and flags nothing.  No peer variant.
 template <bool kPeers, bool kWide, bool kRecords, bool kWindows = false>
 __global__ void __launch_bounds__(R_THREADS, kWide ? R_CTAS_PER_SM_WIDE : R_CTAS_PER_SM)
 render_kernel(DevState st, RasterDev rd, const RenderLayout L, const RenderTargets targets,
@@ -409,8 +414,10 @@ render_kernel(DevState st, RasterDev rd, const RenderLayout L, const RenderTarge
   for (int s = warp; s < S; s += NWARP) {
     // sprite record of this env's current scene, or slot s of record e (warp-uniform loads)
     const int scene = (e * st.K + cur) * S + s;
-    const SlotRecord r = kRecords ? read_record(st, rec, s) : SlotRecord{};
-    const int shape = kRecords ? r.shape : st.p_shape[scene];
+    // kWindows: an undrawn slot (a zero draw byte, warp-uniform) is an empty slot
+    const bool drawn = !kWindows || !wins.draw || wins.draw[(size_t)e_out * S + s];
+    const SlotRecord r = kRecords && drawn ? read_record(st, rec, s) : SlotRecord{};
+    const int shape = !drawn ? 0 : kRecords ? r.shape : st.p_shape[scene];
     const uint32_t col = kRecords ? r.rgb : st.p_rgb[scene];
     const double px = kRecords ? r.f64[POS_X] : st.pos_x[e * S + s];
     const double py = kRecords ? r.f64[POS_Y] : st.pos_y[e * S + s];

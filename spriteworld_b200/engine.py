@@ -505,7 +505,7 @@ class Engine(object):
         self._stream()))
     return frames, status
 
-  def render_windows(self, raster, windows, states=None, frames=None, status=None):
+  def render_windows(self, raster, windows, states=None, frames=None, status=None, draw=None):
     """The scene seen through windows (swb_render_windows): frame (i, v) is `raster`'s PILRenderer
     frame of row i with the window windows[i, v] = (x0, y0, x1, y1) of scene coordinates stretched
     over the whole raster, so (0, 0, 1, 1) draws what render() / render_states() draw.  Rows are the
@@ -513,12 +513,18 @@ class Engine(object):
     contiguous float64 (n, V, 4) tensor on this device, V >= 1.  Returns (frames (n, V, H, W, 3)
     uint8, status (n, V) uint8: ENV_BAD_WINDOW for an empty or non-finite window or a vertex 2^30
     canvas pixels or more away, whose frame is zeros, and ENV_SPAN_OVERFLOW), new unless given.  One
-    launch on the current stream; nothing else changes."""
+    launch on the current stream; nothing else changes.
+
+    `draw` (swb_render_views): a contiguous bool (n, V, n_slots) tensor on this device; view (i, v)
+    then draws only the slots s with draw[i, v, s], as if every other slot were empty, and its
+    status counts those slots only.  None draws every slot."""
     n, rec, rec_bytes = _rows(self, states)
     if not isinstance(windows, torch.Tensor) or windows.dim() != 3 or windows.shape[-1] != 4 or windows.shape[1] < 1:
       raise ValueError('windows must be a float64 (n, V, 4) tensor with V >= 1, got %s' % _describe(windows))
     V = int(windows.shape[1])
     _check_output(windows, 'windows', torch.float64, (n, V, 4), self.device, align=8)
+    if draw is not None:
+      _check_output(draw, 'draw', torch.bool, (n, V, self.n_slots), self.device)
     if frames is None:
       frames = torch.empty((n, V, raster.height, raster.width, 3), dtype=torch.uint8, device=self.device)
     _check_output(frames, 'frames', torch.uint8, (n, V, raster.height, raster.width, 3), self.device)
@@ -526,9 +532,14 @@ class Engine(object):
       status = torch.empty((n, V), dtype=torch.uint8, device=self.device)
     _check_output(status, 'status', torch.uint8, (n, V), self.device)
     span = 1 if states is None else states.span_class
-    _native.check(self._lib.swb_render_windows(
-        self._h, raster._h, rec, n, rec_bytes, span, _address(windows), V, _address(frames), _address(status),
-        self._stream()))
+    if draw is None:
+      _native.check(self._lib.swb_render_windows(
+          self._h, raster._h, rec, n, rec_bytes, span, _address(windows), V, _address(frames), _address(status),
+          self._stream()))
+    else:
+      _native.check(self._lib.swb_render_views(
+          self._h, raster._h, rec, n, rec_bytes, span, _address(windows), _address(draw), V, _address(frames),
+          _address(status), self._stream()))
     return frames, status
 
   def render_masks(self, width, height, anti_aliasing=1, states=None, out=None):

@@ -34,10 +34,11 @@ def _split_renderers(renderers):
 
 def _color_map(pil_renderers):
   """The one colour map of `pil_renderers` (PILRenderers, and in a BatchedEnvironment also
-  SpriteGlimpses: colours are packed into the scenes at upload), or None."""
+  SpriteGlimpses and SpriteLayers: colours are packed into the scenes at upload), or None."""
   maps = {id(r.color_to_rgb): r.color_to_rgb for r in pil_renderers.values()}
   if len(maps) > 1:
-    raise NotImplementedError('all PILRenderers and SpriteGlimpses of one Environment must share color_to_rgb')
+    raise NotImplementedError('all PILRenderers, SpriteGlimpses and SpriteLayers of one Environment must share '
+                              'color_to_rgb')
   return next(iter(maps.values())) if maps else None
 
 
@@ -337,9 +338,9 @@ class BatchedEnvironment(object):
     unsupported = [n for n, r in self._other.items() if not hasattr(r, 'render_batch')]
     if unsupported:
       raise NotImplementedError('renderers %s have no batched form' % unsupported)
-    self._glimpses = collections.OrderedDict(
-        (n, r) for n, r in self._other.items() if isinstance(r, glimpses.SpriteGlimpses))
-    self._color_to_rgb = _color_map(collections.OrderedDict(list(self._pil.items()) + list(self._glimpses.items())))
+    self._views = collections.OrderedDict(
+        (n, r) for n, r in self._other.items() if isinstance(r, glimpses._SpriteViews))
+    self._color_to_rgb = _color_map(collections.OrderedDict(list(self._pil.items()) + list(self._views.items())))
     self._nodes, self._filters = task.compile()
     task._filters_static()
     self._goal_distribs = task.goal_distributions()
@@ -376,12 +377,12 @@ class BatchedEnvironment(object):
         id(r): engine_lib._new_mask_outputs(self._engine, r._kind, E, r.width, r.height)
         for r in self._other.values() if isinstance(r, handcrafted._SpriteMaskRenderer)}
     self._coverage_buffers = self._soft_buffers = self._mask_buffers
-    # rasters of render_windows by (W, H, aa, bg), those of the SpriteGlimpses renderers made here
-    # (a raster the engine refuses fails the constructor, not a step), and each SpriteGlimpses
-    # renderer's views and their status by id(renderer), overwritten every step like the frames
+    # rasters of render_windows by (W, H, aa, bg), those of the SpriteGlimpses and SpriteLayers
+    # renderers made here (a raster the engine refuses fails the constructor, not a step), and each
+    # such renderer's views and their status by id(renderer), overwritten every step like the frames
     self._window_rasters = {}
     self._glimpse_buffers = {}
-    for r in self._glimpses.values():
+    for r in self._views.values():
       self._window_raster(r)
       V = len(r.slot_indices(slots))
       self._glimpse_buffers[id(r)] = (
@@ -944,30 +945,56 @@ class BatchedEnvironment(object):
     observation of the current state (a loaded one, say) into this environment's buffers, and
     returns them: dict name -> uint8 (n_envs, H, W, 3) frames, then uint8 (n_envs, H, W) masks,
     coverage dicts, uint8 (n_envs, n_slots, H, W) soft masks, box dicts and uint8
-    (n_envs, V, H, W, 3) SpriteGlimpses views, in renderer order."""
+    (n_envs, V, H, W, 3) SpriteGlimpses and SpriteLayers views, in renderer order."""
     out = collections.OrderedDict()
     for name, r in self._rasters.items():
       out[name] = self._engine.render(r, self._frames[name])
     for name, r in self._other.items():
       if isinstance(r, handcrafted._SpriteMaskRenderer):
         out[name] = self._render_sprite_masks(type(r), r)
-      elif isinstance(r, glimpses.SpriteGlimpses):
-        out[name] = self._render_glimpses(r)
+      elif isinstance(r, glimpses._SpriteViews):
+        out[name] = self._render_views(r)
     return out
 
-  def render_windows(self, windows, renderer, states=None):
+  def render_windows(self, windows, renderer, states=None, draw=None):
     """The scene seen through windows (Engine.render_windows) on the current stream: (frames uint8
     (n, V, H, W, 3), status uint8 (n, V)) for a float64 (n, V, 4) device tensor of windows
-    (x0, y0, x1, y1), each drawn as `renderer` (a PILRenderer or SpriteGlimpses whose colour map is
-    this environment's) draws its frame, with the window stretched over the whole raster.  Rows are
-    the live envs (n = n_envs), or with `states` EnvStates of any n records, as if loaded.  Status
-    holds ENV_BAD_WINDOW (an empty or non-finite window, or a vertex 2^30 canvas pixels or more
-    away; the frame is zeros) and ENV_SPAN_OVERFLOW.  New tensors; one launch, read-only."""
-    if not isinstance(renderer, (pil_renderer.PILRenderer, glimpses.SpriteGlimpses)):
-      raise ValueError('renderer must be a PILRenderer or SpriteGlimpses, got %s' % type(renderer).__name__)
+    (x0, y0, x1, y1), each drawn as `renderer` (a PILRenderer, SpriteGlimpses or SpriteLayers whose
+    colour map is this environment's) draws its frame, with the window stretched over the whole
+    raster.  Rows are the live envs (n = n_envs), or with `states` EnvStates of any n records, as if
+    loaded.  Status holds ENV_BAD_WINDOW (an empty or non-finite window, or a vertex 2^30 canvas
+    pixels or more away; the frame is zeros) and ENV_SPAN_OVERFLOW.  New tensors; one launch,
+    read-only.
+
+    `draw`: a bool tensor on this environment's device that broadcasts to (n, V, n_slots); view
+    (i, v) then draws only the slots s with draw[i, v, s], as if the others were empty (the scene
+    without sprite k, a sprite without its occluders), and its status counts those slots only.
+    None draws every slot."""
+    if not isinstance(renderer, (pil_renderer.PILRenderer, glimpses._SpriteViews)):
+      raise ValueError('renderer must be a PILRenderer or SpriteGlimpses or SpriteLayers, got %s'
+                       % type(renderer).__name__)
     if renderer.color_to_rgb is not self._color_to_rgb:
       raise ValueError("renderer's color_to_rgb is not this environment's: colours are packed at upload")
-    return self._engine.render_windows(self._window_raster(renderer), windows, states)
+    if draw is not None:
+      draw = self._broadcast_draw(draw, windows)
+    return self._engine.render_windows(self._window_raster(renderer), windows, states, draw=draw)
+
+  def _broadcast_draw(self, draw, windows):
+    """`draw` broadcast to (n, V, n_slots) for windows (n, V, 4), contiguous on the device.  A
+    `windows` that is not (n, V, 4) is left to Engine.render_windows to refuse."""
+    eng = self._engine
+    if not isinstance(draw, torch.Tensor) or draw.dtype != torch.bool or draw.device != eng.device:
+      raise ValueError('draw must be a bool tensor on %s, got %s' % (eng.device, engine_lib._describe(draw)))
+    if not isinstance(windows, torch.Tensor) or windows.dim() != 3:
+      return draw
+    shape = (int(windows.shape[0]), int(windows.shape[1]), eng.n_slots)
+    try:
+      ok = torch.broadcast_shapes(draw.shape, shape) == shape
+    except RuntimeError:
+      ok = False
+    if not ok:
+      raise ValueError('draw must broadcast to (n, V, n_slots) = %s, got %s' % (shape, engine_lib._describe(draw)))
+    return draw.expand(shape).contiguous()
 
   def _window_raster(self, renderer):
     """The Raster of render_windows for `renderer`'s size, anti_aliasing and background."""
@@ -977,15 +1004,15 @@ class BatchedEnvironment(object):
       r = self._window_rasters[key] = engine_lib.Raster(self._engine, *key)
     return r
 
-  def _render_glimpses(self, renderer, states=None, status=None):
-    """SpriteGlimpses `renderer`'s views on the current stream: of the live envs into this
-    environment's buffers for the renderer (new tensors for one it does not own), or of EnvStates
-    `states` into a new tensor.  `status` (uint8 (n,)), if given, is ORed in place with each row's
-    view status (ENV_BAD_WINDOW, ENV_SPAN_OVERFLOW)."""
+  def _render_views(self, renderer, states=None, status=None):
+    """SpriteGlimpses or SpriteLayers `renderer`'s views on the current stream: of the live envs
+    into this environment's buffers for the renderer (new tensors for one it does not own), or of
+    EnvStates `states` into a new tensor.  `status` (uint8 (n,)), if given, is ORed in place with
+    each row's view status (ENV_BAD_WINDOW, ENV_SPAN_OVERFLOW)."""
     pos = self._engine.state_tensors() if states is None else states.fields()
     frames, st = self._glimpse_buffers.get(id(renderer), (None, None)) if states is None else (None, None)
-    windows = renderer.windows(pos['pos_x'], pos['pos_y'])
-    frames, st = self._engine.render_windows(self._window_raster(renderer), windows, states, frames, st)
+    windows, draw = renderer.views(pos['pos_x'], pos['pos_y'])
+    frames, st = self._engine.render_windows(self._window_raster(renderer), windows, states, frames, st, draw)
     if status is not None:
       status.bitwise_or_(st.amax(1))
     return frames
@@ -1033,9 +1060,9 @@ class BatchedEnvironment(object):
     (n, H, W, 3) tensors (one render launch per raster; never this environment's own frame
     buffers), SpriteFactors dicts of (n, n_slots) tensors, SpriteMasks, SpriteCoverage and
     SoftSpriteMasks observations in new tensors (one launch each), SpriteBoxes observations in new
-    tensors (two launches each), SpriteGlimpses views as new uint8 (n, V, H, W, 3) tensors -- and
-    status uint8 (n,), the OR over the rasters of their render status (_native.ENV_SPAN_OVERFLOW)
-    and over the SpriteGlimpses views of theirs (also _native.ENV_BAD_WINDOW).
+    tensors (two launches each), SpriteGlimpses and SpriteLayers views as new uint8
+    (n, V, H, W, 3) tensors -- and status uint8 (n,), the OR over the rasters of their render status
+    (_native.ENV_SPAN_OVERFLOW) and over the views of theirs (also _native.ENV_BAD_WINDOW).
 
     Enqueued on the current stream without a host synchronisation.  Read-only: no env, scene ring,
     frame buffer or `rng` changes, and nothing counts against the ring's refill.  A renderer
@@ -1052,10 +1079,10 @@ class BatchedEnvironment(object):
         frames, st = eng.render_states(self._rasters[name], states)
         obs[name] = frames
         status = st if status is None else status.bitwise_or_(st)
-      elif name in self._glimpses:
+      elif name in self._views:
         if status is None:
           status = torch.zeros(len(states), dtype=torch.uint8, device=eng.device)
-        obs[name] = self._render_glimpses(self._glimpses[name], states, status)
+        obs[name] = self._render_views(self._views[name], states, status)
       else:
         obs[name] = self._other[name].render_states(self, states)
     if status is None:
@@ -1219,9 +1246,10 @@ class ShardedBatchedEnvironment(object):
     if any(isinstance(r, handcrafted.GoalPositions) for r in dict(config.get('renderers') or {}).values()):
       raise NotImplementedError('ShardedBatchedEnvironment does not gather GoalPositions across ranks; '
                                 "each rank's goals are self.local.goal_tensor()")
-    if any(isinstance(r, glimpses.SpriteGlimpses) for r in dict(config.get('renderers') or {}).values()):
-      raise NotImplementedError('ShardedBatchedEnvironment does not gather SpriteGlimpses across ranks; '
-                                "each rank's are in self.local's observations")
+    for cls in (glimpses.SpriteGlimpses, glimpses.SpriteLayers):
+      if any(isinstance(r, cls) for r in dict(config.get('renderers') or {}).values()):
+        raise NotImplementedError('ShardedBatchedEnvironment does not gather %s across ranks; '
+                                  "each rank's are in self.local's observations" % cls.__name__)
     import torch.distributed as dist
     from spriteworld_b200 import distributed
     self.group = group

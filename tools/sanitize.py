@@ -20,7 +20,7 @@ and int64 device ids, valid and refused (out of range either way, 2^32 + 1, repe
 so that memcheck sees that a refused id never indexes engine memory.  Then rollouts from records
 into leaves, from those leaves, and from the live envs into leaves, renders of records, windows of
 live envs and records (swb_render_windows, flagged windows among them) on a narrow and a wide
-raster, the sprite
+raster, and the same with random subsets of the sprites drawn (swb_render_views), the sprite
 coverage (swb_render_coverage) of live envs and records into buffers that are not 16-byte aligned,
 their soft masks (swb_render_soft_masks) into buffers at odd byte offsets, their boxes
 (swb_render_boxes) at 4-byte offsets that are not 16-byte aligned, and an engine
@@ -124,13 +124,22 @@ def device_checked_records(torch):
   lwin = torch.tensor([-2.0, -2.0, 3.0, 3.0], dtype=torch.float64, device='cuda').repeat(len(res.leaves), 2, 1)
   # the workload's raster and a wide one (anti_aliasing 7: render_kernel<false, true, *, true>)
   wide = engine.Raster(eng, 64, 64, 7, (40, 40, 40))
+  # views with random subsets drawn (swb_render_views), the flagged windows among them, and a
+  # draw that leaves the NaN window's row empty
+  draw = torch.rand(win.shape[:2] + (eng.n_slots,), device='cuda') < 0.5
+  draw[-1] = False
+  ldraw = torch.rand((len(res.leaves), 2, eng.n_slots), device='cuda') < 0.5
   for r in (raster, wide):
     _, wstatus = eng.render_windows(r, win.contiguous())
     eng.render_windows(r, lwin, res.leaves)
+    _, vstatus = eng.render_windows(r, win.contiguous(), draw=draw)
+    eng.render_windows(r, lwin, res.leaves, draw=ldraw)
   torch.cuda.synchronize()
   wide.close()
   print('window renders: %d views on 2 rasters, %d flagged, %d kernel launches'
         % (2 * (wstatus.numel() + lwin.shape[0] * 2), int(wstatus.bool().sum()), eng.launch_count()), flush=True)
+  print('view renders: %d views on 2 rasters, %d flagged'
+        % (2 * (vstatus.numel() + lwin.shape[0] * 2), int(vstatus.bool().sum())), flush=True)
   # coverage of the live envs and of the leaves: odd widths at 4-byte offsets that are not
   # 16-byte aligned (the write-out's head and tail), bands of one and many rows, and zero records
   S = eng.n_slots
